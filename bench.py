@@ -26,6 +26,7 @@ from pathlib import Path
 ROOT = Path(__file__).resolve().parent
 sys.path.insert(0, str(ROOT))
 
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 WORKLOAD = 'C2: LJ256 ForwardTransformer inference, B=64/GPU, 128 phonemes -> 1000 mel frames (forced durations+pitch)'
@@ -34,22 +35,12 @@ B, TP, TM = 64, 128, 1000
 METRIC, UNIT = 'mel_frames_per_sec_fwd', 'frames/s'
 
 
-def _traffic(key):
-    """DRAM bytes per launch of the roofline kernel from the committed ncu --set full capture (profiles/traffic.json,
-    written by profiles/summarize.py); None when no capture is committed."""
-    try:
-        with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'profiles', 'traffic.json')) as f:
-            return json.load(f).get(key)
-    except Exception:
-        return None
-
-
 def _peaks():
     f = ROOT / 'MEASURED_PEAKS.json'
     if f.exists():
         d = json.loads(f.read_text())
-        return float(d.get('bf16_tflops_sustained', d.get('bf16_tflops', 1590.0))), float(d.get('hbm_gbs', 6650.0)), 'measured (MEASURED_PEAKS.json, sustained bf16)'
-    return 1590.0, 6650.0, 'fallback (B200_PROFILING.md)'
+        return float(d.get('bf16_tflops_sustained', d.get('bf16_tflops', 989.0))), float(d.get('hbm_gbs', 3350.0)), 'measured (MEASURED_PEAKS.json, sustained bf16)'
+    return 989.0, 3350.0, 'fallback (NVIDIA H100 SXM data sheet: dense bf16, HBM3)'
 
 
 class ClockSampler:
@@ -172,8 +163,7 @@ def cpu_forward_rate(budget_s, min_passes=1, max_passes=8):
 
 def cpu_reference_line(args, rank, world):
     """--impl reference: the CPU path (oracle restatement of the TF2 graph) on the host cores.  Every step is the whole
-    64-row batch of the GPU arm's step (same config); when K+W whole steps do not fit the time budget the number of steps
-    actually run is reduced (and stated), never the step."""
+    64-row batch of the GPU arm's step (same config); exactly K timed steps after W warm-up steps."""
     from oracle import forward_oracle as fo
     if rank != 0:
         return None
@@ -192,9 +182,8 @@ def cpu_reference_line(args, rank, world):
     t0 = time.perf_counter()
     run()                                   # first whole step: also the estimate for the budget
     t1 = time.perf_counter() - t0
-    budget = 240.0
-    warm = max(0, min(args.warmup - 1, int(0.15 * budget / t1)))
-    steps = max(1, min(args.steps, int((budget - (1 + warm) * t1) / t1)))
+    warm = max(0, args.warmup - 1)          # the first step above counts as a warm-up step
+    steps = args.steps
     for _ in range(warm):
         run()
     t0 = time.perf_counter()
@@ -202,7 +191,7 @@ def cpu_reference_line(args, rank, world):
         run()
     dt = time.perf_counter() - t0
     val = B * TM * steps / dt
-    sample = (f'{steps} whole steps of {B} rows x {TM} frames (asked for {args.steps}; a whole step takes {t1:.1f} s on this host), '
+    sample = (f'{steps} whole steps of {B} rows x {TM} frames (a whole step takes {t1:.1f} s on this host), '
               f'torch-CPU fp32 oracle, {cores} threads')
     return {'impl': 'reference', 'metric': METRIC, 'value': val, 'unit': UNIT, 'n_gpus': args.gpus, 'steps': steps,
             'warmup': warm + 1, 'ms_per_step': dt / steps * 1e3, 'higher_is_better': True, 'scaling': 'weak',
@@ -224,8 +213,8 @@ def hbm_bench(args, rank, world, dev, cfg):
     from transformertts_b200 import lib
     from transformertts_b200.data.audio import Audio
     _, peak_hbm, _ = _peaks()
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
-    steps = max(args.steps, 10)
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 50 MB L2
+    steps = args.steps
     times = []
     if args.mode == 'stft':
         n_clips, n_samples = 256, 220500
@@ -394,7 +383,7 @@ def train_bench(args, rank, world, dev, cfg, params, steps=None):
                        'model': CFG_NAME, 'global_batch': Bt * world, 'seq_len': TM,
                        'parallelism': f'dp{world} (NCCL all-reduce of the flat fp32 gradient in 2 buckets, decoder bucket overlapped with the encoder backward)',
                        'launch': 'eager' if args.no_graphs else 'CUDA graphs (forward + decoder backward | encoder backward), Adam and the NCCL all-reduces launched eagerly',
-                       'l2': 'per-step working set exceeds the 126 MB L2'},
+                       'l2': 'per-step working set exceeds the 50 MB L2'},
             'frames_per_sec': sps * Bt * TM * world,
             'ms_per_step_without_allreduce': ms_local, 'nccl_exposed_ms': max(0.0, ms_step - ms_local) if world > 1 else 0.0,
             'allreduce_bytes_per_step': int(eng.flat_g.numel() * 4) if world > 1 else 0,
@@ -517,7 +506,7 @@ def aligner_bench(args, rank, world, dev):
                 'config': {'workload': 'C5: Aligner teacher-forced forward + validation losses (mel MAE, scaled stop CE, diagonal loss), '
                                        '16 rows/GPU, 130 tokens, 800 decoder frames, r=1, aligner_settings as shipped; train_step = the full training step',
                            'model': 'A5', 'global_batch': B * world, 'seq_len': T, 'parallelism': f'independent replicas x{world}',
-                           'l2': 'working set (~0.6 GB of activations + attention maps) exceeds the 126 MB L2'},
+                           'l2': 'working set (~0.6 GB of activations + attention maps) exceeds the 50 MB L2'},
                 'frames_per_sec': sps * B * T * world,
                 'e2e': {'value': args.steps / float(dt.item()) * world, 'unit': 'steps/s',
                         'h2d_bytes_per_step': int(tok.numel() * 4 + mel.numel() * 4 + stop.numel() * 4), 'd2h_bytes_per_step': 4},
@@ -532,6 +521,31 @@ def aligner_bench(args, rank, world, dev):
         print(json.dumps(line), flush=True)
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out: dict, path: str) -> None:
+    """Write every tensor of a step's output dict as <path>/<name>.npy (float32, float64 kept), 64 MB in all at most: an array
+    that does not fit what is left is replaced by a fixed, seeded sample of its flattened elements (indices in order)."""
+    d = Path(path)
+    d.mkdir(parents=True, exist_ok=True)
+    left = DUMP_LIMIT_BYTES
+    for name in sorted(out):
+        v = out[name]
+        if not torch.is_tensor(v):
+            continue
+        a = v.detach().cpu()
+        a = (a.double() if a.dtype == torch.float64 else a.float()).numpy()
+        if a.nbytes > left:
+            n = max(0, left // a.itemsize)
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=min(n, a.size), replace=False))
+            a = a.reshape(-1)[idx]
+        if a.size == 0:
+            continue
+        np.save(d / f'{name}.npy', a)
+        left -= a.nbytes
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
@@ -542,10 +556,16 @@ def main():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-graphs', action='store_true', help='inference: eager launches instead of CUDA-graph replay')
     ap.add_argument('--no-train', action='store_true', help='default mode: skip the C3 training-step record')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last timed step returned as DIR/<name>.npy (float32, <= 64 MB)')
     ap.add_argument('--mode', default='infer', choices=['infer', 'train', 'stft', 'expand', 'aligner'],
                     help="'train': BASELINE configs[2] (fwd+bwd+Adam, bf16, batch 32/GPU, NCCL data parallel); 'stft': configs[3] "
                          "(STFT->mel, 256 clips x 10 s); 'expand': the length regulator alone (C2-LR)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
+    if args.dump_outputs and (args.mode != 'infer' or args.impl != 'ours'):
+        ap.error('--dump-outputs writes the outputs of the default inference path (--mode infer, --impl ours) only')
     args.warmup = max(args.warmup, 3) if args.impl == 'ours' else args.warmup
 
     rank = int(os.environ.get('RANK', '0'))
@@ -614,6 +634,8 @@ def main():
     e1.record()
     barrier()
     launches = lib.launch_count()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(out, args.dump_outputs)
     ms = e0.elapsed_time(e1)
     t = torch.tensor([ms], device=dev)
     if world > 1:
@@ -636,7 +658,7 @@ def main():
     conv_share = sum(dur_ms) / 3 / (ms / args.steps) if dur_ms else None
     roofline = {'bound': 'tensor', 'kernel': 'gemm_tc_kernel (decoder Conv1D k=3 GEMMs: 256->1024 and 1024->256, M=64000)',
                 'achieved': gemm_tf, 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': gemm_tf / peak_tf if gemm_tf else None,
-                'traffic': _traffic('conv_gemm_mean_bytes_per_launch'), 'traffic_source': _traffic('source'),
+                'traffic': None,
                 'peak_source': peak_src, 'launches_timed': len(dur_ms),
                 'avg_launch_ms': sum(dur_ms) / len(dur_ms) if dur_ms else None,
                 'algorithmic_gflop_per_launch': sum(flops) / len(flops) / 1e9 if flops else None,
@@ -722,7 +744,7 @@ def main():
                 'config': {**_config_dict(world),
                            'parallelism': f'batch-sharded replicas x{world}, no collective (inference)',
                            'launch': 'eager' if args.no_graphs else 'CUDA graphs (encoder half + decoder half, replayed; outputs copied out of the static buffers)',
-                           'l2': 'no explicit flush: per-step working set (~1.5 GB of activations) exceeds the 126 MB L2'},
+                           'l2': 'no explicit flush: per-step working set (~1.5 GB of activations) exceeds the 50 MB L2'},
                 'e2e': {'value': e2e_val, 'unit': UNIT, 'h2d_bytes_per_step': int(h2d), 'd2h_bytes_per_step': int(d2h)},
                 'gpu_launches': int(launches), 'clocks': clocks, 'roofline': roofline,
                 'model_tflops': model_tf, 'algorithmic_gflop_per_step_per_gpu': step_flops / 1e9,

@@ -1,5 +1,5 @@
 /*
- * ttsb.h -- C ABI of libttsb.so, the B200 (sm_100a) kernels behind the ForwardTransformer text->mel hot path
+ * ttsb.h -- C ABI of libttsb.so, the H100 (sm_90a) kernels behind the ForwardTransformer text->mel hot path
  * of as-ideas/TransformerTTS.
  *
  * The reference has no FFI/plugin interface: its boundary is the Python API (model/models.py:344-642,
@@ -38,7 +38,7 @@ extern "C" {
 #define TTSB_PREC_BF16X3 1 /* hi*hi + lo*hi + hi*lo, fp32 accumulate (fp32-class accuracy) */
 #define TTSB_PREC_FP16 2   /* ttsb_mha_fwd only: single IEEE fp16 pass (11-bit mantissa), q/k/vT hold fp16 */
 
-/* implementation selector (debug): tcgen05/TMA kernels, or the plain SIMT CUDA kernels kept for bring-up */
+/* implementation selector (debug): the tensor-core (wgmma/TMA) kernels -- TTSB_IMPL named "tcgen05" for API stability -- or the plain SIMT CUDA kernels kept for bring-up */
 #define TTSB_IMPL_TCGEN05 0
 #define TTSB_IMPL_SIMT 1
 

@@ -8,7 +8,7 @@ checker / reported CPU baseline.
 PARITY STATUS: the reference's arithmetic lives in TensorFlow/Keras (``tensorflow>=2.2.0``, ``requirements.txt:7``), which
 is not installed here and cannot be installed (no network), and the reference's own tests hold no golden vectors for this
 path (SURVEY.md section 4).  This restatement is pinned to the REFERENCE'S OWN CODE instead: tests/test_reference_shim.py
-imports the unmodified /root/reference/model/{layers,models,transformer_utils}.py and utils/losses.py, runs them on
+imports the reference's unmodified model/{layers,models,transformer_utils}.py and utils/losses.py, runs them on
 tests/tf_shim (a torch-backed stand-in for the TensorFlow/Keras primitives, semantics from the TF documentation; the
 reference's tests/test_loss.py known answers pass on it) and compares ``ForwardTransformer.call`` / ``predict`` / ``_train_step``
 (loss, every gradient, Keras Adam) with this file on C1 / LJ256 / LJ256-dense / REF384: agreement 2e-5 (mel), 1e-5 (attention),

@@ -1,20 +1,92 @@
-"""Helpers that run the UNMODIFIED reference sources (/root/reference) on top of tests/tf_shim (test infrastructure only).
+"""Helpers that run the UNMODIFIED reference sources on top of tests/tf_shim (test infrastructure only), and the stored
+records of those runs that tests/test_reference_shim.py compares with.
 
-`available()` is False where /root/reference does not exist (the GPU box): the tests that need it skip there and use the
-golden vectors this module's users committed under tests/golden/ instead."""
+The reference checkout is found through $TTS_REFERENCE; it is needed only to regenerate the records
+(tests/golden/make_golden_shim.py, tests/golden/make_golden_ref.py).  The tests themselves read tests/golden/ref_shim.*."""
 from __future__ import annotations
 
+import json
+import os
 import sys
+import zlib
 from pathlib import Path
 
+import numpy as np
 import torch
 
-REFERENCE = Path('/root/reference')
+REFERENCE = Path(os.environ.get('TTS_REFERENCE', '')) if os.environ.get('TTS_REFERENCE') else None
 SHIM = Path(__file__).resolve().parent / 'tf_shim'
+GOLDEN = Path(__file__).resolve().parent / 'golden'
+
+# the cases the records were produced for (tests/golden/make_golden_shim.py and tests/test_reference_shim.py share them)
+CASES = [('C1', 3, 40, 200, 101), ('LJ256', 2, 48, 300, 201), ('LJ256-dense', 2, 32, 180, 202), ('REF384', 2, 24, 150, 203)]
+PRED_SETTINGS = [(1.0, None, None), (0.8, 2.0, None), (1.25, None, 6.0)]   # speed, max duration of symbol a, min of symbol b
+PE_CASES = [(50, 128), (2000, 256), (333, 384)]
+LR_SCHED = [[0, 1.0e-4], [40000, 1.0e-4], [41000, 5.0e-5], [100000, 1.0e-5]]
+LR_STEPS = [0, 1, 39999, 40000, 40500, 40999, 41000, 77777, 100000, 250000]
+RED_SCHED = [[0, 10], [80000, 5], [150000, 3], [250000, 1]]
+RED_STEPS = [0, 79999, 80000, 200000, 999999]
+SPEC_SEED = 12
+TOKENIZER_MODES = [(False, False), (True, False), (False, True), (True, True)]
+META_TEXT = ('LJ001-0001.wav|Printing, in the only sense|printing in the only sense\nLJ001-0002|really?|really?\n'
+             'LJ001-0003|stop!|stop!\n')
+ALIGNER_PRED_CASES = [(4, False), (1, False), (2, True)]
+
+
+def spec_inputs(seed: int):
+    """Seeded inputs of the spectrogram-op / loss comparison."""
+    g = torch.Generator().manual_seed(seed)
+    mel = torch.randn(3, 9, 4, generator=g)
+    mel[0, 6:] = 0
+    mel[1, 2:] = 0
+    ph = torch.tensor([[4, 5, 6, 0, 0], [9, 0, 0, 0, 0], [1, 2, 3, 4, 5]], dtype=torch.int32)
+    tgt, pred = torch.randn(2, 7, 5, generator=g), torch.randn(2, 7, 5, generator=g)
+    logits = torch.randn(2, 6, 3, generator=g)
+    targets = torch.tensor([[1, 1, 1, 2, 0, 0], [1, 2, 0, 0, 0, 0]])
+    return mel, ph, tgt, pred, logits, targets
+
+
+def sample_index(n: int, k: int, key: str) -> np.ndarray:
+    """Fixed, seeded sample of k of n flat indices (all of them when n <= k), in increasing order."""
+    if n <= k:
+        return np.arange(n)
+    return np.sort(np.random.default_rng(zlib.crc32(key.encode())).choice(n, size=k, replace=False))
+
+
+_GOLD = None
+
+
+def golden():
+    """(arrays, records) written by tests/golden/make_golden_shim.py."""
+    global _GOLD
+    if _GOLD is None:
+        with np.load(GOLDEN / 'ref_shim.npz') as z:
+            arrays = {k: z[k] for k in z.files}
+        _GOLD = (arrays, json.loads((GOLDEN / 'ref_shim.json').read_text()))
+    return _GOLD
+
+
+def expect(key: str, got, tol: float = 0.0):
+    """Compare `got` with the stored reference record `key`: same shape, and at the stored (sampled) elements within tol
+    (bit-exact when tol == 0)."""
+    arrays, js = golden()
+    g = torch.as_tensor(got).detach().cpu()
+    assert list(g.shape) == js['shape/' + key], (key, list(g.shape), js['shape/' + key])
+    want = arrays[key]
+    flat = g.reshape(-1)
+    if want.size != flat.numel():
+        flat = flat[torch.from_numpy(sample_index(flat.numel(), want.size, key))]
+    a = flat.numpy()
+    if tol == 0.0:
+        assert np.array_equal(a.astype(want.dtype), want), key
+        return 0.0
+    err = float(np.abs(a.astype(np.float64) - want.astype(np.float64)).max()) if want.size else 0.0
+    assert err <= tol, (key, err)
+    return err
 
 
 def available() -> bool:
-    return (REFERENCE / 'model' / 'models.py').exists()
+    return REFERENCE is not None and (REFERENCE / 'model' / 'models.py').exists()
 
 
 def real_tensorflow_available() -> bool:
@@ -27,7 +99,7 @@ def real_tensorflow_available() -> bool:
 def activate(real_tf: bool = False):
     """Put the reference tree (and, unless real_tf, the shim packages) on sys.path (idempotent)."""
     if not available():
-        raise RuntimeError('/root/reference is not present on this machine')
+        raise RuntimeError('set TTS_REFERENCE to a checkout of the reference to run it')
     paths = (str(REFERENCE),) if real_tf else (str(REFERENCE), str(SHIM))
     for p in paths:
         if p in sys.path:
@@ -122,7 +194,7 @@ def aligner_named_parameters(model, cfg: dict) -> dict:
 
 
 def reference_forward_transformer(cfg: dict, params: dict, warm_inputs, **overrides):
-    """Instantiate /root/reference/model/models.py:ForwardTransformer (unmodified) under the shim with `params`.
+    """Instantiate the reference's model/models.py:ForwardTransformer (unmodified) under the shim with `params`.
     `warm_inputs` = (tokens, durations (B,Tp,1), pitch (B,Tp,1)): one throw-away call creates the Keras variables (the
     reference's own build_model_weights() feeds a 1x1 dummy, which produces an empty decoder input)."""
     activate()
@@ -143,7 +215,7 @@ def reference_forward_transformer(cfg: dict, params: dict, warm_inputs, **overri
 
 
 def reference_aligner(cfg: dict, params: dict, warm_inputs, **overrides):
-    """Instantiate /root/reference/model/models.py:Aligner (unmodified) under the shim with `params`."""
+    """Instantiate the reference's model/models.py:Aligner (unmodified) under the shim with `params`."""
     activate()
     from model.models import Aligner  # the reference class
     kw = {k: v for k, v in cfg.items() if k not in ('vocab_size', 'stop_loss_scaling')}

@@ -65,7 +65,7 @@ def test_argument_validation_without_gpu(cdll):
     # the training attention kernels: the support query is pure host logic; bad arguments are refused before any CUDA call
     assert cdll.ttsb_attn_probs_supported(128, 1008) == 1 and cdll.ttsb_attn_probs_supported(64, 48) == 1
     assert cdll.ttsb_attn_probs_supported(192, 208) == 1
-    assert cdll.ttsb_attn_probs_supported(256, 1008) == 0      # Q tile + K ring + staging boxes exceed 227 KB
+    assert cdll.ttsb_attn_probs_supported(256, 1008) == 0      # head sizes above 192 take the two-kernel path
     assert cdll.ttsb_attn_probs_supported(96, 1008) == 0 and cdll.ttsb_attn_probs_supported(128, 1001) == 0
     assert cdll.ttsb_attn_probs_fwd(None, 768, 0, 256, 1, 2, 100, 128, None, C.c_float(0.1), C.c_float(0.1), 0, 0, None, None, 112, None) == -1
     assert b'ttsb_attn_probs_fwd' in cdll.ttsb_last_error()

@@ -1,6 +1,6 @@
 """Data-parallel training on NCCL (BASELINE.json configs[2]; the reference has no distributed code): a step on two 16-row
 shards with the gradient all-reduce must be the step of one process on the 32-row batch.  Needs 2 GPUs
-(`gpurun --gpus 2 -- python -m pytest tests/test_gpu_dp.py -m gpu`); skipped on a 1-GPU box."""
+(`python -m pytest tests/test_gpu_dp.py -m gpu` on a machine with two GPUs); skipped on a 1-GPU machine."""
 import subprocess
 import sys
 from pathlib import Path
@@ -37,9 +37,8 @@ def test_dp_step_equals_single_process_step(tmp_path):
     # (2) against ONE step on the whole 32-row batch.  The arithmetic per batch row is the same, but the partial sums are
     # cut differently (weight-gradient reductions split over 16 vs 32 batch rows, encoder-side GEMMs of 768 vs 1536 rows
     # tiled differently, fp32 atomics), and a bf16 rounding that flips upstream moves everything downstream of it, so the
-    # difference grows towards the embedding end of the backward chain.  Measured (B200, LJ256, 32 x 320 frames): largest
-    # element 2.1e-4 of the largest gradient (encoder.pos_scalar, a single number summed from 10^5 cancelling products),
-    # 3.4e-4 in norm; check (1) is the one that pins the exchange.
+    # difference grows towards the embedding end of the backward chain, largest at encoder.pos_scalar (a single number
+    # summed from 10^5 cancelling products); check (1) is the one that pins the exchange.
     print('DP vs single process on the whole batch:', worst(g1, g2), float((g1 - g2).norm() / g1.norm()))
     assert float((g1 - g2).abs().max()) < 6e-4 * gscale, worst(g1, g2)
     assert float((g1 - g2).norm() / g1.norm()) < 1e-3

@@ -256,7 +256,7 @@ def test_gemm_predictor_226_columns_and_mel_80(impl):
 
 @pytest.mark.parametrize('precision', PRECS)
 def test_gemm_persistent_many_tiles(precision):
-    """More tiles than SMs: exercises the persistent loop, both TMEM accumulator stages and the smem ring wrap."""
+    """More tiles than SMs: exercises the persistent loop, the accumulator image over the drained ring and the smem ring wrap."""
     from gpu_util import ref_gemm, run_gemm
     g = torch.Generator().manual_seed(14)
     B, T, d, F = 40, 1000, 256, 1024

@@ -226,7 +226,7 @@ def test_train_step_loss_grads_and_adam(cfg_name, B, Tp, Tm, tol_emu, cos_emu, t
     """One deterministic training step (dropout off): loss, every parameter gradient and the Adam update against torch
     autograd on the restated graph -- once with the oracle's matrix products fed bf16-rounded operands like the tensor-core
     path (forward_oracle.EMULATE_BF16: what remains is summation order and the decorrelation of individual roundings), once
-    against the plain fp32 oracle.  Gates come from tools/grad_noise.py measurements (profiles/r02_grad_noise.md) with ~1.5x
+    against the plain fp32 oracle.  Gates come from tools/grad_noise.py measurements of the step's gradient noise with ~1.5x
     margin; the pos_encoding_scalar gradients (one number each, heavy cancellation) are gated on sign and a factor of two."""
     torch.set_num_threads(8)
     from transformertts_b200.model.models import ForwardTransformer
@@ -477,7 +477,7 @@ def test_train_tts_from_disk_dataset(tmp_path):
     assert 1 in losses and math.isfinite(losses[1]) and 'validation loss at step 3' in out and 'Done.' in out
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason='needs 2 GPUs (run with gpurun --gpus 2)')
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason='needs 2 GPUs')
 def test_train_tts_from_disk_dataset_data_parallel(tmp_path):
     """The same under torchrun with 2 ranks: each rank takes its row slice of every global batch, NCCL all-reduce of the
     gradient buckets, identical weights on both ranks afterwards (checked through the printed loss being finite and the run
@@ -618,7 +618,7 @@ def test_layernorm_bwd_vectorised_and_fused_column_sums(C):
 
 @pytest.mark.parametrize('H,dh,T,rate', [(2, 128, 1000, 0.1), (2, 64, 333, 0.1), (2, 192, 200, 0.0), (1, 128, 130, 0.25)])
 def test_fused_attention_probabilities_match_two_kernel_path(H, dh, T, rate):
-    """ttsb_attn_probs_fwd (logits in TMEM, two passes) against the materialised path (ttsb_bgemm fp32 logits +
+    """ttsb_attn_probs_fwd (logits in registers, two passes) against the materialised path (ttsb_bgemm fp32 logits +
     ttsb_softmax_fwd) and an fp64 softmax: same probabilities to bf16 rounding, identical dropout decisions, exact zeros on
     masked keys and padded query rows, poisoned outputs fully overwritten."""
     lib = _lib()

@@ -1,5 +1,5 @@
-# Multi-GPU evidence run (gpurun --gpus 8): NCCL DP test on 2 ranks, then the default bench line under torchrun at the N given
-# in $SCALE_NS (default "8 2").  Box time is charged per GPU, so the list is short; the driver's own SCALE run covers 1/2/4/8.
+# Multi-GPU evidence run (on a machine with 8 GPUs): NCCL DP test on 2 ranks, then the default bench line under torchrun at the N given
+# in $SCALE_NS (default "8 2").
 set -x
 mkdir -p gpurun_out
 timeout 300 python -m pytest tests/test_gpu_dp.py -m gpu -x -q > gpurun_out/r02_dp_test.log 2>&1; tail -5 gpurun_out/r02_dp_test.log

@@ -2,8 +2,7 @@
 
     python tools/kbench.py mha  [--B 64 --T 1000 --H 2 --dh 128 --precision fp16]
 
-Prints one JSON line per case.  Used for A/B measurements of a single kernel (e.g. TTSB_ATT_NARROW=1); the
-numbers the judge reads come from bench.py, not from here.
+Prints one JSON line per case, for A/B measurements of a single kernel; the benchmark of record is bench.py.
 """
 import argparse
 import json
@@ -57,7 +56,7 @@ def bench_mha(a):
     ms = _time(lambda: lib.mha_fwd(m))
     flops = 4.0 * B * H * T * T * dh
     print(json.dumps({'kernel': 'mha_tc', 'B': B, 'T': T, 'H': H, 'dh': dh, 'precision': a.precision,
-                      'narrow': os.environ.get('TTSB_ATT_NARROW', '0'), 'us': round(ms * 1e3, 2),
+                      'us': round(ms * 1e3, 2),
                       'algorithmic_tflops': round(flops / ms / 1e9, 1)}))
 
 

@@ -1,4 +1,4 @@
-"""Build libttsb.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libttsb.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python -m transformertts_b200.build [--force]
 
@@ -20,7 +20,7 @@ INCLUDE = PKG.parent / 'include'
 OUT = PKG / 'libttsb.so'
 OBJ_DIR = PKG / 'build'
 SOURCES = ['host.cu', 'gemm_tc.cu', 'attention_tc.cu', 'bgemm_tc.cu', 'attn_probs_tc.cu', 'rowops.cu', 'stft_mel.cu', 'train_ops.cu', 'alignment.cu', 'dp_nccl.cu', 'griffin_lim.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=default', '--expt-relaxed-constexpr']
 
 
@@ -59,7 +59,7 @@ def build(force: bool = False, verbose: bool = True) -> Path:
 
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(compile_one, srcs))
-    cmd = [nvcc, '-shared', '-o', str(OUT), *objs, '-gencode', 'arch=compute_100a,code=sm_100a', '-Xcompiler', '-fPIC', '-ldl']
+    cmd = [nvcc, '-shared', '-o', str(OUT), *objs, '-gencode', 'arch=compute_90a,code=sm_90a', '-Xcompiler', '-fPIC', '-ldl']
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f'link failed:\n{r.stdout}\n{r.stderr}')

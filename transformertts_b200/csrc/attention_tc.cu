@@ -1,9 +1,10 @@
-// Fused variable-length self-attention on tcgen05 (flash-style, never materialises the (B,H,T,T) tensors):
-//   per CTA one (batch row, head, 128-query tile); loop over 64-key tiles:
-//     S = Q K^T  (tcgen05.mma, fp32 in TMEM)  ->  online softmax in registers (one thread per query row, exp2 domain,
-//     keys >= kv_len masked)  ->  P (bf16 hi/lo or fp16) written to 128B-swizzled shared memory  ->  O += P V
-//     (tcgen05.mma; V is read MN-major straight from the QKV buffer, no transposed copy)  ->  O rescaled in TMEM only
-//     when a row maximum moved.
+// Fused variable-length self-attention on wgmma (flash-style, never materialises the (B,H,T,T) tensors):
+//   per CTA one (batch row, head, 128-query tile); two consumer warpgroups own 64 query rows each, one producer warp streams
+//   64-key tiles of K and V through a two-stage TMA ring.  Per key tile and warpgroup:
+//     S = Q K^T  (wgmma, fp32 accumulators in registers)  ->  online softmax on the accumulator fragment (a row lives in the
+//     four lanes of a quad; exp2 domain, keys >= kv_len masked)  ->  P (bf16 hi/lo or fp16) re-packed in registers as the
+//     A operand of  O += P V  (wgmma; V is read MN-major straight from the QKV buffer, no transposed copy)  ->  O rescaled
+//     in registers only when a row maximum moved.
 // Replaces model/layers.py:123-129,138-147 (split/merge heads) and :176-195 (ScaledDotProductAttention) of the
 // reference, which materialise logits / softmax / dropout tensors of shape (B,H,T,T) in fp32.
 //
@@ -17,16 +18,16 @@
 #include "../../include/ttsb.h"
 #include "ttsb_common.cuh"
 #include "ttsb_host.h"
+#include "wgmma_sm90.cuh"
 
 namespace ttsb {
 
 constexpr int ATT_BQ = 128;
 constexpr int ATT_BKV = 64;
-// narrow layout: warps 0-3 softmax/epilogue (TMEM lane quarters 0-3), warp 4 TMA + MMA issue               (160 threads)
-// wide layout:   warps 0-7 softmax/epilogue, warp w owns lane quarter w&3 and column half w>>2 of every S/P/O tile,
-//                warp 8 TMA + MMA issue                                                                        (288 threads)
-constexpr int ATT_THREADS_NARROW = 160;
-constexpr int ATT_THREADS_WIDE = 288;
+constexpr int ATT_STAGES = 2;
+// warps 0-7: two softmax / MMA warpgroups (query rows [64*wg, +64)), warp 8: TMA producer (warps 9-11 idle: the producer
+// warpgroup hands its registers to the others with setmaxnreg)
+constexpr int ATT_THREADS = 384;
 
 // single MUFU.EX2 (no denormal fix-up code: p < 2^-126 flushes to 0, far below bf16/fp16 resolution of P)
 __device__ __forceinline__ float fast_exp2(float x) {
@@ -46,20 +47,7 @@ struct MhaKParams {
   __nv_bfloat16* out_lo;
   int ld_out;
   float scale_log2;  // log2(e)/sqrt(dh)
-#ifdef TTSB_ATT_TRACE
-  long long* trace;  // debug build only: clock64 stamps of CTA (0,0,0): [2 roles][64 tiles][8 events]
-#endif
 };
-
-#ifdef TTSB_ATT_TRACE
-#define ATT_TRACE(role, j, ev)                                                                         \
-  do {                                                                                                 \
-    if (p.trace && (threadIdx.x & 31) == 0 && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && (j) < 64)                 \
-      p.trace[((role) * 64 + (j)) * 8 + (ev)] = clock64();                                             \
-  } while (0)
-#else
-#define ATT_TRACE(role, j, ev) do {} while (0)
-#endif
 
 template <int DH, bool kSplit>
 struct MhaCfg {
@@ -67,23 +55,32 @@ struct MhaCfg {
   static constexpr int Q_BYTES = ATT_BQ * DH * 2;    // DH/64 panels of [128 x 64]
   static constexpr int K_BYTES = ATT_BKV * DH * 2;   // DH/64 panels of [64 x 64]
   static constexpr int V_BYTES = DH * ATT_BKV * 2;   // DH/64 boxes of [64 keys x 64 dh] (MN-major B operand)
-  static constexpr int P_BYTES = ATT_BQ * ATT_BKV * 2;
   static constexpr int OFF_Q = 0;
-  static constexpr int OFF_K = OFF_Q + kPlanes * Q_BYTES;
-  // three key/value slots: slot j%3 holds K_j until S_j has completed, then V_j until PV_j has completed, then K_{j+3}.
-  // Every load is therefore issued about one key tile ahead of its consumer (no TMA latency on the critical path).
-  static constexpr int K_STAGE = kPlanes * K_BYTES;
-  static constexpr int OFF_P = OFF_K + 3 * K_STAGE;
-  static constexpr int OFF_BAR = OFF_P + kPlanes * P_BYTES;
-  static constexpr int OFF_RED = OFF_BAR + 128;      // wide layout: row max [2 tiles][2 halves][128] + row sum [2][128]
-  static constexpr int kSmemBytes = OFF_RED + 3072 + 1024;
-  static constexpr int kTmemCols = (2 * ATT_BKV + DH) <= 128 ? 128 : ((2 * ATT_BKV + DH) <= 256 ? 256 : 512);
-  static constexpr int S_COL = 0;             // two S accumulators of ATT_BKV columns
-  static constexpr int O_COL = 2 * ATT_BKV;
+  // stage s holds K_j and V_j of every key tile j with j % ATT_STAGES == s: [K planes][V planes]
+  static constexpr int STAGE_BYTES = kPlanes * (K_BYTES + V_BYTES);
+  static constexpr int OFF_KV = OFF_Q + kPlanes * Q_BYTES;
+  static constexpr int OFF_BAR = OFF_KV + ATT_STAGES * STAGE_BYTES;
+  static constexpr int kSmemBytes = OFF_BAR + 128 + 1024;
 };
 
-template <int DH, bool kSplit, bool kF16, bool kWide>
-__global__ void __launch_bounds__(kWide ? ATT_THREADS_WIDE : ATT_THREADS_NARROW, (kWide && !kSplit && DH <= 128) ? 2 : 1)
+// O (+)= P V for one 16-key slice: A = P in registers, B = V (MN-major)
+template <int DH, bool kF16>
+__device__ __forceinline__ void mma_pv(float (&o)[DH / 2], const uint32_t (&a)[4], uint64_t db) {
+  if constexpr (kF16) {
+    if constexpr (DH == 64) wgmma_rs_m64n64_f16<1>(o, a, db, 1);
+    else if constexpr (DH == 128) wgmma_rs_m64n128_f16<1>(o, a, db, 1);
+    else if constexpr (DH == 192) wgmma_rs_m64n192_f16<1>(o, a, db, 1);
+    else wgmma_rs_m64n256_f16<1>(o, a, db, 1);
+  } else {
+    if constexpr (DH == 64) wgmma_rs_m64n64_bf16<1>(o, a, db, 1);
+    else if constexpr (DH == 128) wgmma_rs_m64n128_bf16<1>(o, a, db, 1);
+    else if constexpr (DH == 192) wgmma_rs_m64n192_bf16<1>(o, a, db, 1);
+    else wgmma_rs_m64n256_bf16<1>(o, a, db, 1);
+  }
+}
+
+template <int DH, bool kSplit, bool kF16>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 mha_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
               const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl, const MhaKParams p) {
   using Cfg = MhaCfg<DH, kSplit>;
@@ -91,18 +88,11 @@ mha_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
   uint64_t* bar_q = bars + 0;
-  uint64_t* bar_kv = bars + 1;  // [3] slot full: completes once for K_j (parity 0) and once for V_j (parity 1) per use
-  uint64_t* bar_s = bars + 4;   // [2]
-  uint64_t* bar_p = bars + 6;
-  uint64_t* bar_pv = bars + 7;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
+  uint64_t* kv_full = bars + 1;                 // [ATT_STAGES]
+  uint64_t* kv_empty = kv_full + ATT_STAGES;    // [ATT_STAGES], one arrival per consumer warp
 
-  constexpr int NH = kWide ? 2 : 1;        // column halves per S/P/O tile
-  constexpr int kMmaWarp = 4 * NH;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int quarter = warp & 3;            // TMEM lane quarter this warp may access
-  const int half = kWide ? (warp >> 2) & 1 : 0;
   const int q0 = blockIdx.x * ATT_BQ;
   const int h = blockIdx.y;
   const int b = blockIdx.z;
@@ -111,14 +101,12 @@ mha_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ 
 
   if (len == 0 || (!p.full_queries && q0 >= len)) {
     // whole query tile is padding (or no key at all): defined (zero) output, no tensor work
-    if (warp < kMmaWarp) {
-      const int t = q0 + quarter * 32 + lane;
+    for (int i = threadIdx.x; i < ATT_BQ * (DH / 8); i += blockDim.x) {
+      const int t = q0 + i / (DH / 8);
       if (t < p.T) {
-        const size_t o = ((size_t)b * p.T + t) * p.ld_out + h * DH + half * (DH / NH);
-        for (int c = 0; c < DH / NH; c += 8) {
-          st_global_v4(p.out_hi + o + c, 0, 0, 0, 0);
-          if (p.out_lo) st_global_v4(p.out_lo + o + c, 0, 0, 0, 0);
-        }
+        const size_t o = ((size_t)b * p.T + t) * p.ld_out + h * DH + (i % (DH / 8)) * 8;
+        st_global_v4(p.out_hi + o, 0, 0, 0, 0);
+        if (p.out_lo) st_global_v4(p.out_lo + o, 0, 0, 0, 0);
       }
     }
     return;
@@ -128,36 +116,20 @@ mha_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ 
 
   if (threadIdx.x == 0) {
     mbar_init(bar_q, 1);
-    mbar_init(bar_kv, 1);
-    mbar_init(bar_kv + 1, 1);
-    mbar_init(bar_kv + 2, 1);
-    mbar_init(bar_s, 1);
-    mbar_init(bar_s + 1, 1);
-    mbar_init(bar_p, 4 * NH);
-    mbar_init(bar_pv, 1);
+    for (int s = 0; s < ATT_STAGES; ++s) {
+      mbar_init(kv_full + s, 1);
+      mbar_init(kv_empty + s, 8);
+    }
     fence_mbar_init();
   }
-  if (warp == kMmaWarp) {
-    tmem_alloc(tmem_slot, Cfg::kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  uint8_t* sQ = smem + Cfg::OFF_Q;
 
-  if (warp == kMmaWarp) {
-    {
-      // ===================== TMA + MMA issue warp: warp-uniform control flow, one elected lane issues =====================
+  if (warp >= 8) {
+    setmaxnreg_dec<40>();
+    if (warp == 8) {
+      // ===================== TMA producer: warp-uniform control flow, one elected lane issues =====================
       const bool leader = elect_one();
-      uint8_t* sQ = smem + Cfg::OFF_Q;
-      uint8_t* sKV = smem + Cfg::OFF_K;
-      uint8_t* sP = smem + Cfg::OFF_P;
-      const uint32_t idesc_s = kF16 ? make_idesc_f16(ATT_BQ, ATT_BKV) : make_idesc_bf16(ATT_BQ, ATT_BKV);
-      const uint32_t idesc_o = (kF16 ? make_idesc_f16(ATT_BQ, DH) : make_idesc_bf16(ATT_BQ, DH)) | (1u << 16);  // B (= V) MN-major
-      const uint32_t t_s = tmem_base + Cfg::S_COL;
-      const uint32_t t_o = tmem_base + Cfg::O_COL;
-
       if (leader) {
         mbar_arrive_expect_tx(bar_q, Cfg::kPlanes * Cfg::Q_BYTES);
         for (int pn = 0; pn < DH / 64; ++pn) {
@@ -165,264 +137,175 @@ mha_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ 
           if (kSplit) tma_load_3d(&tmQl, bar_q, sQ + Cfg::Q_BYTES + pn * (ATT_BQ * 128), p.q_col0 + h * DH + pn * 64, q0, b);
         }
       }
-      // K_j and V_j are the same [64 keys x 64 columns] boxes of the QKV buffer, at the K resp. V columns
-      auto load_kv = [&](int j, int col0) {
-        uint8_t* dst = sKV + (j % 3) * Cfg::K_STAGE;
-        uint64_t* bar = bar_kv + (j % 3);
-        if (leader) {
-          mbar_arrive_expect_tx(bar, Cfg::kPlanes * Cfg::K_BYTES);
-          for (int pn = 0; pn < DH / 64; ++pn) {
-            tma_load_3d(&tmKh, bar, dst + pn * (ATT_BKV * 128), col0 + h * DH + pn * 64, j * ATT_BKV, b);
-            if (kSplit) tma_load_3d(&tmKl, bar, dst + Cfg::K_BYTES + pn * (ATT_BKV * 128), col0 + h * DH + pn * 64, j * ATT_BKV, b);
-          }
-        }
-      };
-      // S_j = Q K_j^T into S accumulator j&1
-      auto issue_s = [&](int j) {
-        const uint8_t* kst = sKV + (j % 3) * Cfg::K_STAGE;
-        const uint32_t ts = t_s + (j & 1) * ATT_BKV;
-        mbar_wait(bar_kv + (j % 3), 0);
-        tc_fence_after();
-        if (leader) {
-#pragma unroll
-        for (int kk = 0; kk < DH / 16; ++kk) {
-          const uint64_t a = make_smem_desc_sw128(smem_u32(sQ + (kk / 4) * (ATT_BQ * 128))) + 2 * (kk % 4);
-          const uint64_t bb = make_smem_desc_sw128(smem_u32(kst + (kk / 4) * (ATT_BKV * 128))) + 2 * (kk % 4);
-          umma_bf16(ts, a, bb, idesc_s, kk != 0);
-        }
-        if (kSplit) {
-#pragma unroll
-          for (int kk = 0; kk < DH / 16; ++kk) {
-            const uint64_t a = make_smem_desc_sw128(smem_u32(sQ + Cfg::Q_BYTES + (kk / 4) * (ATT_BQ * 128))) + 2 * (kk % 4);
-            const uint64_t bb = make_smem_desc_sw128(smem_u32(kst + (kk / 4) * (ATT_BKV * 128))) + 2 * (kk % 4);
-            umma_bf16(ts, a, bb, idesc_s, 1);
-          }
-#pragma unroll
-          for (int kk = 0; kk < DH / 16; ++kk) {
-            const uint64_t a = make_smem_desc_sw128(smem_u32(sQ + (kk / 4) * (ATT_BQ * 128))) + 2 * (kk % 4);
-            const uint64_t bb = make_smem_desc_sw128(smem_u32(kst + Cfg::K_BYTES + (kk / 4) * (ATT_BKV * 128))) + 2 * (kk % 4);
-            umma_bf16(ts, a, bb, idesc_s, 1);
-          }
-        }
-        umma_commit(bar_s + (j & 1));
-        }
-      };
-      load_kv(0, p.k_col0);
-      if (n_kv > 1) load_kv(1, p.k_col0);
-      if (n_kv > 2) load_kv(2, p.k_col0);
-      mbar_wait(bar_q, 0);
-      issue_s(0);
-      mbar_wait(bar_s, 0);        // S_0 complete: its K slot takes V_0
-      load_kv(0, p.v_col0);
+      // K_j and V_j are [64 keys x 64 columns] boxes of the same buffer, at the K resp. V columns
       for (int j = 0; j < n_kv; ++j) {
-        const uint32_t ph = j & 1;
-        // ---- software pipeline: S_{j+1} goes to the tensor pipe now, so the softmax warps find it ready when they finish
-        //      tile j (its accumulator was last read for tile j-1, whose bar_p this thread has already seen)
-        ATT_TRACE(1, j, 0);
-        if (j + 1 < n_kv) issue_s(j + 1);
-        ATT_TRACE(1, j, 1);
-        // ---- slot (j-1)%3 is free once PV_{j-1} has completed: refill it with K_{j+2}
-        if (j >= 1 && j + 2 < n_kv) {
-          mbar_wait(bar_pv, (j - 1) & 1);
-          load_kv(j + 2, p.k_col0);
-        }
-        // ---- O += P V
-        const uint8_t* sV = sKV + (j % 3) * Cfg::K_STAGE;
-        ATT_TRACE(1, j, 2);
-        mbar_wait(bar_kv + (j % 3), 1);
-        ATT_TRACE(1, j, 3);
-        mbar_wait(bar_p, ph);
-        ATT_TRACE(1, j, 4);
-        tc_fence_after();
+        const int s = j % ATT_STAGES;
+        mbar_wait(kv_empty + s, ((j / ATT_STAGES) & 1) ^ 1);
+        uint8_t* dst = smem + Cfg::OFF_KV + s * Cfg::STAGE_BYTES;
         if (leader) {
-#pragma unroll
-        for (int kk = 0; kk < ATT_BKV / 16; ++kk) {
-          const uint64_t a = make_smem_desc_sw128(smem_u32(sP)) + 2 * kk;
-          const uint64_t bb = make_smem_desc_mn_sw128(smem_u32(sV), ATT_BKV * 128) + 128 * kk;  // 16 keys = 2048 B
-          umma_bf16(t_o, a, bb, idesc_o, (j | kk) != 0);
-        }
-        if (kSplit) {
-#pragma unroll
-          for (int kk = 0; kk < ATT_BKV / 16; ++kk) {
-            const uint64_t a = make_smem_desc_sw128(smem_u32(sP + Cfg::P_BYTES)) + 2 * kk;
-            const uint64_t bb = make_smem_desc_mn_sw128(smem_u32(sV), ATT_BKV * 128) + 128 * kk;
-            umma_bf16(t_o, a, bb, idesc_o, 1);
-          }
-#pragma unroll
-          for (int kk = 0; kk < ATT_BKV / 16; ++kk) {
-            const uint64_t a = make_smem_desc_sw128(smem_u32(sP)) + 2 * kk;
-            const uint64_t bb = make_smem_desc_mn_sw128(smem_u32(sV + Cfg::K_BYTES), ATT_BKV * 128) + 128 * kk;
-            umma_bf16(t_o, a, bb, idesc_o, 1);
+          mbar_arrive_expect_tx(kv_full + s, Cfg::STAGE_BYTES);
+          for (int pn = 0; pn < DH / 64; ++pn) {
+            tma_load_3d(&tmKh, kv_full + s, dst + pn * (ATT_BKV * 128), p.k_col0 + h * DH + pn * 64, j * ATT_BKV, b);
+            tma_load_3d(&tmKh, kv_full + s, dst + Cfg::kPlanes * Cfg::K_BYTES + pn * (ATT_BKV * 128), p.v_col0 + h * DH + pn * 64,
+                        j * ATT_BKV, b);
+            if (kSplit) {
+              tma_load_3d(&tmKl, kv_full + s, dst + Cfg::K_BYTES + pn * (ATT_BKV * 128), p.k_col0 + h * DH + pn * 64, j * ATT_BKV, b);
+              tma_load_3d(&tmKl, kv_full + s, dst + 2 * Cfg::K_BYTES + Cfg::V_BYTES + pn * (ATT_BKV * 128),
+                          p.v_col0 + h * DH + pn * 64, j * ATT_BKV, b);
+            }
           }
         }
-        umma_commit(bar_pv);
-        }
-        ATT_TRACE(1, j, 5);
-        // ---- S_{j+1} (issued above, ahead of PV_j) completes first: its K slot takes V_{j+1}, a whole softmax ahead of PV_{j+1}
-        if (j + 1 < n_kv) {
-          mbar_wait(bar_s + ((j + 1) & 1), ((j + 1) >> 1) & 1);
-          load_kv(j + 1, p.v_col0);
-        }
-        ATT_TRACE(1, j, 6);
       }
     }
   } else {
-    // ===================== softmax / epilogue warps =====================
-    // one thread per (query row, column half): with the wide layout two partner warps (w, w+4) share a row, each
-    // reading its half of S, writing its half of P and owning its half of O; row max / row sum are combined through
-    // shared memory behind a 64-thread named barrier.
-    constexpr int SW = ATT_BKV / NH;   // S / P columns of this thread
-    constexpr int OW = DH / NH;        // O columns of this thread
-    const int row = quarter * 32 + lane;
-    const int tq = q0 + row;
-    const uint32_t lane_base = (uint32_t)(quarter * 32) << 16;
-    const uint32_t t_s = tmem_base + lane_base + Cfg::S_COL + half * SW;
-    const uint32_t t_o = tmem_base + lane_base + Cfg::O_COL + half * OW;
-    uint8_t* sP = smem + Cfg::OFF_P;
-    float* red_max = reinterpret_cast<float*>(smem + Cfg::OFF_RED);          // [2][2][128]
-    float* red_sum = red_max + 2 * 2 * ATT_BQ;                               // [2][128]
-    float m = -INFINITY, l = 0.f;
-    uint32_t r[16];
+    // ===================== softmax / MMA warpgroups =====================
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int wq = warp & 3;
+    const int r0 = wg * 64 + 16 * wq + (lane >> 2);          // this thread's rows r0 and r0 + 8 of the tile
+    const int tq[2] = {q0 + r0, q0 + r0 + 8};
+    const int cq = 2 * (lane & 3);                            // its columns 8i + cq + {0, 1} of every accumulator
+    float o[DH / 2];
+#pragma unroll
+    for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    mbar_wait(bar_q, 0);
+    const uint32_t sq = smem_u32(sQ) + wg * (64 * 128);
     for (int j = 0; j < n_kv; ++j) {
-      if (threadIdx.x == 0) ATT_TRACE(0, j, 0);
-      mbar_wait(bar_s + (j & 1), (j >> 1) & 1);
-      if (threadIdx.x == 0) ATT_TRACE(0, j, 1);
-      tc_fence_after();
-      const uint32_t t_sj = t_s + (j & 1) * ATT_BKV;
-      // raw scores (un-scaled): the running max is kept in raw units, the softmax scale is folded into one FFMA per
-      // element: p = exp2(s * scale_log2 - m * scale_log2)
-      float s[SW];
-      {
-        // all TMEM loads are issued back to back and waited for once
-        uint32_t qq[SW / 16][16];
+      const int st = j % ATT_STAGES;
+      mbar_wait(kv_full + st, (j / ATT_STAGES) & 1);
+      const uint32_t sk = smem_u32(smem + Cfg::OFF_KV + st * Cfg::STAGE_BYTES);
+      const uint32_t sv = sk + Cfg::kPlanes * Cfg::K_BYTES;
+      // ---- S = Q K_j^T (raw scores: the running max is kept in raw units, the softmax scale is folded into one FFMA per
+      //      element: p = exp2(s * scale_log2 - m * scale_log2))
+      float s[32];
+      wgmma_fence();
 #pragma unroll
-        for (int c = 0; c < SW / 16; ++c) tmem_ld16(t_sj + c * 16, qq[c]);
-        tmem_wait_ld();
-        if (threadIdx.x == 0) ATT_TRACE(0, j, 2);
-#pragma unroll
-        for (int c = 0; c < SW / 16; ++c)
-#pragma unroll
-          for (int i = 0; i < 16; ++i) s[c * 16 + i] = __uint_as_float(qq[c][i]);
+      for (int kk = 0; kk < DH / 16; ++kk) {
+        const uint64_t da = make_smem_desc_sw128(sq + (kk / 4) * (ATT_BQ * 128)) + 2 * (kk % 4);
+        const uint64_t db = make_smem_desc_sw128(sk + (kk / 4) * (ATT_BKV * 128)) + 2 * (kk % 4);
+        if (kF16) wgmma_ss_m64n64_f16<0, 0>(s, da, db, kk != 0);
+        else wgmma_ss_m64n64_bf16<0, 0>(s, da, db, kk != 0);
       }
-      if ((j + 1) * ATT_BKV > len) {  // only the last key tile can hold padded keys
+      if (kSplit) {
 #pragma unroll
-        for (int i = 0; i < SW; ++i)
-          if (j * ATT_BKV + half * SW + i >= len) s[i] = -INFINITY;
-      }
-      if (p.causal && (j + 1) * ATT_BKV - 1 > q0) {  // look-ahead mask: tiles that reach past the first query row of this CTA
-#pragma unroll
-        for (int i = 0; i < SW; ++i)
-          if (j * ATT_BKV + half * SW + i > tq) s[i] = -INFINITY;
-      }
-      float mx = s[0];
-#pragma unroll
-      for (int i = 1; i < SW; ++i) mx = fmaxf(mx, s[i]);
-      if (kWide) {
-        float* rm = red_max + (j & 1) * 2 * ATT_BQ;
-        rm[half * ATT_BQ + row] = mx;
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
-        mx = fmaxf(mx, rm[(half ^ 1) * ATT_BQ + row]);
-      }
-      // lazy running max: the reference point only moves when the row max grew by more than 2^8 (in exponent units), so
-      // P stays <= 256 (exact range for fp16/bf16, fp32 accumulation) and the O rescale below becomes rare.  l and O
-      // use the same reference, so the final O / l is unchanged.
-      const float m_cand = fmaxf(m, mx);
-      const bool grow = (m_cand - m) * p.scale_log2 > 8.f;        // first tile: m = -inf -> true
-      const float m_new = grow ? m_cand : m;
-      const float alpha = grow ? fast_exp2((m - m_new) * p.scale_log2) : 1.f;  // first tile: exp2(-inf) = 0
-      const float neg_m = -m_new * p.scale_log2;
-      float psum = 0.f;
-#pragma unroll
-      for (int i = 0; i < SW; ++i) {
-        s[i] = fast_exp2(fmaf(s[i], p.scale_log2, neg_m));
-        psum += s[i];
-      }
-      l = l * alpha + psum;   // wide layout: partial sum over this thread's column half
-      m = m_new;
-      if (threadIdx.x == 0) ATT_TRACE(0, j, 3);
-      if (j > 0) {
-        mbar_wait(bar_pv, (j - 1) & 1);  // O_{j-1} complete, P buffer free
-        if (threadIdx.x == 0) ATT_TRACE(0, j, 4);
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, alpha != 1.f)) {
-#pragma unroll
-          for (int c = 0; c < OW / 16; ++c) {
-            tmem_ld16(t_o + c * 16, r);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * alpha);
-            tmem_st16(t_o + c * 16, r);
-          }
-          tmem_wait_st();
+        for (int kk = 0; kk < DH / 16; ++kk) {
+          const uint64_t da_lo = make_smem_desc_sw128(sq + Cfg::Q_BYTES + (kk / 4) * (ATT_BQ * 128)) + 2 * (kk % 4);
+          const uint64_t da_hi = make_smem_desc_sw128(sq + (kk / 4) * (ATT_BQ * 128)) + 2 * (kk % 4);
+          const uint64_t db_hi = make_smem_desc_sw128(sk + (kk / 4) * (ATT_BKV * 128)) + 2 * (kk % 4);
+          const uint64_t db_lo = make_smem_desc_sw128(sk + Cfg::K_BYTES + (kk / 4) * (ATT_BKV * 128)) + 2 * (kk % 4);
+          wgmma_ss_m64n64_bf16<0, 0>(s, da_lo, db_hi, 1);
+          wgmma_ss_m64n64_bf16<0, 0>(s, da_hi, db_lo, 1);
         }
       }
-      if (threadIdx.x == 0) ATT_TRACE(0, j, 5);
-      // P -> shared memory, K-major rows of 128 B with the 128B swizzle (16-byte chunk index ^= row & 7)
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      // ---- masks: padded keys (only the last key tile can hold them) and the look-ahead mask
+      const int k0 = j * ATT_BKV + cq;
+      if ((j + 1) * ATT_BKV > len) {
 #pragma unroll
-      for (int c8 = 0; c8 < SW / 8; ++c8) {
-        const int ch = half * (SW / 8) + c8;
-        uint32_t hi[4], lo[4];
+        for (int i = 0; i < 32; ++i)
+          if (k0 + 8 * (i >> 2) + (i & 1) >= len) s[i] = -INFINITY;
+      }
+      if (p.causal && (j + 1) * ATT_BKV - 1 > q0) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i)
+          if (k0 + 8 * (i >> 2) + (i & 1) > tq[(i >> 1) & 1]) s[i] = -INFINITY;
+      }
+      float alpha[2];
+      float psum[2] = {0.f, 0.f};
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        float mx = -INFINITY;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) mx = fmaxf(mx, fmaxf(s[4 * i + 2 * rr], s[4 * i + 2 * rr + 1]));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        // lazy running max: the reference point only moves when the row max grew by more than 2^8 (in exponent units), so
+        // P stays <= 256 (exact range for fp16/bf16, fp32 accumulation) and the O rescale below becomes rare.  l and O
+        // use the same reference, so the final O / l is unchanged.
+        const float m_cand = fmaxf(m[rr], mx);
+        const bool grow = (m_cand - m[rr]) * p.scale_log2 > 8.f;        // first tile: m = -inf -> true
+        const float m_new = grow ? m_cand : m[rr];
+        alpha[rr] = grow ? fast_exp2((m[rr] - m_new) * p.scale_log2) : 1.f;  // first tile: exp2(-inf) = 0
+        const float neg_m = -m_new * p.scale_log2;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          s[4 * i + 2 * rr] = fast_exp2(fmaf(s[4 * i + 2 * rr], p.scale_log2, neg_m));
+          s[4 * i + 2 * rr + 1] = fast_exp2(fmaf(s[4 * i + 2 * rr + 1], p.scale_log2, neg_m));
+          psum[rr] += s[4 * i + 2 * rr] + s[4 * i + 2 * rr + 1];
+        }
+        l[rr] = l[rr] * alpha[rr] + psum[rr];   // partial sum over this thread's columns; the quad is summed at the end
+        m[rr] = m_new;
+      }
+      if (__any_sync(0xffffffffu, alpha[0] != 1.f || alpha[1] != 1.f)) {
+#pragma unroll
+        for (int i = 0; i < DH / 8; ++i) {
+          o[4 * i] *= alpha[0]; o[4 * i + 1] *= alpha[0];
+          o[4 * i + 2] *= alpha[1]; o[4 * i + 3] *= alpha[1];
+        }
+      }
+      // ---- P as the A operand: the fragment of keys [16kk, 16kk + 16) is s[8kk .. 8kk + 8) re-packed pairwise
+      uint32_t phi[4][4], plo[4][4];
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
+          const float x0 = s[8 * kk + 2 * i], x1 = s[8 * kk + 2 * i + 1];
           if (kF16) {
-            const __half2 hh = __floats2half2_rn(s[c8 * 8 + 2 * i], s[c8 * 8 + 2 * i + 1]);
-            hi[i] = *reinterpret_cast<const uint32_t*>(&hh);
-            lo[i] = 0;
+            const __half2 hh = __floats2half2_rn(x0, x1);
+            phi[kk][i] = *reinterpret_cast<const uint32_t*>(&hh);
           } else {
             __nv_bfloat16 h0, l0, h1, l1;
-            split_bf16(s[c8 * 8 + 2 * i], h0, l0);
-            split_bf16(s[c8 * 8 + 2 * i + 1], h1, l1);
-            hi[i] = pack_bf16(h0, h1);
-            lo[i] = pack_bf16(l0, l1);
+            split_bf16(x0, h0, l0);
+            split_bf16(x1, h1, l1);
+            phi[kk][i] = pack_bf16(h0, h1);
+            plo[kk][i] = pack_bf16(l0, l1);
           }
         }
-        const uint32_t off = row * 128 + ((ch ^ (row & 7)) << 4);
-        st_shared_v4(sP + off, hi[0], hi[1], hi[2], hi[3]);
-        if (kSplit) st_shared_v4(sP + Cfg::P_BYTES + off, lo[0], lo[1], lo[2], lo[3]);
       }
-      fence_proxy_async_smem();
-      tc_fence_before();
+      // ---- O += P V_j
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < ATT_BKV / 16; ++kk) {
+        const uint64_t dv = make_smem_desc_mn_sw128(sv, ATT_BKV * 128) + 128 * kk;   // 16 keys = 2048 B
+        mma_pv<DH, kF16>(o, phi[kk], dv);
+        if (kSplit) {
+          const uint64_t dv_lo = make_smem_desc_mn_sw128(sv + Cfg::V_BYTES, ATT_BKV * 128) + 128 * kk;
+          mma_pv<DH, kF16>(o, plo[kk], dv);
+          mma_pv<DH, kF16>(o, phi[kk], dv_lo);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(o);
       __syncwarp();
-      if (lane == 0) mbar_arrive(bar_p);
-      if (threadIdx.x == 0) ATT_TRACE(0, j, 6);
+      if (lane == 0) mbar_arrive(kv_empty + st);
     }
     // ---- epilogue: O / l -> bf16 hi/lo at columns [h*DH, (h+1)*DH)
-    if (kWide) {
-      red_sum[half * ATT_BQ + row] = l;
-      asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
-      l += red_sum[(half ^ 1) * ATT_BQ + row];
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      l[rr] += __shfl_xor_sync(0xffffffffu, l[rr], 1);
+      l[rr] += __shfl_xor_sync(0xffffffffu, l[rr], 2);
     }
-    mbar_wait(bar_pv, (n_kv - 1) & 1);
-    tc_fence_after();
-    const float inv = l > 0.f ? 1.f / l : 0.f;
-    const size_t o = ((size_t)b * p.T + (tq < p.T ? tq : 0)) * p.ld_out + h * DH + half * OW;
+    const float inv[2] = {l[0] > 0.f ? 1.f / l[0] : 0.f, l[1] > 0.f ? 1.f / l[1] : 0.f};
 #pragma unroll
-    for (int c = 0; c < OW / 16; ++c) {
-      tmem_ld16(t_o + c * 16, r);
-      tmem_wait_ld();
-      uint32_t hi[8], lo[8];
+    for (int rr = 0; rr < 2; ++rr) {
+      if (tq[rr] < p.T) {
+        const size_t ob = ((size_t)b * p.T + tq[rr]) * p.ld_out + h * DH + cq;
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        __nv_bfloat16 h0, l0, h1, l1;
-        split_bf16(__uint_as_float(r[2 * i]) * inv, h0, l0);
-        split_bf16(__uint_as_float(r[2 * i + 1]) * inv, h1, l1);
-        hi[i] = pack_bf16(h0, h1);
-        lo[i] = pack_bf16(l0, l1);
-      }
-      if (tq < p.T) {
-        st_global_v8(p.out_hi + o + c * 16, hi);
-        if (p.out_lo) st_global_v8(p.out_lo + o + c * 16, lo);
+        for (int i = 0; i < DH / 8; ++i) {
+          __nv_bfloat16 h0, l0, h1, l1;
+          split_bf16(o[4 * i + 2 * rr] * inv[rr], h0, l0);
+          split_bf16(o[4 * i + 2 * rr + 1] * inv[rr], h1, l1);
+          *reinterpret_cast<uint32_t*>(p.out_hi + ob + 8 * i) = pack_bf16(h0, h1);
+          if (p.out_lo) *reinterpret_cast<uint32_t*>(p.out_lo + ob + 8 * i) = pack_bf16(l0, l1);
+        }
       }
     }
   }
-
-  tc_fence_before();
   __syncthreads();
-  if (warp == kMmaWarp) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
 }
 
 // ----------------------------------------------------------------------------------------------------
@@ -595,7 +478,7 @@ __global__ void __launch_bounds__(256) mha_weights_kernel(const MhaKParams p, co
   }
 }
 
-template <int DH, bool kSplit, bool kF16, bool kWide>
+template <int DH, bool kSplit, bool kF16>
 static int launch_tc(const ttsb_mha_args* a, const MhaKParams& p, cudaStream_t stream) {
   using Cfg = MhaCfg<DH, kSplit>;
   CUtensorMap tmQ[2], tmK[2];
@@ -612,11 +495,11 @@ static int launch_tc(const ttsb_mha_args* a, const MhaKParams& p, cudaStream_t s
   }
   static PerDevice<bool> attr_set;
   if (!attr_set.get()) {
-    TTSB_CUDA_OK(cudaFuncSetAttribute(mha_tc_kernel<DH, kSplit, kF16, kWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    TTSB_CUDA_OK(cudaFuncSetAttribute(mha_tc_kernel<DH, kSplit, kF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_set.get() = true;
   }
   dim3 grid((a->T + ATT_BQ - 1) / ATT_BQ, a->H, a->B);
-  mha_tc_kernel<DH, kSplit, kF16, kWide><<<grid, kWide ? ATT_THREADS_WIDE : ATT_THREADS_NARROW, Cfg::kSmemBytes, stream>>>(tmQ[0], tmQ[1], tmK[0], tmK[1], p);
+  mha_tc_kernel<DH, kSplit, kF16><<<grid, ATT_THREADS, Cfg::kSmemBytes, stream>>>(tmQ[0], tmQ[1], tmK[0], tmK[1], p);
   count_launch();
   return check_cuda(cudaGetLastError(), "mha_tc_kernel launch");
 }
@@ -654,12 +537,6 @@ extern "C" int ttsb_mha_fwd(const ttsb_mha_args* a, void* stream_v) {
   p.out_lo = static_cast<__nv_bfloat16*>(a->out_lo);  // optional second plane of the OUTPUT (consumer may be bf16x3)
   p.ld_out = a->ld_out;
   p.scale_log2 = 1.4426950408889634f / sqrtf((float)a->dh);
-#ifdef TTSB_ATT_TRACE
-  {
-    const char* e = getenv("TTSB_ATT_TRACE_PTR");  // device pointer (hex) of a 2*64*8 int64 buffer
-    p.trace = e ? reinterpret_cast<long long*>(strtoull(e, nullptr, 16)) : nullptr;
-  }
-#endif
 
   MhaSimtPtrs q{};
   q.qk_hi = static_cast<const __nv_bfloat16*>(a->qk_hi);
@@ -692,19 +569,17 @@ extern "C" int ttsb_mha_fwd(const ttsb_mha_args* a, void* stream_v) {
     count_launch();
     return check_cuda(cudaGetLastError(), "mha_simt_kernel launch");
   }
-  // wide (8 softmax warps) is the default layout; TTSB_ATT_NARROW=1 selects the 4-warp layout for A/B measurements
-  static const bool narrow = [] { const char* e = getenv("TTSB_ATT_NARROW"); return e && e[0] == '1'; }();
   int rc;
-#define TTSB_MHA_DISPATCH(DH_, W_)                                                                                  \
-  (split ? launch_tc<DH_, true, false, W_>(a, p, stream)                                                            \
-         : (f16 ? launch_tc<DH_, false, true, W_>(a, p, stream) : launch_tc<DH_, false, false, W_>(a, p, stream)))
-#define TTSB_MHA_DISPATCH1(DH_, W_) \
-  (f16 ? launch_tc<DH_, false, true, W_>(a, p, stream) : launch_tc<DH_, false, false, W_>(a, p, stream))
-  if (a->dh == 128) rc = narrow ? TTSB_MHA_DISPATCH(128, false) : TTSB_MHA_DISPATCH(128, true);
-  else if (a->dh == 64) rc = narrow ? TTSB_MHA_DISPATCH(64, false) : TTSB_MHA_DISPATCH(64, true);
-  else if (a->dh == 192 && !split) rc = narrow ? TTSB_MHA_DISPATCH1(192, false) : TTSB_MHA_DISPATCH1(192, true);
-  else if (a->dh == 256 && !split) rc = narrow ? TTSB_MHA_DISPATCH1(256, false) : TTSB_MHA_DISPATCH1(256, true);
-  else { set_last_error("ttsb_mha_fwd: head_dim %d not supported by the tcgen05 kernel (64, 128; 192, 256 in single-pass modes)", a->dh); return TTSB_ERR_UNSUPPORTED; }
+#define TTSB_MHA_DISPATCH(DH_)                                                                                      \
+  (split ? launch_tc<DH_, true, false>(a, p, stream) : (f16 ? launch_tc<DH_, false, true>(a, p, stream) : launch_tc<DH_, false, false>(a, p, stream)))
+#define TTSB_MHA_DISPATCH1(DH_) (f16 ? launch_tc<DH_, false, true>(a, p, stream) : launch_tc<DH_, false, false>(a, p, stream))
+  if (a->dh == 128) rc = TTSB_MHA_DISPATCH(128);
+  else if (a->dh == 64) rc = TTSB_MHA_DISPATCH(64);
+  else if (a->dh == 192 && !split) rc = TTSB_MHA_DISPATCH1(192);
+  else if (a->dh == 256 && !split) rc = TTSB_MHA_DISPATCH1(256);
+  else { set_last_error("ttsb_mha_fwd: head_dim %d not supported by the tensor-core kernel (64, 128; 192, 256 in single-pass modes)", a->dh); return TTSB_ERR_UNSUPPORTED; }
+#undef TTSB_MHA_DISPATCH
+#undef TTSB_MHA_DISPATCH1
   if (rc) return rc;
   if (a->weights_out) {
     if (!a->weights_all && (a->weights_batch_index < 0 || a->weights_batch_index >= a->B)) { set_last_error("ttsb_mha_fwd: weights_batch_index out of range"); return TTSB_ERR_INVALID_ARGUMENT; }

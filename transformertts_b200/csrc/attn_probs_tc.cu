@@ -1,50 +1,42 @@
 // Attention probabilities of the training step in ONE kernel:  P = softmax(scale * Q K^T + key mask), P_drop = dropout(P)
 // (model/layers.py:176-188: scaled_dot_product_attention up to the attention weights, and the Dropout on them at :189-191
 // of the MultiHeadAttention call).  The two-kernel path (ttsb_bgemm writing fp32 logits, ttsb_softmax_fwd reading them
-// back) moves 4*T*T bytes each way per (batch row, head); here the logits never leave TMEM.
+// back) moves 4*T*T bytes each way per (batch row, head); here the logits never leave the registers.
 //
-// A work item is (z = b*H + h, 128 query rows).  A softmax row spans all keys but TMEM holds 512 fp32 columns, so the
-// logits are produced TWICE: pass 1 sweeps the live 64-key tiles and keeps the running row maximum and sum (online
-// rescaling), pass 2 recomputes every tile and writes the normalised probabilities.  The extra QK^T is cheap (contraction
-// over dh only) next to the 8*T*T bytes of fp32 round trip it replaces.
+// A work item is (z = b*H + h, 128 query rows).  A softmax row spans all keys, so the logits are produced TWICE: pass 1
+// sweeps the live 64-key tiles and keeps the running row maximum and sum (online rescaling), pass 2 recomputes every tile
+// and writes the normalised probabilities.  The extra QK^T is cheap (contraction over dh only) next to the 8*T*T bytes of
+// fp32 round trip it replaces.
 //
-//   warp 0     TMA producer: Q tile of the item once (resident), K tiles (128 keys) through a ring
-//   warp 1     tcgen05.mma issuer: one 128 x 128 product fills TWO adjacent 64-column TMEM buffers (tiles j, j+1); with
-//              one product per 64-key tile the issuer, which shares its scheduler with four softmax warps, starved pass 1
-//   warps 2-17 four groups of four warps (one per TMEM lane quarter); group g takes tiles j with j % 4 == g, a thread owns
-//              one query row of the tile.  After pass 1 the groups merge their (max, sum) through shared memory.
-//              Pass 2 stages one bf16 [32 rows x 32 cols] box (64B swizzle) per output and warp and hands it to TMA;
-//              small boxes leave the shared memory to the K ring (three 128-key stages at dh = 128, two at dh = 192).
-// The softmax side is latency bound (dependent ex2 / hash chains, TMEM and shared-memory round trips), hence sixteen
-// warps of it: the first version with eight ran at half the issue rate (ncu: 2.5 warps per scheduler, 50 % issue slots).
+//   warps 0-7  two wgmma warpgroups, each owning 64 query rows of the item: S = Q K^T with fp32 accumulators in
+//              registers (a row lives in the four lanes of a quad), softmax / dropout on the fragment, bf16 pairs stored
+//              straight from it
+//   warp 8     TMA producer: Q tile of the item once (resident), K tiles (64 keys) through a ring (warps 9-11 idle: the
+//              producer warpgroup hands its registers to the others with setmaxnreg)
 //
 // Masks follow ttsb_softmax_fwd with flags == 0: keys >= len[b] get probability exactly 0, query rows >= len[b] are written
 // as zeros.  Dropout decisions come from the same stateless hash at the same element index ((z*T + m)*ld + k), so the
 // backward pass (MODE 1 below, or the dS epilogue of ttsb_bgemm) regenerates them.
 //
 // MODE 1 of the same kernel is the backward counterpart (softmax gradient fused into the dP product, what ttsb_bgemm does
-// with sm_P set): the MMA is dP = dO V^T (one pass); the saved P box of a warp's next half tile arrives by TMA in its second
-// staging box while the current one is processed, and dS = scale * P * (dropout(dP) - D) leaves through the first.
+// with sm_P set): the MMA is dP = dO V^T (one pass), and dS = scale * P * (dropout(dP) - D) is formed on the fragment with
+// the saved P read next to it.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 
 #include "../../include/ttsb.h"
 #include "ttsb_common.cuh"
 #include "ttsb_host.h"
+#include "wgmma_sm90.cuh"
 
 namespace ttsb {
 
 constexpr int AP_BM = 128;
 constexpr int AP_BN = 64;
-constexpr int AP_GROUPS = 4;
-constexpr int AP_NBUF = 8;
-constexpr int AP_THREADS = 64 + AP_GROUPS * 128;
+constexpr int AP_THREADS = 384;
 constexpr int AP_QBOX_BYTES = 128 * 64 * 2;         // [128 query rows x 64 k] K-major box
-constexpr int AP_KEYS = 2 * AP_BN;                  // keys per MMA job (two softmax tiles)
-constexpr int AP_KBOX_BYTES = AP_KEYS * 64 * 2;     // [128 keys x 64 k]
-constexpr int AP_STAGING_BYTES = AP_GROUPS * 4 * 2 * 2048;   // per softmax warp: one [32 x 32] bf16 box per output
+constexpr int AP_KBOX_BYTES = AP_BN * 64 * 2;       // [64 keys x 64 k]
 constexpr int AP_MAX_STAGES = 8;
-constexpr int AP_STATS_BYTES = 2 * AP_GROUPS * 128 * 8;      // [item parity][group][row] (max, sum)
 constexpr int AP_BAR_BYTES = 512;
 constexpr int AP_MAX_SMEM = 227 * 1024;
 
@@ -58,85 +50,52 @@ struct ApParams {
   float drop_p;
   uint32_t seed, site;
   int two_outputs;
+  __nv_bfloat16* out0;    // MODE 0: P_pre, MODE 1: dS
+  __nv_bfloat16* out1;    // MODE 0: P_drop
   // MODE 1 (dS): saved probabilities (Z, T, ld_p), row statistic D (Z*T), plain scale
   const __nv_bfloat16* sm_P;
   const float* sm_D;
   float scale;
 };
 
-// shared-memory accesses by 32-bit shared address: through generic pointers derived from the dynamic-smem base the compiler
-// emits generic LD / ST.E instead of LDS / STS
-__device__ __forceinline__ void ap_sts128(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ void ap_sts64f(uint32_t saddr, float a, float b) {
-  asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(saddr), "f"(a), "f"(b) : "memory");
-}
-__device__ __forceinline__ uint4 ap_lds128(uint32_t saddr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(saddr) : "memory");
-  return v;
-}
-__device__ __forceinline__ float2 ap_lds64f(uint32_t saddr) {
-  float2 v;
-  asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(saddr) : "memory");
-  return v;
-}
 __device__ __forceinline__ float ap_ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+__device__ __forceinline__ uint32_t ap_pack(float a, float b) {
+  const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&v);
+}
 
 template <int MODE>
 __global__ void __launch_bounds__(AP_THREADS, 1)
-attn_probs_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmD, const ApParams p) {
+attn_probs_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const ApParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int q_bytes = p.kbs * AP_QBOX_BYTES;
   const int k_bytes = p.kbs * AP_KBOX_BYTES;
   uint8_t* q_smem = smem;
   uint8_t* k_smem = smem + q_bytes;
-  uint8_t* staging = k_smem + p.nst * k_bytes;
-  float2* stats = reinterpret_cast<float2*>(staging + AP_STAGING_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + AP_STAGING_BYTES + AP_STATS_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(k_smem + p.nst * k_bytes);
   uint64_t* q_full = bars;
   uint64_t* q_empty = bars + 1;
   uint64_t* k_full = bars + 2;
   uint64_t* k_empty = k_full + AP_MAX_STAGES;
-  uint64_t* t_full = k_empty + AP_MAX_STAGES;
-  uint64_t* t_empty = t_full + AP_NBUF;
-  uint64_t* p_full = t_empty + AP_NBUF;          // MODE 1: one per softmax warp, the P box of its next half tile has landed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(p_full + AP_GROUPS * 4);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmP);
-    tma_prefetch_desc(&tmD);
     mbar_init(q_full, 1);
-    mbar_init(q_empty, 1);
+    mbar_init(q_empty, 8);
     for (int s = 0; s < AP_MAX_STAGES; ++s) {
       mbar_init(k_full + s, 1);
-      mbar_init(k_empty + s, 1);
+      mbar_init(k_empty + s, 8);
     }
-    for (int s = 0; s < AP_NBUF; ++s) {
-      mbar_init(t_full + s, 1);
-      mbar_init(t_empty + s, 4);
-    }
-    for (int s = 0; s < AP_GROUPS * 4; ++s) mbar_init(p_full + s, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int num_items = p.Z * p.m_tiles;
 
   // 64-key tiles of an item that are produced by MMAs: none when every query row of the tile is padding
@@ -144,351 +103,183 @@ attn_probs_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     z = item / p.m_tiles;
     m0 = (item % p.m_tiles) * AP_BM;
     len = min(max(__ldg(p.kv_len + z / p.H), 0), p.Tk);
-    return m0 < len ? 2 * ((len + AP_KEYS - 1) / AP_KEYS) : 0;   // whole MMA jobs: even, the last tile may lie past len
+    return m0 < len ? (len + AP_BN - 1) / AP_BN : 0;
   };
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    const bool leader = elect_one();
-    uint32_t jc = 0, qc = 0;
-    for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-      int z, m0, len;
-      const int nkl = live_tiles(item, z, m0, len);
-      if (nkl == 0) continue;
-      const int b = z / p.H, h = z % p.H;
-      mbar_wait_parked(q_empty, (qc & 1) ^ 1);
-      if (leader) {
-        mbar_arrive_expect_tx(q_full, (uint32_t)q_bytes);
-        for (int kb = 0; kb < p.kbs; ++kb) tma_load_3d(&tmQ, q_full, q_smem + kb * AP_QBOX_BYTES, p.q_col0 + h * p.dh + kb * 64, m0, b);
-      }
-      ++qc;
-      const int njobs = nkl / 2;
-      for (int job = 0; job < (MODE == 0 ? 2 : 1) * njobs; ++job) {       // probabilities: pass 1, then pass 2
-        const int j = job < njobs ? job : job - njobs;
-        const int stage = jc % p.nst;
-        mbar_wait_parked(k_empty + stage, ((jc / p.nst) & 1) ^ 1);
+  if (warp >= 8) {
+    setmaxnreg_dec<40>();
+    if (warp == 8) {
+      // ===================== TMA producer =====================
+      const bool leader = elect_one();
+      uint32_t jc = 0, qc = 0;
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+        int z, m0, len;
+        const int nkl = live_tiles(item, z, m0, len);
+        if (nkl == 0) continue;
+        const int b = z / p.H, h = z % p.H;
+        mbar_wait_parked(q_empty, (qc & 1) ^ 1);
         if (leader) {
-          mbar_arrive_expect_tx(k_full + stage, (uint32_t)k_bytes);
-          for (int kb = 0; kb < p.kbs; ++kb)
-            tma_load_3d(&tmK, k_full + stage, k_smem + stage * k_bytes + kb * AP_KBOX_BYTES, p.k_col0 + h * p.dh + kb * 64, j * AP_KEYS, b);
+          mbar_arrive_expect_tx(q_full, (uint32_t)q_bytes);
+          for (int kb = 0; kb < p.kbs; ++kb) tma_load_3d(&tmQ, q_full, q_smem + kb * AP_QBOX_BYTES, p.q_col0 + h * p.dh + kb * 64, m0, b);
         }
-        ++jc;
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const bool leader = elect_one();
-    const uint32_t idesc = make_idesc_bf16(AP_BM, AP_KEYS);
-    uint32_t jc = 0, qc = 0;
-    for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-      int z, m0, len;
-      const int nkl = live_tiles(item, z, m0, len);
-      if (nkl == 0) continue;
-      mbar_wait_parked(q_full, qc & 1);
-      tc_fence_after();
-      const uint32_t qs = smem_u32(q_smem);
-      for (int job = 0; job < (MODE == 0 ? nkl : nkl / 2); ++job) {   // nkl/2 jobs per pass
-        const int buf = (2 * jc) & (AP_NBUF - 1);      // tiles 2*jc, 2*jc + 1 -> buffers buf, buf + 1 (adjacent columns)
-        const int stage = jc % p.nst;
-        mbar_wait_parked(t_empty + buf, (((2 * jc) / AP_NBUF) & 1) ^ 1);
-        mbar_wait_parked(t_empty + buf + 1, (((2 * jc) / AP_NBUF) & 1) ^ 1);
-        mbar_wait_parked(k_full + stage, (jc / p.nst) & 1);
-        tc_fence_after();
-        const uint32_t ks = smem_u32(k_smem + stage * k_bytes);
-        if (leader) {
-          for (int kb = 0; kb < p.kbs; ++kb) {
-            const uint64_t a = make_smem_desc_sw128(qs + kb * AP_QBOX_BYTES);
-            const uint64_t bd = make_smem_desc_sw128(ks + kb * AP_KBOX_BYTES);
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) umma_bf16(tmem_base + buf * AP_BN, a + 2 * kk, bd + 2 * kk, idesc, (kb | kk) != 0);
+        ++qc;
+        for (int job = 0; job < (MODE == 0 ? 2 : 1) * nkl; ++job) {       // probabilities: pass 1, then pass 2
+          const int j = job < nkl ? job : job - nkl;
+          const int stage = jc % p.nst;
+          mbar_wait_parked(k_empty + stage, ((jc / p.nst) & 1) ^ 1);
+          if (leader) {
+            mbar_arrive_expect_tx(k_full + stage, (uint32_t)k_bytes);
+            for (int kb = 0; kb < p.kbs; ++kb)
+              tma_load_3d(&tmK, k_full + stage, k_smem + stage * k_bytes + kb * AP_KBOX_BYTES, p.k_col0 + h * p.dh + kb * 64, j * AP_BN, b);
           }
-          umma_commit(k_empty + stage);
-          umma_commit(t_full + buf);
-          umma_commit(t_full + buf + 1);
+          ++jc;
         }
-        ++jc;
       }
-      if (leader) umma_commit(q_empty);   // every MMA that reads this Q tile has completed when this arrives
-      ++qc;
     }
   } else {
-    // ===================== softmax warps =====================
-    const int quarter = warp & 3;
-    const int group = (warp - 2) >> 2;
-    const int row = quarter * 32 + lane;
-    uint8_t* box0 = staging + (warp - 2) * 4096;
-    uint8_t* box1 = box0 + 2048;
-    const uint32_t box0_s = smem_u32(box0) + lane * 64, box1_s = box0_s + 2048;   // this lane's row of the two boxes
+    // ===================== wgmma / softmax warpgroups =====================
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int rloc = wg * 64 + 16 * (warp & 3) + (lane >> 2);   // this thread's rows rloc and rloc + 8 of the item
+    const int cq = 2 * (lane & 3);                              // its columns 8i + cq + {0, 1} of every 64-key tile
     const uint32_t thresh16 = dropout_thresh(p.drop_p) >> 16;
     const float ks = p.drop_p > 0.f ? 1.f / (1.f - p.drop_p) : 1.f;
     const float c = p.scale_log2e;
-    const int sw = (lane >> 1) & 3;   // 64B swizzle: 16-byte chunk index ^= bits 7-8 of the address = (row >> 1) & 3
     const uint32_t hterm = dropout_hterm(p.seed, p.site, 0u);
-    const uint32_t tlane = tmem_base + ((uint32_t)(quarter * 32) << 16);
-    uint32_t jc = 0, it = 0, pcount = 0;
+    uint32_t jc = 0, qc = 0;
+    // one 64-key tile of S = Q K^T (MODE 1: dP = dO V^T) for this warpgroup's 64 rows; releases the K stage
+    auto produce = [&](float (&s)[32]) {
+      const int stage = jc % p.nst;
+      mbar_wait_parked(k_full + stage, (jc / p.nst) & 1);
+      const uint32_t qs = smem_u32(q_smem) + wg * (64 * 128);
+      const uint32_t kst = smem_u32(k_smem + stage * k_bytes);
+      wgmma_fence();
+      for (int kb = 0; kb < p.kbs; ++kb) {
+        const uint64_t a = make_smem_desc_sw128(qs + kb * AP_QBOX_BYTES);
+        const uint64_t bd = make_smem_desc_sw128(kst + kb * AP_KBOX_BYTES);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_ss_m64n64_bf16<0, 0>(s, a + 2 * kk, bd + 2 * kk, (kb | kk) != 0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(k_empty + stage);
+      ++jc;
+    };
 
     for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
       int z, m0, len;
       const int nkl = live_tiles(item, z, m0, len);
-      const int m = m0 + row;
-      const bool live = m < len;
+      const int m[2] = {m0 + rloc, m0 + rloc + 8};
+      const bool live[2] = {m[0] < len, m[1] < len};
+      const bool in_t[2] = {m[0] < p.T, m[1] < p.T};
+      if (nkl > 0) mbar_wait_parked(q_full, qc & 1);
+      // element offset of (row m, column 0) in the (Z, T, ld_p) layout; pair indices fit 32 bits (< 2^33 elements)
+      const size_t rowoff[2] = {((size_t)z * p.T + (in_t[0] ? m[0] : 0)) * p.ld_p, ((size_t)z * p.T + (in_t[1] ? m[1] : 0)) * p.ld_p};
+      const int n_out = max(p.n_tiles, nkl);   // every produced tile is consumed, also past the last column of the output
       if constexpr (MODE == 1) {
         // ---------------- dS = scale * P * (keep * dP / (1-p) - D), one pass
-        const float dsum = live ? __ldg(p.sm_D + (size_t)z * p.T + m) : 0.f;
-        const bool any_dead = __any_sync(0xffffffffu, !live);
+        const float dsum[2] = {live[0] ? __ldg(p.sm_D + (size_t)z * p.T + m[0]) : 0.f, live[1] ? __ldg(p.sm_D + (size_t)z * p.T + m[1]) : 0.f};
         const float sc = p.scale, sks = p.scale * ks;
-        const int n_t = max(p.n_tiles, nkl);
-        const uint32_t jc_base = jc;
-        jc += nkl;
-        // The saved P box of a half tile ([32 rows x 32 cols], the layout of the output boxes) is fetched by TMA into this
-        // warp's second staging box one half tile ahead of its use.  Per-thread global loads next to their use left the
-        // kernel on the loads (ncu: 4.5 long-scoreboard stalls per issued instruction); holding the next segment in
-        // registers instead spilled inside the loop.
-        uint64_t* pbar = p_full + (warp - 2);
-        auto want_p = [&](int j, int hf) { return j < nkl && j * AP_BN + 32 * hf < len; };     // warp-uniform
-        auto issue_p = [&](int j, int hf) {
-          if (lane == 0) {
-            mbar_arrive_expect_tx(pbar, 2048u);
-            tma_load_3d(&tmD, pbar, box1, j * AP_BN + 32 * hf, m0 + quarter * 32, z);
-          }
-        };
-        if (want_p(group, 0)) issue_p(group, 0);
-        for (int j = group; j < n_t; j += AP_GROUPS) {
+        for (int j = 0; j < n_out; ++j) {
+          float s[32];
           const bool has_mma = j < nkl;
-          const uint32_t my_jc = jc_base + j;
-          const int buf = my_jc & (AP_NBUF - 1);
-          const int col0 = j * AP_BN;
-          const uint32_t x0 = (uint32_t)(((uint32_t)z * (uint32_t)p.T + (uint32_t)m) * (uint64_t)p.ld_p + (uint64_t)col0 >> 1) * DROPOUT_C1;
-          if (has_mma) {
-            mbar_wait_parked(t_full + buf, (my_jc / AP_NBUF) & 1);
-            tc_fence_after();
-          }
+          if (has_mma) produce(s);
 #pragma unroll
-          for (int hf = 0; hf < 2; ++hf) {
-            uint4 cur[4];
+          for (int rr = 0; rr < 2; ++rr) {
+            if (!in_t[rr]) continue;
 #pragma unroll
-            for (int q = 0; q < 4; ++q) cur[q] = make_uint4(0, 0, 0, 0);
-            if (want_p(j, hf)) {
-              mbar_wait_parked(pbar, pcount & 1);
-              ++pcount;
-#pragma unroll
-              for (int q = 0; q < 4; ++q) cur[q] = ap_lds128(box1_s + ((q ^ sw) << 4));
-              fence_proxy_async_smem();    // the box is overwritten by the next TMA load (async proxy) after these reads
-              __syncwarp();
-            }
-            {
-              const int nj = hf == 0 ? j : j + AP_GROUPS, nhf = hf ^ 1;
-              if (want_p(nj, nhf)) issue_p(nj, nhf);
-            }
-            float y[32];
-            if (has_mma && col0 + 32 * hf < len) {      // warp-uniform (tcgen05.ld is .sync.aligned); dead rows carry P = 0
-              uint32_t ra[16], rb[16];
-              tmem_ld16(tlane + buf * AP_BN + 32 * hf, ra);
-              tmem_ld16(tlane + buf * AP_BN + 32 * hf + 16, rb);
-              tmem_wait_ld();
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                const uint4 qv = cur[i >> 2];
-                const uint32_t w = (i & 3) == 0 ? qv.x : (i & 3) == 1 ? qv.y : (i & 3) == 2 ? qv.z : qv.w;
+            for (int i = 0; i < 8; ++i) {
+              const int col = j * AP_BN + 8 * i + cq;
+              if (col >= p.ld_p) continue;
+              float y0 = 0.f, y1 = 0.f;
+              if (has_mma && live[rr] && col < len) {
+                const uint32_t w = __ldg(reinterpret_cast<const uint32_t*>(p.sm_P + rowoff[rr] + col));
                 const float p0 = __uint_as_float(w << 16), p1 = __uint_as_float(w & 0xffff0000u);
-                const uint32_t hsh = dropout_mix((x0 + (uint32_t)(16 * hf + i) * DROPOUT_C1) ^ hterm);
-                const float r0 = __uint_as_float(i < 8 ? ra[2 * i] : rb[2 * i - 16]);
-                const float r1 = __uint_as_float(i < 8 ? ra[2 * i + 1] : rb[2 * i - 15]);
-                y[2 * i] = fmaf((hsh & 0xffffu) >= thresh16 ? p0 * sks : 0.f, r0, -(p0 * sc) * dsum);
-                y[2 * i + 1] = fmaf((hsh >> 16) >= thresh16 ? p1 * sks : 0.f, r1, -(p1 * sc) * dsum);
+                const uint32_t hsh = dropout_mix((uint32_t)((rowoff[rr] + col) >> 1) * DROPOUT_C1 ^ hterm);
+                y0 = fmaf((hsh & 0xffffu) >= thresh16 ? p0 * sks : 0.f, s[4 * i + 2 * rr], -(p0 * sc) * dsum[rr]);
+                y1 = fmaf((hsh >> 16) >= thresh16 ? p1 * sks : 0.f, s[4 * i + 2 * rr + 1], -(p1 * sc) * dsum[rr]);
+                if (col + 1 >= len) y1 = 0.f;
               }
-              if (col0 + 32 * hf + 32 > len || any_dead) {     // exact (+0) zeros on masked keys and padded query rows
-#pragma unroll
-                for (int i = 0; i < 32; ++i) y[i] = (live && col0 + 32 * hf + i < len) ? y[i] : 0.f;
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) y[i] = 0.f;
-            }
-            if (hf == 1 && has_mma) {   // last TMEM read of the tile
-              tc_fence_before();
-              __syncwarp();
-              if (lane == 0) mbar_arrive(t_empty + buf);
-            }
-            if (lane == 0) tma_store_wait_read();
-            __syncwarp();
-#pragma unroll
-            for (int ch = 0; ch < 4; ++ch) {
-              uint32_t w[4];
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const __nv_bfloat162 hv = __floats2bfloat162_rn(y[8 * ch + 2 * i], y[8 * ch + 2 * i + 1]);
-                w[i] = *reinterpret_cast<const uint32_t*>(&hv);
-              }
-              ap_sts128(box0_s + ((ch ^ sw) << 4), w[0], w[1], w[2], w[3]);
-            }
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0 && col0 + 32 * hf < p.ld_p) {
-              tma_store_3d(&tmP, box0, col0 + 32 * hf, m0 + quarter * 32, z);
-              tma_store_commit();
+              *reinterpret_cast<uint32_t*>(p.out0 + rowoff[rr] + col) = ap_pack(y0, y1);
             }
           }
         }
       } else {
-      float mx = -INFINITY, l = 0.f;
-      // ---------------- pass 1: running maximum and sum over the live key tiles of this group
-      for (int j = 0; j < nkl; ++j, ++jc) {
-        if ((j & (AP_GROUPS - 1)) != group) continue;
-        const int buf = jc & (AP_NBUF - 1);
-        mbar_wait_parked(t_full + buf, (jc / AP_NBUF) & 1);
-        tc_fence_after();
-        const int n0 = j * AP_BN;
-        uint32_t ra[16], rb[16], rc[16], rd[16];
-        tmem_ld16(tlane + buf * AP_BN, ra);
-        tmem_ld16(tlane + buf * AP_BN + 16, rb);
-        tmem_ld16(tlane + buf * AP_BN + 32, rc);
-        tmem_ld16(tlane + buf * AP_BN + 48, rd);
-        tmem_wait_ld();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(t_empty + buf);     // the tile now lives in registers
-        if (n0 >= len) continue;     // second half of the last MMA job: consumed, nothing to add (jc advances in the for)
-        float v[64];
+        float mx[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+        // ---------------- pass 1: running maximum and sum over the live key tiles
+        for (int j = 0; j < nkl; ++j) {
+          float s[32];
+          produce(s);
+          const int n0 = j * AP_BN + cq;
+          if (j * AP_BN + AP_BN > len) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          v[i] = __uint_as_float(ra[i]); v[16 + i] = __uint_as_float(rb[i]);
-          v[32 + i] = __uint_as_float(rc[i]); v[48 + i] = __uint_as_float(rd[i]);
-        }
-        if (n0 + AP_BN > len) {
-#pragma unroll
-          for (int i = 0; i < 64; ++i) v[i] = (n0 + i < len) ? v[i] : -INFINITY;
-        }
-        float c0 = fmaxf(v[0], v[1]), c1 = fmaxf(v[2], v[3]), c2 = fmaxf(v[4], v[5]), c3 = fmaxf(v[6], v[7]);
-#pragma unroll
-        for (int i = 8; i < 64; i += 8) {
-          c0 = fmaxf(c0, fmaxf(v[i], v[i + 1])); c1 = fmaxf(c1, fmaxf(v[i + 2], v[i + 3]));
-          c2 = fmaxf(c2, fmaxf(v[i + 4], v[i + 5])); c3 = fmaxf(c3, fmaxf(v[i + 6], v[i + 7]));
-        }
-        const float cm = fmaxf(fmaxf(c0, c1), fmaxf(c2, c3));   // finite: key n0 of a live tile is < len
-        const float mnew = fmaxf(mx, cm * c);
-        const float neg = -mnew;
-        float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-#pragma unroll
-        for (int i = 0; i < 64; i += 4) {
-          a0 += ap_ex2(fmaf(v[i], c, neg)); a1 += ap_ex2(fmaf(v[i + 1], c, neg));
-          a2 += ap_ex2(fmaf(v[i + 2], c, neg)); a3 += ap_ex2(fmaf(v[i + 3], c, neg));
-        }
-        l = fmaf(l, ap_ex2(mx - mnew), (a0 + a1) + (a2 + a3));   // mx = -inf on the first tile: ex2(-inf) = 0
-        mx = mnew;
-      }
-      float inv = 0.f;
-      if (nkl > 0) {
-        // merge the groups' partial statistics (a group without a tile holds (-inf, 0); group 0 always has tile 0)
-        const uint32_t st = smem_u32(stats) + (it & 1) * (AP_GROUPS * 128 * 8);
-        ap_sts64f(st + (group * 128 + row) * 8, mx, l);
-        asm volatile("bar.sync 1, %0;" ::"n"(AP_GROUPS * 128) : "memory");
-        float2 o[AP_GROUPS];
-#pragma unroll
-        for (int g = 0; g < AP_GROUPS; ++g) o[g] = ap_lds64f(st + (g * 128 + row) * 8);
-        float mall = o[0].x;
-#pragma unroll
-        for (int g = 1; g < AP_GROUPS; ++g) mall = fmaxf(mall, o[g].x);
-        float lall = 0.f;
-#pragma unroll
-        for (int g = 0; g < AP_GROUPS; ++g) lall = fmaf(o[g].y, ap_ex2(o[g].x - mall), lall);
-        mx = live ? mall : INFINITY;      // dead query rows: ex2(x - inf) = 0
-        inv = live ? 1.f / lall : 0.f;
-        ++it;
-      }
-      // ---------------- pass 2: recomputed logits -> probabilities -> staged bf16 boxes -> TMA tile stores
-      const float neg = -mx;
-      const int n_p2 = max(p.n_tiles, nkl);   // every produced tile is consumed, also one past the last column box
-      for (int j = 0; j < n_p2; ++j) {
-        const bool has_mma = j < nkl;
-        const bool mine = (j & (AP_GROUPS - 1)) == group;
-        const uint32_t my_jc = jc;
-        if (has_mma) ++jc;
-        if (!mine) continue;
-        const int buf = my_jc & (AP_NBUF - 1);
-        const int col0 = j * AP_BN;
-        // dropout hash of element pair k of this row segment: mix((x0 + k*C1) ^ hterm); the host admits tensors of
-        // < 2^33 elements only, so the pair index fits 32 bits and its high word is zero
-        const uint32_t x0 = (uint32_t)(((uint32_t)z * (uint32_t)p.T + (uint32_t)m) * (uint64_t)p.ld_p + (uint64_t)col0 >> 1) * DROPOUT_C1;
-        if (has_mma) {
-          mbar_wait_parked(t_full + buf, (my_jc / AP_NBUF) & 1);
-          tc_fence_after();
-        }
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-          float pv[32];
-          if (has_mma && col0 + 32 * hf < len) {      // warp-uniform
-            uint32_t ra[16], rb[16];
-            tmem_ld16(tlane + buf * AP_BN + 32 * hf, ra);
-            tmem_ld16(tlane + buf * AP_BN + 32 * hf + 16, rb);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              pv[i] = ap_ex2(fmaf(__uint_as_float(ra[i]), c, neg)) * inv;
-              pv[16 + i] = ap_ex2(fmaf(__uint_as_float(rb[i]), c, neg)) * inv;
-            }
-            if (col0 + 32 * hf + 32 > len) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) pv[i] = (col0 + 32 * hf + i < len) ? pv[i] : 0.f;
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) pv[i] = 0.f;
+            for (int i = 0; i < 32; ++i) s[i] = (n0 + 8 * (i >> 2) + (i & 1) < len) ? s[i] : -INFINITY;
           }
-          if (hf == 1 && has_mma) {   // last TMEM read of the tile
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(t_empty + buf);
-          }
-          if (lane == 0) tma_store_wait_read();   // the previous half's boxes have been read out by their TMA stores
-          __syncwarp();
 #pragma unroll
-          for (int ch = 0; ch < 4; ++ch) {
-            uint32_t w[4];
+          for (int rr = 0; rr < 2; ++rr) {
+            float cm = -INFINITY;
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const __nv_bfloat162 hv = __floats2bfloat162_rn(pv[8 * ch + 2 * i], pv[8 * ch + 2 * i + 1]);
-              w[i] = *reinterpret_cast<const uint32_t*>(&hv);
+            for (int i = 0; i < 8; ++i) cm = fmaxf(cm, fmaxf(s[4 * i + 2 * rr], s[4 * i + 2 * rr + 1]));
+            cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 1));
+            cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 2));   // finite: key j*64 of a live tile is < len
+            const float mnew = fmaxf(mx[rr], cm * c);
+            const float neg = -mnew;
+            float a0 = 0.f, a1 = 0.f;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              a0 += ap_ex2(fmaf(s[4 * i + 2 * rr], c, neg));
+              a1 += ap_ex2(fmaf(s[4 * i + 2 * rr + 1], c, neg));
             }
-            ap_sts128(box0_s + ((ch ^ sw) << 4), w[0], w[1], w[2], w[3]);
+            l[rr] = fmaf(l[rr], ap_ex2(mx[rr] - mnew), a0 + a1);   // mx = -inf on the first tile: ex2(-inf) = 0
+            mx[rr] = mnew;
           }
-          if (p.two_outputs) {
+        }
+        float inv[2] = {0.f, 0.f};
 #pragma unroll
-            for (int ch = 0; ch < 4; ++ch) {
-              uint32_t w[4];
+        for (int rr = 0; rr < 2; ++rr) {
+          l[rr] += __shfl_xor_sync(0xffffffffu, l[rr], 1);
+          l[rr] += __shfl_xor_sync(0xffffffffu, l[rr], 2);
+          inv[rr] = (nkl > 0 && live[rr]) ? 1.f / l[rr] : 0.f;
+          mx[rr] = live[rr] ? mx[rr] : INFINITY;      // dead query rows: ex2(x - inf) = 0
+        }
+        // ---------------- pass 2: recomputed logits -> probabilities (and dropped probabilities) -> bf16 pairs
+        for (int j = 0; j < n_out; ++j) {
+          float s[32];
+          const bool has_mma = j < nkl;
+          if (has_mma) produce(s);
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const int k = 16 * hf + 4 * ch + i;   // pair index inside the 64-column segment
-                const uint32_t hsh = dropout_mix((x0 + (uint32_t)k * DROPOUT_C1) ^ hterm);
-                const float d0 = (hsh & 0xffffu) >= thresh16 ? pv[8 * ch + 2 * i] * ks : 0.f;
-                const float d1 = (hsh >> 16) >= thresh16 ? pv[8 * ch + 2 * i + 1] * ks : 0.f;
-                const __nv_bfloat162 hv = __floats2bfloat162_rn(d0, d1);
-                w[i] = *reinterpret_cast<const uint32_t*>(&hv);
+          for (int rr = 0; rr < 2; ++rr) {
+            if (!in_t[rr]) continue;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int col = j * AP_BN + 8 * i + cq;
+              if (col >= p.ld_p) continue;
+              float p0 = 0.f, p1 = 0.f;
+              if (has_mma && col < len) {
+                p0 = ap_ex2(fmaf(s[4 * i + 2 * rr], c, -mx[rr])) * inv[rr];
+                p1 = col + 1 < len ? ap_ex2(fmaf(s[4 * i + 2 * rr + 1], c, -mx[rr])) * inv[rr] : 0.f;
               }
-              ap_sts128(box1_s + ((ch ^ sw) << 4), w[0], w[1], w[2], w[3]);
+              *reinterpret_cast<uint32_t*>(p.out0 + rowoff[rr] + col) = ap_pack(p0, p1);
+              if (p.two_outputs) {
+                const uint32_t hsh = dropout_mix((uint32_t)((rowoff[rr] + col) >> 1) * DROPOUT_C1 ^ hterm);
+                const float d0 = (hsh & 0xffffu) >= thresh16 ? p0 * ks : 0.f;
+                const float d1 = (hsh >> 16) >= thresh16 ? p1 * ks : 0.f;
+                *reinterpret_cast<uint32_t*>(p.out1 + rowoff[rr] + col) = ap_pack(d0, d1);
+              }
             }
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0 && col0 + 32 * hf < p.ld_p) {
-            tma_store_3d(&tmP, box0, col0 + 32 * hf, m0 + quarter * 32, z);
-            if (p.two_outputs) tma_store_3d(&tmD, box1, col0 + 32 * hf, m0 + quarter * 32, z);
-            tma_store_commit();
           }
         }
       }
+      if (nkl > 0) {   // every MMA of this warp that reads the Q tile has completed
+        __syncwarp();
+        if (lane == 0) mbar_arrive(q_empty);
+        ++qc;
       }
     }
-    if (lane == 0) tma_store_wait_all();
   }
-
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
 }  // namespace ttsb
@@ -497,34 +288,32 @@ using namespace ttsb;
 
 static int ap_ring_stages(int dh) {
   const int kbs = dh / 64;
-  const int fixed = 1024 + AP_STAGING_BYTES + AP_STATS_BYTES + AP_BAR_BYTES + kbs * AP_QBOX_BYTES;
+  const int fixed = 1024 + AP_BAR_BYTES + kbs * AP_QBOX_BYTES;
   const int n = (AP_MAX_SMEM - fixed) / (kbs * AP_KBOX_BYTES);
   return n > AP_MAX_STAGES ? AP_MAX_STAGES : n;
 }
 
 extern "C" int ttsb_attn_probs_supported(int dh, int ld_p) {
-  return dh > 0 && dh % 64 == 0 && ld_p > 0 && ld_p % 8 == 0 && ap_ring_stages(dh) >= 2;
+  return dh > 0 && dh % 64 == 0 && dh <= 192 && ld_p > 0 && ld_p % 8 == 0 && ap_ring_stages(dh) >= 2;
 }
 
 // shared launcher: A operand = query-side rows (Q or dO), B operand = key-side rows (K or V)
 template <int MODE>
 static int ap_launch(const void* a, int ld_a, int a_col0, const void* bmat, int ld_b, int b_col0, int B, int H, int T, int dh, ApParams p,
-                     const void* out0, const void* out1, int ld_p, cudaStream_t stream) {
+                     void* out0, void* out1, int ld_p, cudaStream_t stream) {
   p.Z = B * H; p.H = H; p.T = T; p.Tk = T; p.dh = dh; p.kbs = dh / 64;
   p.q_col0 = a_col0; p.k_col0 = b_col0;
   p.m_tiles = (T + AP_BM - 1) / AP_BM;
   p.n_tiles = (ld_p + AP_BN - 1) / AP_BN;
   p.ld_p = ld_p;
   p.nst = ap_ring_stages(dh);
-  const int smem_bytes = 1024 + AP_STAGING_BYTES + AP_STATS_BYTES + AP_BAR_BYTES + p.kbs * AP_QBOX_BYTES + p.nst * p.kbs * AP_KBOX_BYTES;
-  CUtensorMap tmQ, tmK, tmP, tmD;
+  p.out0 = static_cast<__nv_bfloat16*>(out0);
+  p.out1 = static_cast<__nv_bfloat16*>(out1);
+  const int smem_bytes = 1024 + AP_BAR_BYTES + p.kbs * AP_QBOX_BYTES + p.nst * p.kbs * AP_KBOX_BYTES;
+  CUtensorMap tmQ, tmK;
   int rc = make_tmap_bf16_3d(&tmQ, a, (uint64_t)ld_a, (uint64_t)T, (uint64_t)B, (uint64_t)ld_a, (uint64_t)ld_a * T, 64, AP_BM);
   if (rc) return rc;
-  rc = make_tmap_bf16_3d(&tmK, bmat, (uint64_t)ld_b, (uint64_t)T, (uint64_t)B, (uint64_t)ld_b, (uint64_t)ld_b * T, 64, AP_KEYS);
-  if (rc) return rc;
-  rc = make_tmap_bf16_3d_sw64(&tmP, out0, (uint64_t)ld_p, (uint64_t)T, (uint64_t)p.Z, (uint64_t)ld_p, (uint64_t)ld_p * T, 32, 32);
-  if (rc) return rc;
-  rc = make_tmap_bf16_3d_sw64(&tmD, out1, (uint64_t)ld_p, (uint64_t)T, (uint64_t)p.Z, (uint64_t)ld_p, (uint64_t)ld_p * T, 32, 32);
+  rc = make_tmap_bf16_3d(&tmK, bmat, (uint64_t)ld_b, (uint64_t)T, (uint64_t)B, (uint64_t)ld_b, (uint64_t)ld_b * T, 64, AP_BN);
   if (rc) return rc;
   static PerDevice<bool> attr_set;
   if (!attr_set.get()) {
@@ -533,7 +322,7 @@ static int ap_launch(const void* a, int ld_a, int a_col0, const void* bmat, int 
   }
   const int items = p.Z * p.m_tiles;
   const int grid = items < num_sms() ? items : num_sms();
-  attn_probs_tc_kernel<MODE><<<grid, AP_THREADS, smem_bytes, stream>>>(tmQ, tmK, tmP, tmD, p);
+  attn_probs_tc_kernel<MODE><<<grid, AP_THREADS, smem_bytes, stream>>>(tmQ, tmK, p);
   count_launch();
   return check_cuda(cudaGetLastError(), MODE == 0 ? "attn_probs_tc_kernel<0> launch" : "attn_probs_tc_kernel<1> launch");
 }
@@ -582,7 +371,7 @@ extern "C" int ttsb_attn_ds_bwd(const void* dO, int ld_do, int do_col0, const vo
   p.drop_p = drop_p; p.seed = seed; p.site = site;
   p.sm_P = static_cast<const __nv_bfloat16*>(P_pre);
   p.sm_D = D;
-  return ap_launch<1>(dO, ld_do, do_col0, v, ld_v, v_col0, B, H, T, dh, p, dS, P_pre, ld_p, static_cast<cudaStream_t>(stream_v));   // second map: P loads
+  return ap_launch<1>(dO, ld_do, do_col0, v, ld_v, v_col0, B, H, T, dh, p, dS, nullptr, ld_p, static_cast<cudaStream_t>(stream_v));
 }
 
 TTSB_DEFINE_SALT_SETTER(set_salt_attn_probs)

@@ -1,5 +1,6 @@
-// Batched / reduction GEMMs of the training step on tcgen05 (single-pass bf16, fp32 accumulate in TMEM).
-// Same pipeline as gemm_tc.cu (TMA -> 128B-swizzled smem ring -> tcgen05.mma -> 8 epilogue warps), different tiling:
+// Batched / reduction GEMMs of the training step on wgmma (single-pass bf16, fp32 accumulate in registers).
+// Same pipeline as gemm_tc.cu (TMA producer warp -> 128B-swizzled smem ring -> two wgmma warpgroups -> accumulator image in
+// shared memory -> the same 8 warps as epilogue, one thread per output row), different tiling:
 //
 //  mode BATCHED : out[z][m][n] = alpha * sum_k A_z[m][k] * B_z[n][k]        z = (batch row b, head h)
 //                 both operands come from activations (per-(b,h) B operand), e.g. S = Q K^T, O = P V, dP = dO V^T,
@@ -9,7 +10,7 @@
 //                 weight gradients of Dense / concat-Dense / Conv1D (k taps = k segments), reduction over all B*T
 //                 rows split across CTAs, partial tiles added with fp32 red.global.add (Keras (K,N) layout).
 //
-// Operand majorness.  tcgen05 reads an operand either K-major (the contraction index is contiguous in memory: rows of
+// Operand majorness.  wgmma reads an operand either K-major (the contraction index is contiguous in memory: rows of
 // 128 B hold 64 k) or MN-major (the M/N index is contiguous: rows of 128 B hold 64 m, one row per k).  Supporting both
 // means NO transposed copies are ever made: P^T, dS^T, dO^T, V^T, K^T and the X^T / G^T of the weight gradients are just
 // the same row-major tensors read MN-major.  An MN-major tile is fetched as ceil(rows/64) TMA boxes of [64 k x 64 mn]
@@ -19,6 +20,7 @@
 
 #include "../../include/ttsb.h"
 #include "ttsb_common.cuh"
+#include "wgmma_sm90.cuh"
 #include "ttsb_host.h"
 
 namespace ttsb {
@@ -26,17 +28,24 @@ namespace ttsb {
 constexpr int BG_BM = 128;
 constexpr int BG_BK = 64;
 constexpr int BG_MAX_BN = 256;
-constexpr int BG_THREADS = 320;
+constexpr int BG_THREADS = 384;   // warps 0-7: two wgmma / epilogue warpgroups, warp 8: TMA producer (warps 9-11 idle: the
+                                   // producer warpgroup hands its registers to the others with setmaxnreg)
 constexpr int BG_STAGES = 4;
+constexpr int BG_NCH = BG_MAX_BN / 64;
 constexpr int BG_A_BYTES = BG_BM * BG_BK * 2;
 constexpr int BG_B_BYTES = BG_MAX_BN * BG_BK * 2;
 constexpr int BG_STAGE_BYTES = BG_A_BYTES + BG_B_BYTES;
-constexpr int BG_BAR_OFFSET = BG_STAGES * BG_STAGE_BYTES;
-// bf16 outputs leave through shared staging boxes and TMA tile stores: 2 alternating boxes x 4 lane quarters of
-// [32 rows x 64 cols] (4 KiB, 128B swizzle) -- see the staged epilogue below
-constexpr int BG_STAGE_OUT_OFFSET = (BG_BAR_OFFSET + 256 + 1023) / 1024 * 1024;
+constexpr int BG_RING_BYTES = BG_STAGES * BG_STAGE_BYTES;
+// accumulator image [128 rows][BG_PITCH floats], written once the ring is drained, so it overlays the ring
+constexpr int BG_PITCH = acc_pitch(BG_MAX_BN);
+constexpr int BG_IMG_BYTES = BG_BM * BG_PITCH * 4;
+// bf16 outputs leave through shared staging boxes and TMA tile stores: 2 alternating boxes x 4 row quarters of
+// [32 rows x 64 cols] (4 KiB, 128B swizzle) -- see the staged epilogue below; they lie in the ring behind the image
+constexpr int BG_STAGE_OUT_OFFSET = (BG_IMG_BYTES + 1023) / 1024 * 1024;
 constexpr int BG_STAGE_OUT_BYTES = 2 * 4 * 4096;
-constexpr int BG_SMEM_BYTES = BG_STAGE_OUT_OFFSET + BG_STAGE_OUT_BYTES + 1024;
+static_assert(BG_STAGE_OUT_OFFSET + BG_STAGE_OUT_BYTES <= BG_RING_BYTES, "image and staging must fit the ring");
+constexpr int BG_BAR_OFFSET = BG_RING_BYTES;
+constexpr int BG_SMEM_BYTES = BG_BAR_OFFSET + 256 + 1024;
 constexpr int BG_MN_BOX_BYTES = 64 * 128;  // one [64 k x 64 mn] box
 
 struct BgOperand {
@@ -84,9 +93,7 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + BG_BAR_OFFSET);
   uint64_t* empty_bar = full_bar + BG_STAGES;
-  uint64_t* tmem_full = empty_bar + BG_STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  uint64_t* img_free = empty_bar + BG_STAGES;   // the epilogue of the previous tile has released the ring / image
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
@@ -94,22 +101,12 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < BG_STAGES; ++s) {
       mbar_init(full_bar + s, 1);
-      mbar_init(empty_bar + s, 1);
+      mbar_init(empty_bar + s, 8);
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tmem_full + s, 1);
-      mbar_init(tmem_empty + s, 8);
-    }
+    mbar_init(img_free, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const bool a_mn = p.mode == 1 || p.opA.mn_major;
   const bool b_mn = p.mode == 1 || p.opB.mn_major;
   const int b_boxes = (p.block_n + 63) / 64;
@@ -125,12 +122,21 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
     return nb > 0 ? nb * t_chunks : 0;
   };
 
-  if (warp == 0) {
+  if (warp >= 8) {
+    setmaxnreg_dec<40>();
+    if (warp > 8) goto done;
     // ===================== TMA producer: warp-uniform control flow, the elected lane issues (see elect_one) ==========
     const bool leader = elect_one();
     int stage = 0;
-    uint32_t phase = 0;
+    uint32_t phase = 0, img_phase = 0;
+    bool first = true;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      if (tile_kblocks(tile) == 0) continue;
+      if (!first) {   // the ring holds the previous tile's accumulator image until its epilogue is done
+        mbar_wait(img_free, img_phase);
+        img_phase ^= 1;
+      }
+      first = false;
       if (p.mode == 0) {
         const int n_tile = tile % p.n_tiles;
         const int m_tile = (tile / p.n_tiles) % p.m_tiles;
@@ -187,53 +193,72 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: warp-uniform control flow, the elected lane issues =====================
-    const bool leader = elect_one();
-    const uint32_t idesc = make_idesc_bf16(BG_BM, p.block_n) | (a_mn ? (1u << 15) : 0u) | (b_mn ? (1u << 16) : 0u);
-    const uint32_t a_step = a_mn ? (16 * 128) >> 4 : 2;  // descriptor advance per 16 k
-    const uint32_t b_step = b_mn ? (16 * 128) >> 4 : 2;
-    int stage = 0, acc = 0;
-    uint32_t phase = 0, acc_phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const int kbs = tile_kblocks(tile);
-      if (kbs == 0) continue;
-      mbar_wait(tmem_empty + acc, acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BG_MAX_BN;
-      for (int kb = 0; kb < kbs; ++kb) {
-        mbar_wait(full_bar + stage, phase);
-        tc_fence_after();
-        const uint32_t st = smem_u32(smem + stage * BG_STAGE_BYTES);
-        const uint64_t a = a_mn ? make_smem_desc_mn_sw128(st, BG_MN_BOX_BYTES) : make_smem_desc_sw128(st);
-        const uint64_t b = b_mn ? make_smem_desc_mn_sw128(st + BG_A_BYTES, BG_MN_BOX_BYTES) : make_smem_desc_sw128(st + BG_A_BYTES);
-        if (leader) {
-#pragma unroll
-          for (int kk = 0; kk < BG_BK / 16; ++kk) umma_bf16(d_tmem, a + a_step * kk, b + b_step * kk, idesc, (kb | kk) != 0);
-          umma_commit(empty_bar + stage);
-        }
-        if (++stage == BG_STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (leader) umma_commit(tmem_full + acc);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  } else if (warp >= 2) {
-    // ===================== epilogue warps =====================
-    const int quarter = warp & 3;
-    const int half = (warp - 2) >> 2;
+  } else {
+    // ===================== two wgmma warpgroups (rows [64*wg, +64) of the tile), then the epilogue =====================
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int quarter = warp & 3;        // epilogue: rows [32*quarter, +32)
+    const int half = warp >> 2;          // epilogue: which half of the tile's column chunks
     const int row = quarter * 32 + lane;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    float* img = reinterpret_cast<float*>(smem);
+    float* arow = img + (size_t)row * BG_PITCH;
+    int stage = 0;
+    uint32_t phase = 0;
     const int nch = p.block_n >> 4;
     const int ch_begin = half ? (nch + 1) >> 1 : 0;
     const int ch_end = half ? nch : (nch + 1) >> 1;
+    const int nmma = (p.block_n + 63) >> 6;   // n64 products per k step; columns past block_n are computed and ignored
+    const uint32_t a_step = a_mn ? (16 * 128) >> 4 : 2;  // descriptor advance per 16 k
+    const uint32_t b_step = b_mn ? (16 * 128) >> 4 : 2;
     uint32_t r[16];
     uint32_t slab_ctr = 0;  // staged epilogue: slabs stored so far (selects the staging box)
+    // the same 64-row / 64-column block offsets hold for both majornesses: a K-major block is 64 rows of 128 B, an MN-major
+    // block one [64 k x 64 mn] TMA box
+    auto mma = [&](float (&d)[32], uint64_t da, uint64_t db, uint32_t accum) {
+      if (a_mn) {
+        if (b_mn) wgmma_ss_m64n64_bf16<1, 1>(d, da, db, accum); else wgmma_ss_m64n64_bf16<1, 0>(d, da, db, accum);
+      } else {
+        if (b_mn) wgmma_ss_m64n64_bf16<0, 1>(d, da, db, accum); else wgmma_ss_m64n64_bf16<0, 0>(d, da, db, accum);
+      }
+    };
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      if (tile_kblocks(tile) == 0) continue;
-      mbar_wait(tmem_full + acc, acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * BG_MAX_BN;
+      const int kbs = tile_kblocks(tile);
+      if (kbs == 0) continue;
+      float acc[BG_NCH][32];
+      int prev_stage = -1;
+      for (int kb = 0; kb < kbs; ++kb) {
+        mbar_wait(full_bar + stage, phase);
+        const uint32_t st = smem_u32(smem + stage * BG_STAGE_BYTES);
+        const uint64_t a = a_mn ? make_smem_desc_mn_sw128(st + wg * 8192, BG_MN_BOX_BYTES) : make_smem_desc_sw128(st + wg * 8192);
+        wgmma_fence();
+#pragma unroll
+        for (int c = 0; c < BG_NCH; ++c) {
+          if (c < nmma) {
+            const uint32_t bs = st + BG_A_BYTES + c * 8192;
+            const uint64_t bd = b_mn ? make_smem_desc_mn_sw128(bs, BG_MN_BOX_BYTES) : make_smem_desc_sw128(bs);
+#pragma unroll
+            for (int kk = 0; kk < BG_BK / 16; ++kk) mma(acc[c], a + a_step * kk, bd + b_step * kk, (kb | kk) != 0);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();   // the products of the previous k block have finished reading their stage: release it
+        if (prev_stage >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar + prev_stage);
+        }
+        prev_stage = stage;
+        if (++stage == BG_STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int c = 0; c < BG_NCH; ++c) wgmma_fence_regs(acc[c]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar + prev_stage);
+      asm volatile("bar.sync 5, 256;" ::: "memory");   // both warpgroups are done reading the ring: park the tile in it
+#pragma unroll
+      for (int c = 0; c < BG_NCH; ++c)
+        if (c < nmma) acc_store_fragment(img, BG_PITCH, wg * 64, c * 64, acc[c]);
+      asm volatile("bar.sync 5, 256;" ::: "memory");
       if (p.mode == 0) {
         const int n_tile = tile % p.n_tiles;
         const int m_tile = (tile / p.n_tiles) % p.m_tiles;
@@ -247,7 +272,7 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
         const size_t o = (size_t)(p.out_by_b ? b : z) * (size_t)p.out_z_stride + (size_t)(row_ok ? m : 0) * p.ld_out + h * p.out_h_col + n0;
         if (p.staged) {
           // ---- bf16 output as TMA tile stores.  A thread owns one output ROW, so direct stores are 32-byte pieces of 32
-          //      different rows per warp instruction (request-rate bound: the fused dS epilogue ran at 240 us for 390 MB).
+          //      different rows per warp instruction (request-rate bound).
           //      The two warps of a lane quarter fill a [32 rows x 64 cols] 128B-swizzled box (warp `half` writes column
           //      chunks 2*half, 2*half+1 of the slab) and one lane hands it to the TMA unit; two boxes alternate, so only
           //      the store issued two slabs ago must have been read out.  Rows >= M / columns past the tensor are clipped
@@ -269,7 +294,7 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
           const float ks = p.sm_drop_p > 0.f ? 1.f / (1.f - p.sm_drop_p) : 1.f;
           uint32_t qa[16], qb[16];
           // fused softmax backward: the P_pre row segments of the NEXT slab are requested before the current slab is
-          // processed: the slab loop is a dependent chain (TMEM load -> math -> shared store -> barrier -> TMA store) with two
+          // processed: the slab loop is a dependent chain (image load -> math -> shared store -> barrier -> TMA store) with two
           // warps per lane quarter and nothing else to hide a global load behind
           uint4 pn00, pn01, pn10, pn11;   // next slab: [chunk u][16-byte half]
           auto prefetch = [&](int s0n) {
@@ -307,13 +332,12 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
               }
             }
             __syncwarp();
-            tmem_ld16(taddr + (ca << 4), qa);
-            tmem_ld16(taddr + (cb << 4), qb);
+            acc_ld16(arow + (ca << 4), qa);
+            acc_ld16(arow + (cb << 4), qb);
             uint8_t* box = stage_out + ((slab_ctr & 1u) ? 4 * 4096 : 0) + quarter * 4096;
             ++slab_ctr;
             if (issuer) tma_store_wait_read_but_one();
             asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
-            tmem_wait_ld();
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
               const int c0 = (u ? cb : ca) << 4;
@@ -382,7 +406,7 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
           }
         } else if (p.sm_P != nullptr) {
           // ---- softmax backward fused into the dP product (see ttsb_bgemm_args): this thread owns query row m of
-          //      problem z.  The P_pre row segments of all its chunks are requested before the first TMEM load.
+          //      problem z.  The P_pre row segments of all its chunks are requested before the first accumulator load.
           int len = min(max(__ldg(p.sm_len + b), 0), p.N);
           const bool live = row_ok && ((p.sm_flags & 2) ? len > 0 : m < len);
           if (p.sm_flags & 1) len = min(len, m + 1);
@@ -390,7 +414,7 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
           const uint32_t thresh = dropout_thresh(p.sm_drop_p);
           const float ks = p.sm_drop_p > 0.f ? 1.f / (1.f - p.sm_drop_p) : 1.f;
           // chunks of this thread in groups of four: the P_pre (and P_drop) row segments of a group are requested before
-          // its first TMEM load.  The dropout decision is read back from the saved P_drop (kept <=> P_drop != 0 wherever
+          // its first accumulator load.  The dropout decision is read back from the saved P_drop (kept <=> P_drop != 0 wherever
           // P_pre != 0) when sm_Pdrop is given; otherwise it is regenerated from the hash.
           constexpr int GRP = 4;
           for (int g0 = ch_begin; g0 < ch_end; g0 += GRP) {
@@ -422,8 +446,7 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
               if (ch < ch_end) {   // warp-uniform
                 const int c0 = ch << 4;
                 __syncwarp();
-                tmem_ld16(taddr + c0, r);
-                tmem_wait_ld();
+                acc_ld16(arow + c0, r);
                 if (row_ok && n0 + c0 < p.out_cols) {
                   const size_t e0 = o + c0;  // element index in the (Z, M, ld_out) layout shared by P_pre, P_drop, dP and dS
                   uint32_t hh[8];
@@ -457,8 +480,7 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
         for (int ch = ch_begin; ch < ch_end; ++ch) {
           const int c0 = ch << 4;
           __syncwarp();
-          tmem_ld16(taddr + c0, r);
-          tmem_wait_ld();
+          acc_ld16(arow + c0, r);
           if (row_ok && n0 + c0 < p.out_cols) {  // out_cols (multiple of 16) bounds the writable part of the row
             float y[16];
 #pragma unroll
@@ -493,8 +515,7 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
         for (int ch = ch_begin; ch < ch_end; ++ch) {
           const int c0 = ch << 4;
           __syncwarp();
-          tmem_ld16(taddr + c0, r);
-          tmem_wait_ld();
+          acc_ld16(arow + c0, r);
           if (row_ok) {
             if ((p.N & 3) == 0 && n0 + c0 + 16 <= p.N) {   // 16-byte aligned: four vector reductions instead of sixteen scalar ones
 #pragma unroll
@@ -510,21 +531,16 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tmem_empty + acc);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      // the staging boxes and the image lie in the ring: TMA stores must have read them before the producer refills it
+      if (p.staged && half == 0 && lane == 0) tma_store_wait_read();
+      fence_proxy_async_smem();
+      asm volatile("bar.sync 5, 256;" ::: "memory");
+      if (threadIdx.x == 0) mbar_arrive(img_free);
     }
     if (p.staged && half == 0 && lane == 0) tma_store_wait_all();  // staged boxes fully written out before exit
   }
-
-  tc_fence_before();
+done:
   __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
 static int launch(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& o, const BgParams& p, cudaStream_t stream) {

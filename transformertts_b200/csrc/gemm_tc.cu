@@ -1,8 +1,10 @@
 // Tensor-core GEMM family for the ForwardTransformer blocks (Dense / concat-projection / Conv1D 'same'):
-// persistent warp-specialised tcgen05 kernel -- TMA (3-D maps over (C,T,B), OOB rows = 'same' zero padding) ->
-// 128B-swizzled shared memory -> tcgen05.mma (kind::f16, bf16 operands, fp32 accumulators in TMEM, double buffered)
-// -> epilogue warps (tcgen05.ld, one thread per output row) fusing bias / ReLU / residual / LayerNorm / row mask and
-// writing fp32 + bf16 hi/lo (or fp16) copies for the next GEMM / the attention kernel.
+// persistent warp-specialised wgmma kernel -- one TMA producer warp (3-D maps over (C,T,B), OOB rows = 'same' zero
+// padding) -> 128B-swizzled shared-memory ring -> two consumer warpgroups, each issuing wgmma (bf16 operands, fp32
+// accumulators in registers) for 64 of the tile's 128 rows.  The finished tile is parked in shared memory (accumulator
+// image, overlaying the drained ring) and the same eight warps run the epilogue one thread per output row, fusing bias /
+// ReLU / residual / LayerNorm / row mask and writing fp32 + bf16 hi/lo (or fp16) copies for the next GEMM / the
+// attention kernel.
 //
 // Replaces, in the reference (TF2/Keras ops): model/layers.py:134-136,149 (q/k/v + concat projection),
 // :93-94 (FFN), :19-26,36-40 (Conv1D stack + residual LayerNorm), :498-524 (predictor convs), model/models.py:422.
@@ -17,6 +19,7 @@
 #include <cuda_fp16.h>
 
 #include "ttsb_common.cuh"
+#include "wgmma_sm90.cuh"
 #include "ttsb_host.h"
 
 namespace ttsb {
@@ -24,11 +27,12 @@ namespace ttsb {
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
 constexpr int GEMM_MAX_BN = 256;
-constexpr int GEMM_THREADS = 320;  // warp0 TMA, warp1 MMA (+TMEM alloc), warps2-9 epilogue (2 per TMEM lane quarter)
+constexpr int GEMM_THREADS = 384;  // warps 0-7: two wgmma / epilogue warpgroups, warp 8: TMA producer (warps 9-11 idle: the
+                                   // producer warpgroup hands its registers to the others with setmaxnreg)
 constexpr int GEMM_EPI_WARPS = 8;
 constexpr int A_TILE_BYTES = GEMM_BM * GEMM_BK * 2;      // 16 KiB
 constexpr int B_TILE_BYTES = GEMM_MAX_BN * GEMM_BK * 2;  // 32 KiB
-constexpr int TMEM_COLS = 512;
+constexpr int GEMM_NCH = GEMM_MAX_BN / 64;               // wgmma n64 products per k step (the tile width rounded up to 64)
 
 struct GemmKParams {
   int B, T, N, block_n, n_tiles, tiles_per_row, num_tiles;
@@ -54,20 +58,7 @@ struct GemmKParams {
   uint32_t drop_pre_site, drop_post_site, drop_seed;
   int h16;  // 1: out_hi receives IEEE fp16 instead of bf16 (single plane; operands of the fp16 attention)
   int staged;  // 1: 16-bit outputs go through shared memory and TMA tile stores (plain epilogue, block_n % 64 == 0)
-#ifdef TTSB_GEMM_TRACE
-  long long* trace;  // debug build only: clock64 stamps of CTA 0: [3 roles][64 tiles][4 events]
-#endif
 };
-
-#ifdef TTSB_GEMM_TRACE
-#define GEMM_TRACE(role, it, ev)                                                              \
-  do {                                                                                        \
-    if (p.trace && blockIdx.x == 0 && (threadIdx.x & 31) == 0 && (it) < 64)                   \
-      p.trace[((role) * 64 + (it)) * 4 + (ev)] = clock64();                                   \
-  } while (0)
-#else
-#define GEMM_TRACE(role, it, ev) do {} while (0)
-#endif
 
 // kPair: the LayerNorm GEMMs run as a cluster of two CTAs that split the N (row) dimension of one 128-row tile in halves
 // (twice as many work items -> no wave-quantisation tail, small-M encoder GEMMs fill the chip) and exchange per-row
@@ -78,15 +69,20 @@ struct GemmCfg {
   static constexpr int kStages = kSplit ? 2 : 4;
   static constexpr int kBTile = kPair ? PAIR_MAX_BN * GEMM_BK * 2 : B_TILE_BYTES;
   static constexpr int kStageBytes = (kSplit ? 2 : 1) * (A_TILE_BYTES + kBTile);
-  static constexpr int kBarOffset = kStages * kStageBytes;
-  static constexpr int kRedOffset = kBarOffset + 256;           // [2 acc][2][2][128] floats of intra-CTA exchange
-  static constexpr int kXchgOffset = kRedOffset + 4096;         // pair mode: [2 slots][128] float2 written by the peer CTA
-  static constexpr int kXbarOffset = kXchgOffset + 2048;        // pair mode: 2 mbarriers
-  // plain (non-LayerNorm) epilogue: two planes x four lane quarters of [32 rows x 64 cols] 16-bit staging boxes (4 KB each,
-  // 128B-swizzled) for TMA tile stores; they overlay the LayerNorm exchange area, which that kernel does not use
-  static constexpr int kStageOutOffset = (kRedOffset + 1023) / 1024 * 1024;
+  static constexpr int kRingBytes = kStages * kStageBytes;
+  // accumulator image [128 rows][kPitch floats]: written once the ring is drained, so it overlays the ring
+  static constexpr int kPitch = acc_pitch(kPair ? PAIR_MAX_BN : GEMM_MAX_BN);
+  static constexpr int kImgBytes = GEMM_BM * kPitch * 4;
+  // plain (non-LayerNorm) epilogue: two planes x four row quarters of [32 rows x 64 cols] 16-bit staging boxes (4 KB each,
+  // 128B-swizzled) for TMA tile stores, in the ring behind the image
+  static constexpr int kStageOutOffset = (kImgBytes + 1023) / 1024 * 1024;
   static constexpr int kStageOutBytes = 2 * 4 * 4096;
-  static constexpr int kSmemBytes = (kStageOutOffset + kStageOutBytes > kXbarOffset + 64 ? kStageOutOffset + kStageOutBytes : kXbarOffset + 64) + 1024;  // + alignment slack
+  static_assert(kImgBytes <= kRingBytes && (kPair || kStageOutOffset + kStageOutBytes <= kRingBytes), "image must fit the ring");
+  static constexpr int kBarOffset = kRingBytes;
+  static constexpr int kRedOffset = kBarOffset + 256;           // [2][2][128] floats of intra-CTA exchange
+  static constexpr int kXchgOffset = kRedOffset + 2048;         // pair mode: [2 slots][128] float2 written by the peer CTA
+  static constexpr int kXbarOffset = kXchgOffset + 2048;        // pair mode: 2 mbarriers
+  static constexpr int kSmemBytes = kXbarOffset + 64 + 1024;    // + alignment slack
 };
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
@@ -123,9 +119,9 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
 }
 
 // ----------------------------------------------------------------------------------------------------
-// Epilogue for one 128 x block_n accumulator tile.  8 epilogue warps: warp (quarter, half) owns TMEM lanes
-// [32*quarter, +32) (thread = one output row) and the lower / upper half of the tile's 16-column chunks, so two warps
-// per SM sub-partition interleave and hide each other's latencies.  Per-column vectors (bias, gamma, beta) are read
+// Epilogue for one 128 x block_n accumulator tile (image rows in shared memory).  8 epilogue warps: warp (quarter, half)
+// owns rows [32*quarter, +32) (thread = one output row) and the lower / upper half of the tile's 16-column chunks, so
+// two warps per SM sub-partition interleave and hide each other's latencies.  Per-column vectors (bias, gamma, beta) are read
 // as warp-uniform float4 loads (buffers are padded to n_pad by the host).
 // ----------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void ldg16(const float* __restrict__ p, float (&v)[16]) {
@@ -209,8 +205,8 @@ struct PairCtx {
 };
 
 template <bool kLN>
-__device__ __forceinline__ void epilogue_tile(const GemmKParams& p, uint32_t taddr, int b, int t0, int n0, int row, int half,
-                                              int quarter, float* red /* [2][2][128] for this accumulator stage */,
+__device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow, int b, int t0, int n0, int row, int half,
+                                              int quarter, float* red /* [2][2][128] */,
                                               const PairCtx& px, uint8_t* stage_out, const CUtensorMap* tmOh, const CUtensorMap* tmOl,
                                               uint32_t& slab_ctr) {
   const int t = t0 + row;
@@ -228,9 +224,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, uint32_t tad
   if constexpr (!kLN) {
     if (p.staged) {
       // 16-bit outputs as TMA tile stores.  A thread owns one output ROW, so direct stores are 32-byte pieces of 32
-      // different rows per warp instruction; the clock64 trace (tools/gemm_trace.py) shows ~1000 clk per 16-column chunk
-      // in that form (request-rate bound: 10 kclk per 128x256 fp16 tile, more than the 6.7 kclk of MMAs at K = 256).
-      // Here the two warps of a lane quarter fill a [32 rows x 64 cols] 128B-swizzled box per plane and one lane hands
+      // different rows per warp instruction (request-rate bound).  Here the two warps of a lane quarter fill a [32 rows x 64 cols] 128B-swizzled box per plane and one lane hands
       // it to the TMA unit (full 128-byte lines, asynchronous, rows >= T and columns >= N clipped by the tensor map).
       uint8_t* box_a = stage_out + quarter * 4096;
       uint8_t* box_b = stage_out + 4 * 4096 + quarter * 4096;
@@ -241,8 +235,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, uint32_t tad
       for (int s0 = 0; s0 < nch; s0 += 4) {   // 64-column slab: this warp handles chunks s0 + 2*half, +1
         const int ca = s0 + 2 * half, cb = ca + 1;
         __syncwarp();
-        tmem_ld16(taddr + (ca << 4), qa);
-        tmem_ld16(taddr + (cb << 4), qb);
+        acc_ld16(arow + (ca << 4), qa);
+        acc_ld16(arow + (cb << 4), qb);
         // two planes: box_a = hi, box_b = lo, reused every slab; one plane: the two boxes alternate, so only the store
         // issued two slabs ago has to have been read out
         uint8_t* box_hi = two ? box_a : ((slab_ctr & 1u) ? box_b : box_a);
@@ -252,7 +246,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, uint32_t tad
           if (two) tma_store_wait_read(); else tma_store_wait_read_but_one();
         }
         asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
-        tmem_wait_ld();
 #pragma unroll
         for (int u = 0; u < 2; ++u) {
           const int c0 = (u ? cb : ca) << 4;
@@ -306,21 +299,14 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, uint32_t tad
       }
       return;
     }
-    // direct stores (fp32 outputs, residual adds, odd tile widths): two TMEM loads in flight per wait
+    // direct stores (fp32 outputs, residual adds, odd tile widths)
     constexpr int IN_FLIGHT = 2;
     uint32_t q[IN_FLIGHT][16];
     for (int g0 = ch_begin; g0 < ch_end; g0 += IN_FLIGHT) {
       __syncwarp();
-#ifdef TTSB_GEMM_TRACE
-      if (p.trace && blockIdx.x == 0 && threadIdx.x == 64) p.trace[(2 * 64 + (g0 - ch_begin) / IN_FLIGHT) * 4 + 0] = clock64();
-#endif
 #pragma unroll
       for (int i = 0; i < IN_FLIGHT; ++i)
-        if (g0 + i < ch_end) tmem_ld16(taddr + ((g0 + i) << 4), q[i]);
-      tmem_wait_ld();
-#ifdef TTSB_GEMM_TRACE
-      if (p.trace && blockIdx.x == 0 && threadIdx.x == 64) p.trace[(2 * 64 + (g0 - ch_begin) / IN_FLIGHT) * 4 + 1] = clock64();
-#endif
+        if (g0 + i < ch_end) acc_ld16(arow + ((g0 + i) << 4), q[i]);
 #pragma unroll
       for (int i = 0; i < IN_FLIGHT; ++i) {
         if (g0 + i < ch_end) {   // warp-uniform
@@ -354,20 +340,17 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, uint32_t tad
           if (row_ok) store_chunk(p, orow, n0 + c0, y);
         }
       }
-#ifdef TTSB_GEMM_TRACE
-      if (p.trace && blockIdx.x == 0 && threadIdx.x == 64) p.trace[(2 * 64 + (g0 - ch_begin) / IN_FLIGHT) * 4 + 2] = clock64();
-#endif
     }
     return;
   } else {
 
-  // ---- LayerNorm epilogue (single N tile), two passes over TMEM:
-  //   pass 1 builds v = acc + bias (+relu) (+dropout) (+residual), parks it back in TMEM and accumulates SHIFTED sums
+  // ---- LayerNorm epilogue (single N tile), two passes over the accumulator image:
+  //   pass 1 builds v = acc + bias (+relu) (+dropout) (+residual), parks it back in the image and accumulates SHIFTED sums
   //          s = sum(v - K), q = sum((v - K)^2) with K = the thread's first value (no cancellation: this is Welford's
   //          statistic for the thread's column range, (mean_h, M2_h) = (K + s/n_h, q - s^2/n_h));
   //   the two warps of a lane quarter (column halves) and, in pair mode, the two CTAs of the cluster combine their
-  //   (mean, M2, n) with Chan's parallel formula; pass 2 normalises.  TMEM loads and the residual row are fetched one
-  //   chunk ahead of their use.
+  //   (mean, M2, n) with Chan's parallel formula; pass 2 normalises.  The residual row is fetched one chunk ahead of its
+  //   use.
   const float inv_n = 1.f / (float)ncols;
   uint32_t r2[16];
   float res[16], res2[16];
@@ -378,7 +361,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, uint32_t tad
   const __nv_bfloat16* res_row_lo = (has_res && pair_res) ? p.res_lo + orow * (size_t)p.ld_res + n0 : nullptr;
   auto fetch = [&](int ch, uint32_t (&rr)[16], float (&rs)[16]) {
     const int c0 = ch << 4;
-    tmem_ld16(taddr + c0, rr);
+    acc_ld16(arow + c0, rr);
     if (has_res) {
       if (pair_res) {
         // 16 columns = 32 bytes of hi + 32 bytes of lo; x = hi + lo (bf16 -> fp32 is a 16-bit shift)
@@ -443,21 +426,18 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, uint32_t tad
       st_global_v8f(dst, y);
       st_global_v8f(dst + 8, y + 8);
     }
-    tmem_st16(taddr + c0, rr);
+    acc_st16(arow + c0, rr);
   };
   __syncwarp();
   if (ch_begin < ch_end) fetch(ch_begin, r, res);
   for (int ch = ch_begin; ch < ch_end; ch += 2) {
-    tmem_wait_ld_tied(r);
     if (ch + 1 < ch_end) fetch(ch + 1, r2, res2);
     pass1_chunk(ch, r, res);
     if (ch + 1 < ch_end) {
-      tmem_wait_ld_tied(r2);
       if (ch + 2 < ch_end) fetch(ch + 2, r, res);
       pass1_chunk(ch + 1, r2, res2);
     }
   }
-  tmem_wait_st();
   // (mean, M2, n) of this thread's column range, then of the CTA's columns (half 0 is always operand 'a': both warps of
   // the pair evaluate the same expression and get bit-identical statistics)
   const int n_mine = max(0, min(ncols, ch_end << 4) - (ch_begin << 4));
@@ -518,14 +498,12 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, uint32_t tad
     if (row_ok) store_chunk(p, orow, n0 + c0, y);
   };
   __syncwarp();
-  if (ch_begin < ch_end) tmem_ld16(taddr + (ch_begin << 4), r);
+  if (ch_begin < ch_end) acc_ld16(arow + (ch_begin << 4), r);
   for (int ch = ch_begin; ch < ch_end; ch += 2) {
-    tmem_wait_ld_tied(r);
-    if (ch + 1 < ch_end) tmem_ld16(taddr + ((ch + 1) << 4), r2);
+    if (ch + 1 < ch_end) acc_ld16(arow + ((ch + 1) << 4), r2);
     pass2_chunk(ch, r);
     if (ch + 1 < ch_end) {
-      tmem_wait_ld_tied(r2);
-      if (ch + 2 < ch_end) tmem_ld16(taddr + ((ch + 2) << 4), r);
+      if (ch + 2 < ch_end) acc_ld16(arow + ((ch + 2) << 4), r);
       pass2_chunk(ch + 1, r2);
     }
   }
@@ -546,9 +524,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kBarOffset);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* tmem_full = empty_bar + Cfg::kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  uint64_t* img_free = empty_bar + Cfg::kStages;   // the epilogue of the previous tile has released the ring / image
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -563,38 +539,37 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
     tma_prefetch_desc(&tmWh);
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(full_bar + s, 1);
-      mbar_init(empty_bar + s, 1);
+      mbar_init(empty_bar + s, GEMM_EPI_WARPS);
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tmem_full + s, 1);
-      mbar_init(tmem_empty + s, GEMM_EPI_WARPS);
+    mbar_init(img_free, 1);
+    for (int s = 0; s < 2; ++s)
       if (kPair) mbar_init(xbar + s, GEMM_EPI_WARPS);  // one arrival per epilogue warp of the PEER CTA
-    }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   if (kPair) cluster_sync_all();  // the peer's exchange barriers are initialised before anyone arrives on them
-  const uint32_t tmem_base = *tmem_slot;
 
   const uint32_t stage_tx = (kSplit ? 2u : 1u) * (uint32_t)(A_TILE_BYTES + p.block_n * GEMM_BK * 2);
 
-  if (warp == 0) {
+  if (warp >= GEMM_EPI_WARPS) {
+    setmaxnreg_dec<40>();
+    if (warp > GEMM_EPI_WARPS) goto done;
     // ===================== TMA producer: warp-uniform control flow, the elected lane issues (see elect_one) ==========
     const bool leader = elect_one();
     int stage = 0;
-    uint32_t phase = 0;
+    uint32_t phase = 0, img_phase = 0;
+    bool first = true;
     for (int tile = p.tile_begin + work_id; tile < p.num_tiles; tile += work_stride) {
       const int n_tile = kPair ? cta_rank : tile % p.n_tiles;
       const int m_tile = kPair ? tile : tile / p.n_tiles;
       const int b = m_tile / p.tiles_per_row;
       const int t0 = (m_tile % p.tiles_per_row) * GEMM_BM;
       const int n0 = n_tile * p.block_n;
+      if (!first) {   // the ring holds the previous tile's accumulator image until its epilogue is done
+        mbar_wait(img_free, img_phase);
+        img_phase ^= 1;
+      }
+      first = false;
       int kglob = 0;
       for (int s = 0; s < p.num_seg; ++s) {
         const CUtensorMap* mh = p.seg_src[s] == 0 ? &tmA0h : &tmA1h;
@@ -616,71 +591,80 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: warp-uniform control flow, the elected lane issues =====================
-    const bool leader = elect_one();
-    const uint32_t idesc = make_idesc_bf16(GEMM_BM, p.block_n);
+  } else {
+    // ===================== two wgmma warpgroups (rows [64*wg, +64) of the tile), then the epilogue =====================
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int quarter = warp & 3;        // epilogue: rows [32*quarter, +32)
+    const int half = warp >> 2;          // epilogue: which half of the tile's column chunks
+    float* red_all = reinterpret_cast<float*>(smem + Cfg::kRedOffset);
+    float* img = reinterpret_cast<float*>(smem);
     int stage = 0;
     uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    int total_kb = 0;
-    for (int s = 0; s < p.num_seg; ++s) total_kb += p.seg_kblocks[s];
-    int trace_it = 0;
-    for (int tile = p.tile_begin + work_id; tile < p.num_tiles; tile += work_stride, ++trace_it) {
-      GEMM_TRACE(1, trace_it, 0);
-      mbar_wait(tmem_empty + acc, acc_phase ^ 1);
-      GEMM_TRACE(1, trace_it, 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * GEMM_MAX_BN;
-      for (int kb = 0; kb < total_kb; ++kb) {
-        mbar_wait(full_bar + stage, phase);
-        if (kb == 0) GEMM_TRACE(1, trace_it, 2);
-        tc_fence_after();
-        const uint32_t st = smem_u32(smem + stage * Cfg::kStageBytes);
-        const uint64_t a_hi = make_smem_desc_sw128(st);
-        const uint64_t b_hi = make_smem_desc_sw128(st + A_TILE_BYTES);
-        if (leader) {
-#pragma unroll
-          for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
-            umma_bf16(d_tmem, a_hi + 2 * kk, b_hi + 2 * kk, idesc, (kb | kk) != 0);
-          }
-          if (kSplit) {
-            const uint64_t a_lo = make_smem_desc_sw128(st + A_TILE_BYTES + Cfg::kBTile);
-            const uint64_t b_lo = make_smem_desc_sw128(st + 2 * A_TILE_BYTES + Cfg::kBTile);
-#pragma unroll
-            for (int kk = 0; kk < GEMM_BK / 16; ++kk) umma_bf16(d_tmem, a_lo + 2 * kk, b_hi + 2 * kk, idesc, 1);
-#pragma unroll
-            for (int kk = 0; kk < GEMM_BK / 16; ++kk) umma_bf16(d_tmem, a_hi + 2 * kk, b_lo + 2 * kk, idesc, 1);
-          }
-          umma_commit(empty_bar + stage);  // frees the smem stage once these MMAs have read it
-        }
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-      }
-      if (leader) umma_commit(tmem_full + acc);  // accumulator complete
-      GEMM_TRACE(1, trace_it, 3);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  } else if (warp >= 2) {
-    // ===================== epilogue warps =====================
-    const int quarter = warp & 3;        // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;    // which half of the tile's column chunks
-    float* red_all = reinterpret_cast<float*>(smem + Cfg::kRedOffset);
-    int acc = 0;
-    uint32_t acc_phase = 0;
     int iter = 0;
     float2* xslots = reinterpret_cast<float2*>(smem + Cfg::kXchgOffset);
     uint32_t slab_ctr = 0;  // staged epilogue: slabs stored so far (selects the staging box of single-plane outputs)
+    int total_kb = 0;
+    for (int s = 0; s < p.num_seg; ++s) total_kb += p.seg_kblocks[s];
+    const int nch = (p.block_n + 63) >> 6;   // n64 products per k step; columns past block_n are computed and ignored
     for (int tile = p.tile_begin + work_id; tile < p.num_tiles; tile += work_stride, ++iter) {
       const int n_tile = kPair ? cta_rank : tile % p.n_tiles;
       const int m_tile = kPair ? tile : tile / p.n_tiles;
       const int b = m_tile / p.tiles_per_row;
       const int t0 = (m_tile % p.tiles_per_row) * GEMM_BM;
-      if (warp == 2) GEMM_TRACE(0, iter, 0);
-      mbar_wait(tmem_full + acc, acc_phase);
-      if (warp == 2) GEMM_TRACE(0, iter, 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * GEMM_MAX_BN;
+      float acc[GEMM_NCH][32];
+      int prev_stage = -1;
+      for (int kb = 0; kb < total_kb; ++kb) {
+        mbar_wait(full_bar + stage, phase);
+        const uint32_t st = smem_u32(smem + stage * Cfg::kStageBytes);
+        const uint32_t a_hi = st + wg * (64 * 128);
+        const uint32_t b_hi = st + A_TILE_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
+          const uint64_t da = make_smem_desc_sw128(a_hi) + 2 * kk;
+#pragma unroll
+          for (int c = 0; c < GEMM_NCH; ++c)
+            if (c < nch) wgmma_ss_m64n64_bf16<0, 0>(acc[c], da, make_smem_desc_sw128(b_hi + c * (64 * 128)) + 2 * kk, (kb | kk) != 0);
+        }
+        if (kSplit) {
+          const uint32_t a_lo = st + A_TILE_BYTES + Cfg::kBTile + wg * (64 * 128);
+          const uint32_t b_lo = st + 2 * A_TILE_BYTES + Cfg::kBTile;
+#pragma unroll
+          for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
+            const uint64_t da_lo = make_smem_desc_sw128(a_lo) + 2 * kk, da_hi = make_smem_desc_sw128(a_hi) + 2 * kk;
+#pragma unroll
+            for (int c = 0; c < GEMM_NCH; ++c) {
+              if (c < nch) {
+                wgmma_ss_m64n64_bf16<0, 0>(acc[c], da_lo, make_smem_desc_sw128(b_hi + c * (64 * 128)) + 2 * kk, 1);
+                wgmma_ss_m64n64_bf16<0, 0>(acc[c], da_hi, make_smem_desc_sw128(b_lo + c * (64 * 128)) + 2 * kk, 1);
+              }
+            }
+          }
+        }
+        wgmma_commit();
+        // the products of the previous k block have finished reading their stage: release it
+        wgmma_wait<1>();
+        if (prev_stage >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar + prev_stage);
+        }
+        prev_stage = stage;
+        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int c = 0; c < GEMM_NCH; ++c) wgmma_fence_regs(acc[c]);
+      if (prev_stage >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_bar + prev_stage);
+      }
+      // both warpgroups are done reading the ring: park the tile in it
+      asm volatile("bar.sync 5, 256;" ::: "memory");
+#pragma unroll
+      for (int c = 0; c < GEMM_NCH; ++c)
+        if (c < nch) acc_store_fragment(img, Cfg::kPitch, wg * 64, c * 64, acc[c]);
+      asm volatile("bar.sync 5, 256;" ::: "memory");
       PairCtx px{};
       if (kPair) {
         const int slot = iter & 1;
@@ -691,25 +675,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
         px.peer_bar = map_to_peer(smem_u32(px.my_bar), (uint32_t)(cta_rank ^ 1));
         px.parity = (uint32_t)((iter >> 1) & 1);
       }
-      epilogue_tile<kLN>(p, taddr, b, t0, n_tile * p.block_n, quarter * 32 + lane, half, quarter, red_all + acc * (4 * GEMM_BM), px,
+      const int row = quarter * 32 + lane;
+      epilogue_tile<kLN>(p, img + (size_t)row * Cfg::kPitch, b, t0, n_tile * p.block_n, row, half, quarter, red_all, px,
                          smem + Cfg::kStageOutOffset, &tmOh, &tmOl, slab_ctr);
-      if (warp == 2) GEMM_TRACE(0, iter, 2);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tmem_empty + acc);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      // the staging boxes and the image lie in the ring: TMA stores must have read them before the producer refills it
+      if (!kLN && p.staged && half == 0 && lane == 0) tma_store_wait_read();
+      fence_proxy_async_smem();
+      asm volatile("bar.sync 5, 256;" ::: "memory");
+      if (threadIdx.x == 0) mbar_arrive(img_free);
     }
     if (!kLN && p.staged && half == 0 && lane == 0) tma_store_wait_all();  // staged boxes fully written out before exit
   }
-
-  tc_fence_before();
+done:
   __syncthreads();
   if (kPair) cluster_sync_all();  // keep this CTA's shared memory alive until the peer's last remote write / arrive landed
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
 }
 
 // ----------------------------------------------------------------------------------------------------
@@ -884,7 +863,7 @@ extern "C" int ttsb_linear_fwd(const ttsb_gemm_args* a, void* stream_v) {
   p.res_lo = static_cast<const __nv_bfloat16*>(a->residual_lo);
   if (!a->residual && (a->residual_hi || a->residual_lo)) {
     if (!a->residual_hi || !a->residual_lo || !a->ln_gamma || a->impl == TTSB_IMPL_SIMT) {
-      set_last_error("ttsb_linear_fwd: a bf16 hi/lo residual needs both planes and the tcgen05 LayerNorm epilogue");
+      set_last_error("ttsb_linear_fwd: a bf16 hi/lo residual needs both planes and the tensor-core LayerNorm epilogue");
       return TTSB_ERR_INVALID_ARGUMENT;
     }
   }
@@ -902,16 +881,10 @@ extern "C" int ttsb_linear_fwd(const ttsb_gemm_args* a, void* stream_v) {
     return TTSB_ERR_INVALID_ARGUMENT;
   }
   if ((a->drop_pre_p > 0.f || a->drop_post_p > 0.f) && a->impl == TTSB_IMPL_SIMT) {
-    set_last_error("ttsb_linear_fwd: dropout is only implemented in the tcgen05 kernel");
+    set_last_error("ttsb_linear_fwd: dropout is only implemented in the tensor-core kernel");
     return TTSB_ERR_UNSUPPORTED;
   }
   if (p.h16) p.out_lo = nullptr;
-#ifdef TTSB_GEMM_TRACE
-  {
-    const char* e = getenv("TTSB_GEMM_TRACE_PTR");  // device pointer (hex) of a 3*64*4 int64 buffer
-    p.trace = e ? reinterpret_cast<long long*>(strtoull(e, nullptr, 16)) : nullptr;
-  }
-#endif
 
   if (a->impl == TTSB_IMPL_SIMT) {
     GemmSimtPtrs q{};

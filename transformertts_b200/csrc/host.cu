@@ -37,7 +37,7 @@ int num_sms() {
   static PerDevice<int> sms;
   int& n = sms.get();
   if (n == 0) {
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, current_device()) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, current_device()) != cudaSuccess || n <= 0) n = 132;  // H100 SXM
   }
   return n;
 }

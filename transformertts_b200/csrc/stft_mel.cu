@@ -160,9 +160,8 @@ stft_mel_kernel(const float* __restrict__ wav, int n_samples, int n_frames, int 
 
 // ----------------------------------------------------------------------------------------------------
 // Version 2 of the fused kernel (the one ttsb_stft_mel_log launches; the kernel above is kept as TTSB_STFT_V1=1 for A/B runs).
-// ncu of version 1 (profiles/r02_stft.md): 38 % of the issue slots used, long-scoreboard stalls dominate (4.9 per issued
-// instruction: global loads of samples, window, filter weights and band bounds with nothing to hide them behind), 17 M
-// shared-memory bank conflicts in the mel loop, ~3700 instructions per frame pair.  Changes:
+// Version 1 waits on global loads of samples, window, filter weights and band bounds with nothing to hide them behind, and
+// its mel loop has shared-memory bank conflicts.  Changes:
 //   * persistent warps; the samples of the NEXT frame pair are requested into the (dead) FFT registers before the
 //     magnitude / mel phase of the current pair, so their latency is hidden behind ~500 instructions of other work;
 //   * window, twiddles (as (cos, -sin) pairs), packed filter weights and band bounds live in shared memory;

@@ -129,7 +129,7 @@ softmax_fwd_vec_kernel(const float* __restrict__ S, int Z, int H, int T, int Tk,
 }
 
 // dS = scale * P_pre * (dPp - sum_k P_pre dPp),  dPp = dP * keep/(1-p).  Two light passes over the row (the second one
-// hits L2); keeping the row in registers instead was measured 2-4x slower (occupancy).
+// hits L2); keeping the whole row in registers instead would cost occupancy.
 __global__ void softmax_bwd_kernel(const __nv_bfloat16* __restrict__ P_pre, const float* __restrict__ dP, int Z, int H, int T, int Tk,
                                    int ld, const int* __restrict__ kv_len, float scale, float drop_p, uint32_t seed, uint32_t site,
                                    int flags, __nv_bfloat16* __restrict__ dS) {
@@ -989,7 +989,7 @@ extern "C" int ttsb_scaled_ce_loss(const float* logits, int B, int Tp, int Tt, i
                                    float scaling, float* loss_out, float grad_weight, float* grad, int ld_grad, void* stream) {
   if (!logits || !targets || !loss_out || B <= 0 || Tp <= 0 || Tt <= 0 || Tt > Tp || C <= 0 || ld < C || (grad && ld_grad < C))
     return bad("ttsb_scaled_ce_loss: bad arguments (need Tt <= Tp, ld >= C)");
-  scaled_ce_kernel<<<148, 256, 0, STREAM(stream)>>>(logits, B, Tp, Tt, C, ld, targets, index, scaling, loss_out, grad_weight, grad, ld_grad);
+  scaled_ce_kernel<<<num_sms(), 256, 0, STREAM(stream)>>>(logits, B, Tp, Tt, C, ld, targets, index, scaling, loss_out, grad_weight, grad, ld_grad);
   LAUNCH_OK("scaled_ce_kernel");
 }
 

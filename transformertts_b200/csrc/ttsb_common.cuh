@@ -1,6 +1,6 @@
-// Shared device helpers for the sm_100a kernels: mbarrier, TMA, tcgen05 (TMEM alloc / MMA / ld / st / commit),
-// shared-memory matrix descriptors and the kind::f16 instruction descriptor.
-// Everything is inline PTX; no CUTLASS dependency.  Compile with -gencode arch=compute_100a,code=sm_100a.
+// Shared device helpers for the sm_90a kernels: mbarrier, TMA, wgmma shared-memory matrix descriptors and the
+// shared-memory accumulator image of the GEMM epilogues (the wgmma instructions themselves are in wgmma_sm90.cuh).
+// Everything is inline PTX; no CUTLASS dependency.  Compile with -gencode arch=compute_90a,code=sm_90a.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -42,8 +42,7 @@ __device__ __forceinline__ uint32_t pack_bf16(__nv_bfloat16 a, __nv_bfloat16 b) 
 // this device-resident word, refreshed by memcpy nodes at the head of the graph.
 static __constant__ uint32_t c_drop_salt = 0;
 // One 32-bit hash serves TWO consecutive elements (16 bits each; the rate is resolved to 2^-16): the per-element cost of the
-// mask is what bounds the attention-probability kernels of the training step (ncu: the fused dS epilogue issued ~42
-// instructions per element with a hash per element).
+// mask is a large share of the per-element work of the attention-probability kernels of the training step.
 // hash(pair) = mix((uint32)pair * C1 ^ hterm(seed, site, pair >> 32)).  Kernels that walk consecutive pairs hoist hterm and
 // step the first term by C1 per pair (dropout_hterm / dropout_mix below) instead of redoing the 64-bit index arithmetic.
 constexpr uint32_t DROPOUT_C1 = 0x9E3779B1u;
@@ -113,9 +112,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 // The same with a suspend-time hint: the hardware parks the warp until the phase completes (or the hint expires) instead of
 // re-issuing the poll, which leaves the issue slots to the other warps of the scheduler.  Used by attn_probs_tc.cu, whose
-// sixteen softmax warps are issue bound (9 % of its instructions were wait loops before).  Measured on the GEMM kernels
-// (gemm_tc / bgemm_tc, A/B on one box, two runs each): C2 step 5.51-5.59 -> 5.60-5.62 ms, C3 step 8.29 -> 8.33 ms -- their
-// producer / issuer warps are on the critical path, so they keep the polling wait above.
+// softmax warpgroups wait for K tiles while sharing schedulers with each other; the GEMM kernels keep the polling wait above
+// for their pipeline barriers.
 __device__ __forceinline__ void mbar_wait_parked(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   for (;;) {
@@ -141,8 +139,6 @@ __device__ __forceinline__ void st_shared_v4(void* p, uint32_t a, uint32_t b, ui
 // fences
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor, tile mode, mbarrier completion)
@@ -180,33 +176,18 @@ __device__ __forceinline__ void tma_store_wait_read_but_one() { asm volatile("cp
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------------
-// TMEM allocation (one warp, .sync.aligned)
+// wgmma shared-memory matrix descriptors (sm_90 format)
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------
-// UMMA descriptors
-// ------------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a K-major operand tile stored as rows of 128 bytes (64 bf16) with the
-// 128-byte swizzle TMA writes (CU_TENSOR_MAP_SWIZZLE_128B): 8-row groups are 1024 B apart (SBO), LBO is unused for
-// swizzled K-major layouts (set to 1), descriptor version 1 (Blackwell), layout type 2 (SWIZZLE_128B).
-// The tile base must be 1024-byte aligned; advancing K by 16 elements adds 32 bytes to the start address.
+// K-major operand tile stored as rows of 128 bytes (64 bf16) with the 128-byte swizzle TMA writes
+// (CU_TENSOR_MAP_SWIZZLE_128B): 8-row groups are 1024 B apart (SBO), LBO is unused for swizzled K-major layouts (set to 1),
+// layout type 1 (SWIZZLE_128B) in bits [62,64).  The tile base must be 1024-byte aligned; advancing K by 16 elements adds
+// 32 bytes to the start address (+2 in descriptor units).
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);       // start address, bits [0,14)
   d |= (uint64_t)1 << 16;                        // leading byte offset (ignored), bits [16,30)
   d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset = 1024 B, bits [32,46)
-  d |= (uint64_t)1 << 46;                        // descriptor version, bits [46,48)
-  d |= (uint64_t)2 << 61;                        // SWIZZLE_128B, bits [61,64)
+  d |= (uint64_t)1 << 62;                        // SWIZZLE_128B
   return d;
 }
 // MN-major operand (the M or N index is contiguous: each 128-byte row holds 64 m/n for ONE k): the tile is stored as
@@ -217,102 +198,79 @@ __device__ __forceinline__ uint64_t make_smem_desc_mn_sw128(uint32_t saddr, uint
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
   d |= (uint64_t)(lbo_bytes >> 4) << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// Instruction descriptor, kind::f16: D=f32, A=B=bf16, both K-major (OR in bit 15 / 16 for an MN-major A / B), dense.
-__host__ __device__ __forceinline__ uint32_t make_idesc_bf16(uint32_t M, uint32_t N) {
-  return (1u << 4)            // c_format = F32
-         | (1u << 7)          // a_format = BF16
-         | (1u << 10)         // b_format = BF16
-         | ((N >> 3) << 17)   // n_dim
-         | ((M >> 4) << 24);  // m_dim
-}
-// Same with IEEE fp16 operands (a_format = b_format = 0).
-__host__ __device__ __forceinline__ uint32_t make_idesc_f16(uint32_t M, uint32_t N) {
-  return (1u << 4) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
 
-// One lane of a fully converged warp.  The TMA / MMA issuing warps run their role code warp-uniformly and predicate only
-// the issuing instructions on this: every operand then lives in uniform registers.  Entering the role under
-// `if (lane == 0)` instead makes ptxas wrap each UTCHMMA / UTMALDG in an ELECT + R2UR + BRA.U.ANY loop (~12 dependent
-// instructions, ~100 clk per MMA measured with clock64 stamps).
+// Register budget hand-over between warpgroups (the producer warpgroup of a warp-specialised kernel needs few registers,
+// the wgmma warpgroups hold their accumulators in registers)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// One lane of a fully converged warp.  The TMA issuing warps run their role code warp-uniformly and predicate only the
+// issuing instructions on this, so every operand stays in uniform registers.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n.reg .pred p;\nelect.sync _|p, 0xffffffff;\nselp.u32 %0, 1, 0, p;\n}" : "=r"(pred));
   return pred != 0;
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+// ------------------------------------------------------------------------------------------------
+// Accumulator image: the GEMM kernels park a finished 128 x N fp32 tile in shared memory as rows of ACC_PITCH(N) floats
+// so that their epilogues run one thread per output row.  A pitch of N + 4 floats (N % 16 == 0) keeps the 16-byte row
+// accesses of eight consecutive rows in distinct banks.
+// ------------------------------------------------------------------------------------------------
+__host__ __device__ constexpr int acc_pitch(int n) { return n + 4; }
+// the wgmma accumulator fragment of one 64 x N warpgroup product (see wgmma_sm90.cuh) -> image rows [row0, row0 + 64)
+template <int R>
+__device__ __forceinline__ void acc_store_fragment(float* img, int pitch, int row0, int col0, const float (&d)[R]) {
+  const int t = threadIdx.x & 127;
+  const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2);
+  const int c = col0 + 2 * (t & 3);
+#pragma unroll
+  for (int i = 0; i < R / 4; ++i) {
+    *reinterpret_cast<float2*>(img + (size_t)r * pitch + c + 8 * i) = make_float2(d[4 * i], d[4 * i + 1]);
+    *reinterpret_cast<float2*>(img + (size_t)(r + 8) * pitch + c + 8 * i) = make_float2(d[4 * i + 2], d[4 * i + 3]);
+  }
 }
-// Arrive on an mbarrier once all tcgen05 ops previously issued BY THIS THREAD have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// 16 consecutive floats of one image row (16-byte aligned)
+__device__ __forceinline__ void acc_ld16(const float* p, uint32_t (&r)[16]) {
+  const uint32_t s = smem_u32(p);
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+    asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(r[4 * j]), "=r"(r[4 * j + 1]), "=r"(r[4 * j + 2]), "=r"(r[4 * j + 3])
+                 : "r"(s + 16 * j) : "memory");
+}
+__device__ __forceinline__ void acc_st16(float* p, const uint32_t (&r)[16]) {
+  const uint32_t s = smem_u32(p);
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+    asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(s + 16 * j), "r"(r[4 * j]), "r"(r[4 * j + 1]), "r"(r[4 * j + 2]),
+                 "r"(r[4 * j + 3]) : "memory");
 }
 
-// ------------------------------------------------------------------------------------------------
-// TMEM <-> registers.  32x32b shape: lane i of the warp reads TMEM lane (base_lane + i), N consecutive columns.
-// A warp may only touch lanes [32*(warp_id%4), 32*(warp_id%4)+32).
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// wait::ld that also ties the destination registers of an earlier tcgen05.ld, so that no use of them can be scheduled
-// above the wait when loads are software-pipelined (issued one chunk ahead of their consumer)
-__device__ __forceinline__ void tmem_wait_ld_tied(uint32_t (&r)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]), "+r"(r[9]),
-                 "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-               :
-               : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32-byte (256-bit, sm_100) global stores / loads: one full sector per lane instead of two half-sector requests
-__device__ __forceinline__ void st_global_v8(void* p, const uint32_t (&v)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]),
-               "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void st_global_v8f(float* p, const float* v) {
-  asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]), "f"(v[4]),
-               "f"(v[5]), "f"(v[6]), "f"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void ld_global_nc_v8f(const float* p, float* v) {
-  asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-               : "l"(p));
-}
-__device__ __forceinline__ void ld_global_nc_v8(const void* p, uint32_t (&v)[8]) {
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "l"(p));
-}
-// 16-byte global stores / loads
+// 32-byte global stores / loads as two 16-byte accesses (one full sector per lane)
 __device__ __forceinline__ void st_global_v4(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+__device__ __forceinline__ void st_global_v8(void* p, const uint32_t (&v)[8]) {
+  st_global_v4(p, v[0], v[1], v[2], v[3]);
+  st_global_v4(static_cast<uint8_t*>(p) + 16, v[4], v[5], v[6], v[7]);
+}
+__device__ __forceinline__ void st_global_v8f(float* p, const float* v) {
+  asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]) : "memory");
+  asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p + 4), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7]) : "memory");
+}
+__device__ __forceinline__ void ld_global_nc_v8f(const float* p, float* v) {
+  asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]) : "l"(p));
+  asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]) : "l"(p + 4));
+}
+__device__ __forceinline__ void ld_global_nc_v8(const void* p, uint32_t (&v)[8]) {
+  const uint8_t* q = static_cast<const uint8_t*>(p);
+  asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "l"(q));
+  asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]) : "l"(q + 16));
 }
 
 }  // namespace ttsb

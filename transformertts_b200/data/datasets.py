@@ -13,7 +13,7 @@ Mirrors ``data/datasets.py`` and ``data/metadata_readers.py`` of the reference:
     pass unless ``drop_remainder``; ``next_batch`` iterates over endless passes.
   * ``pitch_per_char`` (extract_durations.py:108-115).
 
-What is B200-specific: batches are assembled directly into PINNED host tensors and a background thread keeps
+What is GPU-specific: batches are assembled directly into PINNED host tensors and a background thread keeps
 ``prefetch`` batches ahead (``PrefetchLoader``), optionally already copied to the device on a side stream, so that the
 training step's H2D copy (10 MB per LJ256 batch) overlaps the previous step; with ``rank`` / ``world_size`` every rank
 takes a disjoint slice of each emitted batch (data-parallel training, one process per GPU).

@@ -15,7 +15,7 @@ PREC_FP16 = 2
 IMPL_TCGEN05 = 0
 IMPL_SIMT = 1
 
-# TTSB_LIB selects another build of the same library (e.g. the clock-trace debug build made by tools/att_trace.py)
+# TTSB_LIB selects another build of the same library (for example a debug build)
 _LIB_PATH = Path(os.environ.get('TTSB_LIB') or Path(__file__).resolve().parent / 'libttsb.so')
 _lib = None
 

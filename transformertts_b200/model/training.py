@@ -2,7 +2,7 @@
 losses utils/losses.py:41-70 with weights [1,1,3] models.py:485; Adam utils/training_config_manager.py:102-106).
 
 The forward pass is run in single-pass bf16 tensor-core mode (BASELINE.json configs[2]: "bf16") and keeps what the
-backward needs; the backward is hand-written: every gradient GEMM runs on tcgen05 (data gradients through the forward
+backward needs; the backward is hand-written: every gradient GEMM runs on the wgmma tensor-core kernels (data gradients through the forward
 GEMM kernel with re-packed weights, weight gradients and the attention gradients through ttsb_wgrad / ttsb_bgemm),
 everything else through the row kernels of csrc/train_ops.cu.  Parameters, gradients and Adam moments live in flat
 fp32 buffers so that Adam is one launch and data-parallel all-reduce works on contiguous buckets.
