@@ -315,6 +315,13 @@ int ttsb_attention_scores(const float* att, int B, int H, int Tq, int Tk, const 
                           float* scores, void* stream);
 int ttsb_durations_from_attention(const float* att, int B, int H, int Tq, int Tk, const int32_t* mel_len, const int32_t* phon_len,
                                   const float* scores, int weighted, uint8_t* scratch, int32_t* durations, void* stream);
+/* Per-character pitch (extract_durations.py:108-115, batched): character c < n_chars[b] covers frames [cum[c], cum[c+1]) of
+ * the exclusive prefix sum of durations (B,Tp) (non-negative), clipped at pitch_len[b] <= Tm.  A frame value v of pitch
+ * (B,Tm) is kept iff v != 0 and v*pitch_std + pitch_mean < 400 (two rounded float64 operations); out (B,Tp) float64 is the
+ * mean of the kept values, bit-exact with np.mean (numpy's pairwise summation order), or 0 when none is kept.
+ * Characters >= n_chars[b] are 0.  Tp <= 12287. */
+int ttsb_pitch_per_char(const double* pitch, int B, int Tm, const int32_t* pitch_len, const int32_t* durations, int Tp,
+                        const int32_t* n_chars, double pitch_mean, double pitch_std, double* out, void* stream);
 
 /* Aligner losses (SURVEY 8(f) row 1).
  * ttsb_scaled_ce_loss: utils/losses.py:4-21 new_scaled_crossentropy -- sparse softmax CE of logits (B,Tp,ld)[:, :Tt, :C] against

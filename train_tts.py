@@ -8,7 +8,8 @@
     python train_tts.py --config ... --synthetic [--max_steps N] [--batch_size B]  # seeded LJSpeech-shaped batches
     torchrun --nproc-per-node 8 train_tts.py --config ...                          # data parallel, one process per GPU
 
-Training data: the directory layout the reference's ``create_training_data.py`` / ``extract_durations.py`` write
+Training data: the directory layout the reference's ``create_training_data.py`` / ``extract_durations.py`` write (the
+durations and per-character pitch can be produced here with ``train_aligner.py`` + ``extract_durations.py``)
 (``<train_data_directory>.<data_name>/`` with ``train_metadata.*.txt`` / ``valid_metadata.*.txt`` (``name|phonemes``),
 ``mels.*/<name>.npy`` (T,80), ``durations.*/<name>.npy`` int (Tp,), ``char_pitch.*/<name>.npy`` (Tp,)), read by
 ``transformertts_b200/data/datasets.py`` with the bucket boundaries / batch sizes of the config (yaml :22-24), shuffled with

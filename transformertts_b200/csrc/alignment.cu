@@ -154,6 +154,122 @@ __global__ void durations_dp_kernel(const float* __restrict__ att, int H, int Tq
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Per-character pitch (extract_durations.py:108-115 of the reference, batched): the mean of the voiced (!= 0), < 400 Hz
+// (after de-normalisation) frame pitches under each character.  The mean is bit-exact with np.mean: the kept values are
+// summed in numpy's pairwise order (numpy/core/src/umath/loops_utils.h.src, pairwise_sum_DOUBLE) and divided by their
+// count.  That order depends on the count n of kept values only:
+//   n < 8:        sequential from 0.0;
+//   8 <= n <= 128: eight strided accumulators ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)), then the n % 8 tail sequentially;
+//   n > 128:      sum(first n2) + sum(rest), n2 = n/2 rounded down to a multiple of 8.
+// A segment is a handful of frames, so one thread walks one character's frames; the tree of the n > 128 case is evaluated
+// with an explicit stack, consuming the kept values left to right.
+// ---------------------------------------------------------------------------------------------------------------------
+struct KeptPitch {   // the kept frame values of one segment, in order
+  const double* p;
+  int i;
+  double mean, std;
+  __device__ __forceinline__ static bool keep(double v, double mean, double std) {
+    // numpy evaluates values * std + mean as two rounded operations: no FMA contraction
+    return v != 0.0 && __dadd_rn(__dmul_rn(v, std), mean) < 400.0;
+  }
+  __device__ __forceinline__ double next() {
+    while (true) {
+      const double v = p[i++];
+      if (keep(v, mean, std)) return v;
+    }
+  }
+};
+
+__device__ double pairwise_leaf(KeptPitch& src, int n) {   // n <= 128
+  if (n < 8) {
+    double s = 0.0;
+    for (int k = 0; k < n; ++k) s = __dadd_rn(s, src.next());
+    return s;
+  }
+  double r[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) r[j] = src.next();
+  int k = 8;
+  for (; k < n - (n % 8); k += 8) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) r[j] = __dadd_rn(r[j], src.next());
+  }
+  double s = __dadd_rn(__dadd_rn(__dadd_rn(r[0], r[1]), __dadd_rn(r[2], r[3])), __dadd_rn(__dadd_rn(r[4], r[5]), __dadd_rn(r[6], r[7])));
+  for (; k < n; ++k) s = __dadd_rn(s, src.next());
+  return s;
+}
+
+__device__ double pairwise_sum(KeptPitch& src, int n) {
+  int right_n[32];      // pending right halves; depth <= log2(n / 128) + 1 < 32 for any int n
+  double left[32];
+  bool left_done[32];
+  int sp = 0;
+  while (true) {
+    while (n > 128) {
+      int n2 = n / 2;
+      n2 -= n2 % 8;
+      right_n[sp] = n - n2;
+      left_done[sp] = false;
+      ++sp;
+      n = n2;
+    }
+    double s = pairwise_leaf(src, n);
+    while (sp > 0 && left_done[sp - 1]) {   // both halves done: fold into the parent
+      --sp;
+      s = __dadd_rn(left[sp], s);
+    }
+    if (sp == 0) return s;
+    left[sp - 1] = s;                       // left half done: descend into the right half
+    left_done[sp - 1] = true;
+    n = right_n[sp - 1];
+  }
+}
+
+// one block per batch row: exclusive prefix sum of the durations in shared memory, then one thread per character
+__global__ void pitch_per_char_kernel(const double* __restrict__ pitch, int Tm, const int32_t* __restrict__ pitch_len,
+                                      const int32_t* __restrict__ durations, int Tp, const int32_t* __restrict__ n_chars,
+                                      double pitch_mean, double pitch_std, double* __restrict__ out) {
+  extern __shared__ int cum[];   // [Tp + 1]
+  const int b = blockIdx.x;
+  const int32_t* dur = durations + (size_t)b * Tp;
+  if (threadIdx.x < 32) {        // warp 0: 32 contiguous chunks, warp scan of the chunk sums
+    const int lane = threadIdx.x;
+    const int chunk = (Tp + 31) / 32;
+    const int lo = min(lane * chunk, Tp), hi = min(lo + chunk, Tp);
+    int s = 0;
+    for (int i = lo; i < hi; ++i) s += dur[i];
+    int incl = s;
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += t;
+    }
+    int run = incl - s;
+    for (int i = lo; i < hi; ++i) {
+      cum[i] = run;
+      run += dur[i];
+    }
+    if (lane == 31) cum[Tp] = incl;
+  }
+  __syncthreads();
+  const int L = min(max(pitch_len[b], 0), Tm);
+  const int nc = min(max(n_chars[b], 0), Tp);
+  const double* row = pitch + (size_t)b * Tm;
+  for (int c = threadIdx.x; c < Tp; c += blockDim.x) {
+    double v = 0.0;
+    if (c < nc) {
+      const int lo = min(cum[c], L), hi = min(cum[c + 1], L);   // pitch[a:b] clipped at the pitch length, as numpy slices
+      int n = 0;
+      for (int f = lo; f < hi; ++f) n += KeptPitch::keep(row[f], pitch_mean, pitch_std);
+      if (n > 0) {
+        KeptPitch src{row, lo, pitch_mean, pitch_std};
+        v = pairwise_sum(src, n) / (double)n;
+      }
+    }
+    out[(size_t)b * Tp + c] = v;
+  }
+}
+
 static inline int bad(const char* msg) {
   set_last_error("%s", msg);
   return TTSB_ERR_INVALID_ARGUMENT;
@@ -200,4 +316,16 @@ extern "C" int ttsb_durations_from_attention(const float* att, int B, int H, int
                                                                          durations);
   count_launch();
   return check_cuda(cudaGetLastError(), "durations_dp_kernel");
+}
+
+extern "C" int ttsb_pitch_per_char(const double* pitch, int B, int Tm, const int32_t* pitch_len, const int32_t* durations, int Tp,
+                                   const int32_t* n_chars, double pitch_mean, double pitch_std, double* out, void* stream) {
+  if (!pitch || !pitch_len || !durations || !n_chars || !out || B <= 0 || Tm <= 0 || Tp <= 0)
+    return bad("ttsb_pitch_per_char: bad arguments");
+  const size_t sm = ((size_t)Tp + 1) * sizeof(int);
+  if (sm > 48 * 1024) return bad("ttsb_pitch_per_char: Tp too large");
+  pitch_per_char_kernel<<<B, 128, sm, static_cast<cudaStream_t>(stream)>>>(pitch, Tm, pitch_len, durations, Tp, n_chars, pitch_mean,
+                                                                           pitch_std, out);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "pitch_per_char_kernel");
 }

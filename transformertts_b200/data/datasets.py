@@ -85,6 +85,28 @@ class DataReader:
             if training:
                 self.filenames += self.upsample
 
+    KINDS = ('original', 'phonemized', 'train', 'valid')
+
+    @classmethod
+    def from_config(cls, config_manager, kind: str):
+        """datasets.py:47-72: ``original`` reads the corpus metadata with the reader named by ``data_name``; ``phonemized``,
+        ``train`` and ``valid`` read the processed ``name|phonemes`` files, the training list with its upsampled names."""
+        if kind not in cls.KINDS:
+            raise ValueError(f'Invalid kind type. Expected one of: {list(cls.KINDS)}')
+        reader, training, is_processed = post_processed_reader, False, True
+        if kind == 'train':
+            metadata, training = config_manager.train_metadata_path, True
+        elif kind == 'original':
+            metadata = config_manager.metadata_path
+            reader = get_preprocessor_by_name(config_manager.config['data_name'])
+            is_processed = False
+        elif kind == 'valid':
+            metadata = config_manager.valid_metadata_path
+        else:
+            metadata = config_manager.phonemized_metadata_path
+        return cls(metadata_path=metadata, metadata_reading_function=reader, training=training, is_processed=is_processed,
+                   wav_directory=config_manager.wav_directory)
+
 
 # ----------------------------------------------------------------------------------------------------------------------
 # per-sample preprocessors (datasets.py:76-161)
@@ -108,6 +130,13 @@ class AlignerPreprocessor:
     @staticmethod
     def get_sample_length(norm_mel, *_):
         return norm_mel.shape[0]
+
+    @classmethod
+    def from_config(cls, config_manager, tokenizer: Callable):
+        """datasets.py:98-103."""
+        c = config_manager.config
+        return cls(mel_channels=int(c['mel_channels']), mel_start_value=float(c['mel_start_value']),
+                   mel_end_value=float(c['mel_end_value']), tokenizer=tokenizer)
 
 
 class TTSPreprocessor:
@@ -260,6 +289,14 @@ class AlignerDataset(_FileDataset):
     def _process_sample(self, sample_name):
         mel, text = self._read_sample(sample_name)
         return self.preprocessor(mel=mel, text=text, sample_name=sample_name)
+
+    @classmethod
+    def from_config(cls, config_manager, preprocessor: AlignerPreprocessor, kind: str, mel_directory=None):
+        """datasets.py:136-150."""
+        if kind not in DataReader.KINDS:
+            raise ValueError(f'Invalid kind type. Expected one of: {list(DataReader.KINDS)}')
+        return cls(data_reader=DataReader.from_config(config_manager, kind=kind), preprocessor=preprocessor,
+                   mel_directory=config_manager.mel_dir if mel_directory is None else mel_directory)
 
 
 class TTSDataset(_FileDataset):

@@ -26,7 +26,7 @@ EXPORTS = [
     'ttsb_pitch_embed_add_fwd', 'ttsb_durations_to_int', 'ttsb_expand_indices', 'ttsb_length_regulate_fwd',
     'ttsb_expand_ln_pe_fwd', 'ttsb_mel_lengths', 'ttsb_phoneme_lengths', 'ttsb_stft_mel_log',
     'ttsb_bgemm', 'ttsb_wgrad', 'ttsb_rowdot_heads', 'ttsb_softmax_fwd', 'ttsb_attn_probs_supported', 'ttsb_attn_probs_fwd', 'ttsb_attn_ds_bwd', 'ttsb_softmax_bwd', 'ttsb_layernorm_bwd',
-    'ttsb_relu_bwd', 'ttsb_relu_bwd_colsum', 'ttsb_colsum_bf16', 'ttsb_colsum_bf16_x3', 'ttsb_cast_bf16_pad', 'ttsb_mae_loss', 'ttsb_scaled_ce_loss', 'ttsb_diag_loss', 'ttsb_diag_loss_train', 'ttsb_attention_scores', 'ttsb_durations_from_attention', 'ttsb_expand_bwd', 'ttsb_embedding_bwd', 'ttsb_pe_scalar_bwd',
+    'ttsb_relu_bwd', 'ttsb_relu_bwd_colsum', 'ttsb_colsum_bf16', 'ttsb_colsum_bf16_x3', 'ttsb_cast_bf16_pad', 'ttsb_mae_loss', 'ttsb_scaled_ce_loss', 'ttsb_diag_loss', 'ttsb_diag_loss_train', 'ttsb_attention_scores', 'ttsb_durations_from_attention', 'ttsb_pitch_per_char', 'ttsb_expand_bwd', 'ttsb_embedding_bwd', 'ttsb_pe_scalar_bwd',
     'ttsb_pitch_embed_bwd', 'ttsb_statpred_head_bwd', 'ttsb_adam_tf_step', 'ttsb_embed_ln_pe_train_fwd',
     'ttsb_expand_ln_pe_train_fwd', 'ttsb_mel_to_linear', 'ttsb_stft_complex', 'ttsb_istft_workspace_bytes', 'ttsb_istft', 'ttsb_griffinlim_update',
     'ttsb_dp_unique_id', 'ttsb_dp_init', 'ttsb_dp_allreduce_bucket', 'ttsb_dp_destroy',
@@ -386,6 +386,13 @@ def durations_from_attention(att, mel_len, phon_len, scores, weighted, scratch, 
     B, H, Tq, Tk = att.shape
     _check(load().ttsb_durations_from_attention(ptr(att), B, H, Tq, Tk, ptr(mel_len), ptr(phon_len), ptr(scores), int(bool(weighted)),
                                                 ptr(scratch), ptr(durations), _stream()), 'ttsb_durations_from_attention')
+
+
+def pitch_per_char(pitch, pitch_len, durations, n_chars, pitch_mean, pitch_std, out):
+    B, Tm = pitch.shape
+    Tp = durations.shape[1]
+    _check(load().ttsb_pitch_per_char(ptr(pitch), B, Tm, ptr(pitch_len), ptr(durations), Tp, ptr(n_chars), C.c_double(pitch_mean),
+                                      C.c_double(pitch_std), ptr(out), _stream()), 'ttsb_pitch_per_char')
 
 
 def diag_loss(att, q_len, k_len, loss_out):

@@ -523,12 +523,43 @@ class Aligner(ForwardTransformer):
                 break
         return out_dict
 
-    def _compile(self, stop_scaling=8.0, optimizer=None):
-        """models.py:222-227."""
+    def _compile(self, stop_scaling=None, optimizer=None):
+        """models.py:222-227.  stop_scaling None keeps the model's (``stop_loss_scaling`` of its config, default 8), so that
+        restoring optimizer state from a checkpoint does not reset it."""
         from .training import Adam
         self.loss_weights = [1., 1.]
-        self.stop_scaling = float(stop_scaling)
+        if stop_scaling is not None:
+            self.stop_scaling = float(stop_scaling)
         self.optimizer = optimizer if optimizer is not None else Adam(1.0e-4)
+
+    def align(self, text, mel, mels_have_start_end_vectors: bool = False, phonemize: bool = False, encode_phonemes: bool = False,
+              plot: bool = True):
+        """models.py:247-269 -> (last-block cross-attention (N, heads, T, phonemes), model output of ``call``).
+        text: token ids (N, Tp) or (Tp,); mel: (N, T, mel) or (T, mel) without the start vector, or with start and end vectors
+        when ``mels_have_start_end_vectors`` (the end vector is then dropped, as the teacher-forced input drops it).  The
+        input is prepended with the start vector, sliced [:, 0::r] and run through ``call(training=False)``.  ``plot`` is
+        accepted for the reference's signature and ignored."""
+        if phonemize:
+            raise NotImplementedError('phonemization needs the espeak phonemizer, which is outside the built path; '
+                                      'pass token ids')
+        if encode_phonemes:   # phoneme string -> ids with start / end tokens (the Aligner's tokenizer)
+            from ..data.text import Tokenizer
+            text = Tokenizer(add_start_end=True, model_breathing=bool(self.config.get('model_breathing', False)))(text)
+        text = torch.as_tensor(text).to(torch.int32)
+        if text.dim() < 2:
+            text = text[None]
+        mel = torch.as_tensor(mel).to(device=self.device, dtype=torch.float32)
+        if mel.dim() < 3:
+            mel = mel[None]
+        if self.r != 1:
+            print('WARNING: reduction factor != 1.')
+        if mels_have_start_end_vectors:
+            tar_inp = mel[:, :-1]
+        else:
+            start = self.start_vec.to(device=self.device, dtype=torch.float32)[None].expand(mel.shape[0], 1, self.mel_channels)
+            tar_inp = torch.cat([start, mel], dim=1)
+        model_out = self.call(text, tar_inp[:, 0::self.r].contiguous(), training=False)
+        return model_out['decoder_attention']['Decoder_LastBlock_CrossAttention'], model_out
 
     def _set_r(self, r):
         self.r = int(r)
@@ -536,6 +567,8 @@ class Aligner(ForwardTransformer):
     def set_constants(self, learning_rate: float = None, reduction_factor: float = None, decoder_prenet_dropout: float = None,
                       force_encoder_diagonal: bool = None, force_decoder_diagonal: bool = None):
         """models.py:300-312."""
+        if learning_rate is not None and self.optimizer is not None:
+            self.optimizer.lr = float(learning_rate)
         if reduction_factor is not None:
             self._set_r(reduction_factor)
         if force_encoder_diagonal is not None:

@@ -797,7 +797,7 @@ class ForwardTransformer:
     def load_optimizer_state(self, state: dict):
         from .training import Adam
         if self.optimizer is None:
-            self._compile(Adam(state['lr'], beta_1=state['beta_1'], beta_2=state['beta_2'], epsilon=state['epsilon']))
+            self._compile(optimizer=Adam(state['lr'], beta_1=state['beta_1'], beta_2=state['beta_2'], epsilon=state['epsilon']))
         opt = self.optimizer
         opt.lr, opt.iterations = float(state['lr']), int(state['iterations'])
         opt.beta_1, opt.beta_2, opt.epsilon = state['beta_1'], state['beta_2'], state['epsilon']
