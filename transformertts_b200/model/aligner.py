@@ -22,7 +22,8 @@ from typing import Dict
 import torch
 
 from .. import lib
-from .models import LN_EPS, ForwardTransformer, _on_device, _PackedLinear, _round_up
+from .models import (LN_EPS, ForwardTransformer, _capture_graphs, _fill_inputs, _lru_get, _lru_make_room, _on_device, _PackedLinear,
+                     _qkv_block_n, _replay, _round_up, _static_inputs)
 from .transformer_utils import mask_from_lengths, positional_encoding
 
 ALIGNER_VOCAB = 129  # 126 symbols + pad + start + end (reference: data/text/tokenizer.py:17-26 with add_start_end=True)
@@ -57,23 +58,12 @@ class Aligner(ForwardTransformer):
         if int(encoder_prenet_dimension) != int(encoder_model_dimension):
             raise ValueError('the embedding (encoder prenet) feeds the encoder blocks directly: dimensions must match '
                              '(reference: model/models.py:53-65)')
-        self.mel_channels = int(mel_channels)
+        # cuda_graphs / train_graphs replay the teacher-forced validation step / training step as CUDA graphs per input shape
+        # (the steps are ~90 / ~430 dependent launches of small kernels: host-launch bound when issued eagerly)
+        self._init_runtime(mel_channels, debug, kwargs)
         self.vocab_size = int(kwargs.get('vocab_size', ALIGNER_VOCAB))
-        self.device = torch.device(kwargs.get('device', 'cuda:0'))
-        self.precision = kwargs.get('precision', 'bf16x3')
-        self.impl = kwargs.get('impl', 'tcgen05')
-        self.attention_precision = kwargs.get('attention_precision', 'fp16' if self.precision == 'bf16x3' else 'bf16')
         self.return_attention_weights = True      # attention maps are model outputs (models.py:150-153, 297)
-        self._weights_all = True
-        self.debug = debug
-        self.alphabet = kwargs.get('alphabet')
-        self.train_dropout = bool(kwargs.get('train_dropout', True))  # False: deterministic training step (parity tests)
-        # replay the teacher-forced validation step / training step as CUDA graphs per input shape (the steps are ~90 / ~430
-        # dependent launches of small kernels: host-launch bound when issued eagerly)
-        self.cuda_graphs = bool(kwargs.get('cuda_graphs', False))
-        self.train_graphs = bool(kwargs.get('train_graphs', False))
         self._val_graphs = {}
-        self._graph_pool = None
         self.max_r = int(max_r)
         self.r = int(max_r)                        # models.py:46 -- starts at max_r, lowered by the schedule via set_constants
         self.stop_prob_index = 2
@@ -88,14 +78,7 @@ class Aligner(ForwardTransformer):
             'decoder': dict(d=int(decoder_model_dimension), heads=list(decoder_num_heads), n_dense=len(decoder_num_heads),
                             ffn=decoder_feed_forward_dimension, filters=[], kernel=None, max_pos=int(decoder_max_position_encoding)),
         }
-        self.weights: Dict[str, torch.Tensor] = {}
-        self._packed = None
-        self._prof = None
-        self.optimizer = None
         self.loss_weights = [1., 1.]
-        self._engine = None
-        self._drop_seed = 0
-        self._step = 0
         self._init_weights(seed=int(kwargs.get('seed', 42)))
 
     # ------------------------------------------------------------------------------------------------
@@ -157,13 +140,8 @@ class Aligner(ForwardTransformer):
             raise lib.TtsbError('Aligner: model / feed-forward / prenet dimensions must be multiples of 64 (GEMM K blocks)')
         P['encoder.pe'] = self._prepare_pe('encoder')
         for i, _ in enumerate(enc['heads']):
-            pre = f'encoder.b{i}.'
-            wqkv = torch.cat([W[pre + 'wq.w'], W[pre + 'wk.w'], W[pre + 'wv.w']], dim=1)
-            bqkv = torch.cat([W[pre + 'wq.b'], W[pre + 'wk.b'], W[pre + 'wv.b']])
-            P[pre + 'qkv'] = _PackedLinear(wqkv, bqkv, [d_enc], sp, block_n=d_enc if d_enc <= 256 else d_enc // 2)
-            P[pre + 'wo'] = _PackedLinear(W[pre + 'wo.w'], W[pre + 'wo.b'], [d_enc, d_enc], sp, single_tile=True)
-            P[pre + 'ffn1'] = _PackedLinear(W[pre + 'ffn1.w'], W[pre + 'ffn1.b'], [d_enc], sp)
-            P[pre + 'ffn2'] = _PackedLinear(W[pre + 'ffn2.w'], W[pre + 'ffn2.b'], [int(enc['ffn'])], sp, single_tile=True)
+            self._pack_attention(P, f'encoder.b{i}.', d_enc)
+            self._pack_ffn(P, f'encoder.b{i}.', d_enc, int(enc['ffn']))
         # K = mel_channels (80) is padded with zero rows to one 128-wide K block pair
         self._mel_k = _round_up(mel, 64)
 
@@ -176,18 +154,13 @@ class Aligner(ForwardTransformer):
         P['prenet.d2'] = _PackedLinear(W['prenet.d2.w'], W['prenet.d2.b'], [int(self.config['decoder_prenet_dimension'])], sp)
         for i, _ in enumerate(dec['heads']):
             pre = f'decoder.b{i}.'
-            s = pre + 'sa.'
-            wqkv = torch.cat([W[s + 'wq.w'], W[s + 'wk.w'], W[s + 'wv.w']], dim=1)
-            bqkv = torch.cat([W[s + 'wq.b'], W[s + 'wk.b'], W[s + 'wv.b']])
-            P[s + 'qkv'] = _PackedLinear(wqkv, bqkv, [d_dec], sp, block_n=d_dec if d_dec <= 256 else d_dec // 2)
-            P[s + 'wo'] = _PackedLinear(W[s + 'wo.w'], W[s + 'wo.b'], [d_dec, d_dec], sp, single_tile=True)
+            self._pack_attention(P, pre + 'sa.', d_dec)
             c = pre + 'ca.'
             P[c + 'q'] = _PackedLinear(W[c + 'wq.w'], W[c + 'wq.b'], [d_dec], sp)
             P[c + 'kv'] = _PackedLinear(torch.cat([W[c + 'wk.w'], W[c + 'wv.w']], dim=1), torch.cat([W[c + 'wk.b'], W[c + 'wv.b']]),
-                                        [d_enc], sp, block_n=d_dec if d_dec <= 256 else d_dec // 2)
+                                        [d_enc], sp, block_n=_qkv_block_n(d_dec))
             P[c + 'wo'] = _PackedLinear(W[c + 'wo.w'], W[c + 'wo.b'], [d_dec, d_dec], sp, single_tile=True)
-            P[pre + 'ffn1'] = _PackedLinear(W[pre + 'ffn1.w'], W[pre + 'ffn1.b'], [d_dec], sp)
-            P[pre + 'ffn2'] = _PackedLinear(W[pre + 'ffn2.w'], W[pre + 'ffn2.b'], [int(dec['ffn'])], sp, single_tile=True)
+            self._pack_ffn(P, pre, d_dec, int(dec['ffn']))
         # Postnet: mel (80) and stop (3) heads share one GEMM over the padded linear frames
         w_post = pad_rows(torch.cat([W['postnet.mel.w'], W['postnet.stop.w']], dim=1))
         P['postnet'] = _PackedLinear(w_post, torch.cat([W['postnet.mel.b'], W['postnet.stop.b']]), [self._mel_k], sp)
@@ -214,42 +187,15 @@ class Aligner(ForwardTransformer):
         return self._pe_r[r]
 
     # ------------------------------------------------------------------------------------------------
-    def _mha(self, B, T, H, dh, q_buf, ld_q, q_col0, kv_buf, ld_kv, Tk, k_col0, v_col0, lens, causal, weights):
-        d = H * dh
-        _, at_hi, at_lo = self._act(B, T, d, f32=False)
-        ap = self.attention_precision
-        if ap == 'bf16x3':
-            raise lib.TtsbError("Aligner attention runs in the single-pass modes ('fp16' / 'bf16'): head dim 256 needs them")
-        m = lib.MhaArgs()
-        m.B, m.T, m.H, m.dh = B, T, H, dh
-        m.qk_hi = q_buf.data_ptr()
-        m.ld_qk, m.q_col0, m.k_col0, m.v_col0 = ld_q, q_col0, k_col0, v_col0
-        if kv_buf is not None:
-            m.kv_hi = kv_buf.data_ptr()
-            m.ld_kv, m.Tk = ld_kv, Tk
-        m.kv_len = lens.data_ptr()
-        m.out_hi = at_hi.data_ptr()
-        m.out_lo = at_lo.data_ptr() if at_lo is not None else None
-        m.ld_out = d
-        m.causal = int(causal)
-        m.full_queries = 1
-        wts = None
-        if weights:
-            wts = torch.empty((B, H, T, Tk if kv_buf is not None else T), dtype=torch.float32, device=self.device)
-            m.weights_out = wts.data_ptr()
-            m.weights_all = 1
-        m.precision = {'fp16': lib.PREC_FP16, 'bf16': lib.PREC_BF16}[ap]
-        m.impl = self._impl
-        lib.mha_fwd(m)
-        return (at_hi, at_lo), wts
-
     def _cadb(self, P, i: int, x, enc, enc_len, dec_len, B: int, T: int, Tp: int):
-        """CrossAttentionDenseBlock (layers.py:330-349): no row masks inside the block."""
+        """CrossAttentionDenseBlock (layers.py:330-349): no row masks inside the block; every query row is computed."""
         W = self.weights
         dec, d_enc = self._stacks['decoder'], self._stacks['encoder']['d']
         d, H = dec['d'], dec['heads'][i]
         dh = d // H
         pre = f'decoder.b{i}.'
+        if self.attention_precision == 'bf16x3':
+            raise lib.TtsbError("Aligner attention runs in the single-pass modes ('fp16' / 'bf16'): head dim 256 needs them")
         f16 = self.attention_precision == 'fp16'
         adt = torch.float16 if f16 else torch.bfloat16
         x_f, x_hi, x_lo = x
@@ -257,7 +203,7 @@ class Aligner(ForwardTransformer):
         qkv = P[pre + 'sa.qkv']
         qk = torch.empty((B, T, qkv.n_pad), dtype=adt, device=self.device)
         self._gemm(qkv, B, T, [(x_hi, x_lo, d, 0)], [0], [0], out_hi=qk, out_fp16=f16)
-        (a_hi, a_lo), _ = self._mha(B, T, H, dh, qk, qkv.n_pad, 0, None, 0, T, d, 2 * d, dec_len, True, False)
+        (a_hi, a_lo), _ = self._mha(B, T, H, dh, qk, qkv.n_pad, (0, d, 2 * d), dec_len, causal=True, full_queries=True)
         y = self._act(B, T, d)
         self._gemm(P[pre + 'sa.wo'], B, T, [(x_hi, x_lo, d, 0), (a_hi, a_lo, d, 0)], [0, 1], [0, 0], residual=x_f,
                    ln=(W[pre + 'sa.ln.gamma'], W[pre + 'sa.ln.beta']), out_f32=y[0], out_hi=y[1], out_lo=y[2])
@@ -267,7 +213,8 @@ class Aligner(ForwardTransformer):
         kvb = torch.empty((B, Tp, pkv.n_pad), dtype=adt, device=self.device)
         self._gemm(pq, B, T, [(y[1], y[2], d, 0)], [0], [0], out_hi=qb, out_fp16=f16)
         self._gemm(pkv, B, Tp, [(enc[1], enc[2], d_enc, 0)], [0], [0], out_hi=kvb, out_fp16=f16)
-        (c_hi, c_lo), wts = self._mha(B, T, H, dh, qb, pq.n_pad, 0, kvb, pkv.n_pad, Tp, 0, d, enc_len, False, True)
+        (c_hi, c_lo), wts = self._mha(B, T, H, dh, qb, pq.n_pad, (0, 0, d), enc_len, kv=kvb, ld_kv=pkv.n_pad, Tk=Tp,
+                                      full_queries=True, maps='all')
         z = self._act(B, T, d)
         self._gemm(P[pre + 'ca.wo'], B, T, [(y[1], y[2], d, 0), (c_hi, c_lo, d, 0)], [0, 1], [0, 0], residual=y[0],
                    ln=(W[pre + 'ca.ln.gamma'], W[pre + 'ca.ln.beta']), out_f32=z[0], out_hi=z[1], out_lo=z[2])
@@ -300,7 +247,7 @@ class Aligner(ForwardTransformer):
                             W['encoder.pos_scalar'].reshape(1), LN_EPS, h[0], h[1], h[2])
         attn = {}
         for i in range(len(self._stacks['encoder']['heads'])):
-            h = self._block(P, 'encoder', i, h, enc_len, B, Tp, attn, f'Encoder_DenseBlock{i + 1}_SelfAttention')
+            h = self._block(P, 'encoder', i, h, enc_len, B, Tp, attn, f'Encoder_DenseBlock{i + 1}_SelfAttention', maps='all')
         return h, mask_from_lengths(enc_len, Tp), attn, enc_len
 
     def _call_decoder(self, encoder_output, targets, encoder_padding_mask, training=False, enc_len=None):
@@ -424,30 +371,15 @@ class Aligner(ForwardTransformer):
         inp, tar, stop_prob = torch.as_tensor(inp), torch.as_tensor(tar), torch.as_tensor(stop_prob)
         self._prepare()
         key = (tuple(inp.shape), tuple(tar.shape), self.r, self.force_encoder_diagonal, self.force_decoder_diagonal, id(self._packed))
-        ent = self._val_graphs.get(key)
+        ent = _lru_get(self._val_graphs, key)
         if ent is None:
-            dev = self.device
-            ins = [inp.to(device=dev, dtype=torch.int32).contiguous().clone(), tar.to(device=dev, dtype=torch.float32).contiguous().clone(),
-                   stop_prob.to(device=dev, dtype=torch.int32).contiguous().clone()]
-            side = torch.cuda.Stream(device=dev)
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                self._gta_forward(*ins, training=False)
-            torch.cuda.current_stream().wait_stream(side)
-            if self._graph_pool is None:
-                self._graph_pool = torch.cuda.graph_pool_handle()
-            g = torch.cuda.CUDAGraph()
-            n0 = lib.launch_count()
-            with torch.cuda.graph(g, pool=self._graph_pool):
-                out = self._gta_forward(*ins, training=False)[0]
-            if len(self._val_graphs) >= 4:
-                self._val_graphs.pop(next(iter(self._val_graphs)))
-            ent = self._val_graphs[key] = {'ins': ins, 'g': g, 'out': out, 'n': lib.launch_count() - n0}
+            _lru_make_room(self._val_graphs, 4)
+            ins = _static_inputs(self.device, (inp, tar, stop_prob), (torch.int32, torch.float32, torch.int32))
+            [(g, (out, _))] = _capture_graphs(self, self.device, lambda: self._gta_forward(*ins), lambda: self._gta_forward(*ins))
+            ent = self._val_graphs[key] = {'ins': ins, 'g': g, 'out': out}
         else:
-            for dst, src in zip(ent['ins'], (inp, tar, stop_prob)):
-                dst.copy_(src, non_blocking=True)
-        ent['g'].replay()
-        lib.add_launch_count(ent['n'])
+            _fill_inputs(ent['ins'], (inp, tar, stop_prob))
+        _replay(ent['g'])
 
         def cp(v):
             if torch.is_tensor(v):
@@ -485,14 +417,6 @@ class Aligner(ForwardTransformer):
         return out
 
     train_step = _train_step
-
-    def encode_text(self, text):
-        """models.py:338-340: text -> token ids through the attached text pipeline (the espeak phonemizer is external)."""
-        tp = getattr(self, 'text_pipeline', None)
-        if tp is None:
-            raise NotImplementedError('text encoding needs the espeak phonemizer, which is outside the built path; '
-                                      'pass token ids with encode=False or attach a text_pipeline')
-        return tp(text)
 
     def predict(self, inp, max_length=1000, encode=True, verbose=True):
         """models.py:271-292: autoregressive decoding of one token row.  As in the reference the encoder runs once and the
@@ -575,10 +499,6 @@ class Aligner(ForwardTransformer):
             self.force_encoder_diagonal = bool(force_encoder_diagonal)
         if force_decoder_diagonal is not None:
             self.force_decoder_diagonal = bool(force_decoder_diagonal)
-
-    @property
-    def step(self) -> int:
-        return int(self.optimizer.iterations) if self.optimizer is not None else 0
 
     @classmethod
     def from_config(cls, config: dict, max_r: int = 10):

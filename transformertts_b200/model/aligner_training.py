@@ -1,6 +1,6 @@
 """Training step of the Aligner (reference: model/models.py:168-216 ``_gta_forward`` + ``_train_step``): teacher-forced
 forward in single-pass bf16 with saved activations, hand-written backward, Keras-form Adam -- on the same kernels as the
-ForwardTransformer engine (training.py).  The encoder blocks reuse TrainEngine._block_fwd/_block_bwd unchanged; this file
+ForwardTransformer engine (training.py), whose packing, encoder, attention core and graph replay it shares; this file
 adds the CrossAttentionDenseBlock (layers.py:330-349), DecoderPrenet, FinalProj / Postnet and the Aligner losses.
 
 Differences to the ForwardTransformer blocks that matter for the backward pass:
@@ -12,12 +12,10 @@ Differences to the ForwardTransformer blocks that matter for the backward pass:
 """
 from __future__ import annotations
 
-import math
-
 import torch
 
 from .. import lib
-from .models import LN_EPS, _packed_empty, _round_up
+from .models import LN_EPS, _capture_graphs, _PackedLinear, _qkv_block_n, _round_up
 from .training import TrainEngine
 from .transformer_utils import mask_from_lengths
 
@@ -32,168 +30,43 @@ class AlignerTrainEngine(TrainEngine):
     def _build_packs(self):
         m = self.model
         W = m.weights
-        P, descs = {}, []
-        dev = self.dev
-
-        def desc(src, dst_ptr, R, R_pad, C_cols, cb, cb_valid, sr, s_outer, s_inner, dst_ld, f32=0):
-            d_ = lib.PackDesc()
-            d_.src, d_.dst = src.data_ptr() if torch.is_tensor(src) else src, dst_ptr
-            d_.R, d_.R_pad, d_.C_cols, d_.cb, d_.cb_valid = R, R_pad, C_cols, cb, cb_valid
-            d_.sr, d_.s_outer, d_.s_inner, d_.dst_ld, d_.dst_f32 = sr, s_outer, s_inner, dst_ld, f32
-            descs.append(d_)
-
-        def fwd(key, parts, K, seg_k, single=False, block_n=None, k_valid=None):
-            """parts: [(w (Kv,Ni) view, b (Ni))] concatenated along N -- forward packing [N_pad, K]; rows k_valid..K of the
-            contraction are zero (the 80 mel channels are fed as a 128-wide K block)."""
-            kv = K if k_valid is None else k_valid
-            N = sum(w.shape[-1] for w, _ in parts)
-            pl = _packed_empty(K, N, seg_k, dev, single_tile=single, block_n=block_n)
-            if kv != K:
-                pl.w_hi.zero_()
-            row = 0
-            for i, (w, b) in enumerate(parts):
-                Ni = w.shape[-1]
-                last = i == len(parts) - 1
-                desc(w, pl.w_hi.data_ptr() + 2 * row * K, Ni, (pl.n_pad - row) if last else Ni, K, K, kv, 1, 0, Ni, K)
-                desc(b, pl.bias.data_ptr() + 4 * row, 1, 1, (pl.n_pad - row) if last else Ni, pl.n_pad, Ni, 0, 0, 1, pl.n_pad, f32=1)
-                row += Ni
-            P[key] = pl
-
-        def dgrad_dense(key, parts, K):
-            """parts: [w (K,Ni)] concatenated along N -- data-gradient packing [K_pad, N_pad] (contraction over N)."""
-            N = sum(w.shape[-1] for w in parts)
-            npad = _round_up(N, 64)
-            pl = _packed_empty(npad, K, [npad], dev, bias=False)
-            col = 0
-            for i, w in enumerate(parts):
-                Ni = w.shape[-1]
-                last = i == len(parts) - 1
-                width = (npad - col) if last else Ni
-                desc(w, pl.w_hi.data_ptr() + 2 * col, K, pl.n_pad, width, width, Ni, Ni, 0, 1, npad)
-                col += Ni
-            P[key] = pl
-
         enc, dec = m._stacks['encoder'], m._stacks['decoder']
-        d_enc, d_dec, mel = enc['d'], dec['d'], m.mel_channels
+        d_enc, d, mel = enc['d'], dec['d'], m.mel_channels
         for i, _ in enumerate(enc['heads']):
-            pre = f'encoder.b{i}.'
-            d = d_enc
-            qkv = [(W[pre + n + '.w'], W[pre + n + '.b']) for n in ('wq', 'wk', 'wv')]
-            fwd(pre + 'qkv', qkv, d, [d], block_n=d if d <= 256 else d // 2)
-            dgrad_dense(pre + 'qkv.d', [w for w, _ in qkv], d)
-            fwd(pre + 'wo', [(W[pre + 'wo.w'], W[pre + 'wo.b'])], 2 * d, [d, d], single=True)
-            dgrad_dense(pre + 'wo.dx', [W[pre + 'wo.w'][:d]], d)
-            dgrad_dense(pre + 'wo.da', [W[pre + 'wo.w'][d:]], d)
-            F = int(enc['ffn'])
-            fwd(pre + 'ffn1', [(W[pre + 'ffn1.w'], W[pre + 'ffn1.b'])], d, [d])
-            fwd(pre + 'ffn2', [(W[pre + 'ffn2.w'], W[pre + 'ffn2.b'])], F, [F], single=True)
-            dgrad_dense(pre + 'ffn1.d', [W[pre + 'ffn1.w']], d)
-            dgrad_dense(pre + 'ffn2.d', [W[pre + 'ffn2.w']], F)
+            self._pack_attention(f'encoder.b{i}.', d_enc)
+            self._pack_ffn(f'encoder.b{i}.', d_enc, int(enc['ffn']))
         kmel = _round_up(mel, 64)
         pd = int(m.config['decoder_prenet_dimension'])
-        fwd('prenet.d1', [(W['prenet.d1.w'], W['prenet.d1.b'])], kmel, [kmel], k_valid=mel)
-        fwd('prenet.d2', [(W['prenet.d2.w'], W['prenet.d2.b'])], pd, [pd])
-        dgrad_dense('prenet.d2.d', [W['prenet.d2.w']], pd)
-        d = d_dec
+        self._fwd('prenet.d1', [(W['prenet.d1.w'], W['prenet.d1.b'])], kmel, [kmel], k_valid=mel)
+        self._fwd('prenet.d2', [(W['prenet.d2.w'], W['prenet.d2.b'])], pd, [pd])
+        self._dgrad_dense('prenet.d2.d', [W['prenet.d2.w']], pd)
         for i, _ in enumerate(dec['heads']):
             pre = f'decoder.b{i}.'
-            s = pre + 'sa.'
-            qkv = [(W[s + n + '.w'], W[s + n + '.b']) for n in ('wq', 'wk', 'wv')]
-            fwd(s + 'qkv', qkv, d, [d], block_n=d if d <= 256 else d // 2)
-            dgrad_dense(s + 'qkv.d', [w for w, _ in qkv], d)
-            fwd(s + 'wo', [(W[s + 'wo.w'], W[s + 'wo.b'])], 2 * d, [d, d], single=True)
-            dgrad_dense(s + 'wo.dx', [W[s + 'wo.w'][:d]], d)
-            dgrad_dense(s + 'wo.da', [W[s + 'wo.w'][d:]], d)
+            self._pack_attention(pre + 'sa.', d)
             c = pre + 'ca.'
-            fwd(c + 'q', [(W[c + 'wq.w'], W[c + 'wq.b'])], d, [d])
-            dgrad_dense(c + 'q.d', [W[c + 'wq.w']], d)
+            self._fwd(c + 'q', [(W[c + 'wq.w'], W[c + 'wq.b'])], d, [d])
+            self._dgrad_dense(c + 'q.d', [W[c + 'wq.w']], d)
             kv = [(W[c + 'wk.w'], W[c + 'wk.b']), (W[c + 'wv.w'], W[c + 'wv.b'])]
-            fwd(c + 'kv', kv, d_enc, [d_enc], block_n=d if d <= 256 else d // 2)
-            dgrad_dense(c + 'kv.d', [w for w, _ in kv], d_enc)
-            fwd(c + 'wo', [(W[c + 'wo.w'], W[c + 'wo.b'])], 2 * d, [d, d], single=True)
-            dgrad_dense(c + 'wo.dx', [W[c + 'wo.w'][:d]], d)
-            dgrad_dense(c + 'wo.da', [W[c + 'wo.w'][d:]], d)
-            F = int(dec['ffn'])
-            fwd(pre + 'ffn1', [(W[pre + 'ffn1.w'], W[pre + 'ffn1.b'])], d, [d])
-            fwd(pre + 'ffn2', [(W[pre + 'ffn2.w'], W[pre + 'ffn2.b'])], F, [F], single=True)
-            dgrad_dense(pre + 'ffn1.d', [W[pre + 'ffn1.w']], d)
-            dgrad_dense(pre + 'ffn2.d', [W[pre + 'ffn2.w']], F)
+            self._fwd(c + 'kv', kv, d_enc, [d_enc], block_n=_qkv_block_n(d))
+            self._dgrad_dense(c + 'kv.d', [w for w, _ in kv], d_enc)
+            self._pack_wo(c, d)
+            self._pack_ffn(pre, d, int(dec['ffn']))
         # FinalProj[:, :, :r*mel] per reduction factor (models.py:146); Postnet: mel | stop heads in one GEMM
         self._fp = {}
         for r in range(1, m.max_r + 1):
-            n = r * mel
-            w, b = W['final_proj.w'][:, :n], W['final_proj.b'][:n]
-            N = n
-            pl = _packed_empty(d, N, [d], dev)
-            desc(w, pl.w_hi.data_ptr(), N, pl.n_pad, d, d, d, 1, 0, W['final_proj.w'].shape[1], d)
-            desc(b, pl.bias.data_ptr(), 1, 1, pl.n_pad, pl.n_pad, N, 0, 0, 1, pl.n_pad, f32=1)
+            N = r * mel
+            w, b = W['final_proj.w'][:, :N], W['final_proj.b'][:N]
+            pl = _PackedLinear.empty(d, N, [d], self.dev)
+            self._desc(w, pl.w_hi.data_ptr(), N, pl.n_pad, d, d, d, 1, 0, W['final_proj.w'].shape[1], d)
+            self._desc(b, pl.bias.data_ptr(), 1, 1, pl.n_pad, pl.n_pad, N, 0, 0, 1, pl.n_pad, f32=1)
             npad = _round_up(N, 64)
-            pd_ = _packed_empty(npad, d, [npad], dev, bias=False)
-            desc(w, pd_.w_hi.data_ptr(), d, pd_.n_pad, npad, npad, N, W['final_proj.w'].shape[1], 0, 1, npad)
+            pd_ = _PackedLinear.empty(npad, d, [npad], self.dev, bias=False)
+            self._desc(w, pd_.w_hi.data_ptr(), d, pd_.n_pad, npad, npad, N, W['final_proj.w'].shape[1], 0, 1, npad)
             self._fp[r] = (pl, pd_)
         post = [(W['postnet.mel.w'], W['postnet.mel.b']), (W['postnet.stop.w'], W['postnet.stop.b'])]
-        fwd('postnet', post, kmel, [kmel], k_valid=mel)
-        dgrad_dense('postnet.d', [w for w, _ in post], mel)
-        P['encoder.pe'] = m._prepare_pe('encoder')
-        self.P = P
-        self._n_descs = len(descs)
-        self._descs_dev = lib.upload_pack_descs(descs, dev)
-
-    # ------------------------------------------------------------------------------------------------
-    # generic attention core on materialised probabilities (self: q,k,v in one buffer; cross: q buffer + kv buffer)
-    # ------------------------------------------------------------------------------------------------
-    def _attn_fwd(self, B, H, dh, T, Tk, qb, q_ld, q_col, kb, k_ld, k_col, v_col, lens, flags):
-        d = H * dh
-        ldp = _round_up(Tk, 16)
-        Z = B * H
-        S = self._f32(Z, T, ldp)
-        self._bgemm(B, H, T, Tk, dh, qb, (d, T, B), (q_ld, q_ld * T), (dh, 0, 0, q_col), kb, (d, Tk, B), (k_ld, k_ld * Tk),
-                    (dh, 0, 0, k_col), alpha=1.0 / math.sqrt(dh), out_f32=S, ld_out=ldp, out_batch_stride=T * ldp, out_cols=ldp)
-        P_pre = self._bf(Z, T, ldp)
-        rate = self.drop_rate
-        P_drop = self._bf(Z, T, ldp) if rate > 0 else P_pre
-        site = self._site()
-        lib.softmax_fwd(S, B, H, T, Tk, ldp, lens, rate, self.seed, site, P_pre, P_drop, flags=flags)
-        del S
-        out = self._bf(B, T, d)
-        self._bgemm(B, H, T, dh, Tk, P_drop, (Tk, T, Z), (ldp, T * ldp), (0, 0, 1, 0), kb, (d, Tk, B), (k_ld, k_ld * Tk),
-                    (dh, 0, 0, v_col, 1), out_bf16=out, ld_out=d, out_batch_stride=T * d, out_h_col=dh, out_by_b=1, out_cols=dh)
-        return out, dict(P_pre=P_pre, P_drop=P_drop, ldp=ldp, site=site, flags=flags, out=out)
-
-    def _attn_bwd(self, c, B, H, dh, T, Tk, dout, qb, q_ld, q_col, kb, k_ld, k_col, v_col, lens, dq_buf, dq_ld, dq_col, dkv_buf,
-                  dkv_ld, dk_col, dv_col, diag=None):
-        """dout: bf16 (B,T,d) gradient of the attention output.  Writes dQ into dq_buf[:, :, dq_col:], dK / dV into
-        dkv_buf[:, :, dk_col:] / [dv_col:] (bf16).  diag = (grad_scale, q_len, k_len) adds the diagonal-loss term to dP."""
-        d = H * dh
-        ldp = c['ldp']
-        Z = B * H
-        dS = self._bf(Z, T, ldp)
-        scale = 1.0 / math.sqrt(dh)
-        if diag is not None:
-            dP = self._f32(Z, T, ldp)
-            self._bgemm(B, H, T, Tk, dh, dout, (d, T, B), (d, d * T), (dh, 0, 0, 0), kb, (d, Tk, B), (k_ld, k_ld * Tk), (dh, 0, 0, v_col),
-                        out_f32=dP, ld_out=ldp, out_batch_stride=T * ldp, out_cols=ldp)
-            lib.diag_loss_train(c['P_drop'], B, H, T, Tk, ldp, diag[1], diag[2], 0.0, self._scratch1, diag[0], dP)
-            lib.softmax_bwd(c['P_pre'], dP, B, H, T, Tk, ldp, lens, scale, self.drop_rate, self.seed, c['site'], dS, flags=c['flags'])
-            del dP
-        else:  # dS out of the dP product's epilogue (D = dO . O), see TrainEngine._block_bwd
-            D = self._f32(Z * T)
-            lib.rowdot_heads(dout, c['out'], H, dh, D)
-            self._bgemm(B, H, T, Tk, dh, dout, (d, T, B), (d, d * T), (dh, 0, 0, 0), kb, (d, Tk, B), (k_ld, k_ld * Tk), (dh, 0, 0, v_col),
-                        out_bf16=dS, ld_out=ldp, out_batch_stride=T * ldp, out_cols=ldp,
-                        softmax_bwd=(c['P_pre'], D, scale, self.drop_rate, self.seed, c['site'], c['flags'], lens, c['P_drop']))
-        # dQ = dS K : A = dS (K-major over keys), B = K read MN-major
-        self._bgemm(B, H, T, dh, Tk, dS, (Tk, T, Z), (ldp, T * ldp), (0, 0, 1, 0), kb, (d, Tk, B), (k_ld, k_ld * Tk),
-                    (dh, 0, 0, k_col, 1), out_bf16=dq_buf, ld_out=dq_ld, out_batch_stride=T * dq_ld, out_h_col=dh, out_by_b=1,
-                    out_cols=dh, out_ptr_off=dq_col)
-        # dK = dS^T Q : A = dS read MN-major (= dS^T), B = Q read MN-major
-        self._bgemm(B, H, Tk, dh, T, dS, (Tk, T, Z), (ldp, T * ldp), (0, 0, 1, 0, 1), qb, (d, T, B), (q_ld, q_ld * T),
-                    (dh, 0, 0, q_col, 1), out_bf16=dkv_buf, ld_out=dkv_ld, out_batch_stride=Tk * dkv_ld, out_h_col=dh, out_by_b=1,
-                    out_cols=dh, out_ptr_off=dk_col)
-        # dV = P^T dO : A = P_drop read MN-major, B = dO read MN-major
-        self._bgemm(B, H, Tk, dh, T, c['P_drop'], (Tk, T, Z), (ldp, T * ldp), (0, 0, 1, 0, 1), dout, (d, T, B), (d, d * T),
-                    (dh, 0, 0, 0, 1), out_bf16=dkv_buf, ld_out=dkv_ld, out_batch_stride=Tk * dkv_ld, out_h_col=dh, out_by_b=1,
-                    out_cols=dh, out_ptr_off=dv_col)
+        self._fwd('postnet', post, kmel, [kmel], k_valid=mel)
+        self._dgrad_dense('postnet.d', [w for w, _ in post], mel)
+        self.P['encoder.pe'] = m._prepare_pe('encoder')
 
     # ------------------------------------------------------------------------------------------------
     # CrossAttentionDenseBlock
@@ -309,54 +182,24 @@ class AlignerTrainEngine(TrainEngine):
         all-reduce in the middle the eager path is used).  Per-step dropout masks come from the device-resident salt
         (TrainEngine._set_salt); Adam stays an eager launch."""
         m = self.model
-        inp, tar, stop_prob = torch.as_tensor(inp), torch.as_tensor(tar), torch.as_tensor(stop_prob)
-        key = (tuple(inp.shape), tuple(tar.shape), int(m.r), m.force_encoder_diagonal, m.force_decoder_diagonal, bool(m.train_dropout))
-        ent = self._graphs.get(key)
-        if ent is None:
-            dev = self.dev
-            ins = [inp.to(device=dev, dtype=torch.int32).contiguous().clone(), tar.to(device=dev, dtype=torch.float32).contiguous().clone(),
-                   stop_prob.to(device=dev, dtype=torch.int32).contiguous().clone()]
-            self._set_salt(1)
-            side = torch.cuda.Stream(device=dev)
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                self.forward_backward(*ins, training=True)
-            torch.cuda.current_stream().wait_stream(side)
-            if self._graph_pool is None:
-                self._graph_pool = torch.cuda.graph_pool_handle()
-            g = torch.cuda.CUDAGraph()
-            n0 = lib.launch_count()
-            with torch.cuda.graph(g, pool=self._graph_pool):
+        ins = [torch.as_tensor(t) for t in (inp, tar, stop_prob)]
+        key = (tuple(ins[0].shape), tuple(ins[1].shape), int(m.r), m.force_encoder_diagonal, m.force_decoder_diagonal,
+               bool(m.train_dropout))
+
+        def capture(static):
+            def step():
                 lib.set_dropout_salt(self._salt_dev)
-                out = self.forward_backward(*ins, training=True)
-            if len(self._graphs) >= 4:
-                self._graphs.pop(next(iter(self._graphs)))
-            ent = self._graphs[key] = {'ins': ins, 'g': g, 'out': out, 'n': lib.launch_count() - n0}
-        else:
-            for dst, src in zip(ent['ins'], (inp, tar, stop_prob)):
-                dst.copy_(src, non_blocking=True)
-        it = m.optimizer.iterations if m.optimizer else 0
-        self._set_salt(((it + 1) * 40503 + 12345) & 0x7fffffff)
-        self._salt_applied = 1
-        ent['g'].replay()
-        lib.add_launch_count(ent['n'])
-        out = dict(ent['out'])
-        out['loss'] = out['loss'].clone()
-        out['losses'] = {k: v.clone() for k, v in out['losses'].items()}
-        return out
+                return self.forward_backward(*static, training=True)
+            self._set_salt(1)
+            return _capture_graphs(self, self.dev, lambda: self.forward_backward(*static, training=True), step)
+        return self._replay_step(key, ins, (torch.int32, torch.float32, torch.int32), capture)
 
     def forward_backward(self, inp, tar, stop_prob, training=True, sync=None):
         m, W, G = self.model, self.model.weights, self.g
         dev = self.dev
-        self.use_dropout = training and m.train_dropout
-        self.drop_rate = float(m.config.get('dropout_rate', 0.0)) if self.use_dropout else 0.0
-        prenet_rate = float(m.config.get('decoder_prenet_dropout', 0.0)) if self.use_dropout else 0.0
         self.drop_sites = 0
-        self.seed = (self.base_seed * 2654435761 + (m.optimizer.iterations if m.optimizer else 0) * 40503 + self.rank * 97) & 0x7fffffff
-        m._drop_seed = self.seed
-        saved_precision = m.precision
-        m.precision = 'bf16'
-        try:
+        with self._step_state(m.step, training):
+            prenet_rate = float(m.config.get('decoder_prenet_dropout', 0.0)) if self.use_dropout else 0.0
             P = self._pack()
             r = int(m.r)
             mel = m.mel_channels
@@ -370,23 +213,11 @@ class AlignerTrainEngine(TrainEngine):
             B, Tp = x.shape
             T = tgt.shape[1]
             d_enc, d = m._stacks['encoder']['d'], m._stacks['decoder']['d']
-            self._scratch1 = torch.zeros(1, dtype=torch.float32, device=dev)
             enc_len = torch.empty((B,), dtype=torch.int32, device=dev)
             lib.phoneme_lengths(x, 0, enc_len)
             dec_len = torch.empty((B,), dtype=torch.int32, device=dev)
             lib.mel_lengths(tgt, 0.0, dec_len)
-            # ---- encoder
-            e_rows = self._f32(1, B * Tp, d_enc)
-            lib.length_regulate_fwd(W['embedding'].view(1, -1, d_enc), x.view(1, -1), e_rows)
-            h_f, h_bf = self._f32(B, Tp, d_enc), self._bf(B, Tp, d_enc)
-            site_e = self._site()
-            lib.embed_ln_pe_fwd(x, W['embedding'], W['encoder.ln.gamma'], W['encoder.ln.beta'], P['encoder.pe'],
-                                W['encoder.pos_scalar'].reshape(1), LN_EPS, h_f, h_bf, None, drop=(self.drop_rate, self.seed, site_e))
-            enc_ctx = []
-            for i in range(len(m._stacks['encoder']['heads'])):
-                h_f, h_bf, c = self._block_fwd('encoder', i, h_f, h_bf, enc_len, B, Tp)
-                enc_ctx.append(c)
-            enc_bf = h_bf
+            _, enc_bf, enc_ctx = self._encoder_fwd(x, enc_len)
             # ---- decoder prenet (layers.py:420-443): relu Dense -> dropout -> relu Dense -> dropout
             t_pad = self._bf(B, T, kmel)
             lib.cast_bf16_pad(tgt, B * T, mel, t_pad, kmel)
@@ -431,16 +262,17 @@ class AlignerTrainEngine(TrainEngine):
             dstop = self._f32(B, Tr, 3)
             lib.mae_loss(mel_out, B, Tr, mel_len, mel, tar_real, wts[0], losses[0:1], dmel)
             lib.scaled_ce_loss(stop_out, mel_len, 3, tar_stop, m.stop_prob_index, m.stop_scaling, losses[1:2], wts[1], dstop)
-            n_maps = (n_dec if m.force_decoder_diagonal else 0) + (len(enc_ctx) if m.force_encoder_diagonal else 0)
+            enc_blocks = enc_ctx['blocks']
+            n_maps = (n_dec if m.force_decoder_diagonal else 0) + (len(enc_blocks) if m.force_encoder_diagonal else 0)
             norm = 1.0 + n_maps
             if m.force_decoder_diagonal:
                 for i, c in enumerate(dec_ctx):
                     H = m._stacks['decoder']['heads'][i]
                     lib.diag_loss_train(c['cac']['P_drop'], B, H, T, Tp, c['cac']['ldp'], dec_len, enc_len, 1.0 / norm, losses[2:3], 0.0, None)
             if m.force_encoder_diagonal:
-                for i, c in enumerate(enc_ctx):
+                for i, c in enumerate(enc_blocks):
                     H = m._stacks['encoder']['heads'][i]
-                    lib.diag_loss_train(c['P_drop'], B, H, Tp, Tp, c['ldp'], enc_len, enc_len, 1.0 / norm, losses[2:3], 0.0, None)
+                    lib.diag_loss_train(c['sa']['P_drop'], B, H, Tp, Tp, c['sa']['ldp'], enc_len, enc_len, 1.0 / norm, losses[2:3], 0.0, None)
             out = {'mel': mel_out, 'stop_prob': stop_out, 'linear': linear, 'decoder_output': x_f,
                    'mel_mask': mask_from_lengths(dec_len, T), 'text_mask': mask_from_lengths(enc_len, Tp),
                    'mel_lengths': dec_len, 'text_lengths': enc_len, 'decoder_attention': {}, 'encoder_attention': {},
@@ -499,13 +331,5 @@ class AlignerTrainEngine(TrainEngine):
             if sync is not None:
                 sync.bucket_ready(*self.decoder_range)
             # encoder (the encoder maps' diagonal loss adds to dP inside the block backward)
-            dz = d_enc_acc
-            self._enc_diag = (1.0 / norm, enc_len) if m.force_encoder_diagonal else None
-            for i in range(len(enc_ctx) - 1, -1, -1):
-                dz = self._block_bwd('encoder', i, enc_ctx[i], dz, enc_len, B)
-                enc_ctx[i] = None
-            de = self._prologue_bwd('encoder', dz, e_rows.view(B, Tp, d_enc), enc_len, B, Tp, site_e)
-            lib.embedding_bwd(de, x, G['embedding'])
+            self._encoder_bwd(enc_ctx, d_enc_acc, diag=(1.0 / norm, enc_len, enc_len) if m.force_encoder_diagonal else None)
             return out
-        finally:
-            m.precision = saved_precision

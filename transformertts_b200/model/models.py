@@ -60,33 +60,88 @@ class _PackedLinear:
     def __init__(self, w_kn: torch.Tensor, bias: Optional[torch.Tensor], seg_k: List[int], split: bool, single_tile: bool = False,
                  block_n: Optional[int] = None):
         K, N = w_kn.reshape(-1, w_kn.shape[-1]).shape
-        assert sum(seg_k) == K, (seg_k, K)
-        self.N = N
-        self.K = K
-        self.seg_k = seg_k
-        self.block_n = block_n or _pick_block_n(N, single_tile)
-        self.n_tiles = (N + self.block_n - 1) // self.block_n
-        self.n_pad = self.n_tiles * self.block_n
+        self._tile(K, N, seg_k, single_tile, block_n)
         self.w_hi, self.w_lo = lib.pack_weight(w_kn, self.n_pad, split)
         self.bias = None
         if bias is not None:  # the epilogue reads whole 16-column chunks: pad to n_pad
             self.bias = torch.zeros(self.n_pad, dtype=torch.float32, device=bias.device)
             self.bias[:N] = bias.float()
 
+    @classmethod
+    def empty(cls, K: int, N: int, seg_k: List[int], device, single_tile: bool = False, block_n: Optional[int] = None,
+              bias: bool = True) -> '_PackedLinear':
+        """Buffers allocated but not filled (the training engine refreshes them every step with one batched launch,
+        lib.repack_batched)."""
+        pl = cls.__new__(cls)
+        pl._tile(K, N, seg_k, single_tile, block_n)
+        pl.w_hi = torch.empty((pl.n_pad, K), dtype=torch.bfloat16, device=device)
+        pl.w_lo = None
+        pl.bias = torch.zeros(pl.n_pad, dtype=torch.float32, device=device) if bias else None
+        return pl
 
-def _packed_empty(K: int, N: int, seg_k: List[int], device, single_tile: bool = False, block_n: Optional[int] = None, bias: bool = True):
-    """A _PackedLinear whose buffers are allocated but not filled (the training engine refreshes them every step with one
-    batched launch, lib.repack_batched)."""
-    pl = _PackedLinear.__new__(_PackedLinear)
-    assert sum(seg_k) == K, (seg_k, K)
-    pl.N, pl.K, pl.seg_k = N, K, seg_k
-    pl.block_n = block_n or _pick_block_n(N, single_tile)
-    pl.n_tiles = (N + pl.block_n - 1) // pl.block_n
-    pl.n_pad = pl.n_tiles * pl.block_n
-    pl.w_hi = torch.empty((pl.n_pad, K), dtype=torch.bfloat16, device=device)
-    pl.w_lo = None
-    pl.bias = torch.zeros(pl.n_pad, dtype=torch.float32, device=device) if bias else None
-    return pl
+    def _tile(self, K, N, seg_k, single_tile, block_n):
+        assert sum(seg_k) == K, (seg_k, K)
+        self.N, self.K, self.seg_k = N, K, seg_k
+        self.block_n = block_n or _pick_block_n(N, single_tile)
+        self.n_tiles = (N + self.block_n - 1) // self.block_n
+        self.n_pad = self.n_tiles * self.block_n
+
+
+def _qkv_block_n(d: int) -> int:
+    """N tile of a projection onto q|k|v (or k|v): one head-aligned tile of width d, or two of d/2."""
+    return d if d <= 256 else d // 2
+
+
+# ---- CUDA graphs: per-shape caches (least recently used evicted first) whose graphs share one private memory pool
+def _capture_graphs(owner, device, warmup, *stages):
+    """Runs `warmup()` eagerly on a side stream (one-time function attributes, packs, allocator), then captures each stage
+    as one CUDA graph in `owner._graph_pool` (created on first use).  Returns [(graph, stage output)];
+    graph.ttsb_launches is the number of library kernels inside it (added to the launch count per replay)."""
+    side = torch.cuda.Stream(device=device)
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        warmup()
+    torch.cuda.current_stream().wait_stream(side)
+    if owner._graph_pool is None:
+        owner._graph_pool = torch.cuda.graph_pool_handle()
+    captured = []
+    n0 = lib.launch_count()
+    for fn in stages:
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, pool=owner._graph_pool):
+            out = fn()
+        n1 = lib.launch_count()
+        g.ttsb_launches, n0 = n1 - n0, n1
+        captured.append((g, out))
+    return captured
+
+
+def _replay(g):
+    g.replay()
+    lib.add_launch_count(g.ttsb_launches)
+
+
+def _lru_get(cache: dict, key):
+    """The cached entry (now the most recently used), or None."""
+    ent = cache.pop(key, None)
+    if ent is not None:
+        cache[key] = ent
+    return ent
+
+
+def _lru_make_room(cache: dict, limit: int):
+    while len(cache) >= limit:
+        cache.pop(next(iter(cache)))
+
+
+def _static_inputs(device, tensors, dtypes):
+    """Device copies of a step's inputs for a graph to read; _fill_inputs refreshes them before each replay."""
+    return [t.to(device=device, dtype=dt).contiguous().clone() for t, dt in zip(tensors, dtypes)]
+
+
+def _fill_inputs(static, tensors):
+    for dst, src in zip(static, tensors):
+        dst.copy_(src, non_blocking=True)
 
 
 def _pad_vec(v: torch.Tensor, n: int) -> torch.Tensor:
@@ -132,25 +187,10 @@ class ForwardTransformer:
         self.config.update(kwargs)
         if encoder_model_dimension != decoder_model_dimension:
             raise ValueError('Expand feeds the encoder output to the decoder: model dimensions must match')
-        self.mel_channels = int(mel_channels)
+        self._init_runtime(mel_channels, debug, kwargs)
         # reference tokenizer: 126 symbols + pad, one more id when model_breathing adds the breathing token (tokenizer.py:28-33)
         self.vocab_size = int(kwargs.get('vocab_size', DEFAULT_VOCAB + (1 if model_breathing else 0)))
-        self.alphabet = kwargs.get('alphabet')
-        self.device = torch.device(kwargs.get('device', 'cuda:0'))
-        # numerics of the tensor-core products: 'bf16x3' meets the 1e-3 mel parity gate, 'bf16' is the fast mode
-        self.precision = kwargs.get('precision', 'bf16x3')
-        self.impl = kwargs.get('impl', 'tcgen05')
-        # attention products: single-pass IEEE fp16 keeps the mel error below the 1e-3 gate (smoke() measures 4.3e-4) at a third
-        # of the tensor work of bf16x3; 'bf16' / 'bf16x3' remain selectable
-        self.attention_precision = kwargs.get('attention_precision', 'fp16' if self.precision == 'bf16x3' else 'bf16')
-        self.return_attention_weights = bool(kwargs.get('return_attention_weights', False))
-        # inference: capture the two halves of call() as CUDA graphs per input shape and replay them (see call())
-        self.cuda_graphs = bool(kwargs.get('cuda_graphs', False))
-        self.max_cached_graphs = int(kwargs.get('max_cached_graphs', 8))
-        self._enc_graphs = {}
-        self._graph_pool = None
-        self._len_host = None
-        self.debug = debug
+        self.loss_weights = [1., 1., 3.]
         self._stacks = {}
         for name in ('encoder', 'decoder'):
             d = int(self.config[f'{name}_model_dimension'])
@@ -161,17 +201,36 @@ class ForwardTransformer:
                 filters=[int(f) for f in (self.config.get(f'{name}_attention_conv_filters') or [])],
                 kernel=self.config.get(f'{name}_attention_conv_kernel'),
                 max_pos=int(self.config[f'{name}_max_position_encoding']))
+        self._init_weights(seed=int(kwargs.get('seed', 42)))
+
+    def _init_runtime(self, mel_channels, debug, kwargs):
+        """Constructor state shared with the Aligner: device, numerics, CUDA-graph caches, optimizer and engine slots."""
+        self.mel_channels = int(mel_channels)
+        self.alphabet = kwargs.get('alphabet')
+        self.device = torch.device(kwargs.get('device', 'cuda:0'))
+        # numerics of the tensor-core products: 'bf16x3' meets the 1e-3 mel parity gate, 'bf16' is the fast mode
+        self.precision = kwargs.get('precision', 'bf16x3')
+        self.impl = kwargs.get('impl', 'tcgen05')
+        # attention products: single-pass IEEE fp16 keeps the mel error below the 1e-3 gate (smoke() measures 4.3e-4) at a third
+        # of the tensor work of bf16x3; 'bf16' / 'bf16x3' remain selectable
+        self.attention_precision = kwargs.get('attention_precision', 'fp16' if self.precision == 'bf16x3' else 'bf16')
+        self.return_attention_weights = bool(kwargs.get('return_attention_weights', False))
+        # inference: capture the step as CUDA graphs per input shape and replay them (see call())
+        self.cuda_graphs = bool(kwargs.get('cuda_graphs', False))
+        self.max_cached_graphs = int(kwargs.get('max_cached_graphs', 8))
+        self._enc_graphs = {}
+        self._graph_pool = None
+        self._len_host = None
+        self.debug = debug
         self.weights: Dict[str, torch.Tensor] = {}
         self._packed = None
         self._prof = None  # bench.py: {tag: [(start_event, end_event, flops)]} for tagged GEMM launches
         self.optimizer = None
-        self.loss_weights = [1., 1., 3.]
         self.train_dropout = bool(kwargs.get('train_dropout', True))  # False: deterministic training step (parity tests)
-        # training: replay the step as two CUDA graphs per input shape (training.TrainEngine.step_graphed)
+        # training: replay the step as CUDA graphs per input shape (training.TrainEngine.step_graphed)
         self.train_graphs = bool(kwargs.get('train_graphs', False))
         self._engine = None
         self._drop_seed = 0
-        self._init_weights(seed=int(kwargs.get('seed', 42)))
 
     # ------------------------------------------------------------------------------------------------
     # parameters
@@ -304,14 +363,9 @@ class ForwardTransformer:
             P[f'{name}.pe'] = self._prepare_pe(name)
             for i, _ in enumerate(st['heads']):
                 pre = f'{name}.b{i}.'
-                wqkv = torch.cat([W[pre + 'wq.w'], W[pre + 'wk.w'], W[pre + 'wv.w']], dim=1)
-                bqkv = torch.cat([W[pre + 'wq.b'], W[pre + 'wk.b'], W[pre + 'wv.b']])
-                bn = d if d <= 256 else d // 2
-                P[pre + 'qkv'] = _PackedLinear(wqkv, bqkv, [d], sp, block_n=bn)
-                P[pre + 'wo'] = _PackedLinear(W[pre + 'wo.w'], W[pre + 'wo.b'], [d, d], sp, single_tile=True)
+                self._pack_attention(P, pre, d)
                 if i < st['n_dense']:
-                    P[pre + 'ffn1'] = _PackedLinear(W[pre + 'ffn1.w'], W[pre + 'ffn1.b'], [d], sp)
-                    P[pre + 'ffn2'] = _PackedLinear(W[pre + 'ffn2.w'], W[pre + 'ffn2.b'], [int(st['ffn'])], sp, single_tile=True)
+                    self._pack_ffn(P, pre, d, int(st['ffn']))
                 else:
                     cin = d
                     nconv = len(st['filters'])
@@ -332,6 +386,19 @@ class ForwardTransformer:
         P['pitch_embed.w'] = W['pitch_embed.w'].reshape(-1).contiguous()
         self._packed = P
         return P
+
+    def _pack_attention(self, P, pre: str, d: int):
+        """Self-attention sub-block: q|k|v as one GEMM, output projection on concat([x, attn])."""
+        W, sp = self.weights, self._split
+        wqkv = torch.cat([W[pre + 'wq.w'], W[pre + 'wk.w'], W[pre + 'wv.w']], dim=1)
+        bqkv = torch.cat([W[pre + 'wq.b'], W[pre + 'wk.b'], W[pre + 'wv.b']])
+        P[pre + 'qkv'] = _PackedLinear(wqkv, bqkv, [d], sp, block_n=_qkv_block_n(d))
+        P[pre + 'wo'] = _PackedLinear(W[pre + 'wo.w'], W[pre + 'wo.b'], [d, d], sp, single_tile=True)
+
+    def _pack_ffn(self, P, pre: str, d: int, F: int):
+        W, sp = self.weights, self._split
+        P[pre + 'ffn1'] = _PackedLinear(W[pre + 'ffn1.w'], W[pre + 'ffn1.b'], [d], sp)
+        P[pre + 'ffn2'] = _PackedLinear(W[pre + 'ffn2.w'], W[pre + 'ffn2.b'], [F], sp, single_tile=True)
 
     def _prepare_pe(self, name: str) -> torch.Tensor:
         st = self._stacks[name]
@@ -432,8 +499,41 @@ class ForwardTransformer:
     def _conv_shifts(self, k: int) -> List[int]:
         return [j - (k - 1) // 2 for j in range(k)]
 
-    def _block(self, P, name: str, i: int, x, lens, B: int, T: int, attn_out: Optional[dict], key: str, need_f32: bool = True):
-        """One SelfAttentionDenseBlock / SelfAttentionConvBlock (reference: model/layers.py:214-264).
+    def _mha(self, B, T, H, dh, qk, ld_qk, cols, lens, qk_lo=None, kv=None, ld_kv=0, Tk=None, causal=False,
+             full_queries=False, maps=None):
+        """Fused attention (include/ttsb.h: ttsb_mha_fwd).  qk holds Q at column cols[0] and, without a separate `kv` buffer,
+        K / V at cols[1] / cols[2]; with `kv` (Tk rows, leading dimension ld_kv) K and V are read from there.  maps: None,
+        'first' (the probabilities of batch row 0) or 'all' (every row) -> returned fp32 (B or 1, H, T, Tk)."""
+        d = H * dh
+        _, at_hi, at_lo = self._act(B, T, d, f32=False)
+        m = lib.MhaArgs()
+        m.B, m.T, m.H, m.dh = B, T, H, dh
+        m.qk_hi = qk.data_ptr()
+        m.qk_lo = qk_lo.data_ptr() if qk_lo is not None else None
+        m.ld_qk, (m.q_col0, m.k_col0, m.v_col0) = ld_qk, cols
+        if kv is not None:
+            m.kv_hi = kv.data_ptr()
+            m.ld_kv, m.Tk = ld_kv, Tk
+        m.kv_len = lens.data_ptr()
+        m.out_hi = at_hi.data_ptr()
+        m.out_lo = at_lo.data_ptr() if at_lo is not None else None
+        m.ld_out = d
+        m.causal, m.full_queries = int(causal), int(full_queries)
+        wts = None
+        if maps is not None:
+            wts = torch.empty((B if maps == 'all' else 1, H, T, Tk or T), dtype=torch.float32, device=self.device)
+            m.weights_out = wts.data_ptr()
+            m.weights_batch_index = 0
+            m.weights_all = int(maps == 'all')
+        m.precision = {'fp16': lib.PREC_FP16, 'bf16': lib.PREC_BF16, 'bf16x3': lib.PREC_BF16X3}[self.attention_precision]
+        m.impl = self._impl
+        lib.mha_fwd(m)
+        return (at_hi, at_lo), wts
+
+    def _block(self, P, name: str, i: int, x, lens, B: int, T: int, attn_out: Optional[dict], key: str, need_f32: bool = True,
+               maps: str = 'first'):
+        """One SelfAttentionDenseBlock / SelfAttentionConvBlock (reference: model/layers.py:214-264).  With
+        `return_attention_weights` the probabilities (`maps` rows, see _mha) are stored in attn_out[key].
 
         In bf16x3 mode the hi/lo pair of an activation carries 16 mantissa bits and serves as the residual stream itself:
         the LayerNorm GEMMs then write no fp32 copy (x[0] / the returned z[0] are None unless `need_f32`) -- 4 instead of
@@ -455,26 +555,8 @@ class ForwardTransformer:
         qk_lo = torch.empty_like(qk_hi) if att_split else None
         self._gemm(qkv, B, T, [(x_hi, x_lo, d, 0)], [0], [0], out_hi=qk_hi, out_lo=qk_lo, out_fp16=(ap == 'fp16'))
         # --- fused attention
-        _, at_hi, at_lo = self._act(B, T, d, f32=False)
-        m = lib.MhaArgs()
-        m.B, m.T, m.H, m.dh = B, T, H, dh
-        m.qk_hi = qk_hi.data_ptr()
-        m.qk_lo = qk_lo.data_ptr() if qk_lo is not None else None
-        m.ld_qk, m.q_col0, m.k_col0, m.v_col0 = qkv.n_pad, 0, d, 2 * d
-        m.kv_len = lens.data_ptr()
-        m.out_hi = at_hi.data_ptr()
-        m.out_lo = at_lo.data_ptr() if at_lo is not None else None
-        m.ld_out = d
-        wts = None
-        if attn_out is not None and self.return_attention_weights:
-            all_rows = bool(getattr(self, '_weights_all', False))  # Aligner: attention maps of every row are outputs
-            wts = torch.empty((B if all_rows else 1, H, T, T), dtype=torch.float32, device=dev)
-            m.weights_out = wts.data_ptr()
-            m.weights_batch_index = 0
-            m.weights_all = int(all_rows)
-        m.precision = {'fp16': lib.PREC_FP16, 'bf16': lib.PREC_BF16, 'bf16x3': lib.PREC_BF16X3}[ap]
-        m.impl = self._impl
-        lib.mha_fwd(m)
+        (at_hi, at_lo), wts = self._mha(B, T, H, dh, qk_hi, qkv.n_pad, (0, d, 2 * d), lens, qk_lo=qk_lo,
+                                        maps=maps if attn_out is not None and self.return_attention_weights else None)
         if attn_out is not None:
             attn_out[key] = wts
         # --- output projection on concat([x, attn]) + residual + LayerNorm + row mask
@@ -641,34 +723,17 @@ class ForwardTransformer:
 
     # ---- CUDA-graph replay of the two halves (static input / output buffers live in one private memory pool)
     def _capture(self, fn):
-        side = torch.cuda.Stream(device=self.device)
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            fn()                       # eager warm-up on the capture shapes (one-time function attributes, allocator warm-up)
-        torch.cuda.current_stream().wait_stream(side)
-        if self._graph_pool is None:
-            self._graph_pool = torch.cuda.graph_pool_handle()
-        g = torch.cuda.CUDAGraph()
-        n0 = lib.launch_count()
-        with torch.cuda.graph(g, pool=self._graph_pool):
-            out = fn()
-        g.ttsb_launches = lib.launch_count() - n0   # kernels of the library inside this graph (added per replay)
+        [(g, out)] = _capture_graphs(self, self.device, fn, fn)
         return g, out
-
-    @staticmethod
-    def _replay(g):
-        g.replay()
-        lib.add_launch_count(g.ttsb_launches)
 
     def _call_graphed(self, P, x, tgt_dur, tgt_pitch, scalar, mx, mn):
         dev = self.device
         B, Tp = x.shape
         key = (B, Tp, tgt_dur is not None, tgt_pitch is not None, mx is not None, mn is not None, scalar, self.precision,
                self.attention_precision, id(P))
-        ent = self._enc_graphs.get(key)
+        ent = _lru_get(self._enc_graphs, key)
         if ent is None:
-            if len(self._enc_graphs) >= self.max_cached_graphs:
-                self._enc_graphs.pop(next(iter(self._enc_graphs)))
+            _lru_make_room(self._enc_graphs, self.max_cached_graphs)
             f32 = lambda t: None if t is None else torch.empty((B, Tp), dtype=torch.float32, device=dev)  # noqa: E731
             ins = {'x': torch.empty((B, Tp), dtype=torch.int32, device=dev), 'dur': f32(tgt_dur), 'pitch': f32(tgt_pitch),
                    'mx': f32(mx), 'mn': f32(mn)}
@@ -677,23 +742,19 @@ class ForwardTransformer:
             ent = {'ins': ins, 'graph': g, 'st': st, 'dec': {}}
             self._enc_graphs[key] = ent
         else:
-            self._enc_graphs[key] = self._enc_graphs.pop(key)   # most recently used last
             self._fill(ent['ins'], x, tgt_dur, tgt_pitch, mx, mn)
-        self._replay(ent['graph'])
+        _replay(ent['graph'])
         st = ent['st']
         Tm = self._read_lengths(st['dec_len'])
         if Tm == 0:
             return self._outputs(st, torch.zeros((B, 0, self.mel_channels), dtype=torch.float32, device=dev), {}, 0, clone=True)
-        dec = ent['dec'].get(Tm)
+        dec = _lru_get(ent['dec'], Tm)
         if dec is None:
-            if len(ent['dec']) >= self.max_cached_graphs:
-                ent['dec'].pop(next(iter(ent['dec'])))
+            _lru_make_room(ent['dec'], self.max_cached_graphs)
             g, (mel, dec_attn) = self._capture(lambda: self._stage_decoder(P, st, B, Tm))
             dec = {'graph': g, 'mel': mel}
             ent['dec'][Tm] = dec
-        else:
-            ent['dec'][Tm] = ent['dec'].pop(Tm)
-        self._replay(dec['graph'])
+        _replay(dec['graph'])
         # outputs are copied out of the graph's static buffers (20 MB of mel at C2), so a result stays valid
         # across later calls exactly as in eager mode
         return self._outputs(st, dec['mel'], {}, Tm, clone=True)
@@ -721,7 +782,7 @@ class ForwardTransformer:
     def encode_text(self, text):
         tp = getattr(self, 'text_pipeline', None)
         if tp is None:
-            raise NotImplementedError('text encoding needs the espeak phonemizer, which is outside the text->mel hot path; '
+            raise NotImplementedError('text encoding needs the espeak phonemizer, which is outside the built path; '
                                       'pass token ids with encode=False or attach a text_pipeline')
         return tp(text)
 

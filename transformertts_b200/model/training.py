@@ -9,14 +9,15 @@ fp32 buffers so that Adam is one launch and data-parallel all-reduce works on co
 """
 from __future__ import annotations
 
+import contextlib
 import math
-import os
 from typing import Dict
 
 import torch
 
 from .. import lib
-from .models import LN_EPS, _pad_vec, _round_up
+from .models import (LN_EPS, _capture_graphs, _fill_inputs, _lru_get, _lru_make_room, _pad_vec, _PackedLinear, _qkv_block_n, _replay,
+                     _round_up, _static_inputs)
 from .transformer_utils import mask_from_lengths
 
 
@@ -64,88 +65,111 @@ class TrainEngine:
         self._salt_dev = None
         self._graphs = {}
         self._graph_pool = None
-        self.fused_probs = os.environ.get('TTSB_NO_FUSED_PROBS') is None   # attn_probs_tc.cu instead of logits GEMM + softmax
+        self._loss_scratch = torch.zeros(1, dtype=torch.float32, device=self.dev)   # loss word of the diagonal-loss gradient
 
     # ------------------------------------------------------------------------------------------------
     # packed operands for the step (weights change every step)
     # ------------------------------------------------------------------------------------------------
+    def _pack(self):
+        """Every packed operand of the step is allocated once, with one ttsb_pack_desc per destination block that describes
+        how to refresh it from the flat fp32 parameters; every step then repacks them in a single kernel launch."""
+        if self.P is None:
+            self.P, self._descs = {}, []
+            self._build_packs()
+            self._n_descs = len(self._descs)
+            self._descs_dev = lib.upload_pack_descs(self._descs, self.dev)
+        lib.repack_batched(self._descs_dev, self._n_descs)
+        return self.P
+
+    def _desc(self, src, dst_ptr, R, R_pad, C_cols, cb, cb_valid, sr, s_outer, s_inner, dst_ld, f32=0):
+        d_ = lib.PackDesc()
+        d_.src, d_.dst = src.data_ptr() if torch.is_tensor(src) else src, dst_ptr
+        d_.R, d_.R_pad, d_.C_cols, d_.cb, d_.cb_valid = R, R_pad, C_cols, cb, cb_valid
+        d_.sr, d_.s_outer, d_.s_inner, d_.dst_ld, d_.dst_f32 = sr, s_outer, s_inner, dst_ld, f32
+        self._descs.append(d_)
+
+    def _vec(self, src, dst, n_valid):  # zero-padded fp32 vector copy
+        self._desc(src, dst.data_ptr(), 1, 1, dst.numel(), dst.numel(), n_valid, 0, 0, 1, dst.numel(), f32=1)
+
+    def _fwd(self, key, parts, K, seg_k, single=False, block_n=None, k_valid=None):
+        """parts: [(w (Kv,Ni) view, b (Ni))] concatenated along N (q|k|v) -- forward packing [N_pad, K]; rows k_valid..K of
+        the contraction are zero (the Aligner feeds its 80 mel channels as a 128-wide K block)."""
+        kv = K if k_valid is None else k_valid
+        N = sum(w.shape[-1] for w, _ in parts)
+        pl = _PackedLinear.empty(K, N, seg_k, self.dev, single_tile=single, block_n=block_n)
+        if kv != K:
+            pl.w_hi.zero_()
+        row = 0
+        for i, (w, b) in enumerate(parts):
+            Ni = w.shape[-1]
+            last = i == len(parts) - 1
+            self._desc(w, pl.w_hi.data_ptr() + 2 * row * K, Ni, (pl.n_pad - row) if last else Ni, K, K, kv, 1, 0, Ni, K)
+            self._desc(b, pl.bias.data_ptr() + 4 * row, 1, 1, (pl.n_pad - row) if last else Ni, pl.n_pad, Ni, 0, 0, 1, pl.n_pad, f32=1)
+            row += Ni
+        self.P[key] = pl
+
+    def _dgrad_dense(self, key, parts, K):
+        """parts: [w (K,Ni)] concatenated along N -- data-gradient packing [K_pad, N_pad] (contraction over N)."""
+        N = sum(w.shape[-1] for w in parts)
+        npad = _round_up(N, 64)
+        pl = _PackedLinear.empty(npad, K, [npad], self.dev, bias=False)
+        col = 0
+        for i, w in enumerate(parts):
+            Ni = w.shape[-1]
+            last = i == len(parts) - 1
+            width = (npad - col) if last else Ni
+            self._desc(w, pl.w_hi.data_ptr() + 2 * col, K, pl.n_pad, width, width, Ni, Ni, 0, 1, npad)
+            col += Ni
+        self.P[key] = pl
+
+    def _dgrad_conv(self, key, w):
+        k, cin, cout = w.shape
+        cpad = _round_up(cout, 64)
+        pl = _PackedLinear.empty(k * cpad, cin, [cpad] * k, self.dev, bias=False)
+        self._desc(w, pl.w_hi.data_ptr(), cin, pl.n_pad, k * cpad, cpad, cout, cout, cin * cout, 1, k * cpad)
+        self.P[key] = pl
+
+    def _pack_attention(self, pre, d):
+        """Self-attention sub-block: q|k|v as one GEMM and its data gradient, then the output projection."""
+        W = self.model.weights
+        qkv = [(W[pre + n + '.w'], W[pre + n + '.b']) for n in ('wq', 'wk', 'wv')]
+        self._fwd(pre + 'qkv', qkv, d, [d], block_n=_qkv_block_n(d))
+        self._dgrad_dense(pre + 'qkv.d', [w for w, _ in qkv], d)
+        self._pack_wo(pre, d)
+
+    def _pack_wo(self, pre, d):
+        """Output projection on concat([x, attn]) and its data gradients towards x and attn."""
+        W = self.model.weights
+        self._fwd(pre + 'wo', [(W[pre + 'wo.w'], W[pre + 'wo.b'])], 2 * d, [d, d], single=True)
+        self._dgrad_dense(pre + 'wo.dx', [W[pre + 'wo.w'][:d]], d)
+        self._dgrad_dense(pre + 'wo.da', [W[pre + 'wo.w'][d:]], d)
+
+    def _pack_ffn(self, pre, d, F):
+        W = self.model.weights
+        self._fwd(pre + 'ffn1', [(W[pre + 'ffn1.w'], W[pre + 'ffn1.b'])], d, [d])
+        self._fwd(pre + 'ffn2', [(W[pre + 'ffn2.w'], W[pre + 'ffn2.b'])], F, [F], single=True)
+        self._dgrad_dense(pre + 'ffn1.d', [W[pre + 'ffn1.w']], d)
+        self._dgrad_dense(pre + 'ffn2.d', [W[pre + 'ffn2.w']], F)
+
     def _build_packs(self):
-        """Allocate every packed operand of the step once and describe how to refresh it from the flat fp32 parameters
-        (one ttsb_pack_desc per destination block); _pack() then is a single kernel launch per step."""
-        from .models import _packed_empty
         m = self.model
-        W = m.weights
-        P, descs = {}, []
-        dev = self.dev
-
-        def desc(src, dst_ptr, R, R_pad, C_cols, cb, cb_valid, sr, s_outer, s_inner, dst_ld, f32=0):
-            d_ = lib.PackDesc()
-            d_.src, d_.dst = src.data_ptr() if torch.is_tensor(src) else src, dst_ptr
-            d_.R, d_.R_pad, d_.C_cols, d_.cb, d_.cb_valid = R, R_pad, C_cols, cb, cb_valid
-            d_.sr, d_.s_outer, d_.s_inner, d_.dst_ld, d_.dst_f32 = sr, s_outer, s_inner, dst_ld, f32
-            descs.append(d_)
-
-        def vec(src, dst, n_valid):  # zero-padded fp32 vector copy
-            desc(src, dst.data_ptr(), 1, 1, dst.numel(), dst.numel(), n_valid, 0, 0, 1, dst.numel(), f32=1)
-
-        def fwd(key, parts, K, seg_k, single=False, block_n=None):
-            """parts: [(w (K,Ni) view, b (Ni))] concatenated along N (q|k|v) -- forward packing [N_pad, K]."""
-            N = sum(w.shape[-1] for w, _ in parts)
-            pl = _packed_empty(K, N, seg_k, dev, single_tile=single, block_n=block_n)
-            row = 0
-            for i, (w, b) in enumerate(parts):
-                Ni = w.shape[-1]
-                last = i == len(parts) - 1
-                desc(w, pl.w_hi.data_ptr() + 2 * row * K, Ni, (pl.n_pad - row) if last else Ni, K, K, K, 1, 0, Ni, K)
-                desc(b, pl.bias.data_ptr() + 4 * row, 1, 1, (pl.n_pad - row) if last else Ni, pl.n_pad, Ni, 0, 0, 1, pl.n_pad, f32=1)
-                row += Ni
-            P[key] = pl
-
-        def dgrad_dense(key, parts, K):
-            """parts: [w (K,Ni)] concatenated along N -- data-gradient packing [K_pad, N_pad] (contraction over N)."""
-            N = sum(w.shape[-1] for w in parts)
-            npad = _round_up(N, 64)
-            pl = _packed_empty(npad, K, [npad], dev, bias=False)
-            col = 0
-            for i, w in enumerate(parts):
-                Ni = w.shape[-1]
-                last = i == len(parts) - 1
-                width = (npad - col) if last else Ni
-                desc(w, pl.w_hi.data_ptr() + 2 * col, K, pl.n_pad, width, width, Ni, Ni, 0, 1, npad)
-                col += Ni
-            P[key] = pl
-
-        def dgrad_conv(key, w):
-            k, cin, cout = w.shape
-            cpad = _round_up(cout, 64)
-            pl = _packed_empty(k * cpad, cin, [cpad] * k, dev, bias=False)
-            desc(w, pl.w_hi.data_ptr(), cin, pl.n_pad, k * cpad, cpad, cout, cout, cin * cout, 1, k * cpad)
-            P[key] = pl
-
+        W, P, dev = m.weights, self.P, self.dev
         for name, st in m._stacks.items():
             d = st['d']
             for i, _ in enumerate(st['heads']):
                 pre = f'{name}.b{i}.'
-                qkv = [(W[pre + n + '.w'], W[pre + n + '.b']) for n in ('wq', 'wk', 'wv')]
-                fwd(pre + 'qkv', qkv, d, [d], block_n=d if d <= 256 else d // 2)
-                dgrad_dense(pre + 'qkv.d', [w for w, _ in qkv], d)
-                fwd(pre + 'wo', [(W[pre + 'wo.w'], W[pre + 'wo.b'])], 2 * d, [d, d], single=True)
-                dgrad_dense(pre + 'wo.dx', [W[pre + 'wo.w'][:d]], d)
-                dgrad_dense(pre + 'wo.da', [W[pre + 'wo.w'][d:]], d)
+                self._pack_attention(pre, d)
                 if i < st['n_dense']:
-                    F = int(st['ffn'])
-                    fwd(pre + 'ffn1', [(W[pre + 'ffn1.w'], W[pre + 'ffn1.b'])], d, [d])
-                    fwd(pre + 'ffn2', [(W[pre + 'ffn2.w'], W[pre + 'ffn2.b'])], F, [F], single=True)
-                    dgrad_dense(pre + 'ffn1.d', [W[pre + 'ffn1.w']], d)
-                    dgrad_dense(pre + 'ffn2.d', [W[pre + 'ffn2.w']], F)
+                    self._pack_ffn(pre, d, int(st['ffn']))
                 else:
                     cin = d
                     n = len(st['filters'])
                     kk = int(st['kernel'])
                     for j, f in enumerate(st['filters']):
                         w = W[pre + f'conv{j}.w']
-                        fwd(pre + f'conv{j}', [(w.view(kk * cin, f), W[pre + f'conv{j}.b'])], kk * cin, [cin] * kk, single=(j == n - 1))
-                        dgrad_conv(pre + f'conv{j}.d', w)
+                        self._fwd(pre + f'conv{j}', [(w.view(kk * cin, f), W[pre + f'conv{j}.b'])], kk * cin, [cin] * kk,
+                                  single=(j == n - 1))
+                        self._dgrad_conv(pre + f'conv{j}.d', w)
                         cin = f
         d_enc = m._stacks['encoder']['d']
         for name, filt, k in (('dur_pred', m.config['duration_conv_filters'], m.config['duration_kernel_size']),
@@ -156,28 +180,20 @@ class TrainEngine:
                 f = int(f)
                 bn = _round_up(f, 64)  # 226 -> 256 columns so the next contraction is a multiple of 64
                 w = W[f'{name}.conv{j}.w']
-                fwd(f'{name}.conv{j}', [(w.view(kk * cin, f), W[f'{name}.conv{j}.b'])], kk * cin, [cin] * kk, single=True, block_n=bn)
+                self._fwd(f'{name}.conv{j}', [(w.view(kk * cin, f), W[f'{name}.conv{j}.b'])], kk * cin, [cin] * kk, single=True,
+                          block_n=bn)
                 g_pad = torch.zeros(bn, dtype=torch.float32, device=dev)
                 b_pad = torch.zeros(bn, dtype=torch.float32, device=dev)
-                vec(W[f'{name}.ln{j}.gamma'], g_pad, f)
-                vec(W[f'{name}.ln{j}.beta'], b_pad, f)
+                self._vec(W[f'{name}.ln{j}.gamma'], g_pad, f)
+                self._vec(W[f'{name}.ln{j}.beta'], b_pad, f)
                 P[f'{name}.ln{j}'] = (g_pad, b_pad)
-                dgrad_conv(f'{name}.conv{j}.d', w)
+                self._dgrad_conv(f'{name}.conv{j}.d', w)
                 cin = f
         dd = m._stacks['decoder']['d']
-        fwd('out', [(W['out.w'], W['out.b'])], dd, [dd])
-        dgrad_dense('out.d', [W['out.w']], dd)
+        self._fwd('out', [(W['out.w'], W['out.b'])], dd, [dd])
+        self._dgrad_dense('out.d', [W['out.w']], dd)
         for name, st in m._stacks.items():
             P[f'{name}.pe'] = m._prepare_pe(name)
-        self.P = P
-        self._n_descs = len(descs)
-        self._descs_dev = lib.upload_pack_descs(descs, dev)
-
-    def _pack(self):
-        if self.P is None:
-            self._build_packs()
-        lib.repack_batched(self._descs_dev, self._n_descs)
-        return self.P
 
     # ------------------------------------------------------------------------------------------------
     # small helpers
@@ -235,6 +251,82 @@ class TrainEngine:
         lib.bgemm(g)
 
     # ------------------------------------------------------------------------------------------------
+    # attention core on saved probabilities (self: q,k,v in one buffer; cross: q buffer + k|v buffer)
+    # ------------------------------------------------------------------------------------------------
+    @staticmethod
+    def _fused_probs(qb, kb, flags, dh, ldp):
+        """Self-attention without softmax flags runs on attn_probs_tc.cu where that kernel takes the head size; otherwise the
+        fp32 logits are materialised by a batched GEMM and the softmax kernels."""
+        return kb is qb and flags == 0 and lib.attn_probs_supported(dh, ldp)
+
+    def _attn_fwd(self, B, H, dh, T, Tk, qb, q_ld, q_col, kb, k_ld, k_col, v_col, lens, flags=0):
+        d = H * dh
+        ldp = _round_up(Tk, 16)
+        Z = B * H
+        scale = 1.0 / math.sqrt(dh)
+        rate = self.drop_rate
+        P_pre = self._bf(Z, T, ldp)
+        P_drop = self._bf(Z, T, ldp) if rate > 0 else P_pre
+        site = self._site()
+        if self._fused_probs(qb, kb, flags, dh, ldp):
+            # logits, softmax and attention dropout in one kernel: the (Z, T, T) fp32 logits never reach HBM
+            lib.attn_probs_fwd(qb, q_ld, q_col, k_col, B, H, T, dh, lens, scale, rate, self.seed, site, P_pre, P_drop, ldp)
+        else:
+            S = self._f32(Z, T, ldp)
+            self._bgemm(B, H, T, Tk, dh, qb, (d, T, B), (q_ld, q_ld * T), (dh, 0, 0, q_col), kb, (d, Tk, B), (k_ld, k_ld * Tk),
+                        (dh, 0, 0, k_col), alpha=scale, out_f32=S, ld_out=ldp, out_batch_stride=T * ldp, out_cols=ldp)
+            lib.softmax_fwd(S, B, H, T, Tk, ldp, lens, rate, self.seed, site, P_pre, P_drop, flags=flags)
+            del S
+        out = self._bf(B, T, d)
+        # O = P V: V is read MN-major straight from its buffer (columns v_col + h*dh), no transposed copy
+        self._bgemm(B, H, T, dh, Tk, P_drop, (Tk, T, Z), (ldp, T * ldp), (0, 0, 1, 0), kb, (d, Tk, B), (k_ld, k_ld * Tk),
+                    (dh, 0, 0, v_col, 1), out_bf16=out, ld_out=d, out_batch_stride=T * d, out_h_col=dh, out_by_b=1, out_cols=dh)
+        return out, dict(P_pre=P_pre, P_drop=P_drop, ldp=ldp, site=site, flags=flags, out=out)
+
+    def _attn_bwd(self, c, B, H, dh, T, Tk, dout, qb, q_ld, q_col, kb, k_ld, k_col, v_col, lens, dq_buf, dq_ld, dq_col, dkv_buf,
+                  dkv_ld, dk_col, dv_col, diag=None):
+        """dout: bf16 (B,T,d) gradient of the attention output.  Writes dQ into dq_buf[:, :, dq_col:], dK / dV into
+        dkv_buf[:, :, dk_col:] / [dv_col:] (bf16).  diag = (grad_scale, q_len, k_len) adds the gradient of the diagonal loss
+        on the post-dropout probabilities to dP."""
+        d = H * dh
+        ldp, site, flags = c['ldp'], c['site'], c['flags']
+        Z = B * H
+        scale = 1.0 / math.sqrt(dh)
+        rate = self.drop_rate
+        dS = self._bf(Z, T, ldp)
+        if diag is not None:
+            dP = self._f32(Z, T, ldp)
+            self._bgemm(B, H, T, Tk, dh, dout, (d, T, B), (d, d * T), (dh, 0, 0, 0), kb, (d, Tk, B), (k_ld, k_ld * Tk), (dh, 0, 0, v_col),
+                        out_f32=dP, ld_out=ldp, out_batch_stride=T * ldp, out_cols=ldp)
+            lib.diag_loss_train(c['P_drop'], B, H, T, Tk, ldp, diag[1], diag[2], 0.0, self._loss_scratch, diag[0], dP)
+            lib.softmax_bwd(c['P_pre'], dP, B, H, T, Tk, ldp, lens, scale, rate, self.seed, site, dS, flags=flags)
+            del dP
+        else:
+            # dS straight out of the dP = dO V^T product: rowsum(P_drop * dP) = dO . O per (row, head), so the fp32 dP
+            # matrix (Z*T*Tk*4 bytes) is never written or re-read
+            D = self._f32(Z * T)
+            lib.rowdot_heads(dout, c['out'], H, dh, D)
+            if self._fused_probs(qb, kb, flags, dh, ldp):
+                # sixteen-warp epilogue twin of the forward probability kernel (dropout decisions re-drawn from the hash)
+                lib.attn_ds_bwd(dout, d, 0, kb, k_ld, v_col, B, H, T, dh, lens, c['P_pre'], D, scale, rate, self.seed, site, dS, ldp)
+            else:   # dropout decisions read back from the saved P_drop
+                self._bgemm(B, H, T, Tk, dh, dout, (d, T, B), (d, d * T), (dh, 0, 0, 0), kb, (d, Tk, B), (k_ld, k_ld * Tk),
+                            (dh, 0, 0, v_col), out_bf16=dS, ld_out=ldp, out_batch_stride=T * ldp, out_cols=ldp,
+                            softmax_bwd=(c['P_pre'], D, scale, rate, self.seed, site, flags, lens, c['P_drop']))
+        # dQ = dS K : A = dS (K-major over keys), B = K read MN-major
+        self._bgemm(B, H, T, dh, Tk, dS, (Tk, T, Z), (ldp, T * ldp), (0, 0, 1, 0), kb, (d, Tk, B), (k_ld, k_ld * Tk),
+                    (dh, 0, 0, k_col, 1), out_bf16=dq_buf, ld_out=dq_ld, out_batch_stride=T * dq_ld, out_h_col=dh, out_by_b=1,
+                    out_cols=dh, out_ptr_off=dq_col)
+        # dK = dS^T Q : A = dS read MN-major (= dS^T), B = Q read MN-major
+        self._bgemm(B, H, Tk, dh, T, dS, (Tk, T, Z), (ldp, T * ldp), (0, 0, 1, 0, 1), qb, (d, T, B), (q_ld, q_ld * T),
+                    (dh, 0, 0, q_col, 1), out_bf16=dkv_buf, ld_out=dkv_ld, out_batch_stride=Tk * dkv_ld, out_h_col=dh, out_by_b=1,
+                    out_cols=dh, out_ptr_off=dk_col)
+        # dV = P^T dO : A = P_drop read MN-major, B = dO read MN-major
+        self._bgemm(B, H, Tk, dh, T, c['P_drop'], (Tk, T, Z), (ldp, T * ldp), (0, 0, 1, 0, 1), dout, (d, T, B), (d, d * T),
+                    (dh, 0, 0, 0, 1), out_bf16=dkv_buf, ld_out=dkv_ld, out_batch_stride=Tk * dkv_ld, out_h_col=dh, out_by_b=1,
+                    out_cols=dh, out_ptr_off=dv_col)
+
+    # ------------------------------------------------------------------------------------------------
     # one self-attention block: forward (saving) and backward
     # ------------------------------------------------------------------------------------------------
     def _block_fwd(self, name, i, x_f, x_bf, lens, B, T):
@@ -243,28 +335,11 @@ class TrainEngine:
         d, H = st['d'], st['heads'][i]
         dh = d // H
         pre = f'{name}.b{i}.'
+        rate = self.drop_rate
         c = {'x_f': x_f, 'x_bf': x_bf, 'T': T}
         qkv = self._bf(B, T, 3 * d)
         m._gemm(P[pre + 'qkv'], B, T, [(x_bf, None, d, 0)], [0], [0], out_hi=qkv, ld_out=3 * d)
-        ldp = _round_up(T, 16)
-        Z = B * H
-        P_pre = self._bf(Z, T, ldp)
-        rate = self.drop_rate
-        P_drop = self._bf(Z, T, ldp) if rate > 0 else P_pre
-        site_p = self._site()
-        if self.fused_probs and lib.attn_probs_supported(dh, ldp):
-            # logits, softmax and attention dropout in one kernel: the (Z, T, T) fp32 logits never reach HBM
-            lib.attn_probs_fwd(qkv, 3 * d, 0, d, B, H, T, dh, lens, 1.0 / math.sqrt(dh), rate, self.seed, site_p, P_pre, P_drop, ldp)
-        else:
-            S = self._f32(Z, T, ldp)
-            self._bgemm(B, H, T, T, dh, qkv, (3 * d, T, B), (3 * d, 3 * d * T), (dh, 0, 0, 0), qkv, (2 * d, T, B), (3 * d, 3 * d * T),
-                        (dh, 0, 0, d), alpha=1.0 / math.sqrt(dh), out_f32=S, ld_out=ldp, out_batch_stride=T * ldp, out_cols=ldp)
-            lib.softmax_fwd(S, B, H, T, T, ldp, lens, rate, self.seed, site_p, P_pre, P_drop)
-            del S
-        attn = self._bf(B, T, d)
-        # O = P V: V is read MN-major straight from the QKV buffer (columns 2d + h*dh), no transposed copy
-        self._bgemm(B, H, T, dh, T, P_drop, (T, T, Z), (ldp, T * ldp), (0, 0, 1, 0), qkv, (d, T, B), (3 * d, 3 * d * T),
-                    (dh, 0, 0, 2 * d, 1), out_bf16=attn, ld_out=d, out_batch_stride=T * d, out_h_col=dh, out_by_b=1, out_cols=dh)
+        attn, c_sa = self._attn_fwd(B, H, dh, T, T, qkv, 3 * d, 0, qkv, 3 * d, d, 2 * d, lens)
         y_f, y_bf, u1 = self._f32(B, T, d), self._bf(B, T, d), self._f32(B, T, d)
         site_o = self._site()
         m._gemm(P[pre + 'wo'], B, T, [(x_bf, None, d, 0), (attn, None, d, 0)], [0, 1], [0, 0], residual=x_f,
@@ -294,11 +369,11 @@ class TrainEngine:
             m._gemm(P[pre + f'conv{n - 1}'], B, T, [(cur, None, ld, 0)], [0] * k, shifts, residual=y_f,
                     ln=(W[pre + 'ln2.gamma'], W[pre + 'ln2.beta']), row_len=lens, out_f32=z_f, out_hi=z_bf, out_preln=u2,
                     dropout=(rate, site_c))
-        c.update(qkv=qkv, P_pre=P_pre, P_drop=P_drop, attn=attn, y_f=y_f, y_bf=y_bf, u1=u1, u2=u2, hs=hs, ldp=ldp,
-                 sites=(site_p, site_o, site_c))
+        c.update(qkv=qkv, sa=c_sa, attn=attn, y_f=y_f, y_bf=y_bf, u1=u1, u2=u2, hs=hs, sites=(site_o, site_c))
         return z_f, z_bf, c
 
-    def _block_bwd(self, name, i, c, dz, lens, B):
+    def _block_bwd(self, name, i, c, dz, lens, B, diag=None):
+        """diag: see _attn_bwd."""
         m, P, W, G = self.model, self.P, self.model.weights, self.g
         st = m._stacks[name]
         d, H = st['d'], st['heads'][i]
@@ -306,8 +381,7 @@ class TrainEngine:
         T = c['T']
         pre = f'{name}.b{i}.'
         rate = self.drop_rate
-        site_p, site_o, site_c = c['sites']
-        Z = B * H
+        site_o, site_c = c['sites']
         # ---- LayerNorm 2 (+ row mask) ; the branch gradient carries the branch dropout mask
         du2, g2 = self._f32(B, T, d), self._bf(B, T, d)
         last_b = G[pre + ('ffn2.b' if i < st['n_dense'] else f"conv{len(st['filters']) - 1}.b")]
@@ -354,42 +428,11 @@ class TrainEngine:
         m._gemm(P[pre + 'wo.da'], B, T, [(g1, None, d, 0)], [0], [0], out_hi=dattn, ld_out=d)
         dx_acc = self._f32(B, T, d)
         m._gemm(P[pre + 'wo.dx'], B, T, [(g1, None, d, 0)], [0], [0], residual=du1, out_f32=dx_acc, ld_out=d)
-        # ---- attention backward on the materialised probabilities
-        qkv, ldp = c['qkv'], c['ldp']
-        dS = self._bf(Z, T, ldp)
-        diag = getattr(self, '_enc_diag', None)  # Aligner: diagonal loss on the encoder maps adds its gradient to dP
-        if diag is not None and name == 'encoder':
-            dP = self._f32(Z, T, ldp)
-            self._bgemm(B, H, T, T, dh, dattn, (d, T, B), (d, d * T), (dh, 0, 0, 0), qkv, (d, T, B), (3 * d, 3 * d * T), (dh, 0, 0, 2 * d),
-                        out_f32=dP, ld_out=ldp, out_batch_stride=T * ldp, out_cols=ldp)
-            lib.diag_loss_train(c['P_drop'], B, H, T, T, ldp, diag[1], diag[1], 0.0, self._scratch1, diag[0], dP)
-            lib.softmax_bwd(c['P_pre'], dP, B, H, T, T, ldp, lens, 1.0 / math.sqrt(dh), rate, self.seed, site_p, dS)
-            del dP
-        else:
-            # dS straight out of the dP = dO V^T product: rowsum(P_drop * dP) = dO . O per (row, head), so the fp32 dP
-            # matrix (Z*T*T*4 bytes) is never written or re-read
-            D = self._f32(Z * T)
-            lib.rowdot_heads(dattn, c['attn'], H, dh, D)
-            if self.fused_probs and lib.attn_probs_supported(dh, ldp):
-                # sixteen-warp epilogue twin of the forward probability kernel (dropout decisions re-drawn from the hash)
-                lib.attn_ds_bwd(dattn, d, 0, qkv, 3 * d, 2 * d, B, H, T, dh, lens, c['P_pre'], D, 1.0 / math.sqrt(dh), rate, self.seed,
-                                site_p, dS, ldp)
-            else:
-                self._bgemm(B, H, T, T, dh, dattn, (d, T, B), (d, d * T), (dh, 0, 0, 0), qkv, (d, T, B), (3 * d, 3 * d * T), (dh, 0, 0, 2 * d),
-                            out_bf16=dS, ld_out=ldp, out_batch_stride=T * ldp, out_cols=ldp,
-                            softmax_bwd=(c['P_pre'], D, 1.0 / math.sqrt(dh), rate, self.seed, site_p, 0, lens, None))  # (no P_drop re-read)
+        # ---- attention backward on the saved probabilities
+        qkv = c['qkv']
         dqkv = self._bf(B, T, 3 * d)
-        common = dict(out_bf16=dqkv, ld_out=3 * d, out_batch_stride=T * 3 * d, out_h_col=dh, out_by_b=1, out_cols=dh)
-        qkv_dims, qkv_str = (d, T, B), (3 * d, 3 * d * T)
-        # dQ = dS K    : A = dS (K-major over keys),     B = K read MN-major (columns d + h*dh of the QKV buffer)
-        self._bgemm(B, H, T, dh, T, dS, (T, T, Z), (ldp, T * ldp), (0, 0, 1, 0), qkv, qkv_dims, qkv_str, (dh, 0, 0, d, 1),
-                    out_ptr_off=0, **common)
-        # dK = dS^T Q  : A = dS read MN-major (= dS^T),  B = Q read MN-major
-        self._bgemm(B, H, T, dh, T, dS, (T, T, Z), (ldp, T * ldp), (0, 0, 1, 0, 1), qkv, qkv_dims, qkv_str, (dh, 0, 0, 0, 1),
-                    out_ptr_off=d, **common)
-        # dV = P^T dO  : A = P_drop read MN-major,       B = dO read MN-major
-        self._bgemm(B, H, T, dh, T, c['P_drop'], (T, T, Z), (ldp, T * ldp), (0, 0, 1, 0, 1), dattn, (d, T, B), (d, d * T),
-                    (dh, 0, 0, 0, 1), out_ptr_off=2 * d, **common)
+        self._attn_bwd(c['sa'], B, H, dh, T, T, dattn, qkv, 3 * d, 0, qkv, 3 * d, d, 2 * d, lens, dqkv, 3 * d, 0, dqkv, 3 * d, d, 2 * d,
+                       diag=diag)
         # ---- q/k/v projections
         # the three Dense layers own separate (d,d) kernels and biases but share the (B,T,3d) gradient buffer: one column-sum
         # launch with three outputs, one weight-gradient GEMM of width 3d into a scratch matrix, three strided adds
@@ -477,13 +520,8 @@ class TrainEngine:
     def forward_backward(self, phonemes, mel_tgt, dur_tgt, pitch_tgt, training=True, sync=None):
         """Eager step: forward (+ backward when training).  `sync.bucket_ready` is called as soon as the decoder gradients
         are final (the data-parallel all-reduce of that bucket then overlaps the encoder backward)."""
-        m = self.model
         self._set_salt(0)
-        it = m.optimizer.iterations if m.optimizer else 0
-        self.seed = (self.base_seed * 2654435761 + it * 40503 + self.rank * 97) & 0x7fffffff
-        saved_precision = m.precision
-        m.precision = 'bf16'
-        try:
+        with self._step_state(self.model.step, training):
             gen = self._fb_gen(phonemes, mel_tgt, dur_tgt, pitch_tgt, training)
             out = next(gen)                 # forward (+ decoder backward)
             if training:
@@ -493,6 +531,22 @@ class TrainEngine:
             else:
                 gen.close()
             return out
+
+    def _seed(self, iteration: int) -> int:
+        """Dropout seed of the step at `iteration` (per rank)."""
+        return (self.base_seed * 2654435761 + iteration * 40503 + self.rank * 97) & 0x7fffffff
+
+    @contextlib.contextmanager
+    def _step_state(self, iteration: int, training: bool):
+        """While a step is issued: its dropout rate and seed, and the model's GEMMs in single-pass bf16."""
+        m = self.model
+        self.use_dropout = training and m.train_dropout
+        self.drop_rate = float(m.config.get('dropout_rate', 0.0)) if self.use_dropout else 0.0
+        self.seed = m._drop_seed = self._seed(iteration)
+        saved_precision = m.precision
+        m.precision = 'bf16'
+        try:
+            yield
         finally:
             m.precision = saved_precision
 
@@ -514,175 +568,167 @@ class TrainEngine:
 
     def _fb_gen(self, phonemes, mel_tgt, dur_tgt, pitch_tgt, training=True, Tm_hint=None):
         """The step as a generator: yields the output dictionary after the forward pass + decoder backward (decoder
-        gradients final), finishes with the encoder-side backward.  The caller owns m.precision / self.seed."""
+        gradients final), finishes with the encoder-side backward.  The caller holds the _step_state."""
         m, W, G = self.model, self.model.weights, self.g
         dev = self.dev
-        self.use_dropout = training and m.train_dropout
-        self.drop_rate = float(m.config.get('dropout_rate', 0.0)) if self.use_dropout else 0.0
         self.drop_sites = 0
-        m._drop_seed = self.seed
-        if True:
-            P = self._pack()
-            x = torch.as_tensor(phonemes).to(device=dev, dtype=torch.int32).contiguous()
-            mel_tgt = torch.as_tensor(mel_tgt).to(device=dev, dtype=torch.float32).contiguous()
-            dur_tgt = torch.as_tensor(dur_tgt).to(device=dev, dtype=torch.int32).contiguous()
-            pitch_tgt = torch.as_tensor(pitch_tgt).to(device=dev, dtype=torch.float32).contiguous()
-            B, Tp = x.shape
-            d = m._stacks['encoder']['d']
-            enc_len = torch.empty((B,), dtype=torch.int32, device=dev)
-            lib.phoneme_lengths(x, 0, enc_len)
-            # ---- encoder prologue (embedding rows are kept as the LayerNorm input for the backward pass)
-            e_rows = self._f32(1, B * Tp, d)
-            lib.length_regulate_fwd(W['embedding'].view(1, -1, d), x.view(1, -1), e_rows)
-            h_f, h_bf = self._f32(B, Tp, d), self._bf(B, Tp, d)
-            site_e = self._site()
-            lib.embed_ln_pe_fwd(x, W['embedding'], W['encoder.ln.gamma'], W['encoder.ln.beta'], P['encoder.pe'],
-                                W['encoder.pos_scalar'].reshape(1), LN_EPS, h_f, h_bf, None, drop=(self.drop_rate, self.seed, site_e))
-            enc_ctx = []
-            for i in range(len(m._stacks['encoder']['heads'])):
-                h_f, h_bf, c = self._block_fwd('encoder', i, h_f, h_bf, enc_len, B, Tp)
-                enc_ctx.append(c)
-            dur_out, dur_ctx = self._pred_fwd('dur_pred', h_bf, enc_len, B, Tp, True)
-            pit_out, pit_ctx = self._pred_fwd('pitch_pred', h_bf, enc_len, B, Tp, False)
-            h_pe = self._f32(B, Tp, d)
-            pw = W['pitch_embed.w'].reshape(-1)
-            lib.pitch_embed_add_fwd(h_f, pitch_tgt, pw, W['pitch_embed.b'], h_pe)
-            dur_int = torch.empty((B, Tp), dtype=torch.int32, device=dev)
-            dec_len = torch.empty((B,), dtype=torch.int32, device=dev)
-            lib.durations_to_int(dur_tgt.float(), 1.0, None, None, dur_int, dec_len)
-            mel_len = mel_tgt.shape[1]
-            # decoder length = longest expanded row, but never shorter than the target: a data-parallel shard (or a batch
-            # padded to a bucket length) may hold only rows shorter than the padded target of the GLOBAL batch, which the
-            # reference would have processed at the global length (extra frames are padding rows, masked like any other)
-            Tm = Tm_hint if Tm_hint is not None else max(int(dec_len.max().item()), mel_len)
-            idx = torch.empty((B, Tm), dtype=torch.int32, device=dev)
-            lib.expand_indices(dur_int, Tm, idx)
-            dd = m._stacks['decoder']['d']
-            expanded = self._f32(B, Tm, dd)
-            lib.length_regulate_fwd(h_pe, idx, expanded)
-            m_f, m_bf = self._f32(B, Tm, dd), self._bf(B, Tm, dd)
-            site_d = self._site()
-            lib.expand_ln_pe_fwd(h_pe, idx, W['decoder.ln.gamma'], W['decoder.ln.beta'], P['decoder.pe'],
-                                 W['decoder.pos_scalar'].reshape(1), LN_EPS, m_f, m_bf, None, drop=(self.drop_rate, self.seed, site_d))
-            dec_ctx = []
-            for i in range(len(m._stacks['decoder']['heads'])):
-                m_f, m_bf, c = self._block_fwd('decoder', i, m_f, m_bf, dec_len, B, Tm)
-                dec_ctx.append(c)
-            mel = self._f32(B, Tm, m.mel_channels)
-            m._gemm(P['out'], B, Tm, [(m_bf, None, dd, 0)], [0], [0], out_f32=mel, ld_out=m.mel_channels)
-            # ---- losses (utils/losses.py:41-70, weights [1,1,3]) and their gradients
-            losses = torch.zeros(3, dtype=torch.float32, device=dev)
-            wts = m.loss_weights
-            dmel = self._f32(B, Tm, m.mel_channels)
-            ddur, dpit = self._f32(B, Tp), self._f32(B, Tp)
-            lib.mae_loss(mel, B, Tm, mel_len, m.mel_channels, mel_tgt, wts[0], losses[0:1], dmel)
-            lib.mae_loss(dur_out, B, Tp, Tp, 1, dur_tgt, wts[1], losses[1:2], ddur)
-            lib.mae_loss(pit_out, B, Tp, Tp, 1, pitch_tgt, wts[2], losses[2:3], dpit)
-            out = {'mel': mel, 'duration': dur_out[..., None], 'pitch': pit_out[..., None],
-                   'expanded_mask': mask_from_lengths(dec_len, Tm), 'encoder_attention': {}, 'decoder_attention': {},
-                   'losses': {'mel': losses[0], 'duration': losses[1], 'pitch': losses[2]},
-                   'loss': wts[0] * losses[0] + wts[1] * losses[1] + wts[2] * losses[2], 'mel_lengths': dec_len}
-            if not training:
-                yield out
-                return
-            # =============================== backward ===============================
-            self.flat_g.zero_()
-            C = m.mel_channels
-            kpad = _round_up(C, 64)
-            g = self._bf(B, Tm, kpad)
-            lib.cast_bf16_pad(dmel, B * Tm, C, g, kpad)
-            lib.colsum_bf16(g, B * Tm, C, kpad, G['out.b'])
-            self._wgrad([(m_bf, dd)], g, kpad, B, Tm, dd, C, [(0, 0)], G['out.w'])
-            dz = self._f32(B, Tm, dd)
-            m._gemm(P['out.d'], B, Tm, [(g, None, kpad, 0)], [0], [0], out_f32=dz, ld_out=dd)
-            for i in range(len(dec_ctx) - 1, -1, -1):
-                dz = self._block_bwd('decoder', i, dec_ctx[i], dz, dec_len, B)
-                dec_ctx[i] = None
-            d_exp = self._prologue_bwd('decoder', dz, expanded, dec_len, B, Tm, site_d)
-            yield out             # decoder gradients are final
-            dh_pe = self._f32(B, Tp, d)
-            lib.expand_bwd(d_exp, dur_int, dh_pe)
-            lib.pitch_embed_bwd(dh_pe, pitch_tgt, pw, W['pitch_embed.b'], G['pitch_embed.w'].view(-1), G['pitch_embed.b'])
-            # predictors read the encoder output; their input gradient is accumulated onto dh_pe
-            acc = self._pred_bwd('dur_pred', dur_ctx, ddur, enc_len, B, Tp, dh_pe)
-            acc = self._pred_bwd('pitch_pred', pit_ctx, dpit, enc_len, B, Tp, acc)
-            dz = acc
-            for i in range(len(enc_ctx) - 1, -1, -1):
-                dz = self._block_bwd('encoder', i, enc_ctx[i], dz, enc_len, B)
-                enc_ctx[i] = None
-            de = self._prologue_bwd('encoder', dz, e_rows.view(B, Tp, d), enc_len, B, Tp, site_e)
-            lib.embedding_bwd(de, x, G['embedding'])
+        P = self._pack()
+        x = torch.as_tensor(phonemes).to(device=dev, dtype=torch.int32).contiguous()
+        mel_tgt = torch.as_tensor(mel_tgt).to(device=dev, dtype=torch.float32).contiguous()
+        dur_tgt = torch.as_tensor(dur_tgt).to(device=dev, dtype=torch.int32).contiguous()
+        pitch_tgt = torch.as_tensor(pitch_tgt).to(device=dev, dtype=torch.float32).contiguous()
+        B, Tp = x.shape
+        d = m._stacks['encoder']['d']
+        enc_len = torch.empty((B,), dtype=torch.int32, device=dev)
+        lib.phoneme_lengths(x, 0, enc_len)
+        h_f, h_bf, enc_ctx = self._encoder_fwd(x, enc_len)
+        dur_out, dur_ctx = self._pred_fwd('dur_pred', h_bf, enc_len, B, Tp, True)
+        pit_out, pit_ctx = self._pred_fwd('pitch_pred', h_bf, enc_len, B, Tp, False)
+        h_pe = self._f32(B, Tp, d)
+        pw = W['pitch_embed.w'].reshape(-1)
+        lib.pitch_embed_add_fwd(h_f, pitch_tgt, pw, W['pitch_embed.b'], h_pe)
+        dur_int = torch.empty((B, Tp), dtype=torch.int32, device=dev)
+        dec_len = torch.empty((B,), dtype=torch.int32, device=dev)
+        lib.durations_to_int(dur_tgt.float(), 1.0, None, None, dur_int, dec_len)
+        mel_len = mel_tgt.shape[1]
+        # decoder length = longest expanded row, but never shorter than the target: a data-parallel shard (or a batch
+        # padded to a bucket length) may hold only rows shorter than the padded target of the GLOBAL batch, which the
+        # reference would have processed at the global length (extra frames are padding rows, masked like any other)
+        Tm = Tm_hint if Tm_hint is not None else max(int(dec_len.max().item()), mel_len)
+        idx = torch.empty((B, Tm), dtype=torch.int32, device=dev)
+        lib.expand_indices(dur_int, Tm, idx)
+        dd = m._stacks['decoder']['d']
+        expanded = self._f32(B, Tm, dd)
+        lib.length_regulate_fwd(h_pe, idx, expanded)
+        m_f, m_bf = self._f32(B, Tm, dd), self._bf(B, Tm, dd)
+        site_d = self._site()
+        lib.expand_ln_pe_fwd(h_pe, idx, W['decoder.ln.gamma'], W['decoder.ln.beta'], P['decoder.pe'],
+                             W['decoder.pos_scalar'].reshape(1), LN_EPS, m_f, m_bf, None, drop=(self.drop_rate, self.seed, site_d))
+        dec_ctx = []
+        for i in range(len(m._stacks['decoder']['heads'])):
+            m_f, m_bf, c = self._block_fwd('decoder', i, m_f, m_bf, dec_len, B, Tm)
+            dec_ctx.append(c)
+        mel = self._f32(B, Tm, m.mel_channels)
+        m._gemm(P['out'], B, Tm, [(m_bf, None, dd, 0)], [0], [0], out_f32=mel, ld_out=m.mel_channels)
+        # ---- losses (utils/losses.py:41-70, weights [1,1,3]) and their gradients
+        losses = torch.zeros(3, dtype=torch.float32, device=dev)
+        wts = m.loss_weights
+        dmel = self._f32(B, Tm, m.mel_channels)
+        ddur, dpit = self._f32(B, Tp), self._f32(B, Tp)
+        lib.mae_loss(mel, B, Tm, mel_len, m.mel_channels, mel_tgt, wts[0], losses[0:1], dmel)
+        lib.mae_loss(dur_out, B, Tp, Tp, 1, dur_tgt, wts[1], losses[1:2], ddur)
+        lib.mae_loss(pit_out, B, Tp, Tp, 1, pitch_tgt, wts[2], losses[2:3], dpit)
+        out = {'mel': mel, 'duration': dur_out[..., None], 'pitch': pit_out[..., None],
+               'expanded_mask': mask_from_lengths(dec_len, Tm), 'encoder_attention': {}, 'decoder_attention': {},
+               'losses': {'mel': losses[0], 'duration': losses[1], 'pitch': losses[2]},
+               'loss': wts[0] * losses[0] + wts[1] * losses[1] + wts[2] * losses[2], 'mel_lengths': dec_len}
+        if not training:
+            yield out
+            return
+        # =============================== backward ===============================
+        self.flat_g.zero_()
+        C = m.mel_channels
+        kpad = _round_up(C, 64)
+        g = self._bf(B, Tm, kpad)
+        lib.cast_bf16_pad(dmel, B * Tm, C, g, kpad)
+        lib.colsum_bf16(g, B * Tm, C, kpad, G['out.b'])
+        self._wgrad([(m_bf, dd)], g, kpad, B, Tm, dd, C, [(0, 0)], G['out.w'])
+        dz = self._f32(B, Tm, dd)
+        m._gemm(P['out.d'], B, Tm, [(g, None, kpad, 0)], [0], [0], out_f32=dz, ld_out=dd)
+        for i in range(len(dec_ctx) - 1, -1, -1):
+            dz = self._block_bwd('decoder', i, dec_ctx[i], dz, dec_len, B)
+            dec_ctx[i] = None
+        d_exp = self._prologue_bwd('decoder', dz, expanded, dec_len, B, Tm, site_d)
+        yield out             # decoder gradients are final
+        dh_pe = self._f32(B, Tp, d)
+        lib.expand_bwd(d_exp, dur_int, dh_pe)
+        lib.pitch_embed_bwd(dh_pe, pitch_tgt, pw, W['pitch_embed.b'], G['pitch_embed.w'].view(-1), G['pitch_embed.b'])
+        # predictors read the encoder output; their input gradient is accumulated onto dh_pe
+        acc = self._pred_bwd('dur_pred', dur_ctx, ddur, enc_len, B, Tp, dh_pe)
+        acc = self._pred_bwd('pitch_pred', pit_ctx, dpit, enc_len, B, Tp, acc)
+        self._encoder_bwd(enc_ctx, acc)
 
     # ------------------------------------------------------------------------------------------------
-    # the training step as two CUDA graphs (forward + decoder backward | encoder-side backward), Adam launched eagerly
+    # encoder: embedding, LayerNorm, PE and the self-attention blocks (both engines)
+    # ------------------------------------------------------------------------------------------------
+    def _encoder_fwd(self, x, enc_len):
+        m, W = self.model, self.model.weights
+        B, Tp = x.shape
+        d = m._stacks['encoder']['d']
+        # the embedding rows are kept as the LayerNorm input for the backward pass
+        e_rows = self._f32(1, B * Tp, d)
+        lib.length_regulate_fwd(W['embedding'].view(1, -1, d), x.view(1, -1), e_rows)
+        h_f, h_bf = self._f32(B, Tp, d), self._bf(B, Tp, d)
+        site = self._site()
+        lib.embed_ln_pe_fwd(x, W['embedding'], W['encoder.ln.gamma'], W['encoder.ln.beta'], self.P['encoder.pe'],
+                            W['encoder.pos_scalar'].reshape(1), LN_EPS, h_f, h_bf, None, drop=(self.drop_rate, self.seed, site))
+        blocks = []
+        for i in range(len(m._stacks['encoder']['heads'])):
+            h_f, h_bf, c = self._block_fwd('encoder', i, h_f, h_bf, enc_len, B, Tp)
+            blocks.append(c)
+        return h_f, h_bf, dict(x=x, lens=enc_len, e_rows=e_rows.view(B, Tp, d), site=site, blocks=blocks)
+
+    def _encoder_bwd(self, ctx, dz, diag=None):
+        """dz: fp32 gradient of the encoder output; diag: see _attn_bwd (diagonal loss on the encoder maps)."""
+        blocks, lens, (B, Tp, _) = ctx['blocks'], ctx['lens'], ctx['e_rows'].shape
+        for i in range(len(blocks) - 1, -1, -1):
+            dz = self._block_bwd('encoder', i, blocks[i], dz, lens, B, diag=diag)
+            blocks[i] = None
+        de = self._prologue_bwd('encoder', dz, ctx['e_rows'], lens, B, Tp, ctx['site'])
+        lib.embedding_bwd(de, ctx['x'], self.g['embedding'])
+
+    # ------------------------------------------------------------------------------------------------
+    # the step as CUDA graphs, Adam launched eagerly
     # ------------------------------------------------------------------------------------------------
     def step_graphed(self, phonemes, mel_tgt, dur_tgt, pitch_tgt, sync=None):
-        """Replays the captured step for this input shape (captures it on first use).  ~400 launches, each with host-side
-        tensor-map encoding, become two graph launches: the eager step is host-launch bound (tools/step_cpu_time.py).
-        Per-step state that the captured kernel arguments cannot carry lives in device memory: the dropout salt (see
-        _set_salt); Adam's scalars are not captured (one eager launch).  Outputs are views of static buffers, valid until
-        the next step of the same shape (loss / losses are copied out)."""
+        """Replays the step captured for this input shape (captures it on first use) as two graphs: forward + decoder
+        backward | encoder-side backward.  ~400 launches, each with host-side tensor-map encoding, become two graph
+        launches: the eager step is host-launch bound (tools/step_cpu_time.py)."""
         m = self.model
-        phonemes, mel_tgt, dur_tgt, pitch_tgt = (torch.as_tensor(t) for t in (phonemes, mel_tgt, dur_tgt, pitch_tgt))
-        B, Tp = phonemes.shape
-        mel_len = mel_tgt.shape[1]
-        Tm = max(int(dur_tgt.sum(1).max()), mel_len)          # host sync only if the durations live on the device
+        ins = [torch.as_tensor(t) for t in (phonemes, mel_tgt, dur_tgt, pitch_tgt)]
+        B, Tp = ins[0].shape
+        mel_len = ins[1].shape[1]
+        Tm = max(int(ins[2].sum(1).max()), mel_len)          # host sync only if the durations live on the device
         key = (B, Tp, mel_len, Tm, bool(m.train_dropout), float(m.config.get('dropout_rate', 0.0)))
-        ent = self._graphs.get(key)
+
+        def capture(static):
+            with self._step_state(0, True):      # the seed is frozen in the graph; the salt varies per step
+                self._set_salt(1)
+                gen = self._fb_gen(*static, training=True, Tm_hint=Tm)
+
+                def forward():
+                    lib.set_dropout_salt(self._salt_dev)
+                    return next(gen)
+                return _capture_graphs(self, self.dev, lambda: list(self._fb_gen(*static, training=True, Tm_hint=Tm)),
+                                       forward, lambda: next(gen, None))
+        return self._replay_step(key, ins, (torch.int32, torch.float32, torch.int32, torch.float32), capture, sync)
+
+    def _replay_step(self, key, inputs, dtypes, capture, sync=None):
+        """Replays the graphs of `key` in self._graphs, captured on first use by `capture(static inputs)` -> [(graph, output)]
+        (the first graph's output is the step's output dictionary).  Per-step state that the captured kernel arguments
+        cannot carry lives in device memory: the dropout salt (see _set_salt); Adam's scalars are not captured (one eager
+        launch).  Outputs are views of static buffers, valid until the next step of the same shape (loss / losses are
+        copied out)."""
+        ent = _lru_get(self._graphs, key)
         if ent is None:
-            ent = self._capture_step(key, phonemes, mel_tgt, dur_tgt, pitch_tgt, Tm)
+            _lru_make_room(self._graphs, 4)
+            static = _static_inputs(self.dev, inputs, dtypes)
+            captured = capture(static)
+            ent = self._graphs[key] = {'ins': static, 'graphs': [g for g, _ in captured], 'out': captured[0][1]}
         else:
-            for dst, src in zip(ent['ins'], (phonemes, mel_tgt, dur_tgt, pitch_tgt)):
-                dst.copy_(src, non_blocking=True)
-        it = m.optimizer.iterations if m.optimizer else 0
-        self._set_salt(((it + 1) * 40503 + 12345) & 0x7fffffff)
+            _fill_inputs(ent['ins'], inputs)
+        self._set_salt(((self.model.step + 1) * 40503 + 12345) & 0x7fffffff)
         self._salt_applied = 1
-        ent['g1'].replay()
-        lib.add_launch_count(ent['n1'])
-        if sync is not None:
+        first, *rest = ent['graphs']
+        _replay(first)
+        if sync is not None:      # decoder gradients are final
             sync.bucket_ready(*self.decoder_range)
-        ent['g2'].replay()
-        lib.add_launch_count(ent['n2'])
+        for g in rest:
+            _replay(g)
         out = dict(ent['out'])
         out['loss'] = out['loss'].clone()
         out['losses'] = {k: v.clone() for k, v in out['losses'].items()}
         return out
-
-    def _capture_step(self, key, phonemes, mel_tgt, dur_tgt, pitch_tgt, Tm):
-        m = self.model
-        dev = self.dev
-        ins = [phonemes.to(device=dev, dtype=torch.int32).contiguous().clone(), mel_tgt.to(device=dev, dtype=torch.float32).contiguous().clone(),
-               dur_tgt.to(device=dev, dtype=torch.int32).contiguous().clone(), pitch_tgt.to(device=dev, dtype=torch.float32).contiguous().clone()]
-        self.seed = (self.base_seed * 2654435761 + self.rank * 97) & 0x7fffffff    # frozen in the graph; the salt varies per step
-        saved_precision = m.precision
-        m.precision = 'bf16'
-        try:
-            self._set_salt(1)
-            side = torch.cuda.Stream(device=dev)
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):          # eager warm-up on the capture shapes (packs, function attributes, allocator)
-                for _ in self._fb_gen(*ins, training=True, Tm_hint=Tm):
-                    pass
-            torch.cuda.current_stream().wait_stream(side)
-            if self._graph_pool is None:
-                self._graph_pool = torch.cuda.graph_pool_handle()
-            g1, g2 = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
-            n0 = lib.launch_count()
-            with torch.cuda.graph(g1, pool=self._graph_pool):
-                lib.set_dropout_salt(self._salt_dev)
-                gen = self._fb_gen(*ins, training=True, Tm_hint=Tm)
-                out = next(gen)
-            n1 = lib.launch_count()
-            with torch.cuda.graph(g2, pool=self._graph_pool):
-                next(gen, None)
-            n2 = lib.launch_count()
-        finally:
-            m.precision = saved_precision
-        if len(self._graphs) >= 4:
-            self._graphs.pop(next(iter(self._graphs)))
-        ent = {'ins': ins, 'g1': g1, 'g2': g2, 'out': out, 'n1': n1 - n0, 'n2': n2 - n1}
-        self._graphs[key] = ent
-        return ent
 
     def _prologue_bwd(self, name, g, u, lens, B, T, site):
         m, W, G = self.model, self.model.weights, self.g
