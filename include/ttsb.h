@@ -193,6 +193,72 @@ typedef struct ttsb_mha_args {
 int ttsb_mha_fwd(const ttsb_mha_args* args, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Cached autoregressive decoding of the Aligner  (model/models.py:271-292 Aligner.predict, a batch of sentences at a time)
+ *   The decoder is causal, so one iteration computes ONE new decoder row per sentence: each self-attention block keeps the
+ *   keys / values of the rows already decoded in a cache, and every position lives in device memory (pos[b] = index of the
+ *   row being decoded), so one captured step replays for every iteration.
+ *
+ * ttsb_decode_attn: one query row per (sentence b, head h); logits scaled by 1/sqrt(dh), fp32 softmax, as ttsb_mha_fwd.
+ *   q: 16-bit (B, ld_q), head h at columns q_col0 + h*dh.
+ *   self mode (new_kv != NULL): the new row's key and value (new_kv (B, ld_new), head h at new_k_col0 / new_v_col0 + h*dh: the
+ *     QKV GEMM output) are copied bit for bit into the cache kv (B, Tk, ld_kv) at row pos[b] (columns k_col0 / v_col0 + h*dh),
+ *     and the query attends over keys 0..pos[b] (look-ahead mask); kv_len is not read.  pos[b] < Tk.
+ *   cross mode (new_kv == NULL): attends over the keys < kv_len[b] (padding mask, kv_len[b] >= 1) of kv, which is not written.
+ *   Masked keys get probability exactly 0, as the reference's additive -1e9 mask gives after the fp32 softmax.
+ *   out: bf16 hi (and lo when non-NULL) (B, ld_out), head h at columns h*dh: the attention operand of the concat projection.
+ *   probs (optional): the fp32 probability row of (b, h), written at (b, h, pos[b], :) of a (B, H, probs_T, Tk) buffer.
+ *   done (optional, [B]): rows with done[b] != 0 are skipped; nothing is read or written for them.
+ *   precision: TTSB_PREC_FP16 (q / kv hold IEEE fp16) or TTSB_PREC_BF16.  dh in {64, 128, 256}; leading dimensions and
+ *   column offsets are multiples of 8 (16-byte loads).
+ *   Keys are split across the warps of a CTA and, when B*H is small against the SM count, across CTAs sized for Tk; the CTAs
+ *   whose range holds keys at the row's current length park partial results, and the last of them to finish combines them in
+ *   a fixed order (deterministic).  workspace: at least ttsb_decode_attn_workspace_bytes(B, H, dh) bytes of device memory.
+ *   It starts with B*H counter words, which must be zero before the first call and which every call leaves at zero; the
+ *   partial results follow at an offset that depends on B*H and keep whatever the last call wrote there.  So calls may share
+ *   one workspace (stream-ordered) only when they have the same B and H; calls with another B or H need their own.
+ * ttsb_decode_prologue: the decoder prologue (model/layers.py:406-410) for one row per sentence at a device-side position:
+ *   out[b] = LayerNorm(x[b]) + pos_scalar * pe[pos[b]]  (x fp32 (B, d); pe (pe_rows, d) is the table whose row t is position
+ *   t*r; positions are clamped to [0, pe_rows)); writes the fp32 + bf16 hi/lo triple (B, d).  d % 4 == 0, d <= 512.
+ * ttsb_decode_commit: the end of one iteration (model/models.py:280-289), one CTA, for every row b with done[b] == 0:
+ *   post fp32 (B*r, ld_post) is the step's postnet output (frame j of row b at row b*r + j; mel in columns [0, mel), the
+ *   three stop logits from column stop_col);
+ *   mel_out[b, pos[b]*r + j, :] = frame j  (mel_out fp32 (B, max_iters*r, mel)); stop_out (optional, fp32 (B, max_iters*r, 3))
+ *   the same for the stop logits;
+ *   next_hi / next_lo (B, ld_next) bf16, columns [0, mel) = frame r-1 split into hi/lo: the next input (next_lo may be NULL);
+ *   n[b] = pos[b] + 1; done[b] = 1 when the first arg-max of the last stop row is stop_index or n[b] == max_iters, else
+ *   pos[b] += 1;  *all_done = 1 when every row is done, else 0.
+ * ------------------------------------------------------------------------------------------------------- */
+typedef struct ttsb_decode_attn_args {
+  int B, H, dh;
+  const void* q;
+  int ld_q, q_col0;
+  void* kv;
+  int ld_kv, Tk, k_col0, v_col0;
+  const void* new_kv;         /* NULL: cross mode */
+  int ld_new, new_k_col0, new_v_col0;
+  const int32_t* pos;         /* [B] */
+  const int32_t* kv_len;      /* [B], cross mode */
+  const int32_t* done;        /* [B] or NULL */
+  void* out_hi;
+  void* out_lo;
+  int ld_out;
+  float* probs;               /* or NULL */
+  int probs_T;
+  int precision;
+  void* workspace;
+  int64_t workspace_bytes;
+} ttsb_decode_attn_args;
+
+int64_t ttsb_decode_attn_workspace_bytes(int B, int H, int dh);
+int ttsb_decode_attn(const ttsb_decode_attn_args* args, void* stream);
+int ttsb_decode_prologue(const float* x, const int32_t* pos, const float* gamma, const float* beta, const float* pe, int pe_rows,
+                         const float* pos_scalar, int B, int d, float eps, float* out_f32, void* out_hi, void* out_lo,
+                         void* stream);
+int ttsb_decode_commit(const float* post, int ld_post, int B, int r, int mel, int stop_col, int stop_index, int max_iters,
+                       float* mel_out, float* stop_out, void* next_hi, void* next_lo, int ld_next, int32_t* pos, int32_t* done,
+                       int32_t* n, int32_t* all_done, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Training-step GEMMs (single-pass bf16, fp32 accumulate) -- gradients of the layers above
  *
  * ttsb_bgemm: per-(batch row b, head h) products  out_z[m][n] = alpha * sum_k A_z[m][k] * B_z[n][k]  where both operands

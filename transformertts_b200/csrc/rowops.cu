@@ -109,6 +109,27 @@ __global__ void expand_ln_pe_kernel(const float* __restrict__ x, const int* __re
               out_hi ? out_hi + o : nullptr, out_lo ? out_lo + o : nullptr, drop_p, seed, site, (uint64_t)o);
 }
 
+// Decoder prologue of one row per sentence at a device-side position (cached autoregressive decoding): the PE row is
+// pe[pos[b]] instead of the output frame index of expand_ln_pe_kernel.
+__global__ void decode_prologue_kernel(const float* __restrict__ x, const int* __restrict__ pos, const float* gamma,
+                                       const float* beta, const float* pe, int pe_rows, const float* pos_scalar, int B, int d,
+                                       float eps, float* out_f32, __nv_bfloat16* out_hi, __nv_bfloat16* out_lo) {
+  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= B) return;
+  const int lane = threadIdx.x & 31;
+  const int t = min(max(__ldg(pos + row), 0), pe_rows - 1);
+  const int nv = (d + 127) / 128;
+  float4 v[ROW_MAX_V4];
+#pragma unroll
+  for (int i = 0; i < ROW_MAX_V4; ++i) {
+    const int c0 = (i * 32 + lane) * 4;
+    v[i] = (i < nv && c0 < d) ? __ldg(reinterpret_cast<const float4*>(x + (size_t)row * d + c0)) : make_float4(0, 0, 0, 0);
+  }
+  const size_t o = (size_t)row * d;
+  ln_pe_store(v, nv, d, lane, gamma, beta, eps, pe + (size_t)t * d, __ldg(pos_scalar), out_f32 ? out_f32 + o : nullptr,
+              out_hi ? out_hi + o : nullptr, out_lo ? out_lo + o : nullptr);
+}
+
 // Stand-alone LayerNorm + row mask for model dimensions whose row does not fit one 256-column accumulator tile (d = 384):
 // the GEMM writes the pre-norm value (acc + bias + residual), this kernel normalises it (model/layers.py:211,40,102).
 __global__ void layernorm_fwd_kernel(const float* __restrict__ x, const float* gamma, const float* beta, int rows, int T, int d,
@@ -446,6 +467,16 @@ extern "C" int ttsb_expand_ln_pe_fwd(const float* x, const int32_t* idx, const f
                                      const float* pos_scalar, int B, int Tp, int Tm, int d, float eps, float* out_f32, void* out_hi,
                                      void* out_lo, void* stream) {
   return ttsb_expand_ln_pe_train_fwd(x, idx, gamma, beta, pe, pos_scalar, B, Tp, Tm, d, eps, 0.f, 0u, 0u, out_f32, out_hi, out_lo, stream);
+}
+
+extern "C" int ttsb_decode_prologue(const float* x, const int32_t* pos, const float* gamma, const float* beta, const float* pe, int pe_rows,
+                                    const float* pos_scalar, int B, int d, float eps, float* out_f32, void* out_hi, void* out_lo,
+                                    void* stream) {
+  if (!x || !pos || !gamma || !beta || !pe || !pos_scalar) return bad("ttsb_decode_prologue: NULL input");
+  if (B <= 0 || pe_rows <= 0 || d <= 0 || d % 4 || d > 128 * ROW_MAX_V4) return bad("ttsb_decode_prologue: need B, pe_rows > 0, d % 4 == 0, d <= 512");
+  decode_prologue_kernel<<<(B + 7) / 8, 256, 0, STREAM(stream)>>>(x, pos, gamma, beta, pe, pe_rows, pos_scalar, B, d, eps, out_f32,
+                                                                  static_cast<__nv_bfloat16*>(out_hi), static_cast<__nv_bfloat16*>(out_lo));
+  LAUNCH_OK("decode_prologue_kernel");
 }
 
 extern "C" int ttsb_layernorm_fwd(const float* x, const float* gamma, const float* beta, int B, int T, int d, int ld, float eps,

@@ -30,6 +30,7 @@ EXPORTS = [
     'ttsb_pitch_embed_bwd', 'ttsb_statpred_head_bwd', 'ttsb_adam_tf_step', 'ttsb_embed_ln_pe_train_fwd',
     'ttsb_expand_ln_pe_train_fwd', 'ttsb_mel_to_linear', 'ttsb_stft_complex', 'ttsb_istft_workspace_bytes', 'ttsb_istft', 'ttsb_griffinlim_update',
     'ttsb_dp_unique_id', 'ttsb_dp_init', 'ttsb_dp_allreduce_bucket', 'ttsb_dp_destroy',
+    'ttsb_decode_attn_workspace_bytes', 'ttsb_decode_attn', 'ttsb_decode_prologue', 'ttsb_decode_commit',
 ]
 
 
@@ -95,6 +96,17 @@ class MhaArgs(C.Structure):
     ]
 
 
+class DecodeAttnArgs(C.Structure):
+    _fields_ = [
+        ('B', C.c_int), ('H', C.c_int), ('dh', C.c_int), ('q', C.c_void_p), ('ld_q', C.c_int), ('q_col0', C.c_int),
+        ('kv', C.c_void_p), ('ld_kv', C.c_int), ('Tk', C.c_int), ('k_col0', C.c_int), ('v_col0', C.c_int),
+        ('new_kv', C.c_void_p), ('ld_new', C.c_int), ('new_k_col0', C.c_int), ('new_v_col0', C.c_int),
+        ('pos', C.c_void_p), ('kv_len', C.c_void_p), ('done', C.c_void_p), ('out_hi', C.c_void_p), ('out_lo', C.c_void_p),
+        ('ld_out', C.c_int), ('probs', C.c_void_p), ('probs_T', C.c_int), ('precision', C.c_int),
+        ('workspace', C.c_void_p), ('workspace_bytes', C.c_int64),
+    ]
+
+
 def library_path() -> Path:
     return _LIB_PATH
 
@@ -113,6 +125,7 @@ def load() -> C.CDLL:
     lib.ttsb_add_launch_count.restype = None
     lib.ttsb_add_launch_count.argtypes = [C.c_int64]
     lib.ttsb_istft_workspace_bytes.restype = C.c_int64
+    lib.ttsb_decode_attn_workspace_bytes.restype = C.c_int64
     for name in EXPORTS:
         if not hasattr(lib, name):
             raise TtsbError(f'libttsb.so does not export {name}')
@@ -485,3 +498,29 @@ def istft_workspace_bytes(n_frames: int) -> int:
 def griffinlim_update(rebuilt, previous, magnitude, momentum, projected_out):
     _check(load().ttsb_griffinlim_update(ptr(rebuilt), ptr(previous), ptr(magnitude), C.c_float(momentum), C.c_int64(magnitude.numel()),
                                          ptr(projected_out), _stream()), 'ttsb_griffinlim_update')
+
+
+# ------------------------------------------------------------------------------------------------------------
+# cached autoregressive decoding (Aligner.predict_batch)
+# ------------------------------------------------------------------------------------------------------------
+def decode_attn_workspace_bytes(B: int, H: int, dh: int) -> int:
+    return int(load().ttsb_decode_attn_workspace_bytes(int(B), int(H), int(dh)))
+
+
+def decode_attn(args: DecodeAttnArgs):
+    _check(load().ttsb_decode_attn(C.byref(args), _stream()), 'ttsb_decode_attn')
+
+
+def decode_prologue(x, pos, gamma, beta, pe, pos_scalar, eps, out_f32, out_hi, out_lo):
+    """out[b] = LayerNorm(x[b]) + pos_scalar * pe[pos[b]]; x fp32 (B, d)."""
+    d = x.shape[-1]
+    B = x.numel() // d
+    _check(load().ttsb_decode_prologue(ptr(x), ptr(pos), ptr(gamma), ptr(beta), ptr(pe), pe.shape[0], ptr(pos_scalar), B, d,
+                                       C.c_float(eps), ptr(out_f32), ptr(out_hi), ptr(out_lo), _stream()), 'ttsb_decode_prologue')
+
+
+def decode_commit(post, B, r, mel, stop_col, stop_index, max_iters, mel_out, stop_out, next_hi, next_lo, pos, done, n, all_done):
+    """End of one decode iteration (include/ttsb.h: ttsb_decode_commit); post fp32 (B*r, ld_post), next_hi / next_lo (B, ld_next)."""
+    _check(load().ttsb_decode_commit(ptr(post), post.shape[-1], int(B), int(r), int(mel), int(stop_col), int(stop_index), int(max_iters),
+                                     ptr(mel_out), ptr(stop_out), ptr(next_hi), ptr(next_lo), next_hi.shape[-1], ptr(pos), ptr(done),
+                                     ptr(n), ptr(all_done), _stream()), 'ttsb_decode_commit')

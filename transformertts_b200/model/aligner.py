@@ -17,8 +17,9 @@ Parameter names (flat dict, Keras layouts):
 """
 from __future__ import annotations
 
-from typing import Dict
+from typing import Dict, List
 
+import numpy as np
 import torch
 
 from .. import lib
@@ -27,6 +28,10 @@ from .models import (LN_EPS, ForwardTransformer, _capture_graphs, _fill_inputs, 
 from .transformer_utils import mask_from_lengths, positional_encoding
 
 ALIGNER_VOCAB = 129  # 126 symbols + pad + start + end (reference: data/text/tokenizer.py:17-26 with add_start_end=True)
+# predict_batch: decode steps issued between two host reads of the "all rows done" word (finished rows stay frozen, so the
+# result does not depend on it; it only bounds the steps run after the last row has stopped)
+_DECODE_SYNC_EVERY = 8
+_DECODE_GRAPH_CACHE = 2   # captured decode steps kept per model (each holds its caches and map buffers)
 
 
 class Aligner(ForwardTransformer):
@@ -64,6 +69,8 @@ class Aligner(ForwardTransformer):
         self.vocab_size = int(kwargs.get('vocab_size', ALIGNER_VOCAB))
         self.return_attention_weights = True      # attention maps are model outputs (models.py:150-153, 297)
         self._val_graphs = {}
+        self._decode_graphs = {}
+        self.decode_stats = None   # predict_batch: {'steps', 'host_reads'} of the last call
         self.max_r = int(max_r)
         self.r = int(max_r)                        # models.py:46 -- starts at max_r, lowered by the schedule via set_constants
         self.stop_prob_index = 2
@@ -176,6 +183,19 @@ class Aligner(ForwardTransformer):
             self._final_proj[r] = _PackedLinear(self.weights['final_proj.w'][:, :n].contiguous(), self.weights['final_proj.b'][:n].contiguous(),
                                                 [self._stacks['decoder']['d']], self._split)
         return self._final_proj[r]
+
+    def _final_proj_frames_r(self, r: int) -> _PackedLinear:
+        """The first r*mel columns of FinalProj with every frame padded to _mel_k columns (zero weights and bias): the GEMM
+        output, viewed as (rows*r, _mel_k), is the zero-padded postnet input of the cached decode step."""
+        key = ('frames', r)
+        if key not in self._final_proj:
+            mel, k, d = self.mel_channels, self._mel_k, self._stacks['decoder']['d']
+            w = torch.zeros((d, r, k), dtype=torch.float32, device=self.device)
+            b = torch.zeros((r, k), dtype=torch.float32, device=self.device)
+            w[:, :, :mel] = self.weights['final_proj.w'][:, :r * mel].reshape(d, r, mel)
+            b[:, :mel] = self.weights['final_proj.b'][:r * mel].reshape(r, mel)
+            self._final_proj[key] = _PackedLinear(w.reshape(d, r * k), b.reshape(-1), [d], self._split)
+        return self._final_proj[key]
 
     def _decoder_pe(self, r: int) -> torch.Tensor:
         """pos_encoding[:, :T*r:r] (layers.py:409) as a dense table so row t of the table is position t*r."""
@@ -446,6 +466,225 @@ class Aligner(ForwardTransformer):
                     print('Stopping')
                 break
         return out_dict
+
+    # ------------------------------------------------------------------------------------------------
+    # cached autoregressive decoding of a batch of sentences
+    # ------------------------------------------------------------------------------------------------
+    def predict_batch(self, inputs, max_length=1000, verbose=False) -> List[dict]:
+        """`predict` (models.py:271-292) for a batch of token rows, with a key/value cache instead of the re-run of the decoder
+        over the whole prefix.  inputs: a list of 1-D token-id sequences, or a (B, Tp) array padded with 0 at the end.
+
+        Returns one dict per row in the shape `predict` returns for that row alone: 'mel' (n_b*r, mel_channels),
+        'decoder_attention' {key: (1, H, n_b, Tp_b)}, 'encoder_attention' {key: (1, H, Tp_b, Tp_b)}, plus 'stop_prob'
+        (n_b*r, 3), the stop logits.  n_b is the first iteration whose last stop distribution has its arg-max at
+        `stop_prob_index`, or max_length // r + 1; Tp_b is the row's token count.
+
+        The decoder is causal and its rows do not depend on later ones, so each iteration decodes one row per sentence: the
+        encoder and every block's cross-attention K|V run once, each self-attention block appends the new row's K and V to its
+        cache, and the step reads its positions from device memory.  One difference from the re-run is left out on purpose:
+        the reference masks a decoder key whose input frame sums to exactly 0 in every channel (transformer_utils.py:29-32);
+        a predicted frame does that with probability zero, and the cached decode never masks one.  With `cuda_graphs` the
+        step is captured once per (B, Tp, max_length, r, precisions) and replayed; the host reads one "all rows done" word
+        every few steps."""
+        r = int(self.r)
+        max_iters = int(max_length) // r + 1
+        if max_iters * r > self._stacks['decoder']['max_pos']:
+            raise ValueError('target length * r exceeds decoder_max_position_encoding')
+        return self._predict_batch(self._token_batch(inputs), max_iters, r, verbose)
+
+    @staticmethod
+    def _token_batch(inputs) -> torch.Tensor:
+        if torch.is_tensor(inputs) or isinstance(inputs, np.ndarray):
+            tokens = torch.as_tensor(inputs).to(torch.int32)
+            if tokens.dim() != 2:
+                raise ValueError('inputs must be a list of token sequences or a (batch, length) array')
+        else:
+            rows = [torch.as_tensor(np.asarray(row)).reshape(-1).to(torch.int32) for row in inputs]
+            if not rows:
+                raise ValueError('inputs is empty')
+            tokens = torch.zeros((len(rows), max(len(row) for row in rows)), dtype=torch.int32)
+            for b, row in enumerate(rows):
+                tokens[b, :len(row)] = row
+        nz = tokens.cpu() != 0
+        if tokens.shape[0] == 0 or tokens.shape[1] == 0 or not bool(nz[:, 0].all()):
+            raise ValueError('every row needs at least one token')
+        if bool((nz[:, 1:] & ~nz[:, :-1]).any()):
+            raise ValueError('pad id 0 inside a sequence: batches must be padded at the end')
+        return tokens
+
+    @_on_device
+    def _predict_batch(self, tokens, max_iters: int, r: int, verbose: bool) -> List[dict]:
+        P = self._prepare()
+        B, Tp = tokens.shape
+        enc, _, enc_attn, enc_len = self._call_encoder(tokens, training=False)
+        if self.cuda_graphs and self.impl != 'simt':
+            key = (B, Tp, max_iters, r, self.precision, self.attention_precision, id(P))
+            ent = _lru_get(self._decode_graphs, key)
+            if ent is None:
+                _lru_make_room(self._decode_graphs, _DECODE_GRAPH_CACHE)
+                st = self._decode_state(P, B, Tp, max_iters, r)
+                self._decode_prefill(P, st, enc, enc_len)   # the capture's warm-up step runs on a valid state
+                [(g, _)] = _capture_graphs(self, self.device, lambda: self._decode_step(P, st), lambda: self._decode_step(P, st))
+                ent = self._decode_graphs[key] = {'st': st, 'g': g, 'P': P}
+            st = ent['st']
+
+            def step():
+                _replay(ent['g'])
+        else:
+            st = self._decode_state(P, B, Tp, max_iters, r)
+
+            def step():
+                self._decode_step(P, st)
+        self._decode_prefill(P, st, enc, enc_len)
+        flag = torch.empty((1,), dtype=torch.int32, pin_memory=True)
+        steps = reads = 0
+        while steps < max_iters:
+            for _ in range(min(_DECODE_SYNC_EVERY, max_iters - steps)):
+                step()
+                steps += 1
+            if steps == max_iters:   # every row is done at the iteration cap
+                break
+            flag.copy_(st['all_done'], non_blocking=True)
+            torch.cuda.current_stream().synchronize()
+            reads += 1
+            if int(flag[0]):
+                break
+        lens = torch.stack([st['n'], enc_len]).cpu()
+        reads += 1
+        self.decode_stats = {'steps': steps, 'host_reads': reads}
+        n_dec = len(self._stacks['decoder']['heads'])
+        out = []
+        for b in range(B):
+            nb, tb = int(lens[0, b]), int(lens[1, b])
+            if verbose and nb < max_iters:
+                print(f'row {b}: stopping after {nb} iterations')
+            out.append({
+                'mel': st['mel'][b, :nb * r].clone(),
+                'stop_prob': st['stop'][b, :nb * r].clone(),
+                'decoder_attention': {('Decoder_LastBlock_CrossAttention' if i == n_dec - 1 else f'Decoder_DenseBlock{i + 1}_CrossAttention'):
+                                      st['maps'][i][b:b + 1, :, :nb, :tb].clone() for i in range(n_dec)},
+                'encoder_attention': {k: w[b:b + 1, :, :tb, :tb].clone() for k, w in enc_attn.items()},
+            })
+        return out
+
+    def _decode_state(self, P, B: int, Tp: int, max_iters: int, r: int) -> dict:
+        """Device buffers of one batch decode: caches, maps and outputs for the whole call plus the step's activations."""
+        if self.attention_precision == 'bf16x3':
+            raise lib.TtsbError("Aligner attention runs in the single-pass modes ('fp16' / 'bf16'): head dim 256 needs them")
+        dev, dec = self.device, self._stacks['decoder']
+        d, mel, k = dec['d'], self.mel_channels, self._mel_k
+        adt = torch.float16 if self.attention_precision == 'fp16' else torch.bfloat16
+        i32 = dict(dtype=torch.int32, device=dev)
+        fp = self._final_proj_frames_r(r)
+        start = torch.zeros((B, k), dtype=torch.float32, device=dev)
+        start[:, :mel] = self.start_vec.to(dev)
+        start_hi, start_lo = lib.split_bf16(start, self._split)
+        return {
+            'B': B, 'Tp': Tp, 'r': r, 'max_iters': max_iters, 'fp': fp, 'pe': self._decoder_pe(r),
+            'pos': torch.zeros((B,), **i32), 'done': torch.zeros((B,), **i32), 'n': torch.zeros((B,), **i32),
+            'all_done': torch.zeros((1,), **i32), 'enc_len': torch.zeros((B,), **i32),
+            'start': (start_hi, start_lo), 'in': (torch.empty_like(start_hi), torch.empty_like(start_lo) if start_lo is not None else None),
+            # ttsb_decode_attn's workspace layout depends on the head count: one per head count of the stack (A5: 4 and 1)
+            'workspace': {H: torch.zeros((lib.decode_attn_workspace_bytes(B, H, d // H),), dtype=torch.uint8, device=dev)
+                          for H in set(dec['heads'])},
+            'cache': [torch.empty((B, max_iters, 2 * d), dtype=adt, device=dev) for _ in dec['heads']],
+            'kv': [torch.empty((B, Tp, P[f'decoder.b{i}.ca.kv'].n_pad), dtype=adt, device=dev) for i in range(len(dec['heads']))],
+            'maps': [torch.empty((B, H, max_iters, Tp), dtype=torch.float32, device=dev) for H in dec['heads']],
+            'mel': torch.empty((B, max_iters * r, mel), dtype=torch.float32, device=dev),
+            'stop': torch.empty((B, max_iters * r, 3), dtype=torch.float32, device=dev),
+            # one step's activations: rows = sentences
+            'h1': self._act(1, B, P['prenet.d1'].n_pad, f32=False), 'pre': torch.empty((B, d), dtype=torch.float32, device=dev),
+            'x': self._act(1, B, d), 'y': self._act(1, B, d), 'z': self._act(1, B, d), 'o': [self._act(1, B, d), self._act(1, B, d)],
+            'qkv': torch.empty((B, P['decoder.b0.sa.qkv'].n_pad), dtype=adt, device=dev),
+            'q': torch.empty((B, P['decoder.b0.ca.q'].n_pad), dtype=adt, device=dev),
+            'att': self._act(1, B, d, f32=False), 'h': self._act(1, B, P['decoder.b0.ffn1'].n_pad, f32=False),
+            'lin': self._act(1, B, fp.n_pad, f32=False),
+            'post': torch.empty((B * r, P['postnet'].n_pad), dtype=torch.float32, device=dev),
+        }
+
+    def _decode_prefill(self, P, st, enc, enc_len):
+        """Once per call: every block's cross-attention K|V of the encoder output, the start frame as every row's first input,
+        positions and flags at zero."""
+        d_enc = self._stacks['encoder']['d']
+        f16 = self.attention_precision == 'fp16'
+        for i, kv in enumerate(st['kv']):
+            self._gemm(P[f'decoder.b{i}.ca.kv'], st['B'], st['Tp'], [(enc[1], enc[2], d_enc, 0)], [0], [0], out_hi=kv, out_fp16=f16)
+        st['enc_len'].copy_(enc_len)
+        for t in ('pos', 'done', 'n', 'all_done'):
+            st[t].zero_()
+        for dst, src in zip(st['in'], st['start']):
+            if dst is not None:
+                dst.copy_(src)
+
+    def _decode_attn(self, st, H, dh, q, ld_q, kv, ld_kv, Tk, new=False, probs=None):
+        """ttsb_decode_attn: self mode (`new`: K and V of the new row at columns d / 2d of q, cached at (0, d) of kv) or
+        cross mode over the encoder K|V (keys < enc_len)."""
+        d = H * dh
+        a = lib.DecodeAttnArgs()
+        a.B, a.H, a.dh = st['B'], H, dh
+        a.q, a.ld_q, a.q_col0 = q.data_ptr(), ld_q, 0
+        a.kv, a.ld_kv, a.Tk, a.k_col0, a.v_col0 = kv.data_ptr(), ld_kv, Tk, 0, d
+        if new:
+            a.new_kv, a.ld_new, a.new_k_col0, a.new_v_col0 = q.data_ptr(), ld_q, d, 2 * d
+        else:
+            a.kv_len = st['enc_len'].data_ptr()
+        a.pos, a.done = st['pos'].data_ptr(), st['done'].data_ptr()
+        _, at_hi, at_lo = st['att']
+        a.out_hi = at_hi.data_ptr()
+        a.out_lo = at_lo.data_ptr() if at_lo is not None else None
+        a.ld_out = d
+        if probs is not None:
+            a.probs, a.probs_T = probs.data_ptr(), probs.shape[2]
+        a.precision = lib.PREC_FP16 if self.attention_precision == 'fp16' else lib.PREC_BF16
+        ws = st['workspace'][H]
+        a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+        lib.decode_attn(a)
+
+    def _decode_step(self, P, st):
+        """One iteration for every row: prenet, prologue at pos[b], the blocks with cached self-attention, FinalProj, postnet,
+        commit.  Every GEMM takes the B rows as one sequence (a Dense has no time shift), so they share 128-row tiles."""
+        W = self.weights
+        dec = self._stacks['decoder']
+        d, B, r, k = dec['d'], st['B'], st['r'], self._mel_k
+        f16 = self.attention_precision == 'fp16'
+        in_hi, in_lo = st['in']
+        _, h_hi, h_lo = st['h1']
+        self._gemm(P['prenet.d1'], 1, B, [(in_hi, in_lo, k, 0)], [0], [0], relu=True, out_hi=h_hi, out_lo=h_lo)
+        self._gemm(P['prenet.d2'], 1, B, [(h_hi, h_lo, P['prenet.d1'].n_pad, 0)], [0], [0], relu=True, out_f32=st['pre'])
+        x = st['x']
+        lib.decode_prologue(st['pre'], st['pos'], W['decoder.ln.gamma'], W['decoder.ln.beta'], st['pe'], W['decoder.pos_scalar'].reshape(1),
+                            LN_EPS, x[0], x[1], x[2])
+        _, a_hi, a_lo = st['att']
+        for i, H in enumerate(dec['heads']):
+            pre = f'decoder.b{i}.'
+            qkv = P[pre + 'sa.qkv']
+            self._gemm(qkv, 1, B, [(x[1], x[2], d, 0)], [0], [0], out_hi=st['qkv'], out_fp16=f16)
+            self._decode_attn(st, H, d // H, st['qkv'], qkv.n_pad, st['cache'][i], 2 * d, st['max_iters'], new=True)
+            y = st['y']
+            self._gemm(P[pre + 'sa.wo'], 1, B, [(x[1], x[2], d, 0), (a_hi, a_lo, d, 0)], [0, 1], [0, 0], residual=x[0],
+                       ln=(W[pre + 'sa.ln.gamma'], W[pre + 'sa.ln.beta']), out_f32=y[0], out_hi=y[1], out_lo=y[2])
+            pq, pkv = P[pre + 'ca.q'], P[pre + 'ca.kv']
+            self._gemm(pq, 1, B, [(y[1], y[2], d, 0)], [0], [0], out_hi=st['q'], out_fp16=f16)
+            self._decode_attn(st, H, d // H, st['q'], pq.n_pad, st['kv'][i], pkv.n_pad, st['Tp'], probs=st['maps'][i])
+            z = st['z']
+            self._gemm(P[pre + 'ca.wo'], 1, B, [(y[1], y[2], d, 0), (a_hi, a_lo, d, 0)], [0, 1], [0, 0], residual=y[0],
+                       ln=(W[pre + 'ca.ln.gamma'], W[pre + 'ca.ln.beta']), out_f32=z[0], out_hi=z[1], out_lo=z[2])
+            f1 = P[pre + 'ffn1']
+            _, f_hi, f_lo = st['h']
+            self._gemm(f1, 1, B, [(z[1], z[2], d, 0)], [0], [0], relu=True, out_hi=f_hi, out_lo=f_lo)
+            o = st['o'][i % 2]
+            self._gemm(P[pre + 'ffn2'], 1, B, [(f_hi, f_lo, f1.n_pad, 0)], [0], [0], residual=z[0],
+                       ln=(W[pre + 'ln2.gamma'], W[pre + 'ln2.beta']), out_f32=o[0], out_hi=o[1], out_lo=o[2])
+            x = o
+        # FinalProj[:, :r*mel] with frames padded to k columns = the postnet's input rows (models.py:146-150)
+        fp = st['fp']
+        _, l_hi, l_lo = st['lin']
+        self._gemm(fp, 1, B, [(x[1], x[2], d, 0)], [0], [0], out_hi=l_hi, out_lo=l_lo)
+        pn = P['postnet']
+        self._gemm(pn, 1, B * r, [(l_hi, l_lo, k, 0)], [0], [0], out_f32=st['post'])
+        mel = self.mel_channels
+        lib.decode_commit(st['post'], B, r, mel, mel, self.stop_prob_index, st['max_iters'], st['mel'], st['stop'], in_hi, in_lo,
+                          st['pos'], st['done'], st['n'], st['all_done'])
 
     def _compile(self, stop_scaling=None, optimizer=None):
         """models.py:222-227.  stop_scaling None keeps the model's (``stop_loss_scaling`` of its config, default 8), so that
