@@ -490,6 +490,21 @@ int ttsb_istft(const float* spec, int n_frames, void* workspace, int64_t workspa
  * NULL: first iteration); a /= |a| + 1e-16; projected_out = magnitude * a.  rebuilt / previous / projected_out are complex64. */
 int ttsb_griffinlim_update(const float* rebuilt, const float* previous, const float* magnitude, float momentum, int64_t n,
                            float* projected_out, void* stream);
+/* Griffin-Lim for a packed ragged batch of clips: librosa.griffinlim (0.7.1, "fast", momentum) of every clip, n_iter iterations
+ * plus the final iSTFT, with a number of launches that does not depend on n_clips (1 + 3 n_iter + 2).
+ *   Clip c owns frames frame_offsets[c] .. frame_offsets[c+1] - 1 of the packed arrays (frame_offsets: int32 (n_clips + 1) in
+ *   device memory, frame_offsets[0] = 0, frame_offsets[n_clips] = total_frames, every clip >= 4 frames -- the host checks this;
+ *   a malformed table gives wrong numbers, never an access outside the buffers).  Its waveform has 256 (T_c - 1) samples and
+ *   starts at sample 256 (frame_offsets[c] - c) of wav_out, so wav_out holds 256 (total_frames - n_clips) fp32 samples.
+ *   magnitude fp32 (total_frames, 513); init_angles complex64 (total_frames, 513) of unit modulus.
+ *   Each clip is transformed on its own: reflect padding at the clip's own edges, no overlap-add across clips, and a clip's
+ *   waveform does not depend, bit for bit, on the other clips of the batch or its position in it.
+ *   workspace: ttsb_griffinlim_batch_workspace_bytes(total_frames, n_clips) bytes of device memory, 16-byte aligned.
+ *   Needs n_clips >= 1, 4 n_clips <= total_frames <= 2097151, n_iter >= 0, momentum finite and >= 0. */
+int64_t ttsb_griffinlim_batch_workspace_bytes(int total_frames, int n_clips);   /* -1 for an invalid shape */
+int ttsb_griffinlim_batch(const float* magnitude, const float* init_angles, const int32_t* frame_offsets, int n_clips,
+                          int total_frames, int n_iter, float momentum, void* workspace, int64_t workspace_bytes,
+                          float* wav_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Data-parallel gradient exchange (BASELINE.json: "NCCL allreduce over NVLink on gradient buckets only"; the reference has

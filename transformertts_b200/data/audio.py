@@ -40,6 +40,28 @@ def slaney_mel_basis(sr: int, n_fft: int, n_mels: int, fmin: float, fmax: float)
     return basis.astype(np.float32)
 
 
+def _random_phase(shape, seed):
+    """exp(2 pi i u), u uniform from a fresh CPU generator (seeded when `seed` is given) -> complex64 CPU tensor."""
+    g = torch.Generator(device='cpu')
+    if seed is not None:
+        g.manual_seed(seed)
+    ph = 2 * np.pi * torch.rand(shape, generator=g, dtype=torch.float64)
+    return torch.polar(torch.ones_like(ph), ph).to(torch.complex64)
+
+
+def _clip_frame_counts(frame_offsets, total_frames: int) -> np.ndarray:
+    """Host check of a packed batch's frame offsets (n_clips + 1, from 0 to total_frames) -> frames per clip.  Griffin-Lim needs
+    at least 4 frames per clip: the STFT of a shorter clip's 256 (T - 1) samples has no room for the 512-sample reflect padding."""
+    off = np.asarray(frame_offsets.cpu() if torch.is_tensor(frame_offsets) else frame_offsets, dtype=np.int64)
+    if off.ndim != 1 or len(off) < 2 or off[0] != 0 or off[-1] != total_frames:
+        raise ValueError(f'frame offsets must run from 0 to {total_frames} over n_clips + 1 entries, got {off.tolist()}')
+    counts = np.diff(off)
+    for c, t in enumerate(counts):
+        if t < 4:
+            raise ValueError(f'clip {c} has {t} frames; Griffin-Lim needs at least 4 frames per clip')
+    return counts
+
+
 class Normalizer:
     code = -1
 
@@ -132,11 +154,7 @@ class Audio:
             dev = self.device
             T = S.shape[0]
             if init_angles is None:
-                g = torch.Generator(device='cpu')
-                if seed is not None:
-                    g.manual_seed(seed)
-                ph = 2 * np.pi * torch.rand(S.shape, generator=g, dtype=torch.float64)
-                init_angles = torch.polar(torch.ones_like(ph), ph).to(torch.complex64)
+                init_angles = _random_phase(tuple(S.shape), seed)
             proj = torch.view_as_real((S.to(torch.complex64) * init_angles.to(dev)).contiguous()).contiguous()
             ws = torch.empty(lib.istft_workspace_bytes(T) // 4, dtype=torch.float32, device=dev)
             wav = torch.empty(self.hop_length * (T - 1), dtype=torch.float32, device=dev)
@@ -158,6 +176,65 @@ class Audio:
         S = self.mel_to_linear_device(amp, nnls_iter)
         ia = None if init_angles is None else torch.as_tensor(np.ascontiguousarray(np.asarray(init_angles).T)).to(torch.complex64)
         return self.griffinlim_device(S, n_iter=n_iter, init_angles=ia, seed=seed).cpu().numpy()
+
+    def griffinlim_batch_device(self, S: torch.Tensor, frame_offsets, n_iter: int = 32, momentum: float = 0.99,
+                                init_angles: torch.Tensor = None, seeds=None) -> torch.Tensor:
+        """griffinlim_device for every clip of a packed batch in one pass (ttsb_griffinlim_batch, one launch per stage and
+        iteration whatever the number of clips).  S: magnitudes (F, 513) on the device, clip c in frames
+        frame_offsets[c] .. frame_offsets[c+1] - 1 -> packed waveform (256 (F - n_clips)); clip c starts at sample
+        256 (frame_offsets[c] - c).  init_angles: unit-modulus complex64 (F, 513); default: clip c draws its phase as
+        griffinlim_device(S_c, seed=seeds[c]) does (seeds=None: as griffinlim_device(S_c))."""
+        with torch.cuda.device(self.device):
+            dev = self.device
+            F = S.shape[0]
+            counts = _clip_frame_counts(frame_offsets, F)
+            n_clips = len(counts)
+            if init_angles is None:
+                if seeds is not None and len(seeds) != n_clips:
+                    raise ValueError(f'{len(seeds)} seeds for {n_clips} clips')
+                init_angles = torch.cat([_random_phase((int(t), S.shape[1]), None if seeds is None else seeds[c])
+                                         for c, t in enumerate(counts)])
+            init_angles = init_angles.to(device=dev, dtype=torch.complex64).contiguous()
+            off = torch.from_numpy(np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)).to(dev)
+            ws = torch.empty(lib.griffinlim_batch_workspace_bytes(F, n_clips) // 4, dtype=torch.float32, device=dev)
+            wav = torch.empty(self.hop_length * (F - n_clips), dtype=torch.float32, device=dev)
+            lib.griffinlim_batch(S.contiguous(), init_angles, off, n_iter, momentum, ws, wav)
+            return wav
+
+    def reconstruct_waveform_batch(self, mels, n_iter: int = 32, nnls_iter: int = 64, init_angles=None, seed: int = None) -> list:
+        """reconstruct_waveform for a list of normalised mels (n_mels, T_c) in one pass: one mel inversion over the frames of all
+        clips, one batched Griffin-Lim -> list of float32 waveforms (256 (T_c - 1)).  With seed=s, clip c gets the phase of
+        reconstruct_waveform(mels[c], seed=s + c); init_angles: a list of (513, T_c) arrays, as reconstruct_waveform takes."""
+        ms = [np.asarray(m, dtype=np.float32) for m in mels]
+        if not ms:
+            return []
+        for c, m in enumerate(ms):
+            if m.ndim != 2 or m.shape[1] < 4:
+                raise ValueError(f'mel {c} has shape {m.shape}; Griffin-Lim needs (n_mels, T) with T >= 4 frames')
+        counts = [m.shape[1] for m in ms]
+        amp = np.concatenate([self._denormalize(m).T.astype(np.float32) for m in ms])       # (F, n_mels)
+        S = self.mel_to_linear_device(torch.from_numpy(np.ascontiguousarray(amp)).to(self.device), nnls_iter)
+        ia = None
+        if init_angles is not None:
+            ia = torch.cat([torch.as_tensor(np.ascontiguousarray(np.asarray(a).T)).to(torch.complex64) for a in init_angles])
+        seeds = None if seed is None else [seed + c for c in range(len(ms))]
+        off = np.concatenate([[0], np.cumsum(counts)])
+        wav = self.griffinlim_batch_device(S, off, n_iter=n_iter, init_angles=ia, seeds=seeds).cpu().numpy()
+        starts = self.hop_length * (off[:-1] - np.arange(len(ms)))
+        return [wav[s:s + self.hop_length * (t - 1)] for s, t in zip(starts, counts)]
+
+    def save_wav(self, y: np.ndarray, wav_path):
+        """reference: data/audio.py:143-144 (soundfile.write(wav_path, y, sampling_rate): 16-bit PCM for .wav).  Samples are
+        scaled by 32767 and rounded to nearest as libsndfile does; samples beyond full scale are clipped to the int16 range
+        (libsndfile, without its clipping option, wraps them around)."""
+        import wave
+        x = np.asarray(y, dtype=np.float32).reshape(-1)
+        pcm = np.clip(np.rint(x * np.float32(32767)), -32768, 32767).astype('<i2')
+        with wave.open(str(wav_path), 'wb') as f:
+            f.setnchannels(1)
+            f.setsampwidth(2)
+            f.setframerate(int(self.sampling_rate))
+            f.writeframes(pcm.tobytes())
 
     def _denormalize(self, S):
         return self.normalizer.denormalize(S)

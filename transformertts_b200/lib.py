@@ -29,6 +29,7 @@ EXPORTS = [
     'ttsb_relu_bwd', 'ttsb_relu_bwd_colsum', 'ttsb_colsum_bf16', 'ttsb_colsum_bf16_x3', 'ttsb_cast_bf16_pad', 'ttsb_mae_loss', 'ttsb_scaled_ce_loss', 'ttsb_diag_loss', 'ttsb_diag_loss_train', 'ttsb_attention_scores', 'ttsb_durations_from_attention', 'ttsb_pitch_per_char', 'ttsb_expand_bwd', 'ttsb_embedding_bwd', 'ttsb_pe_scalar_bwd',
     'ttsb_pitch_embed_bwd', 'ttsb_statpred_head_bwd', 'ttsb_adam_tf_step', 'ttsb_embed_ln_pe_train_fwd',
     'ttsb_expand_ln_pe_train_fwd', 'ttsb_mel_to_linear', 'ttsb_stft_complex', 'ttsb_istft_workspace_bytes', 'ttsb_istft', 'ttsb_griffinlim_update',
+    'ttsb_griffinlim_batch_workspace_bytes', 'ttsb_griffinlim_batch',
     'ttsb_dp_unique_id', 'ttsb_dp_init', 'ttsb_dp_allreduce_bucket', 'ttsb_dp_destroy',
     'ttsb_decode_attn_workspace_bytes', 'ttsb_decode_attn', 'ttsb_decode_prologue', 'ttsb_decode_commit',
 ]
@@ -125,6 +126,7 @@ def load() -> C.CDLL:
     lib.ttsb_add_launch_count.restype = None
     lib.ttsb_add_launch_count.argtypes = [C.c_int64]
     lib.ttsb_istft_workspace_bytes.restype = C.c_int64
+    lib.ttsb_griffinlim_batch_workspace_bytes.restype = C.c_int64
     lib.ttsb_decode_attn_workspace_bytes.restype = C.c_int64
     for name in EXPORTS:
         if not hasattr(lib, name):
@@ -498,6 +500,22 @@ def istft_workspace_bytes(n_frames: int) -> int:
 def griffinlim_update(rebuilt, previous, magnitude, momentum, projected_out):
     _check(load().ttsb_griffinlim_update(ptr(rebuilt), ptr(previous), ptr(magnitude), C.c_float(momentum), C.c_int64(magnitude.numel()),
                                          ptr(projected_out), _stream()), 'ttsb_griffinlim_update')
+
+
+def griffinlim_batch_workspace_bytes(total_frames: int, n_clips: int) -> int:
+    n = int(load().ttsb_griffinlim_batch_workspace_bytes(int(total_frames), int(n_clips)))
+    if n < 0:
+        raise TtsbError(load().ttsb_last_error().decode())
+    return n
+
+
+def griffinlim_batch(magnitude, init_angles, frame_offsets, n_iter, momentum, workspace, wav_out):
+    """Griffin-Lim of every clip of a packed batch (include/ttsb.h: ttsb_griffinlim_batch).  magnitude fp32 (F, 513),
+    init_angles complex64 (F, 513), frame_offsets int32 (n_clips + 1) on the device, wav_out fp32 (256 (F - n_clips))."""
+    F = magnitude.shape[0]
+    _check(load().ttsb_griffinlim_batch(ptr(magnitude), ptr(init_angles), ptr(frame_offsets), frame_offsets.numel() - 1, F, int(n_iter),
+                                        C.c_float(momentum), ptr(workspace), C.c_int64(workspace.numel() * workspace.element_size()),
+                                        ptr(wav_out), _stream()), 'ttsb_griffinlim_batch')
 
 
 # ------------------------------------------------------------------------------------------------------------
