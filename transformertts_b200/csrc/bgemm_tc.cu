@@ -1,6 +1,5 @@
-// Batched / reduction GEMMs of the training step on wgmma (single-pass bf16, fp32 accumulate in registers).
-// Same pipeline as gemm_tc.cu (TMA producer warp -> 128B-swizzled smem ring -> two wgmma warpgroups -> accumulator image in
-// shared memory -> the same 8 warps as epilogue, one thread per output row), different tiling:
+// Batched / reduction GEMMs of the training step on wgmma (single-pass bf16, fp32 accumulate in registers), run on the
+// pipeline of gemm_pipeline.cuh (4-stage ring, one [128 x 64] A and one [<=256 x 64] B tile per stage):
 //
 //  mode BATCHED : out[z][m][n] = alpha * sum_k A_z[m][k] * B_z[n][k]        z = (batch row b, head h)
 //                 both operands come from activations (per-(b,h) B operand), e.g. S = Q K^T, O = P V, dP = dO V^T,
@@ -16,37 +15,17 @@
 // the same row-major tensors read MN-major.  An MN-major tile is fetched as ceil(rows/64) TMA boxes of [64 k x 64 mn]
 // (8 KiB each, 128B swizzle) and described to the MMA with LBO = 8192 B (next 64-wide MN block), SBO = 1024 B (next 8 k).
 #include <cuda_fp16.h>
-#include <stdlib.h>
 
 #include "../../include/ttsb.h"
-#include "ttsb_common.cuh"
-#include "wgmma_sm90.cuh"
-#include "ttsb_host.h"
+#include "gemm_pipeline.cuh"
 
 namespace ttsb {
 
-constexpr int BG_BM = 128;
-constexpr int BG_BK = 64;
-constexpr int BG_MAX_BN = 256;
-constexpr int BG_THREADS = 384;   // warps 0-7: two wgmma / epilogue warpgroups, warp 8: TMA producer (warps 9-11 idle: the
-                                   // producer warpgroup hands its registers to the others with setmaxnreg)
-constexpr int BG_STAGES = 4;
-constexpr int BG_NCH = BG_MAX_BN / 64;
-constexpr int BG_A_BYTES = BG_BM * BG_BK * 2;
-constexpr int BG_B_BYTES = BG_MAX_BN * BG_BK * 2;
-constexpr int BG_STAGE_BYTES = BG_A_BYTES + BG_B_BYTES;
-constexpr int BG_RING_BYTES = BG_STAGES * BG_STAGE_BYTES;
-// accumulator image [128 rows][BG_PITCH floats], written once the ring is drained, so it overlays the ring
-constexpr int BG_PITCH = acc_pitch(BG_MAX_BN);
-constexpr int BG_IMG_BYTES = BG_BM * BG_PITCH * 4;
-// bf16 outputs leave through shared staging boxes and TMA tile stores: 2 alternating boxes x 4 row quarters of
-// [32 rows x 64 cols] (4 KiB, 128B swizzle) -- see the staged epilogue below; they lie in the ring behind the image
-constexpr int BG_STAGE_OUT_OFFSET = (BG_IMG_BYTES + 1023) / 1024 * 1024;
-constexpr int BG_STAGE_OUT_BYTES = 2 * 4 * 4096;
-static_assert(BG_STAGE_OUT_OFFSET + BG_STAGE_OUT_BYTES <= BG_RING_BYTES, "image and staging must fit the ring");
-constexpr int BG_BAR_OFFSET = BG_RING_BYTES;
-constexpr int BG_SMEM_BYTES = BG_BAR_OFFSET + 256 + 1024;
-constexpr int BG_MN_BOX_BYTES = 64 * 128;  // one [64 k x 64 mn] box
+using BgRing = GemmRing<4, A_TILE_BYTES + B_TILE_BYTES>;
+constexpr int BG_PITCH = acc_pitch(GEMM_MAX_BN);
+constexpr int BG_STAGE_OUT_OFFSET = stage_out_offset(GEMM_MAX_BN);
+static_assert(BG_STAGE_OUT_OFFSET + STAGE_OUT_BYTES <= BgRing::kBytes, "image and staging must fit the ring");
+constexpr int BG_SMEM_BYTES = BgRing::kBytes + GEMM_RING_BAR_BYTES + 1024;  // + alignment slack
 
 struct BgOperand {
   int h_col;     // added to coordinate 0 (contiguous dim) per head
@@ -86,85 +65,68 @@ struct BgParams {
   int staged;  // 1: bf16 output through shared staging + TMA tile stores (batched mode, block_n % 64 == 0)
 };
 
-__global__ void __launch_bounds__(BG_THREADS, 1)
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                 const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO, const BgParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + BG_BAR_OFFSET);
-  uint64_t* empty_bar = full_bar + BG_STAGES;
-  uint64_t* img_free = empty_bar + BG_STAGES;   // the epilogue of the previous tile has released the ring / image
+  uint8_t* smem = align_smem_1024(smem_raw);
+  BgRing ring(smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA0);
     tma_prefetch_desc(&tmB);
-    for (int s = 0; s < BG_STAGES; ++s) {
-      mbar_init(full_bar + s, 1);
-      mbar_init(empty_bar + s, 8);
-    }
-    mbar_init(img_free, 1);
+    ring.init();
     fence_mbar_init();
   }
   __syncthreads();
   const bool a_mn = p.mode == 1 || p.opA.mn_major;
   const bool b_mn = p.mode == 1 || p.opB.mn_major;
   const int b_boxes = (p.block_n + 63) / 64;
-  const uint32_t stage_tx = (uint32_t)(BG_A_BYTES + (b_mn ? b_boxes * BG_MN_BOX_BYTES : p.block_n * BG_BK * 2));
-  const int t_chunks = (p.T + BG_BK - 1) / BG_BK;
+  const uint32_t stage_tx = (uint32_t)(A_TILE_BYTES + (b_mn ? b_boxes * MN_BOX_BYTES : p.block_n * GEMM_BK * 2));
+  const int t_chunks = (p.T + GEMM_BK - 1) / GEMM_BK;
 
   // number of k-blocks of a tile (uniform across roles)
   auto tile_kblocks = [&](int tile) -> int {
-    if (p.mode == 0) return (p.K + BG_BK - 1) / BG_BK;
+    if (p.mode == 0) return (p.K + GEMM_BK - 1) / GEMM_BK;
     const int split = tile % p.splits;
     const int b0 = split * p.b_per_split;
     const int nb = min(p.b_per_split, p.B - b0);
     return nb > 0 ? nb * t_chunks : 0;
   };
 
-  if (warp >= 8) {
+  if (warp >= GEMM_EPI_WARPS) {
     setmaxnreg_dec<40>();
-    if (warp > 8) goto done;
-    // ===================== TMA producer: warp-uniform control flow, the elected lane issues (see elect_one) ==========
+    if (warp > GEMM_EPI_WARPS) goto done;
+    // ===================== TMA producer =====================
     const bool leader = elect_one();
-    int stage = 0;
-    uint32_t phase = 0, img_phase = 0;
-    bool first = true;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       if (tile_kblocks(tile) == 0) continue;
-      if (!first) {   // the ring holds the previous tile's accumulator image until its epilogue is done
-        mbar_wait(img_free, img_phase);
-        img_phase ^= 1;
-      }
-      first = false;
+      ring.wait_image_free();
       if (p.mode == 0) {
         const int n_tile = tile % p.n_tiles;
         const int m_tile = (tile / p.n_tiles) % p.m_tiles;
         const int z = tile / (p.n_tiles * p.m_tiles);
         const int b = z / p.H, h = z % p.H;
-        const int m0 = m_tile * BG_BM, n0 = n_tile * p.block_n;
-        const int kbs = (p.K + BG_BK - 1) / BG_BK;
+        const int m0 = m_tile * GEMM_BM, n0 = n_tile * p.block_n;
+        const int kbs = (p.K + GEMM_BK - 1) / GEMM_BK;
         const int za = p.opA.z_batch ? z : b, zb = p.opB.z_batch ? z : b;
         for (int kb = 0; kb < kbs; ++kb) {
-          mbar_wait(empty_bar + stage, phase ^ 1);
-          uint8_t* st = smem + stage * BG_STAGE_BYTES;
-          if (leader) {
-            mbar_arrive_expect_tx(full_bar + stage, stage_tx);
+          ring.produce(leader, stage_tx, [&](uint64_t* bar, uint8_t* st) {
             if (a_mn) {
-              for (int i = 0; i < BG_BM / 64; ++i)
-                tma_load_3d(&tmA0, full_bar + stage, st + i * BG_MN_BOX_BYTES, m0 + 64 * i + h * p.opA.h_col, kb * BG_BK + h * p.opA.h_row, za);
+              for (int i = 0; i < GEMM_BM / 64; ++i)
+                tma_load_3d(&tmA0, bar, st + i * MN_BOX_BYTES, m0 + 64 * i + h * p.opA.h_col, kb * GEMM_BK + h * p.opA.h_row, za);
             } else {
-              tma_load_3d(&tmA0, full_bar + stage, st, kb * BG_BK + h * p.opA.h_col, m0 + h * p.opA.h_row, za);
+              tma_load_3d(&tmA0, bar, st, kb * GEMM_BK + h * p.opA.h_col, m0 + h * p.opA.h_row, za);
             }
             if (b_mn) {
               for (int i = 0; i < b_boxes; ++i)
-                tma_load_3d(&tmB, full_bar + stage, st + BG_A_BYTES + i * BG_MN_BOX_BYTES, n0 + 64 * i + h * p.opB.h_col,
-                            kb * BG_BK + h * p.opB.h_row, zb);
+                tma_load_3d(&tmB, bar, st + A_TILE_BYTES + i * MN_BOX_BYTES, n0 + 64 * i + h * p.opB.h_col,
+                            kb * GEMM_BK + h * p.opB.h_row, zb);
             } else {
-              tma_load_3d(&tmB, full_bar + stage, st + BG_A_BYTES, kb * BG_BK + h * p.opB.h_col, n0 + h * p.opB.h_row, zb);
+              tma_load_3d(&tmB, bar, st + A_TILE_BYTES, kb * GEMM_BK + h * p.opB.h_col, n0 + h * p.opB.h_row, zb);
             }
-          }
-          if (++stage == BG_STAGES) { stage = 0; phase ^= 1; }
+          });
         }
       } else {
         int r = tile;
@@ -173,22 +135,18 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
         const int m_tile = r % p.m_tiles; r /= p.m_tiles;
         const int seg = r;
         const CUtensorMap* mA = p.seg_src[seg] == 0 ? &tmA0 : &tmA1;
-        const int c0 = m_tile * BG_BM, n0 = n_tile * p.block_n;
+        const int c0 = m_tile * GEMM_BM, n0 = n_tile * p.block_n;
         const int b0 = split * p.b_per_split;
         const int b1 = min(b0 + p.b_per_split, p.B);
         const int shift = p.seg_shift[seg];
         for (int b = b0; b < b1; ++b) {
           for (int tc = 0; tc < t_chunks; ++tc) {
-            mbar_wait(empty_bar + stage, phase ^ 1);
-            uint8_t* st = smem + stage * BG_STAGE_BYTES;
-            if (leader) {
-              mbar_arrive_expect_tx(full_bar + stage, stage_tx);
-              for (int i = 0; i < BG_BM / 64; ++i)
-                tma_load_3d(mA, full_bar + stage, st + i * BG_MN_BOX_BYTES, c0 + 64 * i, tc * BG_BK + shift, b);
+            ring.produce(leader, stage_tx, [&](uint64_t* bar, uint8_t* st) {
+              for (int i = 0; i < GEMM_BM / 64; ++i)
+                tma_load_3d(mA, bar, st + i * MN_BOX_BYTES, c0 + 64 * i, tc * GEMM_BK + shift, b);
               for (int i = 0; i < b_boxes; ++i)
-                tma_load_3d(&tmB, full_bar + stage, st + BG_A_BYTES + i * BG_MN_BOX_BYTES, n0 + 64 * i, tc * BG_BK, b);
-            }
-            if (++stage == BG_STAGES) { stage = 0; phase ^= 1; }
+                tma_load_3d(&tmB, bar, st + A_TILE_BYTES + i * MN_BOX_BYTES, n0 + 64 * i, tc * GEMM_BK, b);
+            });
           }
         }
       }
@@ -202,8 +160,6 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
     const int row = quarter * 32 + lane;
     float* img = reinterpret_cast<float*>(smem);
     float* arow = img + (size_t)row * BG_PITCH;
-    int stage = 0;
-    uint32_t phase = 0;
     const int nch = p.block_n >> 4;
     const int ch_begin = half ? (nch + 1) >> 1 : 0;
     const int ch_end = half ? nch : (nch + 1) >> 1;
@@ -224,59 +180,34 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       const int kbs = tile_kblocks(tile);
       if (kbs == 0) continue;
-      float acc[BG_NCH][32];
-      int prev_stage = -1;
-      for (int kb = 0; kb < kbs; ++kb) {
-        mbar_wait(full_bar + stage, phase);
-        const uint32_t st = smem_u32(smem + stage * BG_STAGE_BYTES);
-        const uint64_t a = a_mn ? make_smem_desc_mn_sw128(st + wg * 8192, BG_MN_BOX_BYTES) : make_smem_desc_sw128(st + wg * 8192);
-        wgmma_fence();
+      float acc[GEMM_NCH][32];
+      ring.mma_tile(kbs, acc, [&](uint32_t st, int kb) {
+        const uint64_t a = a_mn ? make_smem_desc_mn_sw128(st + wg * 8192, MN_BOX_BYTES) : make_smem_desc_sw128(st + wg * 8192);
 #pragma unroll
-        for (int c = 0; c < BG_NCH; ++c) {
+        for (int c = 0; c < GEMM_NCH; ++c) {
           if (c < nmma) {
-            const uint32_t bs = st + BG_A_BYTES + c * 8192;
-            const uint64_t bd = b_mn ? make_smem_desc_mn_sw128(bs, BG_MN_BOX_BYTES) : make_smem_desc_sw128(bs);
+            const uint32_t bs = st + A_TILE_BYTES + c * 8192;
+            const uint64_t bd = b_mn ? make_smem_desc_mn_sw128(bs, MN_BOX_BYTES) : make_smem_desc_sw128(bs);
 #pragma unroll
-            for (int kk = 0; kk < BG_BK / 16; ++kk) mma(acc[c], a + a_step * kk, bd + b_step * kk, (kb | kk) != 0);
+            for (int kk = 0; kk < GEMM_BK / 16; ++kk) mma(acc[c], a + a_step * kk, bd + b_step * kk, (kb | kk) != 0);
           }
         }
-        wgmma_commit();
-        wgmma_wait<1>();   // the products of the previous k block have finished reading their stage: release it
-        if (prev_stage >= 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(empty_bar + prev_stage);
-        }
-        prev_stage = stage;
-        if (++stage == BG_STAGES) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-#pragma unroll
-      for (int c = 0; c < BG_NCH; ++c) wgmma_fence_regs(acc[c]);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty_bar + prev_stage);
-      asm volatile("bar.sync 5, 256;" ::: "memory");   // both warpgroups are done reading the ring: park the tile in it
-#pragma unroll
-      for (int c = 0; c < BG_NCH; ++c)
-        if (c < nmma) acc_store_fragment(img, BG_PITCH, wg * 64, c * 64, acc[c]);
-      asm volatile("bar.sync 5, 256;" ::: "memory");
+      });
+      park_tile(img, BG_PITCH, wg, nmma, acc);
       if (p.mode == 0) {
         const int n_tile = tile % p.n_tiles;
         const int m_tile = (tile / p.n_tiles) % p.m_tiles;
         const int z = tile / (p.n_tiles * p.m_tiles);
         const int b = z / p.H, h = z % p.H;
-        const int m = m_tile * BG_BM + row;
+        const int m = m_tile * GEMM_BM + row;
         const int n0 = n_tile * p.block_n;
         const bool row_ok = m < p.M;
         const bool row_keep = row_ok && (p.row_len == nullptr || m < __ldg(p.row_len + b));
         const int clen = p.col_len ? __ldg(p.col_len + b) : p.N;
         const size_t o = (size_t)(p.out_by_b ? b : z) * (size_t)p.out_z_stride + (size_t)(row_ok ? m : 0) * p.ld_out + h * p.out_h_col + n0;
         if (p.staged) {
-          // ---- bf16 output as TMA tile stores.  A thread owns one output ROW, so direct stores are 32-byte pieces of 32
-          //      different rows per warp instruction (request-rate bound).
-          //      The two warps of a lane quarter fill a [32 rows x 64 cols] 128B-swizzled box (warp `half` writes column
-          //      chunks 2*half, 2*half+1 of the slab) and one lane hands it to the TMA unit; two boxes alternate, so only
-          //      the store issued two slabs ago must have been read out.  Rows >= M / columns past the tensor are clipped
-          //      by the tensor map.  With sm_P set the value is the fused softmax backward of the row (see below).
+          // ---- bf16 output as TMA tile stores, one plane (staged_slab_begin / _end).  Rows >= M / columns past the tensor are clipped by
+          //      the tensor map.  With sm_P set the value is the fused softmax backward of the row (see below).
           uint8_t* stage_out = smem + BG_STAGE_OUT_OFFSET;
           const bool issuer = half == 0 && lane == 0;
           const int lrow = row & 31;
@@ -334,10 +265,7 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
             __syncwarp();
             acc_ld16(arow + (ca << 4), qa);
             acc_ld16(arow + (cb << 4), qb);
-            uint8_t* box = stage_out + ((slab_ctr & 1u) ? 4 * 4096 : 0) + quarter * 4096;
-            ++slab_ctr;
-            if (issuer) tma_store_wait_read_but_one();
-            asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
+            uint8_t* box = staged_slab_begin(stage_out, quarter, issuer, false, slab_ctr);
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
               const int c0 = (u ? cb : ca) << 4;
@@ -388,21 +316,13 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
                 }
               }
               uint32_t hh[8];
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const __nv_bfloat162 v = __floats2bfloat162_rn(y[2 * j], y[2 * j + 1]);
-                hh[j] = *reinterpret_cast<const uint32_t*>(&v);
-              }
-              const int k0 = 2 * (2 * half + u);
-              const uint32_t o0 = lrow * 128 + (((k0) ^ (lrow & 7)) << 4), o1 = lrow * 128 + (((k0 + 1) ^ (lrow & 7)) << 4);
-              st_shared_v4(box + o0, hh[0], hh[1], hh[2], hh[3]);
-              st_shared_v4(box + o1, hh[4], hh[5], hh[6], hh[7]);
+              pack_hi(y, hh);
+              st_box_chunk(box, lrow, 2 * (2 * half + u), hh);
             }
-            fence_proxy_async_smem();
-            asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
-            if (issuer && n0 + (s0 << 4) < p.out_cols)
-              tma_store_3d(&tmO, box, h * p.out_h_col + n0 + (s0 << 4), m_tile * BG_BM + quarter * 32, p.out_by_b ? b : z);
-            if (issuer) tma_store_commit();
+            staged_slab_end(quarter, issuer, [&] {
+              if (n0 + (s0 << 4) < p.out_cols)
+                tma_store_3d(&tmO, box, h * p.out_h_col + n0 + (s0 << 4), m_tile * GEMM_BM + quarter * 32, p.out_by_b ? b : z);
+            });
           }
         } else if (p.sm_P != nullptr) {
           // ---- softmax backward fused into the dP product (see ttsb_bgemm_args): this thread owns query row m of
@@ -462,11 +382,7 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
                       const float g = keep ? __uint_as_float(r[j]) * ks : 0.f;
                       y[j] = k < len ? p.sm_scale * __bfloat162float(pp[j]) * (g - dsum) : 0.f;
                     }
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                      const __nv_bfloat162 v = __floats2bfloat162_rn(y[2 * j], y[2 * j + 1]);
-                      hh[j] = *reinterpret_cast<const uint32_t*>(&v);
-                    }
+                    pack_hi(y, hh);
                   } else {
 #pragma unroll
                     for (int j = 0; j < 8; ++j) hh[j] = 0u;
@@ -494,11 +410,7 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
             }
             if (p.out_bf16) {
               uint32_t hh[8];
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const __nv_bfloat162 v = __floats2bfloat162_rn(y[2 * j], y[2 * j + 1]);
-                hh[j] = *reinterpret_cast<const uint32_t*>(&v);
-              }
+              pack_hi(y, hh);
               st_global_v8(p.out_bf16 + o + c0, hh);
             }
           }
@@ -508,7 +420,7 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
         const int n_tile = rr % p.n_tiles; rr /= p.n_tiles;
         const int m_tile = rr % p.m_tiles; rr /= p.m_tiles;
         const int seg = rr;
-        const int c = m_tile * BG_BM + row;
+        const int c = m_tile * GEMM_BM + row;
         const int n0 = n_tile * p.block_n;
         const bool row_ok = c < p.Cin;
         float* dst = p.dw + ((size_t)seg * p.Cin + (row_ok ? c : 0)) * p.N + n0;
@@ -531,33 +443,17 @@ bgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
           }
         }
       }
-      // the staging boxes and the image lie in the ring: TMA stores must have read them before the producer refills it
-      if (p.staged && half == 0 && lane == 0) tma_store_wait_read();
-      fence_proxy_async_smem();
-      asm volatile("bar.sync 5, 256;" ::: "memory");
-      if (threadIdx.x == 0) mbar_arrive(img_free);
+      ring.release_tile(p.staged && half == 0 && lane == 0);
     }
-    if (p.staged && half == 0 && lane == 0) tma_store_wait_all();  // staged boxes fully written out before exit
+    BgRing::finish(p.staged && half == 0 && lane == 0);
   }
 done:
   __syncthreads();
 }
 
-static int launch(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& o, const BgParams& p, cudaStream_t stream) {
-  static PerDevice<bool> attr_set;
-  if (!attr_set.get()) {
-    TTSB_CUDA_OK(cudaFuncSetAttribute(bgemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BG_SMEM_BYTES));
-    attr_set.get() = true;
-  }
-  const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
-  bgemm_tc_kernel<<<grid, BG_THREADS, BG_SMEM_BYTES, stream>>>(a0, a1, b, o, p);
-  count_launch();
-  return check_cuda(cudaGetLastError(), "bgemm_tc_kernel launch");
-}
-
 static int pick_block_n(int N) {
   const int n16 = (N + 15) / 16 * 16;
-  return n16 < BG_MAX_BN ? n16 : BG_MAX_BN;
+  return n16 < GEMM_MAX_BN ? n16 : GEMM_MAX_BN;
 }
 
 }  // namespace ttsb
@@ -597,28 +493,26 @@ extern "C" int ttsb_bgemm(const ttsb_bgemm_args* a, void* stream_v) {
   }
   p.block_n = pick_block_n(a->N);
   p.n_tiles = (a->N + p.block_n - 1) / p.block_n;
-  p.m_tiles = (a->M + BG_BM - 1) / BG_BM;
+  p.m_tiles = (a->M + GEMM_BM - 1) / GEMM_BM;
   p.num_tiles = p.Z * p.m_tiles * p.n_tiles;
   p.T = 1;
   CUtensorMap tmA, tmB;
   int rc = make_tmap_bf16_3d(&tmA, a->a, (uint64_t)a->a_dim0, (uint64_t)a->a_dim1, (uint64_t)a->a_dim2, (uint64_t)a->a_stride1,
-                             (uint64_t)a->a_stride2, BG_BK, a->a_mn_major ? 64 : BG_BM);
+                             (uint64_t)a->a_stride2, GEMM_BK, a->a_mn_major ? 64 : GEMM_BM);
   if (rc) return rc;
   rc = make_tmap_bf16_3d(&tmB, a->b, (uint64_t)a->b_dim0, (uint64_t)a->b_dim1, (uint64_t)a->b_dim2, (uint64_t)a->b_stride1,
-                         (uint64_t)a->b_stride2, BG_BK, a->b_mn_major ? 64 : p.block_n);
+                         (uint64_t)a->b_stride2, GEMM_BK, a->b_mn_major ? 64 : p.block_n);
   if (rc) return rc;
   // bf16-only outputs of a tile width that fills whole 64-column boxes go through shared staging + TMA tile stores
-  // (TTSB_NO_STAGED_STORE=1 keeps the direct thread-per-row stores)
-  static const bool no_staged = getenv("TTSB_NO_STAGED_STORE") != nullptr;
   CUtensorMap tmO = tmB;
-  if (!no_staged && p.out_bf16 && !p.out_f32 && p.block_n % 64 == 0 && (reinterpret_cast<uintptr_t>(p.out_bf16) & 15) == 0) {
+  if (p.out_bf16 && !p.out_f32 && p.block_n % 64 == 0 && (reinterpret_cast<uintptr_t>(p.out_bf16) & 15) == 0) {
     const uint64_t cols = p.out_by_b ? (uint64_t)p.H * p.out_h_col : (uint64_t)p.out_cols;
     rc = make_tmap_bf16_3d(&tmO, p.out_bf16, cols, (uint64_t)p.M, (uint64_t)(p.out_by_b ? a->B : p.Z), (uint64_t)p.ld_out,
                            (uint64_t)p.out_z_stride, 64, 32);
     if (rc) return rc;
     p.staged = 1;
   }
-  return launch(tmA, tmA, tmB, tmO, p, stream);
+  return launch_pipeline<bgemm_tc_kernel>(BG_SMEM_BYTES, p.num_tiles, false, stream, "bgemm_tc_kernel launch", tmA, tmA, tmB, tmO, p);
 }
 
 extern "C" int ttsb_wgrad(const ttsb_wgrad_args* a, void* stream_v) {
@@ -643,7 +537,7 @@ extern "C" int ttsb_wgrad(const ttsb_wgrad_args* a, void* stream_v) {
   p.dw = a->dw;
   p.block_n = pick_block_n(a->N);
   p.n_tiles = (a->N + p.block_n - 1) / p.block_n;
-  p.m_tiles = (a->Cin + BG_BM - 1) / BG_BM;
+  p.m_tiles = (a->Cin + GEMM_BM - 1) / GEMM_BM;
   const int base_tiles = a->num_segments * p.m_tiles * p.n_tiles;
   int splits = (2 * num_sms() + base_tiles - 1) / base_tiles;
   if (splits > a->B) splits = a->B;
@@ -655,12 +549,12 @@ extern "C" int ttsb_wgrad(const ttsb_wgrad_args* a, void* stream_v) {
   for (int i = 0; i < 2; ++i) {
     const int use = a->x[i] ? i : 0;
     int rc = make_tmap_bf16_3d(&tmA[i], a->x[use], (uint64_t)a->Cin, (uint64_t)a->T, (uint64_t)a->B, (uint64_t)a->ldx[use],
-                               (uint64_t)a->ldx[use] * a->T, BG_BK, 64);
+                               (uint64_t)a->ldx[use] * a->T, GEMM_BK, 64);
     if (rc) return rc;
   }
-  int rc = make_tmap_bf16_3d(&tmB, a->g, (uint64_t)a->N, (uint64_t)a->T, (uint64_t)a->B, (uint64_t)a->ldg, (uint64_t)a->ldg * a->T, BG_BK, 64);
+  int rc = make_tmap_bf16_3d(&tmB, a->g, (uint64_t)a->N, (uint64_t)a->T, (uint64_t)a->B, (uint64_t)a->ldg, (uint64_t)a->ldg * a->T, GEMM_BK, 64);
   if (rc) return rc;
-  return launch(tmA[0], tmA[1], tmB, tmB, p, stream);
+  return launch_pipeline<bgemm_tc_kernel>(BG_SMEM_BYTES, p.num_tiles, false, stream, "bgemm_tc_kernel launch", tmA[0], tmA[1], tmB, tmB, p);
 }
 
 TTSB_DEFINE_SALT_SETTER(set_salt_bgemm)

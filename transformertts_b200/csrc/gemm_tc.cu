@@ -1,38 +1,19 @@
-// Tensor-core GEMM family for the ForwardTransformer blocks (Dense / concat-projection / Conv1D 'same'):
-// persistent warp-specialised wgmma kernel -- one TMA producer warp (3-D maps over (C,T,B), OOB rows = 'same' zero
-// padding) -> 128B-swizzled shared-memory ring -> two consumer warpgroups, each issuing wgmma (bf16 operands, fp32
-// accumulators in registers) for 64 of the tile's 128 rows.  The finished tile is parked in shared memory (accumulator
-// image, overlaying the drained ring) and the same eight warps run the epilogue one thread per output row, fusing bias /
-// ReLU / residual / LayerNorm / row mask and writing fp32 + bf16 hi/lo (or fp16) copies for the next GEMM / the
-// attention kernel.
+// Tensor-core GEMM family for the ForwardTransformer blocks (Dense / concat-projection / Conv1D 'same') on the pipeline of
+// gemm_pipeline.cuh: the producer reads activations through 3-D maps over (C,T,B) (OOB rows = 'same' zero padding), and
+// the thread-per-row epilogue fuses bias / ReLU / residual / LayerNorm / row mask and writes fp32 + bf16 hi/lo (or fp16)
+// copies for the next GEMM / the attention kernel.
 //
 // Replaces, in the reference (TF2/Keras ops): model/layers.py:134-136,149 (q/k/v + concat projection),
 // :93-94 (FFN), :19-26,36-40 (Conv1D stack + residual LayerNorm), :498-524 (predictor convs), model/models.py:422.
 //
 // Precision modes: TTSB_PREC_BF16 (one product) and TTSB_PREC_BF16X3 (A_hi*W_hi + A_lo*W_hi + A_hi*W_lo), the
 // latter gives fp32-class products (needed for the 1e-3 mel parity gate) at 3x the tensor-core work.
-#include <stdarg.h>
-#include <stdio.h>
-#include <stdlib.h>
-
-#include "../../include/ttsb.h"
 #include <cuda_fp16.h>
 
-#include "ttsb_common.cuh"
-#include "wgmma_sm90.cuh"
-#include "ttsb_host.h"
+#include "../../include/ttsb.h"
+#include "gemm_pipeline.cuh"
 
 namespace ttsb {
-
-constexpr int GEMM_BM = 128;
-constexpr int GEMM_BK = 64;
-constexpr int GEMM_MAX_BN = 256;
-constexpr int GEMM_THREADS = 384;  // warps 0-7: two wgmma / epilogue warpgroups, warp 8: TMA producer (warps 9-11 idle: the
-                                   // producer warpgroup hands its registers to the others with setmaxnreg)
-constexpr int GEMM_EPI_WARPS = 8;
-constexpr int A_TILE_BYTES = GEMM_BM * GEMM_BK * 2;      // 16 KiB
-constexpr int B_TILE_BYTES = GEMM_MAX_BN * GEMM_BK * 2;  // 32 KiB
-constexpr int GEMM_NCH = GEMM_MAX_BN / 64;               // wgmma n64 products per k step (the tile width rounded up to 64)
 
 struct GemmKParams {
   int B, T, N, block_n, n_tiles, tiles_per_row, num_tiles;
@@ -69,17 +50,13 @@ struct GemmCfg {
   static constexpr int kStages = kSplit ? 2 : 4;
   static constexpr int kBTile = kPair ? PAIR_MAX_BN * GEMM_BK * 2 : B_TILE_BYTES;
   static constexpr int kStageBytes = (kSplit ? 2 : 1) * (A_TILE_BYTES + kBTile);
-  static constexpr int kRingBytes = kStages * kStageBytes;
-  // accumulator image [128 rows][kPitch floats]: written once the ring is drained, so it overlays the ring
-  static constexpr int kPitch = acc_pitch(kPair ? PAIR_MAX_BN : GEMM_MAX_BN);
-  static constexpr int kImgBytes = GEMM_BM * kPitch * 4;
-  // plain (non-LayerNorm) epilogue: two planes x four row quarters of [32 rows x 64 cols] 16-bit staging boxes (4 KB each,
-  // 128B-swizzled) for TMA tile stores, in the ring behind the image
-  static constexpr int kStageOutOffset = (kImgBytes + 1023) / 1024 * 1024;
-  static constexpr int kStageOutBytes = 2 * 4 * 4096;
-  static_assert(kImgBytes <= kRingBytes && (kPair || kStageOutOffset + kStageOutBytes <= kRingBytes), "image must fit the ring");
-  static constexpr int kBarOffset = kRingBytes;
-  static constexpr int kRedOffset = kBarOffset + 256;           // [2][2][128] floats of intra-CTA exchange
+  using Ring = GemmRing<kStages, kStageBytes>;
+  static constexpr int kMaxBn = kPair ? PAIR_MAX_BN : GEMM_MAX_BN;
+  static constexpr int kPitch = acc_pitch(kMaxBn);
+  // the plain (non-LayerNorm) epilogue stages two planes; pair mode is LayerNorm-only
+  static constexpr int kStageOutOffset = stage_out_offset(kMaxBn);
+  static_assert(img_bytes(kMaxBn) <= Ring::kBytes && (kPair || kStageOutOffset + STAGE_OUT_BYTES <= Ring::kBytes), "image must fit the ring");
+  static constexpr int kRedOffset = Ring::kBytes + GEMM_RING_BAR_BYTES;  // [2][2][128] floats of intra-CTA exchange
   static constexpr int kXchgOffset = kRedOffset + 2048;         // pair mode: [2 slots][128] float2 written by the peer CTA
   static constexpr int kXbarOffset = kXchgOffset + 2048;        // pair mode: 2 mbarriers
   static constexpr int kSmemBytes = kXbarOffset + 64 + 1024;    // + alignment slack
@@ -133,23 +110,6 @@ __device__ __forceinline__ void ldg16(const float* __restrict__ p, float (&v)[16
   }
 }
 
-// bf16 hi (and lo = bf16(y - hi)) of 16 floats, packed pairwise with cvt.rn.bf16x2
-__device__ __forceinline__ void pack_hi_lo(const float (&y)[16], uint32_t (&h)[8], uint32_t (&l)[8], bool want_lo) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const __nv_bfloat162 hh = __floats2bfloat162_rn(y[2 * j], y[2 * j + 1]);
-    h[j] = *reinterpret_cast<const uint32_t*>(&hh);
-  }
-  if (want_lo) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float f0 = __uint_as_float(h[j] << 16), f1 = __uint_as_float(h[j] & 0xffff0000u);
-      const __nv_bfloat162 ll = __floats2bfloat162_rn(y[2 * j] - f0, y[2 * j + 1] - f1);
-      l[j] = *reinterpret_cast<const uint32_t*>(&ll);
-    }
-  }
-}
-
 __device__ __forceinline__ void store_chunk(const GemmKParams& p, size_t orow, int col0, const float (&y)[16]) {
   const size_t o = orow * (size_t)p.ld_out + col0;
   if (p.out_f32) {
@@ -191,7 +151,7 @@ __device__ __forceinline__ void apply_dropout16(float (&y)[16], float p, uint32_
 // exchange of per-row partial sums between the two warps that share a lane quarter
 __device__ __forceinline__ float pair_sum(float part, float* red, int half, int row, int quarter) {
   red[half * GEMM_BM + row] = part;
-  asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
+  quarter_sync(quarter);
   return part + red[(half ^ 1) * GEMM_BM + row];
 }
 
@@ -223,29 +183,18 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
 
   if constexpr (!kLN) {
     if (p.staged) {
-      // 16-bit outputs as TMA tile stores.  A thread owns one output ROW, so direct stores are 32-byte pieces of 32
-      // different rows per warp instruction (request-rate bound).  Here the two warps of a lane quarter fill a [32 rows x 64 cols] 128B-swizzled box per plane and one lane hands
-      // it to the TMA unit (full 128-byte lines, asynchronous, rows >= T and columns >= N clipped by the tensor map).
-      uint8_t* box_a = stage_out + quarter * 4096;
-      uint8_t* box_b = stage_out + 4 * 4096 + quarter * 4096;
+      // 16-bit outputs as TMA tile stores (staged_slab_begin / _end); rows >= T and columns >= N are clipped by the tensor map
       const bool issuer = half == 0 && (threadIdx.x & 31) == 0;
       const int lrow = row & 31;
       const bool two = p.out_lo != nullptr && !p.h16;
+      uint8_t* box_lo = staged_slab_lo_box(stage_out, quarter);
       uint32_t qa[16], qb[16];
       for (int s0 = 0; s0 < nch; s0 += 4) {   // 64-column slab: this warp handles chunks s0 + 2*half, +1
         const int ca = s0 + 2 * half, cb = ca + 1;
         __syncwarp();
         acc_ld16(arow + (ca << 4), qa);
         acc_ld16(arow + (cb << 4), qb);
-        // two planes: box_a = hi, box_b = lo, reused every slab; one plane: the two boxes alternate, so only the store
-        // issued two slabs ago has to have been read out
-        uint8_t* box_hi = two ? box_a : ((slab_ctr & 1u) ? box_b : box_a);
-        uint8_t* box_lo = box_b;
-        ++slab_ctr;
-        if (issuer) {
-          if (two) tma_store_wait_read(); else tma_store_wait_read_but_one();
-        }
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
+        uint8_t* box_hi = staged_slab_begin(stage_out, quarter, issuer, two, slab_ctr);
 #pragma unroll
         for (int u = 0; u < 2; ++u) {
           const int c0 = (u ? cb : ca) << 4;
@@ -279,23 +228,13 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
           } else {
             pack_hi_lo(y, h, l, two);
           }
-          // 16-byte chunk ids of this 16-column chunk inside the 128-byte box row: 2*(2*half+u), +1; swizzle ^= row & 7
-          const int k0 = 2 * (2 * half + u);
-          const uint32_t o0 = lrow * 128 + (((k0) ^ (lrow & 7)) << 4), o1 = lrow * 128 + (((k0 + 1) ^ (lrow & 7)) << 4);
-          st_shared_v4(box_hi + o0, h[0], h[1], h[2], h[3]);
-          st_shared_v4(box_hi + o1, h[4], h[5], h[6], h[7]);
-          if (two) {
-            st_shared_v4(box_lo + o0, l[0], l[1], l[2], l[3]);
-            st_shared_v4(box_lo + o1, l[4], l[5], l[6], l[7]);
-          }
+          st_box_chunk(box_hi, lrow, 2 * (2 * half + u), h);
+          if (two) st_box_chunk(box_lo, lrow, 2 * (2 * half + u), l);
         }
-        fence_proxy_async_smem();
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
-        if (issuer) {
+        staged_slab_end(quarter, issuer, [&] {
           tma_store_3d(tmOh, box_hi, n0 + (s0 << 4), t0 + quarter * 32, b);
           if (two) tma_store_3d(tmOl, box_lo, n0 + (s0 << 4), t0 + quarter * 32, b);
-          tma_store_commit();
-        }
+        });
       }
       return;
     }
@@ -450,7 +389,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
   float* red_m2 = red + 2 * GEMM_BM;
   red[half * GEMM_BM + row] = mean_h;
   red_m2[half * GEMM_BM + row] = m2_h;
-  asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
+  quarter_sync(quarter);
   const float mean_o = red[(half ^ 1) * GEMM_BM + row], m2_o = red_m2[(half ^ 1) * GEMM_BM + row];
   const float n_a = half == 0 ? nf : (float)(ncols - n_mine), n_b = (float)ncols - n_a;
   const float mean_a = half == 0 ? mean_h : mean_o, mean_b = half == 0 ? mean_o : mean_h;
@@ -521,10 +460,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
                const __grid_constant__ CUtensorMap tmOh, const __grid_constant__ CUtensorMap tmOl, const GemmKParams p) {
   using Cfg = GemmCfg<kSplit, kPair>;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kBarOffset);
-  uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* img_free = empty_bar + Cfg::kStages;   // the epilogue of the previous tile has released the ring / image
+  uint8_t* smem = align_smem_1024(smem_raw);
+  typename Cfg::Ring ring(smem);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -537,11 +474,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA0h);
     tma_prefetch_desc(&tmWh);
-    for (int s = 0; s < Cfg::kStages; ++s) {
-      mbar_init(full_bar + s, 1);
-      mbar_init(empty_bar + s, GEMM_EPI_WARPS);
-    }
-    mbar_init(img_free, 1);
+    ring.init();
     for (int s = 0; s < 2; ++s)
       if (kPair) mbar_init(xbar + s, GEMM_EPI_WARPS);  // one arrival per epilogue warp of the PEER CTA
     fence_mbar_init();
@@ -554,40 +487,29 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
   if (warp >= GEMM_EPI_WARPS) {
     setmaxnreg_dec<40>();
     if (warp > GEMM_EPI_WARPS) goto done;
-    // ===================== TMA producer: warp-uniform control flow, the elected lane issues (see elect_one) ==========
+    // ===================== TMA producer =====================
     const bool leader = elect_one();
-    int stage = 0;
-    uint32_t phase = 0, img_phase = 0;
-    bool first = true;
     for (int tile = p.tile_begin + work_id; tile < p.num_tiles; tile += work_stride) {
       const int n_tile = kPair ? cta_rank : tile % p.n_tiles;
       const int m_tile = kPair ? tile : tile / p.n_tiles;
       const int b = m_tile / p.tiles_per_row;
       const int t0 = (m_tile % p.tiles_per_row) * GEMM_BM;
       const int n0 = n_tile * p.block_n;
-      if (!first) {   // the ring holds the previous tile's accumulator image until its epilogue is done
-        mbar_wait(img_free, img_phase);
-        img_phase ^= 1;
-      }
-      first = false;
+      ring.wait_image_free();
       int kglob = 0;
       for (int s = 0; s < p.num_seg; ++s) {
         const CUtensorMap* mh = p.seg_src[s] == 0 ? &tmA0h : &tmA1h;
         const CUtensorMap* ml = p.seg_src[s] == 0 ? &tmA0l : &tmA1l;
         for (int kb = 0; kb < p.seg_kblocks[s]; ++kb, ++kglob) {
-          mbar_wait(empty_bar + stage, phase ^ 1);
-          uint8_t* st = smem + stage * Cfg::kStageBytes;
-          if (leader) {
-            mbar_arrive_expect_tx(full_bar + stage, stage_tx);
-            tma_load_3d(mh, full_bar + stage, st, kb * GEMM_BK, t0 + p.seg_shift[s], b);
-            tma_load_2d(&tmWh, full_bar + stage, st + A_TILE_BYTES, kglob * GEMM_BK, n0);
+          ring.produce(leader, stage_tx, [&](uint64_t* bar, uint8_t* st) {
+            tma_load_3d(mh, bar, st, kb * GEMM_BK, t0 + p.seg_shift[s], b);
+            tma_load_2d(&tmWh, bar, st + A_TILE_BYTES, kglob * GEMM_BK, n0);
             if (kSplit) {
               uint8_t* st2 = st + A_TILE_BYTES + Cfg::kBTile;
-              tma_load_3d(ml, full_bar + stage, st2, kb * GEMM_BK, t0 + p.seg_shift[s], b);
-              tma_load_2d(&tmWl, full_bar + stage, st2 + A_TILE_BYTES, kglob * GEMM_BK, n0);
+              tma_load_3d(ml, bar, st2, kb * GEMM_BK, t0 + p.seg_shift[s], b);
+              tma_load_2d(&tmWl, bar, st2 + A_TILE_BYTES, kglob * GEMM_BK, n0);
             }
-          }
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+          });
         }
       }
     }
@@ -599,8 +521,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
     const int half = warp >> 2;          // epilogue: which half of the tile's column chunks
     float* red_all = reinterpret_cast<float*>(smem + Cfg::kRedOffset);
     float* img = reinterpret_cast<float*>(smem);
-    int stage = 0;
-    uint32_t phase = 0;
     int iter = 0;
     float2* xslots = reinterpret_cast<float2*>(smem + Cfg::kXchgOffset);
     uint32_t slab_ctr = 0;  // staged epilogue: slabs stored so far (selects the staging box of single-plane outputs)
@@ -613,13 +533,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
       const int b = m_tile / p.tiles_per_row;
       const int t0 = (m_tile % p.tiles_per_row) * GEMM_BM;
       float acc[GEMM_NCH][32];
-      int prev_stage = -1;
-      for (int kb = 0; kb < total_kb; ++kb) {
-        mbar_wait(full_bar + stage, phase);
-        const uint32_t st = smem_u32(smem + stage * Cfg::kStageBytes);
+      ring.mma_tile(total_kb, acc, [&](uint32_t st, int kb) {
         const uint32_t a_hi = st + wg * (64 * 128);
         const uint32_t b_hi = st + A_TILE_BYTES;
-        wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
           const uint64_t da = make_smem_desc_sw128(a_hi) + 2 * kk;
@@ -642,29 +558,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
             }
           }
         }
-        wgmma_commit();
-        // the products of the previous k block have finished reading their stage: release it
-        wgmma_wait<1>();
-        if (prev_stage >= 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(empty_bar + prev_stage);
-        }
-        prev_stage = stage;
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-#pragma unroll
-      for (int c = 0; c < GEMM_NCH; ++c) wgmma_fence_regs(acc[c]);
-      if (prev_stage >= 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty_bar + prev_stage);
-      }
-      // both warpgroups are done reading the ring: park the tile in it
-      asm volatile("bar.sync 5, 256;" ::: "memory");
-#pragma unroll
-      for (int c = 0; c < GEMM_NCH; ++c)
-        if (c < nch) acc_store_fragment(img, Cfg::kPitch, wg * 64, c * 64, acc[c]);
-      asm volatile("bar.sync 5, 256;" ::: "memory");
+      });
+      park_tile(img, Cfg::kPitch, wg, nch, acc);
       PairCtx px{};
       if (kPair) {
         const int slot = iter & 1;
@@ -678,13 +573,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
       const int row = quarter * 32 + lane;
       epilogue_tile<kLN>(p, img + (size_t)row * Cfg::kPitch, b, t0, n_tile * p.block_n, row, half, quarter, red_all, px,
                          smem + Cfg::kStageOutOffset, &tmOh, &tmOl, slab_ctr);
-      // the staging boxes and the image lie in the ring: TMA stores must have read them before the producer refills it
-      if (!kLN && p.staged && half == 0 && lane == 0) tma_store_wait_read();
-      fence_proxy_async_smem();
-      asm volatile("bar.sync 5, 256;" ::: "memory");
-      if (threadIdx.x == 0) mbar_arrive(img_free);
+      ring.release_tile(!kLN && p.staged && half == 0 && lane == 0);
     }
-    if (!kLN && p.staged && half == 0 && lane == 0) tma_store_wait_all();  // staged boxes fully written out before exit
+    Cfg::Ring::finish(!kLN && p.staged && half == 0 && lane == 0);
   }
 done:
   __syncthreads();
@@ -778,6 +669,14 @@ __global__ void gemm_simt_kernel(const GemmKParams p, const GemmSimtPtrs q) {
 // ----------------------------------------------------------------------------------------------------
 // host
 // ----------------------------------------------------------------------------------------------------
+template <bool kSplit, bool kPair, bool kLN>
+static int launch_tc(const CUtensorMap (&tmA)[2][2], const CUtensorMap (&tmW)[2], const CUtensorMap (&tmO)[2], const GemmKParams& q,
+                     int work, cudaStream_t stream) {
+  return launch_pipeline<gemm_tc_kernel<kSplit, kPair, kLN>>(GemmCfg<kSplit, kPair>::kSmemBytes, work, kPair, stream,
+                                                             kPair ? "gemm_tc_kernel<pair> launch" : "gemm_tc_kernel launch", tmA[0][0], tmA[0][1], tmA[1][0],
+                                                             tmA[1][1], tmW[0], tmW[1], tmO[0], tmO[1], q);
+}
+
 static int validate(const ttsb_gemm_args* a, int* k_total_out) {
   if (!a) { set_last_error("ttsb_linear_fwd: args is NULL"); return TTSB_ERR_INVALID_ARGUMENT; }
   if (a->B <= 0 || a->T <= 0 || a->N <= 0) { set_last_error("ttsb_linear_fwd: B,T,N must be positive"); return TTSB_ERR_INVALID_ARGUMENT; }
@@ -832,14 +731,13 @@ extern "C" int ttsb_linear_fwd(const ttsb_gemm_args* a, void* stream_v) {
   // LayerNorm GEMMs whose row splits into two equal halves can run as CTA pairs (see GemmCfg): a pair finishes a 128-row
   // tile in ~0.57 of the single-CTA time, so work is handed out at half-tile granularity.  The schedule with the fewest
   // (weighted) rounds wins: all single-CTA tiles, all pairs, or full waves of single-CTA tiles followed by a pair-mode
-  // tail (two launches).  TTSB_NO_PAIR=1 forces single-CTA tiles where the row fits one accumulator.
-  static const bool no_pair = getenv("TTSB_NO_PAIR") != nullptr;
+  // tail (two launches).
   const bool pair_ok = a->impl != TTSB_IMPL_SIMT && a->ln_gamma != nullptr && p.n_tiles == 1 && a->N == a->block_n &&
                        a->N % 32 == 0 && a->N / 2 <= PAIR_MAX_BN && a->N >= 64;
   const bool single_ok = a->block_n <= GEMM_MAX_BN;
   bool pair = false;
   int hybrid_full = 0;  // > 0: tiles [0, hybrid_full) single-CTA, the rest as pairs
-  if (pair_ok && !(no_pair && single_ok)) {
+  if (pair_ok) {
     const int t = a->B * p.tiles_per_row, sms = num_sms(), clusters = sms / 2;
     const float kPairCost = 0.57f;
     const float c_single = single_ok ? (float)((t + sms - 1) / sms) : 1e30f;
@@ -929,11 +827,10 @@ extern "C" int ttsb_linear_fwd(const ttsb_gemm_args* a, void* stream_v) {
       int rc2 = make_tmap_bf16_2d(&tmW[h], base, k_total, as_pair ? a->N : q.n_tiles * q.block_n, (uint64_t)k_total, GEMM_BK, q.block_n);
       if (rc2) return rc2;
     }
-    // plain epilogue with 16-bit outputs only: tile stores through shared memory (TTSB_NO_STAGED_STORE=1 keeps direct stores)
-    static const bool no_staged = getenv("TTSB_NO_STAGED_STORE") != nullptr;
+    // plain epilogue with 16-bit outputs only: tile stores through shared memory
     CUtensorMap tmO[2] = {tmW[0], tmW[1]};  // placeholders when the staged path is off
     q.staged = 0;
-    if (!no_staged && !as_pair && q.gamma == nullptr && q.out_hi != nullptr && q.out_f32 == nullptr && q.out_preln == nullptr &&
+    if (!as_pair && q.gamma == nullptr && q.out_hi != nullptr && q.out_f32 == nullptr && q.out_preln == nullptr &&
         q.residual == nullptr && q.block_n % 64 == 0 && q.ld_out % 8 == 0) {
       const int width = q.n_tiles * q.block_n;
       int rc3 = make_tmap_bf16_3d(&tmO[0], q.out_hi, (uint64_t)width, (uint64_t)a->T, (uint64_t)a->B, (uint64_t)q.ld_out,
@@ -946,59 +843,12 @@ extern "C" int ttsb_linear_fwd(const ttsb_gemm_args* a, void* stream_v) {
       }
       q.staged = 1;
     }
-    if (as_pair) {
-      // cluster of two CTAs per 128-row tile; grid = 2 x min(tiles, SMs/2)
-      const int pairs = work < num_sms() / 2 ? work : num_sms() / 2;
-      cudaLaunchConfig_t cfg{};
-      cfg.gridDim = dim3(2 * pairs);
-      cfg.blockDim = dim3(GEMM_THREADS);
-      cfg.stream = stream;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = 2;
-      attr[0].val.clusterDim.y = 1;
-      attr[0].val.clusterDim.z = 1;
-      cfg.attrs = attr;
-      cfg.numAttrs = 1;
-      if (split) {
-        static PerDevice<bool> attr_set;
-        if (!attr_set.get()) {
-          TTSB_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<true, true>::kSmemBytes));
-          attr_set.get() = true;
-        }
-        cfg.dynamicSmemBytes = GemmCfg<true, true>::kSmemBytes;
-        TTSB_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<true, true, true>, tmA[0][0], tmA[0][1], tmA[1][0], tmA[1][1], tmW[0], tmW[1], tmO[0], tmO[1], q));
-      } else {
-        static PerDevice<bool> attr_set;
-        if (!attr_set.get()) {
-          TTSB_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<false, true>::kSmemBytes));
-          attr_set.get() = true;
-        }
-        cfg.dynamicSmemBytes = GemmCfg<false, true>::kSmemBytes;
-        TTSB_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<false, true, true>, tmA[0][0], tmA[0][1], tmA[1][0], tmA[1][1], tmW[0], tmW[1], tmO[0], tmO[1], q));
-      }
-      count_launch();
-      return check_cuda(cudaGetLastError(), "gemm_tc_kernel<pair> launch");
-    }
-    const int grid = work < num_sms() ? work : num_sms();
-    const bool ln = q.gamma != nullptr;
-#define TTSB_GEMM_LAUNCH(SPLIT, LN)                                                                                                  \
-  do {                                                                                                                               \
-    static PerDevice<bool> attr_set;                                                                                                    \
-    if (!attr_set.get()) {                                                                                                                 \
-      TTSB_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<SPLIT, false, LN>, cudaFuncAttributeMaxDynamicSharedMemorySize,                \
-                                        GemmCfg<SPLIT, false>::kSmemBytes));                                                         \
-      attr_set.get() = true;                                                                                                               \
-    }                                                                                                                                \
-    gemm_tc_kernel<SPLIT, false, LN><<<grid, GEMM_THREADS, GemmCfg<SPLIT, false>::kSmemBytes, stream>>>(                               \
-        tmA[0][0], tmA[0][1], tmA[1][0], tmA[1][1], tmW[0], tmW[1], tmO[0], tmO[1], q);                                                              \
-  } while (0)
-    // separate instantiations for the LayerNorm and the plain epilogue: each gets its own register allocation
-    if (split) { if (ln) TTSB_GEMM_LAUNCH(true, true); else TTSB_GEMM_LAUNCH(true, false); }
-    else { if (ln) TTSB_GEMM_LAUNCH(false, true); else TTSB_GEMM_LAUNCH(false, false); }
-#undef TTSB_GEMM_LAUNCH
-    count_launch();
-    return check_cuda(cudaGetLastError(), "gemm_tc_kernel launch");
+    // pair mode: a cluster of two CTAs per 128-row tile.  Separate instantiations for the LayerNorm and the plain epilogue:
+    // each gets its own register allocation
+    if (as_pair) return split ? launch_tc<true, true, true>(tmA, tmW, tmO, q, work, stream) : launch_tc<false, true, true>(tmA, tmW, tmO, q, work, stream);
+    if (q.gamma != nullptr)
+      return split ? launch_tc<true, false, true>(tmA, tmW, tmO, q, work, stream) : launch_tc<false, false, true>(tmA, tmW, tmO, q, work, stream);
+    return split ? launch_tc<true, false, false>(tmA, tmW, tmO, q, work, stream) : launch_tc<false, false, false>(tmA, tmW, tmO, q, work, stream);
   };
   if (pair && hybrid_full > 0) {
     rc = launch(false, 0, hybrid_full);
