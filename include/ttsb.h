@@ -538,6 +538,65 @@ int ttsb_griffinlim_batch(const float* magnitude, const float* init_angles, cons
                           float* wav_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Ragged-batch Conv1D on the tensor cores (the MelGAN generator, transformertts_b200/model/melgan.py).
+ * Layout: a packed ragged batch of n_clips clips, channels-last 16-bit (rows, ld).  Clip c has L_c rows, given as the int32
+ * prefix sums clip_offsets[0..n_clips] (HOST memory, clip_offsets[0] = 0), framed by TTSB_CONV1D_HALO halo rows on each
+ * side: its rows are clip_offsets[c] + (2c + 1) HALO + [0, L_c), and the buffer holds clip_offsets[n_clips] + 2 HALO n_clips
+ * rows.  Each call computes, for every clip row t in [0, L_c),
+ *   y[c, t, :] = bias + sum_s  in_{tap_src[s]}[c, t + tap_shift[s], :] @ W[koff_s : koff_s + ld_in[tap_src[s]], :]
+ * (|tap_shift| <= HALO, so a tap reads the clip's own halos; koff_s = the ld_in of the earlier taps).  W is the (K_total, N)
+ * matrix packed by ttsb_pack_weight (n_pad = N); ld_in[src] is a multiple of 64 and every input column is read.
+ * With up > 1 (a transposed conv phrased over its input rows), column n of y[c, t] is channel n % ld_out of output row
+ * t up + n / ld_out: the outputs use the same layout with up L_c rows per clip, and N = up ld_out.
+ * Outputs (bf16; the lo planes only in bf16x3; any may be NULL): out_hi/out_lo = y, act_hi/act_lo = LeakyReLU_0.2(y).
+ * halo_mode: TTSB_HALO_NONE leaves the outputs' halos alone; TTSB_HALO_REFLECT writes output row L-1+k of a clip as a copy of
+ * row L-1-k and row -k as a copy of row k (k = 1..HALO, needs up L_c > HALO); TTSB_HALO_ZERO writes zeros there (needs
+ * up L_c >= HALO).  A halo row is written only by the store of the row it mirrors, never by a computed row.
+ * N is a multiple of 64, and at most 256 or a multiple of 256; ld_out (= N / up) is a multiple of 16.  No atomics: a clip's
+ * output is bit-identical wherever it sits in the batch.  workspace: ttsb_conv1d_workspace_bytes(n_clips) bytes of device
+ * memory, 4-byte aligned; the entry points copy the clip table there.  Malformed offsets, clips too short for the halo
+ * mode and a short workspace give TTSB_ERR_INVALID_ARGUMENT before any CUDA call.
+ * ------------------------------------------------------------------------------------------------------- */
+#define TTSB_CONV1D_HALO 9
+#define TTSB_CONV1D_MAX_TAPS 7
+#define TTSB_HALO_NONE 0
+#define TTSB_HALO_REFLECT 1
+#define TTSB_HALO_ZERO 2
+typedef struct ttsb_conv1d_args {
+  int n_clips;
+  const int32_t* clip_offsets; /* HOST, int32 (n_clips + 1) */
+  int num_taps;
+  int tap_src[TTSB_CONV1D_MAX_TAPS];
+  int tap_shift[TTSB_CONV1D_MAX_TAPS];
+  const void* in_hi[2];
+  const void* in_lo[2];
+  int ld_in[2];
+  const void* w_hi;
+  const void* w_lo;
+  const float* bias; /* fp32 (N), or NULL */
+  int N;
+  int up;
+  void* out_hi;
+  void* out_lo;
+  void* act_hi;
+  void* act_lo;
+  int ld_out;
+  int halo_mode;
+  int precision; /* TTSB_PREC_BF16 or TTSB_PREC_BF16X3 */
+  void* workspace;
+  int64_t workspace_bytes;
+} ttsb_conv1d_args;
+int64_t ttsb_conv1d_workspace_bytes(int n_clips); /* -1 for n_clips < 1 */
+int ttsb_conv1d_tc(const ttsb_conv1d_args* a, void* stream);
+/* The generator's output layer: wav = tanh(bias + sum_{k=-3..3} in[t + k, :channels] . weight[k + 3, :]) for every clip row t
+ * in [0, L_c - drop_tail), in = hi (+ lo) planes in the layout above (ld_in columns; the halos hold the reflect padding).
+ * Clip c's samples go to wav_out[clip_offsets[c] - c drop_tail ...].  weight: fp32 (7, channels) on the device,
+ * channels <= ld_in <= 256, every L_c > drop_tail >= 0. */
+int ttsb_conv1d_out_tanh(const void* in_hi, const void* in_lo, int ld_in, int channels, const int32_t* clip_offsets, int n_clips,
+                         int drop_tail, const float* weight, float bias, void* workspace, int64_t workspace_bytes, float* wav_out,
+                         void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Data-parallel gradient exchange (BASELINE.json: "NCCL allreduce over NVLink on gradient buckets only"; the reference has
  * no distributed code).  One communicator per process / GPU.  NCCL is loaded at run time (libnccl.so.2 of the host
  * process, or $TTSB_NCCL_LIB); without it these return TTSB_ERR_UNSUPPORTED.

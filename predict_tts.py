@@ -3,10 +3,14 @@
 
     python predict_tts.py -f lines.txt [-p MODEL_DIR | --step 95000] [-o OUTDIR] [-m] [-s] [-v]
     python predict_tts.py -t "phoneme string" ...
+    python predict_tts.py -f lines.txt --vocoder melgan --vocoder_checkpoint melgan.pt ...
 
 Every input line is tokenised, turned into a mel by ``ForwardTransformer.predict`` (one line per call, as the reference does)
 and vocoded on the GPU with ``Audio.reconstruct_waveform_batch`` (mel inversion + 32 Griffin-Lim iterations), in chunks of
-``VOCODE_CHUNK`` lines so that device memory stays bounded however long the file is.  Output:
+``VOCODE_CHUNK`` lines so that device memory stays bounded however long the file is.  With ``--vocoder melgan`` the chunks
+go through a MelGAN generator instead (``MelGANGenerator.vocode_batch``, weights from ``--vocoder_checkpoint``), as the
+reference's synthesis notebook does one line at a time; a line of T frames then gives 256 T samples (Griffin-Lim:
+256 (T - 1)).  Output:
 ``<outdir>/outputs/<fname>/<fname>_<data_name>_<git_hash>_<step>.wav``, the concatenation of all lines; with ``--single`` also
 ``..._<i>.wav`` per line, with ``--store_mel`` ``..._<i>.mel.npy`` (the (T, n_mels) mel of line i).
 
@@ -26,7 +30,7 @@ from pathlib import Path
 
 import numpy as np
 
-VOCODE_CHUNK = 16    # lines vocoded per reconstruct_waveform_batch call
+VOCODE_CHUNK = 16    # lines vocoded per reconstruct_waveform_batch / vocode_batch call
 MISSING = 'unknown'  # file-name placeholder for a config key the model does not carry
 
 
@@ -40,7 +44,12 @@ def parse_args(argv=None):
     parser.add_argument('--store_mel', '-m', dest='store_mel', action='store_true')
     parser.add_argument('--verbose', '-v', dest='verbose', action='store_true')
     parser.add_argument('--single', '-s', dest='single', action='store_true')
-    return parser.parse_args(argv)
+    parser.add_argument('--vocoder', dest='vocoder', default='griffinlim', choices=('griffinlim', 'melgan'))
+    parser.add_argument('--vocoder_checkpoint', dest='vocoder_checkpoint', default=None, type=str)
+    args = parser.parse_args(argv)
+    if args.vocoder == 'melgan' and args.vocoder_checkpoint is None:
+        parser.error('--vocoder melgan needs --vocoder_checkpoint PATH')
+    return args
 
 
 NO_INPUT_MESSAGE = 'Specify either an input text (-t "some text") or a text input file (-f /path/to/file.txt)'
@@ -105,6 +114,10 @@ def main(argv=None):
     from transformertts_b200.data.audio import Audio
     audio = Audio.from_config(model.config)
     tokenizer = make_tokenizer(model)
+    vocoder = None
+    if args.vocoder == 'melgan':
+        from transformertts_b200.model.melgan import MelGANGenerator
+        vocoder = MelGANGenerator.from_checkpoint(args.vocoder_checkpoint, device=model.device)
     print(f'Output wav under {output_path.parent}')
     wavs = []
     for start in range(0, len(text), VOCODE_CHUNK):
@@ -121,7 +134,10 @@ def main(argv=None):
             mels.append(mel)
             if args.store_mel:
                 np.save(line_paths(outdir, file_name, i)[1], mel)
-        chunk = audio.reconstruct_waveform_batch([m.T for m in mels], seed=start)
+        if vocoder is None:
+            chunk = audio.reconstruct_waveform_batch([m.T for m in mels], seed=start)
+        else:
+            chunk = vocoder.vocode_batch([m.T for m in mels])
         for j, wav in enumerate(chunk):
             if args.single:
                 audio.save_wav(wav, line_paths(outdir, file_name, start + j)[0])

@@ -1,0 +1,114 @@
+"""Mel -> waveform with the MelGAN generator for a file's worth of utterances.
+
+    python tools/vocoder_bench.py [--clips 64] [--reps 3] [--out DIR]
+
+Workload: that of tools/synth_bench.py -- `--clips` seeded ragged clips of 2-10 s (T_c uniform in 173..862 frames), mels from
+the CUDA front end (Audio.mel_spectrogram) -- and a seeded generator checkpoint (oracle/melgan_oracle.py, seed 0).  Paths:
+  notebook   the generator as a torch module in fp32 on the GPU (cuDNN, TF32 off), one clip per call with its 10-frame pad,
+             as the reference's synthesis notebook runs it
+  bf16x3     MelGANGenerator.vocode_batch, all clips in one call, parity mode
+  bf16       the same in fast mode
+  griffinlim Audio.reconstruct_waveform_batch (32 iterations), for context
+Every path runs once before timing; a timing is the host clock around whole calls followed by torch.cuda.synchronize(),
+averaged over `--reps` calls.  FLOPs are counted from the layer shapes (multiply-adds x 2, the useful products only: the
+zero-padded columns of the 32-channel stage are not counted).  Prints one JSON line: seconds per call, seconds of audio per
+second, library launches per call, achieved TFLOP/s, the largest |difference| of each vocode_batch mode from the notebook
+path, and the card name and power limit read in the same run.  `--out` also writes it to DIR/vocoder_bench.json."""
+import argparse
+import json
+import subprocess
+import sys
+import time
+from pathlib import Path
+
+import numpy as np
+import torch
+
+sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+from oracle import audio_oracle as ao  # noqa: E402
+from oracle import melgan_oracle as mo  # noqa: E402
+from transformertts_b200 import lib  # noqa: E402
+from transformertts_b200.data.audio import Audio  # noqa: E402
+from transformertts_b200.model import melgan as mg  # noqa: E402
+
+
+def card():
+    try:
+        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True,
+                           timeout=30).stdout.strip().splitlines()
+        return q[0] if q else 'unknown'
+    except (OSError, subprocess.SubprocessError):
+        return 'unknown'
+
+
+def timed(fn, reps):
+    out = fn()
+    torch.cuda.synchronize()
+    lib.reset_launch_count()
+    t0 = time.perf_counter()
+    for _ in range(reps):
+        out = fn()
+    torch.cuda.synchronize()
+    return (time.perf_counter() - t0) / reps, lib.launch_count() / reps, out
+
+
+def generator_flops(frames) -> float:
+    """FLOPs of one forward over clips of frames[c] frames (10-frame pad included), from the layer shapes."""
+    total = 0.0
+    for L in frames:
+        total += 2.0 * L * 512 * 80 * 7
+        rows = L
+        for _, _, cin, cout, _, u in mg.STAGES:
+            rows *= u
+            total += 2.0 * rows * cout * cin * 2          # each output row of a transposed conv sums 2 of its k taps per input channel
+            total += 3 * 2.0 * rows * cout * cout * 5     # per ResStack block: 3-tap conv + two 1x1 convs
+        total += 2.0 * rows * 32 * 7
+    return total
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--clips', type=int, default=64)
+    ap.add_argument('--reps', type=int, default=3)
+    ap.add_argument('--out', default=None)
+    args = ap.parse_args()
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    audio = Audio(sampling_rate=22050, n_fft=1024, mel_channels=80, hop_length=256, win_length=1024, f_min=0, f_max=8000,
+                  normalizer='MelGAN')
+    lengths = np.random.default_rng(2024).integers(173, 863, size=args.clips)
+    mels = [audio.mel_spectrogram(ao.make_clips(1, 256 * (int(T) - 1), seed=500 + c)[0]).T for c, T in enumerate(lengths)]
+    sd = mo.init_state_dict(seed=0)
+    module = mo.build(sd, dtype=torch.float32).cuda()
+    pad = torch.full((1, 80, mo.PAD_FRAMES), mo.PAD_VALUE, device='cuda')
+
+    def notebook():
+        with torch.no_grad():
+            return [module(torch.cat([torch.from_numpy(m).cuda()[None], pad], 2))[0, 0, :-mo.HOP * mo.PAD_FRAMES].cpu().numpy() for m in mels]
+
+    res = dict(workload='melgan_vocode', clips=args.clips, frames=int(lengths.sum()), min_frames=int(lengths.min()),
+               max_frames=int(lengths.max()), reps=args.reps, audio_s=round(float(256 * lengths.sum() / 22050), 1))
+    flops = generator_flops([int(T) + mo.PAD_FRAMES for T in lengths])
+    res['gflop_per_call'] = round(flops / 1e9, 1)
+    res['gflop_per_audio_s'] = round(flops / 1e9 / res['audio_s'], 2)
+    t, launches, w_ref = timed(notebook, args.reps)
+    res.update(notebook_s=round(t, 5), notebook_audio_s_per_s=round(res['audio_s'] / t, 1), notebook_tflops=round(flops / t / 1e12, 2))
+    for prec in ('bf16x3', 'bf16'):
+        g = mg.MelGANGenerator(device='cuda', precision=prec).load_state_dict(sd)
+        t, launches, w = timed(lambda: g.vocode_batch(mels), args.reps)
+        res.update({f'{prec}_s': round(t, 5), f'{prec}_audio_s_per_s': round(res['audio_s'] / t, 1), f'{prec}_launches': launches,
+                    f'{prec}_tflops': round(flops / t / 1e12, 2),
+                    f'{prec}_max_abs_diff_vs_notebook': float(max(np.abs(a - b).max() for a, b in zip(w, w_ref)))})
+        del g
+    t, launches, _ = timed(lambda: audio.reconstruct_waveform_batch(mels, seed=0), args.reps)
+    res.update(griffinlim_s=round(t, 5), griffinlim_audio_s_per_s=round(res['audio_s'] / t, 1), griffinlim_launches=launches)
+    res['card'] = card()
+    line = json.dumps(res)
+    print(line)
+    if args.out:
+        Path(args.out).mkdir(parents=True, exist_ok=True)
+        (Path(args.out) / 'vocoder_bench.json').write_text(line + '\n')
+
+
+if __name__ == '__main__':
+    main()

@@ -1,0 +1,387 @@
+// Ragged-batch Conv1D on the pipeline of gemm_pipeline.cuh (ttsb_conv1d_tc), for the MelGAN generator: dilated 3-tap convs,
+// the ResStack's shortcut + 1x1 conv as one two-source product, transposed convs phrased over their input rows, and the
+// 7-tap input conv.  Clips are packed channels-last with TTSB_CONV1D_HALO halo rows on each side (include/ttsb.h), so a tap
+// is a row shift of a 2-D TMA load and a 128-row tile may span several clips.  The epilogue (one thread per row) maps the
+// row to its clip, skips halo rows, adds the bias, writes y and LeakyReLU(y) as bf16 hi/lo planes and mirrors the rows next
+// to each clip edge into the halos the next conv reads.  ttsb_conv1d_out_tanh is the generator's N = 1 output layer.
+#include <vector>
+
+#include "../../include/ttsb.h"
+#include "gemm_pipeline.cuh"
+
+namespace ttsb {
+
+constexpr int CONV_HALO = TTSB_CONV1D_HALO;
+constexpr float LRELU_SLOPE = 0.2f;
+
+struct ConvKParams {
+  int rows;  // GEMM rows: every row of the packed input layout, halos included
+  int N, block_n, n_tiles, num_tiles;
+  int num_taps;
+  int tap_src[TTSB_CONV1D_MAX_TAPS], tap_shift[TTSB_CONV1D_MAX_TAPS];
+  int kblocks[2];
+  int n_clips;
+  const int32_t* tab;  // device: region start rows [n_clips + 1], then the clip_offsets prefix sums [n_clips + 1]
+  int up, halo_mode, ld_out;
+  const float* bias;
+  __nv_bfloat16* out_hi;
+  __nv_bfloat16* out_lo;
+  __nv_bfloat16* act_hi;
+  __nv_bfloat16* act_lo;
+};
+
+template <bool kSplit>
+struct ConvCfg {
+  static constexpr int kStages = kSplit ? 2 : 4;
+  static constexpr int kStageBytes = (kSplit ? 2 : 1) * (A_TILE_BYTES + B_TILE_BYTES);
+  using Ring = GemmRing<kStages, kStageBytes>;
+  static constexpr int kPitch = acc_pitch(GEMM_MAX_BN);
+  static_assert(img_bytes(GEMM_MAX_BN) <= Ring::kBytes, "image must fit the ring");
+  static constexpr int kSmemBytes = Ring::kBytes + GEMM_RING_BAR_BYTES + 1024;  // + alignment slack
+};
+
+// last c with tab[c] <= x (tab ascending, tab[0] <= x)
+__device__ __forceinline__ int conv_find_clip(const int32_t* __restrict__ tab, int n, int x) {
+  int lo = 0, hi = n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(tab + mid) <= x) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// 16 columns of output row orow: y (and LeakyReLU(y)) as bf16 hi/lo, or zeros
+__device__ __forceinline__ void conv_store16(const ConvKParams& p, size_t orow, int col, const float (&y)[16], bool zero) {
+  const size_t o = orow * (size_t)p.ld_out + col;
+  uint32_t h[8], l[8];
+  float v[16];
+  if (p.out_hi) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) v[j] = zero ? 0.f : y[j];
+    pack_hi_lo(v, h, l, p.out_lo != nullptr);
+    st_global_v8(p.out_hi + o, h);
+    if (p.out_lo) st_global_v8(p.out_lo + o, l);
+  }
+  if (p.act_hi) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) v[j] = zero ? 0.f : (y[j] > 0.f ? y[j] : LRELU_SLOPE * y[j]);
+    pack_hi_lo(v, h, l, p.act_lo != nullptr);
+    st_global_v8(p.act_hi + o, h);
+    if (p.act_lo) st_global_v8(p.act_lo + o, l);
+  }
+}
+
+__device__ __forceinline__ void conv_epilogue(const ConvKParams& p, const float* arow, int g, int n0, int half) {
+  if (g >= p.rows) return;
+  const int32_t* reg = p.tab;
+  const int32_t* off = p.tab + p.n_clips + 1;
+  const int c = conv_find_clip(reg, p.n_clips, g);
+  const int off_c = __ldg(off + c);
+  const int L = __ldg(off + c + 1) - off_c;
+  const int j = g - __ldg(reg + c) - CONV_HALO;
+  if (j < 0 || j >= L) return;  // a halo row: written only by the mirror stores of the rows it copies
+  const int Lo = L * p.up;
+  const long long base = (long long)off_c * p.up + (long long)(2 * c + 1) * CONV_HALO;  // output row of clip position 0
+  const int nch = p.block_n >> 4;
+  const int ch_begin = half ? (nch + 1) >> 1 : 0;
+  const int ch_end = half ? nch : (nch + 1) >> 1;
+  uint32_t q[16];
+  float y[16], bs[16];
+  for (int ch = ch_begin; ch < ch_end; ++ch) {
+    const int col = n0 + (ch << 4);
+    acc_ld16(arow + (ch << 4), q);
+#pragma unroll
+    for (int k = 0; k < 16; ++k) y[k] = __uint_as_float(q[k]);
+    if (p.bias) {
+      const float4* b4 = reinterpret_cast<const float4*>(p.bias + col);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float4 f = __ldg(b4 + k);
+        bs[4 * k] = f.x; bs[4 * k + 1] = f.y; bs[4 * k + 2] = f.z; bs[4 * k + 3] = f.w;
+      }
+#pragma unroll
+      for (int k = 0; k < 16; ++k) y[k] += bs[k];
+    }
+    const int phase = col / p.ld_out, cc = col - phase * p.ld_out;
+    const int pos = j * p.up + phase;  // position in the output clip
+    conv_store16(p, (size_t)(base + pos), cc, y, false);
+    if (p.halo_mode == TTSB_HALO_REFLECT) {
+      if (pos >= 1 && pos <= CONV_HALO) conv_store16(p, (size_t)(base - pos), cc, y, false);
+      if (pos >= Lo - 1 - CONV_HALO && pos <= Lo - 2) conv_store16(p, (size_t)(base + 2 * (Lo - 1) - pos), cc, y, false);
+    } else if (p.halo_mode == TTSB_HALO_ZERO) {
+      if (pos < CONV_HALO) conv_store16(p, (size_t)(base - 1 - pos), cc, y, true);
+      if (pos >= Lo - CONV_HALO) conv_store16(p, (size_t)(base + 2 * Lo - 1 - pos), cc, y, true);
+    }
+  }
+}
+
+// tensor maps: A[src][hi/lo] (ld_in[src], rows) boxes (64, 128); W[hi/lo] (K_total, N) boxes (64, block_n)
+template <bool kSplit>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant__ CUtensorMap tmA0l,
+                 const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUtensorMap tmA1l,
+                 const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const ConvKParams p) {
+  using Cfg = ConvCfg<kSplit>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = align_smem_1024(smem_raw);
+  typename Cfg::Ring ring(smem);
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA0h);
+    tma_prefetch_desc(&tmWh);
+    ring.init();
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  const uint32_t stage_tx = (kSplit ? 2u : 1u) * (uint32_t)(A_TILE_BYTES + p.block_n * GEMM_BK * 2);
+  if (warp >= GEMM_EPI_WARPS) {
+    setmaxnreg_dec<40>();
+    if (warp > GEMM_EPI_WARPS) goto done;
+    // ===================== TMA producer =====================
+    const bool leader = elect_one();
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      const int m0 = (tile / p.n_tiles) * GEMM_BM;
+      const int n0 = (tile % p.n_tiles) * p.block_n;
+      ring.wait_image_free();
+      int kglob = 0;
+      for (int s = 0; s < p.num_taps; ++s) {
+        const int src = p.tap_src[s];
+        const CUtensorMap* mh = src == 0 ? &tmA0h : &tmA1h;
+        const CUtensorMap* ml = src == 0 ? &tmA0l : &tmA1l;
+        for (int kb = 0; kb < p.kblocks[src]; ++kb, ++kglob) {
+          ring.produce(leader, stage_tx, [&](uint64_t* bar, uint8_t* st) {
+            tma_load_2d(mh, bar, st, kb * GEMM_BK, m0 + p.tap_shift[s]);   // rows outside the buffer load as zeros
+            tma_load_2d(&tmWh, bar, st + A_TILE_BYTES, kglob * GEMM_BK, n0);
+            if (kSplit) {
+              uint8_t* st2 = st + A_TILE_BYTES + B_TILE_BYTES;
+              tma_load_2d(ml, bar, st2, kb * GEMM_BK, m0 + p.tap_shift[s]);
+              tma_load_2d(&tmWl, bar, st2 + A_TILE_BYTES, kglob * GEMM_BK, n0);
+            }
+          });
+        }
+      }
+    }
+  } else {
+    // ===================== two wgmma warpgroups, then the epilogue =====================
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int quarter = warp & 3;
+    const int half = warp >> 2;
+    float* img = reinterpret_cast<float*>(smem);
+    int total_kb = 0;
+    for (int s = 0; s < p.num_taps; ++s) total_kb += p.kblocks[p.tap_src[s]];
+    const int nch = p.block_n >> 6;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      const int m0 = (tile / p.n_tiles) * GEMM_BM;
+      const int n0 = (tile % p.n_tiles) * p.block_n;
+      float acc[GEMM_NCH][32];
+      ring.mma_tile(total_kb, acc, [&](uint32_t st, int kb) {
+        const uint32_t a_hi = st + wg * (64 * 128);
+        const uint32_t b_hi = st + A_TILE_BYTES;
+#pragma unroll
+        for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
+          const uint64_t da = make_smem_desc_sw128(a_hi) + 2 * kk;
+#pragma unroll
+          for (int c = 0; c < GEMM_NCH; ++c)
+            if (c < nch) wgmma_ss_m64n64_bf16<0, 0>(acc[c], da, make_smem_desc_sw128(b_hi + c * (64 * 128)) + 2 * kk, (kb | kk) != 0);
+        }
+        if (kSplit) {
+          const uint32_t a_lo = st + A_TILE_BYTES + B_TILE_BYTES + wg * (64 * 128);
+          const uint32_t b_lo = st + 2 * A_TILE_BYTES + B_TILE_BYTES;
+#pragma unroll
+          for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
+            const uint64_t da_lo = make_smem_desc_sw128(a_lo) + 2 * kk, da_hi = make_smem_desc_sw128(a_hi) + 2 * kk;
+#pragma unroll
+            for (int c = 0; c < GEMM_NCH; ++c) {
+              if (c < nch) {
+                wgmma_ss_m64n64_bf16<0, 0>(acc[c], da_lo, make_smem_desc_sw128(b_hi + c * (64 * 128)) + 2 * kk, 1);
+                wgmma_ss_m64n64_bf16<0, 0>(acc[c], da_hi, make_smem_desc_sw128(b_lo + c * (64 * 128)) + 2 * kk, 1);
+              }
+            }
+          }
+        }
+      });
+      park_tile(img, Cfg::kPitch, wg, nch, acc);
+      const int row = quarter * 32 + lane;
+      __syncwarp();
+      conv_epilogue(p, img + (size_t)row * Cfg::kPitch, m0 + row, n0, half);
+      ring.release_tile(false);
+    }
+  }
+done:
+  __syncthreads();
+}
+
+// one thread per output sample: tanh(bias + 7-tap dot product over the reflect-padded channels), fixed summation order
+__global__ void __launch_bounds__(256)
+conv1d_out_tanh_kernel(const __nv_bfloat16* __restrict__ in_hi, const __nv_bfloat16* __restrict__ in_lo, int ld_in, int channels,
+                       const int32_t* __restrict__ tab, int n_clips, int drop_tail, const float* __restrict__ weight, float bias,
+                       int total, float* __restrict__ wav_out) {
+  extern __shared__ float sw[];  // (7, channels)
+  for (int i = threadIdx.x; i < 7 * channels; i += blockDim.x) sw[i] = weight[i];
+  __syncthreads();
+  const int32_t* off = tab + n_clips + 1;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    const int c = conv_find_clip(off, n_clips, i);
+    const int off_c = __ldg(off + c);
+    const int j = i - off_c;
+    if (j >= __ldg(off + c + 1) - off_c - drop_tail) continue;
+    const size_t row = (size_t)__ldg(tab + c) + CONV_HALO + j;
+    float acc = bias;
+    for (int k = 0; k < 7; ++k) {
+      const __nv_bfloat16* h = in_hi + (row + k - 3) * (size_t)ld_in;
+      const __nv_bfloat16* l = in_lo ? in_lo + (row + k - 3) * (size_t)ld_in : nullptr;
+      for (int ch = 0; ch < channels; ++ch) {
+        float x = __bfloat162float(h[ch]);
+        if (l) x += __bfloat162float(l[ch]);
+        acc = fmaf(x, sw[k * channels + ch], acc);
+      }
+    }
+    wav_out[off_c - (size_t)c * drop_tail + j] = tanhf(acc);
+  }
+}
+
+// checks the host offset table and fills tab (region starts, prefix sums); min_out_len: the least up * L_c; 0 on success
+static int conv_table(const char* what, const int32_t* clip_offsets, int n_clips, int up, int min_out_len, std::vector<int32_t>& tab,
+                      long long* rows) {
+  if (!clip_offsets) { set_last_error("%s: clip_offsets is NULL", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (n_clips < 1) { set_last_error("%s: n_clips must be >= 1", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (clip_offsets[0] != 0) { set_last_error("%s: clip_offsets[0] must be 0", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  tab.assign(2 * (size_t)(n_clips + 1), 0);
+  for (int c = 0; c < n_clips; ++c) {
+    const long long L = (long long)clip_offsets[c + 1] - clip_offsets[c];
+    if (L < 1) { set_last_error("%s: clip_offsets must be increasing (clip %d has %lld rows)", what, c, L); return TTSB_ERR_INVALID_ARGUMENT; }
+    if (L * up < min_out_len) {
+      set_last_error("%s: clip %d has %lld output rows; this halo mode needs at least %d", what, c, L * up, min_out_len);
+      return TTSB_ERR_INVALID_ARGUMENT;
+    }
+  }
+  const long long total = (long long)clip_offsets[n_clips] * up + 2LL * CONV_HALO * n_clips;
+  if (total > INT32_MAX) { set_last_error("%s: too many rows", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  for (int c = 0; c <= n_clips; ++c) {
+    tab[c] = clip_offsets[c] + 2 * CONV_HALO * c;
+    tab[n_clips + 1 + c] = clip_offsets[c];
+  }
+  *rows = (long long)clip_offsets[n_clips] + 2LL * CONV_HALO * n_clips;
+  return 0;
+}
+
+static int check_workspace(const char* what, const void* ws, int64_t bytes, int n_clips) {
+  if (!ws || bytes < 2 * (int64_t)(n_clips + 1) * 4 || reinterpret_cast<uintptr_t>(ws) % 4) {
+    set_last_error("%s: workspace missing, too small (ttsb_conv1d_workspace_bytes) or not 4-byte aligned", what);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  return 0;
+}
+
+}  // namespace ttsb
+
+using namespace ttsb;
+
+extern "C" int64_t ttsb_conv1d_workspace_bytes(int n_clips) {
+  if (n_clips < 1) {
+    set_last_error("ttsb_conv1d_workspace_bytes: n_clips < 1");
+    return -1;
+  }
+  return 2 * (int64_t)(n_clips + 1) * (int64_t)sizeof(int32_t);
+}
+
+extern "C" int ttsb_conv1d_tc(const ttsb_conv1d_args* a, void* stream_v) {
+  const char* what = "ttsb_conv1d_tc";
+  if (!a) { set_last_error("ttsb_conv1d_tc: args is NULL"); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (a->precision != TTSB_PREC_BF16 && a->precision != TTSB_PREC_BF16X3) { set_last_error("ttsb_conv1d_tc: unknown precision"); return TTSB_ERR_INVALID_ARGUMENT; }
+  const bool split = a->precision == TTSB_PREC_BF16X3;
+  if (a->num_taps < 1 || a->num_taps > TTSB_CONV1D_MAX_TAPS) { set_last_error("ttsb_conv1d_tc: num_taps must be in [1, 7]"); return TTSB_ERR_INVALID_ARGUMENT; }
+  int k_total = 0;
+  for (int s = 0; s < a->num_taps; ++s) {
+    const int src = a->tap_src[s];
+    if (src < 0 || src > 1 || !a->in_hi[src] || (split && !a->in_lo[src])) {
+      set_last_error("ttsb_conv1d_tc: tap %d reads source %d, which is missing (bf16x3 needs in_lo too)", s, src);
+      return TTSB_ERR_INVALID_ARGUMENT;
+    }
+    if (a->ld_in[src] < GEMM_BK || a->ld_in[src] % GEMM_BK) { set_last_error("ttsb_conv1d_tc: ld_in[%d] = %d must be a positive multiple of 64", src, a->ld_in[src]); return TTSB_ERR_INVALID_ARGUMENT; }
+    if (a->tap_shift[s] < -CONV_HALO || a->tap_shift[s] > CONV_HALO) { set_last_error("ttsb_conv1d_tc: |tap_shift| must be <= %d", CONV_HALO); return TTSB_ERR_INVALID_ARGUMENT; }
+    k_total += a->ld_in[src];
+  }
+  if (!a->w_hi || (split && !a->w_lo)) { set_last_error("ttsb_conv1d_tc: missing packed weights"); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (a->N < 64 || a->N % 64 || (a->N > GEMM_MAX_BN && a->N % GEMM_MAX_BN)) { set_last_error("ttsb_conv1d_tc: N = %d must be a multiple of 64, at most 256 or a multiple of 256", a->N); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (a->up < 1 || a->N % a->up || a->N / a->up != a->ld_out || a->ld_out % 16) { set_last_error("ttsb_conv1d_tc: need N = up * ld_out with ld_out a multiple of 16"); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (a->halo_mode < TTSB_HALO_NONE || a->halo_mode > TTSB_HALO_ZERO) { set_last_error("ttsb_conv1d_tc: unknown halo_mode"); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (!a->out_hi && !a->act_hi) { set_last_error("ttsb_conv1d_tc: no output"); return TTSB_ERR_INVALID_ARGUMENT; }
+  const int min_len = a->halo_mode == TTSB_HALO_REFLECT ? CONV_HALO + 1 : (a->halo_mode == TTSB_HALO_ZERO ? CONV_HALO : 1);
+  std::vector<int32_t> tab;
+  long long rows = 0;
+  int rc = conv_table(what, a->clip_offsets, a->n_clips, a->up, min_len, tab, &rows);
+  if (rc) return rc;
+  rc = check_workspace(what, a->workspace, a->workspace_bytes, a->n_clips);
+  if (rc) return rc;
+
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  ConvKParams p{};
+  p.rows = (int)rows;
+  p.N = a->N;
+  p.block_n = a->N < GEMM_MAX_BN ? a->N : GEMM_MAX_BN;
+  p.n_tiles = a->N / p.block_n;
+  p.num_tiles = (int)((rows + GEMM_BM - 1) / GEMM_BM) * p.n_tiles;
+  p.num_taps = a->num_taps;
+  for (int s = 0; s < a->num_taps; ++s) { p.tap_src[s] = a->tap_src[s]; p.tap_shift[s] = a->tap_shift[s]; }
+  for (int i = 0; i < 2; ++i) p.kblocks[i] = a->in_hi[i] ? a->ld_in[i] / GEMM_BK : 0;
+  p.n_clips = a->n_clips;
+  p.tab = static_cast<const int32_t*>(a->workspace);
+  p.up = a->up;
+  p.halo_mode = a->halo_mode;
+  p.ld_out = a->ld_out;
+  p.bias = a->bias;
+  p.out_hi = static_cast<__nv_bfloat16*>(a->out_hi);
+  p.out_lo = split && a->out_hi ? static_cast<__nv_bfloat16*>(a->out_lo) : nullptr;
+  p.act_hi = static_cast<__nv_bfloat16*>(a->act_hi);
+  p.act_lo = split && a->act_hi ? static_cast<__nv_bfloat16*>(a->act_lo) : nullptr;
+
+  CUtensorMap tmA[2][2], tmW[2];
+  for (int i = 0; i < 2; ++i) {
+    const int use = a->in_hi[i] ? i : (a->in_hi[0] ? 0 : 1);  // an unused slot aliases the other source
+    for (int h = 0; h < 2; ++h) {
+      const void* base = (h == 1 && split) ? a->in_lo[use] : a->in_hi[use];
+      rc = make_tmap_bf16_2d(&tmA[i][h], base, (uint64_t)a->ld_in[use], (uint64_t)rows, (uint64_t)a->ld_in[use], GEMM_BK, GEMM_BM);
+      if (rc) return rc;
+    }
+  }
+  for (int h = 0; h < 2; ++h) {
+    rc = make_tmap_bf16_2d(&tmW[h], (h == 1 && split) ? a->w_lo : a->w_hi, (uint64_t)k_total, (uint64_t)a->N, (uint64_t)k_total, GEMM_BK, p.block_n);
+    if (rc) return rc;
+  }
+  TTSB_CUDA_OK(cudaMemcpyAsync(a->workspace, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  if (split)
+    return launch_pipeline<conv1d_tc_kernel<true>>(ConvCfg<true>::kSmemBytes, p.num_tiles, false, stream, "conv1d_tc_kernel launch",
+                                                   tmA[0][0], tmA[0][1], tmA[1][0], tmA[1][1], tmW[0], tmW[1], p);
+  return launch_pipeline<conv1d_tc_kernel<false>>(ConvCfg<false>::kSmemBytes, p.num_tiles, false, stream, "conv1d_tc_kernel launch",
+                                                  tmA[0][0], tmA[0][1], tmA[1][0], tmA[1][1], tmW[0], tmW[1], p);
+}
+
+extern "C" int ttsb_conv1d_out_tanh(const void* in_hi, const void* in_lo, int ld_in, int channels, const int32_t* clip_offsets, int n_clips,
+                                    int drop_tail, const float* weight, float bias, void* workspace, int64_t workspace_bytes, float* wav_out,
+                                    void* stream_v) {
+  const char* what = "ttsb_conv1d_out_tanh";
+  if (!in_hi || !weight || !wav_out) { set_last_error("ttsb_conv1d_out_tanh: NULL pointer"); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (channels < 1 || ld_in < channels || ld_in > 256 || ld_in % 8) { set_last_error("ttsb_conv1d_out_tanh: need 1 <= channels <= ld_in <= 256, ld_in % 8 == 0"); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (drop_tail < 0) { set_last_error("ttsb_conv1d_out_tanh: drop_tail < 0"); return TTSB_ERR_INVALID_ARGUMENT; }
+  std::vector<int32_t> tab;
+  long long rows = 0;
+  // the 3-row reflect padding lies in the halos: the clip needs rows 1..3 and must outlast drop_tail
+  int rc = conv_table(what, clip_offsets, n_clips, 1, (drop_tail + 1 > 4 ? drop_tail + 1 : 4), tab, &rows);
+  if (rc) return rc;
+  rc = check_workspace(what, workspace, workspace_bytes, n_clips);
+  if (rc) return rc;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  TTSB_CUDA_OK(cudaMemcpyAsync(workspace, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  const int total = clip_offsets[n_clips];
+  const int grid = min((total + 255) / 256, 8 * num_sms());
+  conv1d_out_tanh_kernel<<<grid, 256, 7 * channels * sizeof(float), stream>>>(
+      static_cast<const __nv_bfloat16*>(in_hi), static_cast<const __nv_bfloat16*>(in_lo), ld_in, channels, static_cast<const int32_t*>(workspace),
+      n_clips, drop_tail, weight, bias, total, wav_out);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "conv1d_out_tanh_kernel launch");
+}

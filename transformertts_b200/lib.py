@@ -33,6 +33,7 @@ EXPORTS = [
     'ttsb_stft_mel_log_batch_workspace_bytes', 'ttsb_stft_mel_log_batch', 'ttsb_pitch_workspace_bytes', 'ttsb_pitch_dio_stonemask',
     'ttsb_dp_unique_id', 'ttsb_dp_init', 'ttsb_dp_allreduce_bucket', 'ttsb_dp_destroy',
     'ttsb_decode_attn_workspace_bytes', 'ttsb_decode_attn', 'ttsb_decode_prologue', 'ttsb_decode_commit',
+    'ttsb_conv1d_workspace_bytes', 'ttsb_conv1d_tc', 'ttsb_conv1d_out_tanh',
 ]
 
 
@@ -131,6 +132,9 @@ def load() -> C.CDLL:
     lib.ttsb_decode_attn_workspace_bytes.restype = C.c_int64
     lib.ttsb_stft_mel_log_batch_workspace_bytes.restype = C.c_int64
     lib.ttsb_pitch_workspace_bytes.restype = C.c_int64
+    lib.ttsb_conv1d_workspace_bytes.restype = C.c_int64
+    lib.ttsb_conv1d_out_tanh.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_float,
+                                         C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     lib.ttsb_pitch_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double]
     lib.ttsb_pitch_dio_stonemask.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double,
                                              C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
@@ -594,3 +598,42 @@ def decode_commit(post, B, r, mel, stop_col, stop_index, max_iters, mel_out, sto
     _check(load().ttsb_decode_commit(ptr(post), post.shape[-1], int(B), int(r), int(mel), int(stop_col), int(stop_index), int(max_iters),
                                      ptr(mel_out), ptr(stop_out), ptr(next_hi), ptr(next_lo), next_hi.shape[-1], ptr(pos), ptr(done),
                                      ptr(n), ptr(all_done), _stream()), 'ttsb_decode_commit')
+
+
+# ------------------------------------------------------------------------------------------------------------
+# ragged-batch Conv1D (the MelGAN generator)
+# ------------------------------------------------------------------------------------------------------------
+CONV1D_HALO = 9
+CONV1D_MAX_TAPS = 7
+HALO_NONE, HALO_REFLECT, HALO_ZERO = 0, 1, 2
+
+
+class Conv1dArgs(C.Structure):
+    _fields_ = [
+        ('n_clips', C.c_int), ('clip_offsets', C.c_void_p), ('num_taps', C.c_int),
+        ('tap_src', C.c_int * CONV1D_MAX_TAPS), ('tap_shift', C.c_int * CONV1D_MAX_TAPS),
+        ('in_hi', C.c_void_p * 2), ('in_lo', C.c_void_p * 2), ('ld_in', C.c_int * 2),
+        ('w_hi', C.c_void_p), ('w_lo', C.c_void_p), ('bias', C.c_void_p), ('N', C.c_int), ('up', C.c_int),
+        ('out_hi', C.c_void_p), ('out_lo', C.c_void_p), ('act_hi', C.c_void_p), ('act_lo', C.c_void_p), ('ld_out', C.c_int),
+        ('halo_mode', C.c_int), ('precision', C.c_int), ('workspace', C.c_void_p), ('workspace_bytes', C.c_int64),
+    ]
+
+
+def conv1d_workspace_bytes(n_clips: int) -> int:
+    n = int(load().ttsb_conv1d_workspace_bytes(int(n_clips)))
+    if n < 0:
+        raise TtsbError(load().ttsb_last_error().decode())
+    return n
+
+
+def conv1d_tc(args: Conv1dArgs):
+    """One ragged-batch conv (include/ttsb.h: ttsb_conv1d_tc).  args.clip_offsets points at a host int32 table."""
+    _check(load().ttsb_conv1d_tc(C.byref(args), _stream()), 'ttsb_conv1d_tc')
+
+
+def conv1d_out_tanh(in_hi, in_lo, channels, clip_offsets, drop_tail, weight, bias, workspace, wav_out):
+    """The generator's output layer (include/ttsb.h: ttsb_conv1d_out_tanh); clip_offsets: host sequence (n_clips + 1)."""
+    co, n = _host_offsets(clip_offsets)
+    _check(load().ttsb_conv1d_out_tanh(ptr(in_hi), ptr(in_lo), in_hi.shape[-1], int(channels), co, n, int(drop_tail), ptr(weight),
+                                       C.c_float(bias), ptr(workspace), C.c_int64(workspace.numel() * workspace.element_size()),
+                                       ptr(wav_out), _stream()), 'ttsb_conv1d_out_tanh')
