@@ -1,21 +1,88 @@
 """Helpers shared by the GPU parity tests: drive single kernels of libttsb.so through the C ABI."""
 from __future__ import annotations
 
+import numpy as np
 import torch
 
 from transformertts_b200 import lib
 from transformertts_b200.model.models import _PackedLinear, _round_up
 
 DEV = 'cuda:0'
+# what the columns of a source buffer outside [a_col0, a_col0 + C) hold: a GEMM that reads them is far off its reference
+WIDE_SOURCE_FILL = 3.0e4
 
 
 def split_or_none(x: torch.Tensor, split: bool):
     return lib.split_bf16(x, split)
 
 
+# ----------------------------------------------------------------------------------------------------------
+# the stateless dropout mask of csrc/ttsb_common.cuh (dropout_hterm, dropout_mix, dropout_keep, dropout_thresh) in numpy
+# uint32 arithmetic: element idx of (seed, site) is kept when its 16-bit half of the hash of pair idx >> 1 is >= thresh >> 16
+# ----------------------------------------------------------------------------------------------------------
+DROPOUT_C1 = 0x9E3779B1
+
+
+def _u32(x):
+    """uint32 array (at least 1-D, so products wrap silently as in C)."""
+    return np.atleast_1d(np.asarray(x, dtype=np.uint64) & np.uint64(0xFFFFFFFF)).astype(np.uint32)
+
+
+def dropout_thresh(p: float) -> int:
+    return int(float(np.float32(p)) * 4294967296.0) if p > 0 else 0
+
+
+def dropout_hterm(seed: int, site: int, pair_hi, salt: int = 0):
+    s = _u32(seed ^ salt)
+    return (_u32(pair_hi) * np.uint32(0x85EBCA77)) ^ (s * np.uint32(0xC2B2AE3D)) ^ (_u32(site) * np.uint32(0x27D4EB2F))
+
+
+def dropout_mix(x):
+    x = _u32(x)
+    x = x ^ (x >> np.uint32(16))
+    x = x * np.uint32(0x7FEB352D)
+    x = x ^ (x >> np.uint32(15))
+    x = x * np.uint32(0x846CA68B)
+    return x ^ (x >> np.uint32(16))
+
+
+def dropout_keep(seed: int, site: int, idx, p: float, salt: int = 0) -> np.ndarray:
+    """Keep decisions of the elements `idx` (any integer array) at rate p."""
+    idx = np.asarray(idx, dtype=np.uint64)
+    pair = idx >> np.uint64(1)
+    h = dropout_mix((_u32(pair & np.uint64(0xFFFFFFFF)) * np.uint32(DROPOUT_C1)) ^ dropout_hterm(seed, site, pair >> np.uint64(32), salt))
+    half = np.where((idx & np.uint64(1)) != 0, h >> np.uint32(16), h & np.uint32(0xFFFF))
+    return half >= np.uint32(dropout_thresh(p) >> 16)
+
+
+def dropout_mask(B: int, T: int, N: int, ld: int, seed: int, site: int, p: float, salt: int = 0) -> np.ndarray:
+    """(B,T,N) keep mask of a (B,T,ld) tensor whose element (b,t,n) is drawn at index (b*T + t)*ld + n."""
+    idx = (np.arange(B * T, dtype=np.uint64)[:, None] * np.uint64(ld) + np.arange(N, dtype=np.uint64)[None, :]).reshape(B, T, N)
+    return dropout_keep(seed, site, idx, p, salt)
+
+
+def dropout_scale(p: float) -> float:
+    """1/(1-p) as the kernels compute it, in fp32."""
+    return float(np.float32(1.0) / (np.float32(1.0) - np.float32(p)))
+
+
+def _poison16(shape):
+    """16-bit buffer of all-ones bit patterns: NaN read as bf16 and as fp16."""
+    t = torch.empty(shape, device=DEV, dtype=torch.bfloat16)
+    t.view(torch.int16).fill_(-1)
+    return t
+
+
 def run_gemm(x_list, w_kn, bias, seg_src, seg_shift, seg_k, *, precision='bf16x3', impl='tcgen05', relu=False,
-             residual=None, ln=None, row_len=None, block_n=None, single_tile=False, out_fp16=False):
-    """x_list: fp32 (B,T,C) sources (on GPU).  Returns dict with requested outputs."""
+             residual=None, ln=None, row_len=None, block_n=None, single_tile=False, out_fp16=False, outputs=None, ld_out=None,
+             lda=None, a_col0=None, residual_pair=None, out_preln=False, dropout=None, dropout_post=None, seed=0):
+    """x_list: fp32 (B,T,C) sources (on GPU).  Returns dict with requested outputs.
+
+    outputs: any subset of 'f32', 'hi', 'lo' (default: all three, 'lo' only in bf16x3); with out_fp16 'hi' holds fp16.
+    ld_out: row stride of the outputs (default n_pad).  lda / a_col0: per source, the source is placed at column a_col0 of
+    a buffer with lda columns whose other columns hold WIDE_SOURCE_FILL.  residual_pair: bf16 (hi, lo) residual.
+    out_preln: also return the pre-LayerNorm value.  dropout / dropout_post: (p, site) of drop_pre / drop_post.
+    Every output starts as NaN; out['launches'] is the number of kernel launches of the call."""
     split = precision == 'bf16x3'
     B, T, _ = x_list[0].shape
     pl = _PackedLinear(w_kn, bias, seg_k, split, single_tile=single_tile, block_n=block_n)
@@ -26,12 +93,20 @@ def run_gemm(x_list, w_kn, bias, seg_src, seg_shift, seg_k, *, precision='bf16x3
     for s in range(len(seg_k)):
         a.seg_src[s], a.seg_shift[s], a.seg_k[s] = seg_src[s], seg_shift[s], seg_k[s]
     for i, x in enumerate(x_list):
+        C = x.shape[-1]
+        ld = lda[i] if lda is not None else C
+        c0 = a_col0[i] if a_col0 is not None else 0
+        if ld != C or c0 != 0:
+            assert c0 + C <= ld
+            buf = torch.full((B, T, ld), WIDE_SOURCE_FILL, device=x.device)
+            buf[..., c0:c0 + C] = x
+            x = buf
         hi, lo = lib.split_bf16(x, split)
         keep += [hi, lo]
         a.a_hi[i] = hi.data_ptr()
         a.a_lo[i] = lo.data_ptr() if lo is not None else None
-        a.lda[i] = x.shape[-1]
-        a.a_col0[i] = 0
+        a.lda[i] = ld
+        a.a_col0[i] = c0
     a.w_hi = pl.w_hi.data_ptr()
     a.w_lo = pl.w_lo.data_ptr() if pl.w_lo is not None else None
     a.bias = pl.bias.data_ptr() if pl.bias is not None else None
@@ -39,6 +114,9 @@ def run_gemm(x_list, w_kn, bias, seg_src, seg_shift, seg_k, *, precision='bf16x3
     if residual is not None:
         a.residual = residual.data_ptr()
         a.ld_res = residual.shape[-1]
+    if residual_pair is not None:
+        a.residual_hi, a.residual_lo = residual_pair[0].data_ptr(), residual_pair[1].data_ptr()
+        a.ld_res = residual_pair[0].shape[-1]
     if ln is not None:
         from transformertts_b200.model.models import _pad_vec
         g_pad, b_pad = _pad_vec(ln[0], pl.n_pad), _pad_vec(ln[1], pl.n_pad)
@@ -46,35 +124,53 @@ def run_gemm(x_list, w_kn, bias, seg_src, seg_shift, seg_k, *, precision='bf16x3
         a.ln_gamma, a.ln_beta, a.ln_eps = g_pad.data_ptr(), b_pad.data_ptr(), 1e-6
     if row_len is not None:
         a.row_len = row_len.data_ptr()
+    if outputs is None:
+        outputs = ('f32', 'hi', 'lo')
+    ld = ld_out or pl.n_pad
     out = {}
     # poison the outputs so unwritten elements are visible
-    out_f32 = torch.full((B, T, pl.n_pad), float('nan'), device=DEV)
-    out_hi = torch.full((B, T, pl.n_pad), float('nan'), device=DEV, dtype=torch.bfloat16)
-    out_lo = torch.full((B, T, pl.n_pad), float('nan'), device=DEV, dtype=torch.bfloat16)
-    a.out_f32, a.out_hi = out_f32.data_ptr(), out_hi.data_ptr()
-    a.out_lo = out_lo.data_ptr() if split else None
-    a.ld_out = pl.n_pad
+    out_f32 = torch.full((B, T, ld), float('nan'), device=DEV) if 'f32' in outputs else None
+    out_hi = _poison16((B, T, ld)) if 'hi' in outputs else None
+    out_lo = _poison16((B, T, ld)) if 'lo' in outputs and split else None
+    preln = torch.full((B, T, ld), float('nan'), device=DEV) if out_preln else None
+    a.out_f32 = out_f32.data_ptr() if out_f32 is not None else None
+    a.out_hi = out_hi.data_ptr() if out_hi is not None else None
+    a.out_lo = out_lo.data_ptr() if out_lo is not None else None
+    a.out_preln = preln.data_ptr() if preln is not None else None
+    a.ld_out = ld
     a.out_fp16 = int(out_fp16)
+    if dropout is not None:
+        a.drop_pre_p, a.drop_pre_site = dropout
+    if dropout_post is not None:
+        a.drop_post_p, a.drop_post_site = dropout_post
+    a.drop_seed = seed
     a.precision = lib.PREC_BF16X3 if split else lib.PREC_BF16
     a.impl = lib.IMPL_SIMT if impl == 'simt' else lib.IMPL_TCGEN05
+    lib.reset_launch_count()
     lib.linear_fwd(a)
+    out['launches'] = lib.launch_count()
     torch.cuda.synchronize()
     out['f32'] = out_f32
     out['hi'] = out_hi
-    out['lo'] = out_lo if split else None
+    out['lo'] = out_lo
+    out['preln'] = preln
     out['n_pad'] = pl.n_pad
     return out
 
 
-def ref_gemm(x_list, w_kn, bias, seg_src, seg_shift, seg_k, *, precision, relu=False, residual=None, ln=None, row_len=None):
-    """float64 CPU reference of the same contract.  In 'bf16' mode the operands are first rounded to bf16 (that is the
-    kernel's arithmetic); in 'bf16x3' mode the fp32 operands are used as they are."""
-    xs = [x.detach().cpu().double() if precision == 'bf16x3' else x.detach().cpu().bfloat16().double() for x in x_list]
-    w = w_kn.detach().cpu().reshape(-1, w_kn.shape[-1])
+def ref_gemm(x_list, w_kn, bias, seg_src, seg_shift, seg_k, *, precision, relu=False, residual=None, ln=None, row_len=None,
+             residual_pair=None, dropout=None, dropout_post=None, seed=0, salt=0, ld_out=None, device='cpu', return_preln=False):
+    """float64 reference of the same contract (on `device`).  In 'bf16' mode the operands are first rounded to bf16 (that is
+    the kernel's arithmetic); in 'bf16x3' mode the fp32 operands are used as they are.  residual_pair adds
+    float(hi) + float(lo); dropout / dropout_post = (p, site) apply the restated masks, drawn at (b*T + t)*ld_out + n, as
+    keep * x * fp32(1/(1-p)).  return_preln: also return the value before the LayerNorm (not row-masked)."""
+    dev = torch.device(device)
+    xs = [x.detach().to(dev).double() if precision == 'bf16x3' else x.detach().to(dev).bfloat16().double() for x in x_list]
+    w = w_kn.detach().to(dev).reshape(-1, w_kn.shape[-1])
     w = w.double() if precision == 'bf16x3' else w.bfloat16().double()
     B, T, _ = xs[0].shape
     N = w.shape[1]
-    acc = torch.zeros(B, T, N, dtype=torch.float64)
+    acc = torch.zeros(B, T, N, dtype=torch.float64, device=dev)
     koff = 0
     for s, k in enumerate(seg_k):
         x = xs[seg_src[s]]
@@ -84,20 +180,33 @@ def ref_gemm(x_list, w_kn, bias, seg_src, seg_shift, seg_k, *, precision, relu=F
             acc[:, lo:hi] += x[:, lo + sh:hi + sh, :k] @ w[koff:koff + k]
         koff += k
     if bias is not None:
-        acc += bias.detach().cpu().double()
+        acc += bias.detach().to(dev).double()
     if relu:
         acc = torch.relu(acc)
+
+    def drop(v, spec):
+        p, site = spec
+        keep = torch.from_numpy(dropout_mask(B, T, N, ld_out, seed, site, p, salt)).to(dev)
+        return v * keep * dropout_scale(p)
+
+    if dropout is not None:
+        acc = drop(acc, dropout)
     if residual is not None:
-        acc += residual.detach().cpu().double()[..., :N]
+        acc += residual.detach().to(dev).double()[..., :N]
+    if residual_pair is not None:
+        acc += residual_pair[0].detach().to(dev).double()[..., :N] + residual_pair[1].detach().to(dev).double()[..., :N]
+    preln = acc
     if ln is not None:
-        g, b = ln[0].detach().cpu().double(), ln[1].detach().cpu().double()
+        g, b = ln[0].detach().to(dev).double(), ln[1].detach().to(dev).double()
         mean = acc.mean(-1, keepdim=True)
         var = ((acc - mean) ** 2).mean(-1, keepdim=True)
         acc = (acc - mean) * torch.rsqrt(var + 1e-6) * g + b
+    if dropout_post is not None:
+        acc = drop(acc, dropout_post)
     if row_len is not None:
-        keep = torch.arange(T)[None, :] < row_len.detach().cpu()[:, None]
+        keep = torch.arange(T, device=dev)[None, :] < row_len.detach().to(dev)[:, None]
         acc = acc * keep[..., None]
-    return acc
+    return (acc, preln) if return_preln else acc
 
 
 def _to16(x, precision, split):
