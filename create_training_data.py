@@ -16,13 +16,20 @@ The wavs are processed in batches of about ``BATCH_SAMPLES`` samples: a thread p
 GPU, each batch is uploaded once, its log-mels (``ttsb_stft_mel_log_batch``) and pitch (``ttsb_pitch_dio_stonemask``) are
 computed on the same packed buffer, and another thread pool writes the ``.npy`` files.
 
+Wavs at another rate than the audio settings' ``sampling_rate`` are resampled to it as the reference's ``librosa.load(path,
+sr=sampling_rate)`` does (resampy's ``kaiser_best`` filter): the off-rate files of a batch go through one
+``ttsb_resample_batch`` launch, then through the same ``Audio.preprocess`` (volume normalisation, hop padding) as every other file.
+Files already at ``sampling_rate`` take exactly the path they take without resampling.
+
 Differences from the reference:
   * Without the ``phonemizer`` package (and espeak), the text column of the metadata is taken to BE phonemes in the model's
     alphabet, as ``predict_tts.py`` does; the script says so when it starts.  With it, the reference's arguments are used.
   * Files are processed in metadata order, so the pitch statistics and the phonemized metadata are in that order; the
     reference's process pool completes them in no fixed order, so its statistics differ in the last bits from run to run.
-  * A wav at another sampling rate is refused (no resampling), and the ``trim_silence`` / ``trim_long_silences`` settings are
-    refused (no librosa or webrtcvad); see ``Audio.load_wav`` and ``Audio.preprocess``.
+  * The ``trim_silence`` / ``trim_long_silences`` settings are refused (no librosa or webrtcvad); see ``Audio.preprocess``.
+  * Resampling restates resampy's ``kaiser_best`` table from its published parameters rather than reading resampy's precomputed
+    file, so it may differ from librosa's result in the last bits of the filter.  A file too short to resample (fewer output
+    samples than one) stops the script with its name; the reference's worker would raise inside resampy.
   * ``max_mel_len``, ``min_mel_len`` and ``n_test`` default to the reference's 1200, 80 and 100 when the config lacks them.
   * No TensorBoard summaries.
 """
@@ -79,13 +86,14 @@ def make_phonemizer(config):
     return phonemizer
 
 
-def batches(paths, budget: int, load):
-    """Consecutive groups of (path, wav) whose samples add up to about `budget`; files are read by a thread pool ahead of use."""
+def batches(paths, budget: int, load, size=len):
+    """Consecutive groups of (path, load(path)) whose sizes (`size` of each loaded item: its samples) add up to about `budget`;
+    files are read by a thread pool ahead of use."""
     with ThreadPoolExecutor(max_workers=4) as pool:
         batch, n = [], 0
         for path, y in zip(paths, pool.map(load, paths)):
             batch.append((path, y))
-            n += len(y)
+            n += size(y)
             if n >= budget:
                 yield batch
                 batch, n = [], 0
@@ -93,14 +101,57 @@ def batches(paths, budget: int, load):
             yield batch
 
 
+class TooShortToResample(ValueError):
+    pass
+
+
+def wav_loader(audio):
+    """path -> (samples, None) preprocessed as Audio.load_wav does when the file is at the configured rate, else the raw mono
+    samples and their rate, to be resampled with the rest of the batch."""
+    from transformertts_b200.data.audio import resampled_length
+
+    def load(path):
+        y, sr = audio.read_wav(str(path))
+        if sr == audio.sampling_rate:
+            return audio.preprocess(y), None
+        try:
+            resampled_length(len(y), sr, audio.sampling_rate)
+        except ValueError as e:
+            raise TooShortToResample(f'{path}: {e}') from None
+        return y, sr
+    return load
+
+
+def loaded_samples(audio):
+    """Size of a wav_loader item in the batch budget: its samples at the configured rate, so a batch of resampled files packs
+    about as many samples for the mel and pitch kernels as a batch of files already at that rate."""
+    from transformertts_b200.data.audio import resampled_length
+
+    def size(item):
+        y, sr = item
+        return len(y) if sr is None else resampled_length(len(y), sr, audio.sampling_rate)
+    return size
+
+
+def resample_batch(audio, batch, rates_seen: dict):
+    """Resample the off-rate files of a batch in one launch, then preprocess them -> batch of (path, samples at the configured rate)."""
+    off = [c for c, (_, (_, sr)) in enumerate(batch) if sr is not None]
+    done = dict(zip(off, audio.resample_ragged([batch[c][1] for c in off]))) if off else {}
+    for c in off:
+        sr = batch[c][1][1]
+        rates_seen[sr] = rates_seen.get(sr, 0) + 1
+    return [(path, audio.preprocess(done[c]) if c in done else y) for c, (path, (y, _)) in enumerate(batch)]
+
+
 def process_mels(cm, audio, wav_files, budget: int = BATCH_SAMPLES):
     """reference :39-99 -> (len_dict, remove_files)."""
     cm.mel_dir.mkdir(parents=True, exist_ok=True)
     cm.pitch_dir.mkdir(parents=True, exist_ok=True)
     max_len, min_len = config_value(cm, 'max_mel_len'), config_value(cm, 'min_mel_len')
-    len_dict, remove_files, mel_lens, pitches = {}, [], [], {}
+    len_dict, remove_files, mel_lens, pitches, rates_seen = {}, [], [], {}, {}
     with ThreadPoolExecutor(max_workers=2) as writer:
-        for batch in batches(wav_files, budget, lambda p: audio.load_wav(str(p))[0]):
+        for raw in batches(wav_files, budget, wav_loader(audio), loaded_samples(audio)):
+            batch = resample_batch(audio, raw, rates_seen)
             wav, so = audio._pack([y for _, y in batch])
             mel, fo_mel = audio.mel_spectrogram_ragged_device(wav, so)
             f0, fo_f0 = audio.extract_pitch_device(wav, so)
@@ -126,6 +177,9 @@ def process_mels(cm, audio, wav_files, budget: int = BATCH_SAMPLES):
         pickle.dump(len_dict, f)
     with open(cm.data_dir / 'under-over_sized_mels.pkl', 'wb') as f:
         pickle.dump(remove_files, f)
+    if rates_seen:
+        print(f"Resampled {sum(rates_seen.values())} file(s) to {audio.sampling_rate} Hz: "
+              + ', '.join(f'{n} from {sr} Hz' for sr, n in sorted(rates_seen.items())))
     total_wav_len = np.sum(mel_lens) * audio.config['hop_length']
     print(f"Total duration (hours): {total_wav_len / audio.config['sampling_rate'] / 60. ** 2:.4f}")
     return len_dict, remove_files
@@ -235,7 +289,10 @@ def main(argv=None):
         from transformertts_b200.data.audio import Audio
         print(f'\nMels will be stored under\n{cm.mel_dir}')
         audio = Audio.from_config(cm.config)
-        process_mels(cm, audio, [reader.wav_paths[k] for k in cross_file_ids])
+        try:
+            process_mels(cm, audio, [reader.wav_paths[k] for k in cross_file_ids])
+        except TooShortToResample as e:
+            raise SystemExit(f'error: {e}') from None
 
     if not args.skip_phonemes:
         process_phonemes(cm, reader, cross_file_ids, phonemizer)

@@ -502,6 +502,28 @@ int ttsb_pitch_dio_stonemask(const float* wav, const int32_t* sample_offsets, in
                              const int32_t* f0_offsets, double* f0_out, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Resampling  (Audio.resample_ragged_device; data/audio.py:126-130: librosa.load(path, sr=...) -> librosa.resample(res_type=
+ * 'kaiser_best') -> resampy.resample(filter='kaiser_best') + fix_length; tests/resample_oracle.py restates the algorithm)
+ *   wav: fp32 clips packed end to end, clip c at samples sample_offsets[c] .. sample_offsets[c+1] - 1, sampled at src_rates[c]
+ *   Hz (sample_offsets int32 (n_clips + 1) and src_rates int32 (n_clips), both in HOST memory; mixed rates share one launch).
+ *   half_window: the interpolation filter's half window, float64 (n_window) in device memory, 512 entries per zero crossing
+ *   (resampy's kaiser_best: n_window 32769).  Clip c becomes ceil(L_c ratio_c) samples at dst_rate, ratio_c = (double) dst_rate /
+ *   src_rates[c]: int(L_c ratio_c) computed samples then zeros; a clip already at dst_rate is copied unchanged.  out_offsets (int32
+ *   (n_clips + 1), HOST memory, from 0) must hold the prefix sums of those lengths; out: fp32 (out_offsets[n_clips]) on the device.
+ *   Every sample follows resampy's resample_f in float64 without contraction, the accumulator rounded to float32 after each tap,
+ *   and the float64 time register r_{t+1} = r_t + 1/ratio is reproduced bit for bit (see csrc/resample.cu), so clip c's output
+ *   does not depend on the other clips or its position in the batch.
+ *   workspace: ttsb_resample_batch_workspace_bytes(...) bytes of device memory, 16-byte aligned (about 530 KB per distinct
+ *   downsampling ratio, plus the clip and time-register tables).  Offsets that do not start at 0 or decrease, a rate <= 0,
+ *   out_offsets that disagree with ceil(L ratio), a clip with int(L ratio) < 1 and a short workspace give
+ *   TTSB_ERR_INVALID_ARGUMENT before any CUDA call. */
+int64_t ttsb_resample_batch_workspace_bytes(const int32_t* sample_offsets, const int32_t* src_rates, int n_clips, int dst_rate,
+                                            int n_window);   /* -1 for invalid arguments */
+int ttsb_resample_batch(const float* wav, const int32_t* sample_offsets, const int32_t* src_rates, int n_clips, int dst_rate,
+                        const double* half_window, int n_window, const int32_t* out_offsets, void* workspace, int64_t workspace_bytes,
+                        float* out, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * mel -> waveform  (Audio.reconstruct_waveform, data/audio.py:94-110: librosa mel_to_stft(power=1) + griffinlim(32, momentum .99))
  *   n_fft 1024, hop 256, periodic Hann, centred frames with reflect padding (the reference configuration).
  * ------------------------------------------------------------------------------------------------------- */

@@ -1,10 +1,12 @@
 """Audio front-end mirror of the reference's ``data/audio.py``: STFT -> 80-bin mel -> log normalisation (reference:
 data/audio.py:72-92, 196-231) by the fused CUDA kernels ``ttsb_stft_mel_log`` / ``ttsb_stft_mel_log_batch``, f0 by DIO +
 StoneMask (data/audio.py:146-151) by ``ttsb_pitch_dio_stonemask``, wav loading and preprocessing (data/audio.py:126-141,
-154-162) on the host, and mel -> waveform by Griffin-Lim.
+154-162) on the host, resampling to ``sampling_rate`` (librosa.load's ``kaiser_best`` resampy filter, data/audio.py:126-130) by
+``ttsb_resample_batch``, and mel -> waveform by Griffin-Lim.
 
-Silence trimming (librosa, webrtcvad) and resampling are not implemented: ``preprocess`` refuses the two trim settings and
-``load_wav`` refuses a file whose rate differs from ``sampling_rate``.
+Silence trimming (librosa, webrtcvad) is not implemented: ``preprocess`` refuses the two trim settings.  ``load_wav`` refuses a
+file whose rate differs from ``sampling_rate``; such files are read with ``read_wav`` and resampled a batch at a time with
+``resample_ragged`` / ``resample_ragged_device``, as ``create_training_data.py`` does.
 """
 from __future__ import annotations
 
@@ -41,6 +43,28 @@ def slaney_mel_basis(sr: int, n_fft: int, n_mels: int, fmin: float, fmax: float)
         falling = (right - bin_hz) / (right - centre)
         basis[m] = np.clip(np.minimum(rising, falling), 0.0, None) * (2.0 / (right - left))
     return basis.astype(np.float32)
+
+
+def kaiser_best_half_window() -> np.ndarray:
+    """resampy's `kaiser_best` interpolation filter (the one librosa.load(sr=...) uses at its default res_type), restated from its
+    published parameters: the right half of rolloff * sinc(rolloff * z) * kaiser(2n + 1, beta), z = linspace(0, 64, n + 1),
+    n = 64 zero crossings * 512 entries per crossing -> float64 (32769,).  resampy ships this table precomputed."""
+    from scipy.signal.windows import kaiser
+    num_zeros, num_table, beta, rolloff = 64, 512, 14.769656459379492, 0.9475937167399596
+    n = num_zeros * num_table
+    sinc_win = rolloff * np.sinc(rolloff * np.linspace(0, num_zeros, num=n + 1, endpoint=True))
+    return kaiser(2 * n + 1, beta)[n:] * sinc_win
+
+
+def resampled_length(n_samples: int, sr_orig: int, sr_new: int) -> int:
+    """Samples of a clip of `n_samples` at sr_orig after resampling to sr_new: ceil(n ratio) in float64, as librosa's fix_length.
+    Raises ValueError when int(n ratio) < 1 (resampy has no output sample to compute)."""
+    if sr_orig == sr_new:
+        return int(n_samples)
+    ratio = float(sr_new) / sr_orig
+    if int(n_samples * ratio) < 1:
+        raise ValueError(f'{n_samples} samples at {sr_orig} Hz are too short to resample to {sr_new} Hz')
+    return int(np.ceil(n_samples * ratio))
 
 
 def _random_phase(shape, seed):
@@ -311,14 +335,45 @@ class Audio:
         mel = mel.cpu().numpy()
         return [mel[a:b] for a, b in zip(fo[:-1], fo[1:])]
 
-    def load_wav(self, wav_path, preprocess: bool = True):
-        """reference: data/audio.py:126-130 (librosa.load(path, sr=sampling_rate)) -> (float32 samples, rate).  PCM and float WAV,
-        several channels averaged to mono; PCM is scaled as libsndfile reads it into float (int16 / 32768, ...).  A file at another
-        rate is refused: librosa would resample it, which is not implemented here."""
+    def _resample_window(self) -> torch.Tensor:
+        if getattr(self, '_rs_window', None) is None:
+            self._rs_window = torch.from_numpy(kaiser_best_half_window()).to(self.device).contiguous()
+        return self._rs_window
+
+    def resample_ragged_device(self, wav: torch.Tensor, sample_offsets, src_rates) -> tuple:
+        """ttsb_resample_batch: packed fp32 clips on the device, clip c sampled at src_rates[c] Hz -> (packed fp32 clips at
+        sampling_rate on the device, output sample offsets).  What librosa.load(sr=sampling_rate) does after reading and mixing to
+        mono (resampy kaiser_best, then fix_length to ceil(L ratio)); a clip already at sampling_rate comes back unchanged.  Clip
+        c's output does not depend on the other clips.  A clip too short to resample raises ValueError."""
+        with torch.cuda.device(self.device):
+            so = np.asarray(sample_offsets, dtype=np.int64)
+            rates = np.asarray(src_rates, dtype=np.int64).reshape(-1)
+            if len(rates) != len(so) - 1:
+                raise ValueError(f'{len(rates)} source rates for {len(so) - 1} clips')
+            lengths = []
+            for c, (L, sr) in enumerate(zip(np.diff(so), rates)):
+                try:
+                    lengths.append(resampled_length(int(L), int(sr), self.sampling_rate))
+                except ValueError as e:
+                    raise ValueError(f'clip {c}: {e}') from None
+            oo = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
+            out = torch.empty(int(oo[-1]), dtype=torch.float32, device=self.device)
+            lib.resample_batch(wav.contiguous(), so, rates, self.sampling_rate, self._resample_window(), oo, out)
+            return out, oo
+
+    def resample_ragged(self, clips) -> list:
+        """resample_ragged_device for a list of (float32 samples, rate) in one launch -> list of float32 arrays at sampling_rate."""
+        clips = list(clips)
+        wav, so = self._pack([y for y, _ in clips])
+        out, oo = self.resample_ragged_device(wav, so, [sr for _, sr in clips])
+        out = out.cpu().numpy()
+        return [out[a:b] for a, b in zip(oo[:-1], oo[1:])]
+
+    def read_wav(self, wav_path):
+        """The decoding half of librosa.load (data/audio.py:126-130) -> (float32 mono samples, the file's own rate).  PCM and float
+        WAV, several channels averaged to mono; PCM is scaled as libsndfile reads it into float (int16 / 32768, ...)."""
         from scipy.io import wavfile
         sr, data = wavfile.read(str(wav_path))
-        if sr != self.sampling_rate:
-            raise ValueError(f'{wav_path}: sampled at {sr} Hz, expected {self.sampling_rate} Hz (resampling is not implemented)')
         if data.dtype == np.uint8:
             y = (data.astype(np.float32) - np.float32(128)) / np.float32(128)
         elif data.dtype.kind == 'i':
@@ -327,6 +382,16 @@ class Audio:
             y = data.astype(np.float32)
         if y.ndim == 2:
             y = np.mean(y, axis=1)
+        return y, sr
+
+    def load_wav(self, wav_path, preprocess: bool = True):
+        """reference: data/audio.py:126-130 (librosa.load(path, sr=sampling_rate)) -> (float32 samples, rate): read_wav, then
+        preprocess.  A file at another rate is refused here; read it with read_wav and resample it with resample_ragged (what
+        create_training_data.py does for a whole corpus)."""
+        y, sr = self.read_wav(wav_path)
+        if sr != self.sampling_rate:
+            raise ValueError(f'{wav_path}: sampled at {sr} Hz, expected {self.sampling_rate} Hz; read_wav + resample_ragged '
+                             f'resample it')
         if preprocess:
             y = self.preprocess(y)
         return y, sr

@@ -34,6 +34,7 @@ EXPORTS = [
     'ttsb_dp_unique_id', 'ttsb_dp_init', 'ttsb_dp_allreduce_bucket', 'ttsb_dp_destroy',
     'ttsb_decode_attn_workspace_bytes', 'ttsb_decode_attn', 'ttsb_decode_prologue', 'ttsb_decode_commit',
     'ttsb_conv1d_workspace_bytes', 'ttsb_conv1d_tc', 'ttsb_conv1d_out_tanh',
+    'ttsb_resample_batch_workspace_bytes', 'ttsb_resample_batch',
 ]
 
 
@@ -138,6 +139,10 @@ def load() -> C.CDLL:
     lib.ttsb_pitch_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double]
     lib.ttsb_pitch_dio_stonemask.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double,
                                              C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+    lib.ttsb_resample_batch_workspace_bytes.restype = C.c_int64
+    lib.ttsb_resample_batch_workspace_bytes.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
+    lib.ttsb_resample_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                        C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     for name in EXPORTS:
         if not hasattr(lib, name):
             raise TtsbError(f'libttsb.so does not export {name}')
@@ -349,6 +354,36 @@ def pitch_dio_stonemask(wav, sample_offsets, fs, frame_period_ms, f0_offsets, f0
     _check(load().ttsb_pitch_dio_stonemask(ptr(wav), so, n, int(fs), float(frame_period_ms), float(f0_floor), float(f0_ceil),
                                            float(channels_in_octave), float(allowed_range), fo, ptr(f0_out), ptr(workspace),
                                            C.c_int64(workspace.numel() * workspace.element_size()), _stream()), 'ttsb_pitch_dio_stonemask')
+
+
+def _host_rates(rates, n: int):
+    import numpy as np
+    a = np.asarray(rates.cpu() if torch.is_tensor(rates) else rates, dtype=np.int64).reshape(-1)
+    if len(a) != n or (len(a) and (a.min() < -2**31 or a.max() > 2**31 - 1)):
+        raise TtsbError(f'{len(a)} source rates for {n} clips (int32 each)')
+    return (C.c_int32 * n)(*a.tolist())
+
+
+def resample_batch_workspace_bytes(sample_offsets, src_rates, dst_rate: int, n_window: int) -> int:
+    so, n = _host_offsets(sample_offsets)
+    nb = int(load().ttsb_resample_batch_workspace_bytes(so, _host_rates(src_rates, n), n, int(dst_rate), int(n_window)))
+    if nb < 0:
+        raise TtsbError(load().ttsb_last_error().decode())
+    return nb
+
+
+def resample_batch(wav, sample_offsets, src_rates, dst_rate, half_window, out_offsets, out):
+    """Resample every clip of a packed ragged batch to dst_rate (include/ttsb.h: ttsb_resample_batch).  wav fp32, half_window
+    fp64 and out fp32 on the device; the offset tables (n_clips + 1) and src_rates (n_clips) are host sequences."""
+    so, n = _host_offsets(sample_offsets)
+    oo, n_o = _host_offsets(out_offsets)
+    if n_o != n:
+        raise TtsbError(f'{n} clips in sample_offsets, {n_o} in out_offsets')
+    rates = _host_rates(src_rates, n)
+    nb = resample_batch_workspace_bytes(sample_offsets, src_rates, dst_rate, half_window.numel())
+    ws = torch.empty(nb, dtype=torch.uint8, device=wav.device)
+    _check(load().ttsb_resample_batch(ptr(wav), so, rates, n, int(dst_rate), ptr(half_window), half_window.numel(), oo, ptr(ws),
+                                      C.c_int64(nb), ptr(out), _stream()), 'ttsb_resample_batch')
 
 
 # ------------------------------------------------------------------------------------------------------------
