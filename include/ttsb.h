@@ -404,6 +404,8 @@ int ttsb_diag_loss_train(const void* P_bf16, int B, int H, int Tq, int Tk, int l
                          float loss_scale, float* loss_out, float grad_scale, float* dP, void* stream);
 int ttsb_diag_loss(const float* att, int B, int H, int Tq, int Tk, const int32_t* q_len, const int32_t* k_len,
                    float* loss_out, void* stream);
+/* Expand backward: dx[b,i,:] = sum of dm[b,t,:] over t in [s_i, s_i + max(dur_i, 0)) clipped to [0, Tm), s_i the exclusive
+ * prefix sum of the non-negative durations (fp32, d multiple of 4, Tp <= 12000) */
 int ttsb_expand_bwd(const float* dm, const int32_t* dur_int, int B, int Tp, int Tm, int d, float* dx, void* stream);
 int ttsb_embedding_bwd(const float* dx, const int32_t* tokens, int B, int T, int d, int vocab, float* demb, void* stream);
 /* d(pos_encoding_scalar) = sum dropout(g) * PE[t]; (drop_p, seed, site) regenerate the prologue dropout mask */

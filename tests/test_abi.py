@@ -71,6 +71,13 @@ def test_argument_validation_without_gpu(cdll):
     assert b'ttsb_attn_probs_fwd' in cdll.ttsb_last_error()
     assert cdll.ttsb_attn_ds_bwd(None, 256, 0, None, 768, 512, 1, 2, 100, 128, None, None, None, C.c_float(0.1), C.c_float(0.1), 0, 0, None, 112, None) == -1
     assert b'ttsb_attn_ds_bwd' in cdll.ttsb_last_error()
+    # the length-regulator backward reads rows as float4 and scans a row's durations in shared memory: widths that are not
+    # a multiple of 4 and more than 12000 phonemes are refused (fake non-null pointers: nothing is launched)
+    p = C.c_void_p(16)
+    assert cdll.ttsb_expand_bwd(p, p, 1, 8, 16, 6, p, None) == -1
+    assert b'ttsb_expand_bwd: need d % 4 == 0' in cdll.ttsb_last_error()
+    assert cdll.ttsb_expand_bwd(p, p, 1, 12001, 16, 256, p, None) == -1
+    assert b'ttsb_expand_bwd: Tp too large' in cdll.ttsb_last_error()
 
 
 def test_product_package_never_imports_the_oracle():

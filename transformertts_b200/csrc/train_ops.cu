@@ -729,11 +729,6 @@ __global__ void expand_bwd_kernel(const float* __restrict__ dm, const int* __res
       }
       reinterpret_cast<float4*>(dx + ((size_t)b * Tp + i) * d)[c] = make_float4(a0.x + a1.x, a0.y + a1.y, a0.z + a1.z, a0.w + a1.w);
     }
-    for (int c = (d4 << 2) + lane; c < d; c += 32) {   // d % 4 tail
-      float acc = 0.f;
-      for (int t = s; t < e; ++t) acc += dm[((size_t)b * Tm + t) * d + c];
-      dx[((size_t)b * Tp + i) * d + c] = acc;
-    }
   }
 }
 
@@ -1018,6 +1013,9 @@ extern "C" int ttsb_rowdot_heads(const void* x, const void* y, int B, int T, int
 
 extern "C" int ttsb_expand_bwd(const float* dm, const int32_t* dur_int, int B, int Tp, int Tm, int d, float* dx, void* stream) {
   if (!dm || !dur_int || !dx || B <= 0 || Tp <= 0 || Tm <= 0 || d <= 0) return bad("ttsb_expand_bwd: bad arguments");
+  // rows are read and written as float4 (row stride d/4 vectors), and the prefix sum of a row lives in shared memory
+  if (d % 4) return bad("ttsb_expand_bwd: need d % 4 == 0");
+  if (Tp > 12000) return bad("ttsb_expand_bwd: Tp too large for the shared-memory scan");
   const int chunks = std::min(32, (Tp + 7) / 8);
   expand_bwd_kernel<<<dim3(B, chunks), 256, (Tp + 1) * sizeof(int), STREAM(stream)>>>(dm, dur_int, Tp, Tm, d, dx);
   LAUNCH_OK("expand_bwd_kernel");
