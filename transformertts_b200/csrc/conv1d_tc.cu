@@ -32,23 +32,12 @@ struct ConvKParams {
 
 template <bool kSplit>
 struct ConvCfg {
-  static constexpr int kStages = kSplit ? 2 : 4;
-  static constexpr int kStageBytes = (kSplit ? 2 : 1) * (A_TILE_BYTES + B_TILE_BYTES);
-  using Ring = GemmRing<kStages, kStageBytes>;
+  using Stage = KMajorStage<kSplit, B_TILE_BYTES>;
+  using Ring = typename Stage::Ring;
   static constexpr int kPitch = acc_pitch(GEMM_MAX_BN);
   static_assert(img_bytes(GEMM_MAX_BN) <= Ring::kBytes, "image must fit the ring");
   static constexpr int kSmemBytes = Ring::kBytes + GEMM_RING_BAR_BYTES + 1024;  // + alignment slack
 };
-
-// last c with tab[c] <= x (tab ascending, tab[0] <= x)
-__device__ __forceinline__ int conv_find_clip(const int32_t* __restrict__ tab, int n, int x) {
-  int lo = 0, hi = n;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (__ldg(tab + mid) <= x) lo = mid; else hi = mid;
-  }
-  return lo;
-}
 
 // 16 columns of output row orow: y (and LeakyReLU(y)) as bf16 hi/lo, or zeros
 __device__ __forceinline__ void conv_store16(const ConvKParams& p, size_t orow, int col, const float (&y)[16], bool zero) {
@@ -75,7 +64,7 @@ __device__ __forceinline__ void conv_epilogue(const ConvKParams& p, const float*
   if (g >= p.rows) return;
   const int32_t* reg = p.tab;
   const int32_t* off = p.tab + p.n_clips + 1;
-  const int c = conv_find_clip(reg, p.n_clips, g);
+  const int c = find_clip(reg, p.n_clips, g);
   const int off_c = __ldg(off + c);
   const int L = __ldg(off + c + 1) - off_c;
   const int j = g - __ldg(reg + c) - CONV_HALO;
@@ -93,12 +82,7 @@ __device__ __forceinline__ void conv_epilogue(const ConvKParams& p, const float*
 #pragma unroll
     for (int k = 0; k < 16; ++k) y[k] = __uint_as_float(q[k]);
     if (p.bias) {
-      const float4* b4 = reinterpret_cast<const float4*>(p.bias + col);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float4 f = __ldg(b4 + k);
-        bs[4 * k] = f.x; bs[4 * k + 1] = f.y; bs[4 * k + 2] = f.z; bs[4 * k + 3] = f.w;
-      }
+      ldg16(p.bias + col, bs);
 #pragma unroll
       for (int k = 0; k < 16; ++k) y[k] += bs[k];
     }
@@ -136,7 +120,7 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constan
   }
   __syncthreads();
 
-  const uint32_t stage_tx = (kSplit ? 2u : 1u) * (uint32_t)(A_TILE_BYTES + p.block_n * GEMM_BK * 2);
+  const uint32_t stage_tx = Cfg::Stage::tx_bytes(p.block_n);
   if (warp >= GEMM_EPI_WARPS) {
     setmaxnreg_dec<40>();
     if (warp > GEMM_EPI_WARPS) goto done;
@@ -152,14 +136,8 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constan
         const CUtensorMap* mh = src == 0 ? &tmA0h : &tmA1h;
         const CUtensorMap* ml = src == 0 ? &tmA0l : &tmA1l;
         for (int kb = 0; kb < p.kblocks[src]; ++kb, ++kglob) {
-          ring.produce(leader, stage_tx, [&](uint64_t* bar, uint8_t* st) {
-            tma_load_2d(mh, bar, st, kb * GEMM_BK, m0 + p.tap_shift[s]);   // rows outside the buffer load as zeros
-            tma_load_2d(&tmWh, bar, st + A_TILE_BYTES, kglob * GEMM_BK, n0);
-            if (kSplit) {
-              uint8_t* st2 = st + A_TILE_BYTES + B_TILE_BYTES;
-              tma_load_2d(ml, bar, st2, kb * GEMM_BK, m0 + p.tap_shift[s]);
-              tma_load_2d(&tmWl, bar, st2 + A_TILE_BYTES, kglob * GEMM_BK, n0);
-            }
+          Cfg::Stage::produce(ring, leader, stage_tx, mh, ml, &tmWh, &tmWl, kglob, n0, [&](const CUtensorMap* m, uint64_t* bar, uint8_t* dst) {
+            tma_load_2d(m, bar, dst, kb * GEMM_BK, m0 + p.tap_shift[s]);   // rows outside the buffer load as zeros
           });
         }
       }
@@ -178,32 +156,7 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constan
       const int m0 = (tile / p.n_tiles) * GEMM_BM;
       const int n0 = (tile % p.n_tiles) * p.block_n;
       float acc[GEMM_NCH][32];
-      ring.mma_tile(total_kb, acc, [&](uint32_t st, int kb) {
-        const uint32_t a_hi = st + wg * (64 * 128);
-        const uint32_t b_hi = st + A_TILE_BYTES;
-#pragma unroll
-        for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
-          const uint64_t da = make_smem_desc_sw128(a_hi) + 2 * kk;
-#pragma unroll
-          for (int c = 0; c < GEMM_NCH; ++c)
-            if (c < nch) wgmma_ss_m64n64_bf16<0, 0>(acc[c], da, make_smem_desc_sw128(b_hi + c * (64 * 128)) + 2 * kk, (kb | kk) != 0);
-        }
-        if (kSplit) {
-          const uint32_t a_lo = st + A_TILE_BYTES + B_TILE_BYTES + wg * (64 * 128);
-          const uint32_t b_lo = st + 2 * A_TILE_BYTES + B_TILE_BYTES;
-#pragma unroll
-          for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
-            const uint64_t da_lo = make_smem_desc_sw128(a_lo) + 2 * kk, da_hi = make_smem_desc_sw128(a_hi) + 2 * kk;
-#pragma unroll
-            for (int c = 0; c < GEMM_NCH; ++c) {
-              if (c < nch) {
-                wgmma_ss_m64n64_bf16<0, 0>(acc[c], da_lo, make_smem_desc_sw128(b_hi + c * (64 * 128)) + 2 * kk, 1);
-                wgmma_ss_m64n64_bf16<0, 0>(acc[c], da_hi, make_smem_desc_sw128(b_lo + c * (64 * 128)) + 2 * kk, 1);
-              }
-            }
-          }
-        }
-      });
+      ring.mma_tile(total_kb, acc, [&](uint32_t st, int kb) { Cfg::Stage::mma(acc, st, wg, nch, kb); });
       park_tile(img, Cfg::kPitch, wg, nch, acc);
       const int row = quarter * 32 + lane;
       __syncwarp();
@@ -225,7 +178,7 @@ conv1d_out_tanh_kernel(const __nv_bfloat16* __restrict__ in_hi, const __nv_bfloa
   __syncthreads();
   const int32_t* off = tab + n_clips + 1;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    const int c = conv_find_clip(off, n_clips, i);
+    const int c = find_clip(off, n_clips, i);
     const int off_c = __ldg(off + c);
     const int j = i - off_c;
     if (j >= __ldg(off + c + 1) - off_c - drop_tail) continue;

@@ -8,9 +8,10 @@
 //               tile's 16-column chunks, so two warps per SM sub-partition hide each other's latencies
 //   warps 9-11  idle: the producer warpgroup hands its registers to the others with setmaxnreg
 // The producer refills the ring only after the epilogue has released the previous tile's image (no double buffering).
-// A kernel supplies the TMA loads of a stage, the wgmma products of a k block and its epilogue.  16-bit outputs leave
-// through staging boxes in the ring (stage_out_offset, staged_slab_begin / _end) as TMA tile stores: a thread owns one
-// output ROW, so direct stores are 32-byte pieces of 32 different rows per warp instruction (request-rate bound).
+// A kernel supplies the TMA loads of a stage, the wgmma products of a k block (KMajorStage for K-major A and B tiles) and
+// its epilogue.  16-bit outputs leave through staging boxes in the ring (stage_out_offset, staged_slab_begin / _end) as
+// TMA tile stores: a thread owns one output ROW, so direct stores are 32-byte pieces of 32 different rows per warp
+// instruction (request-rate bound).
 #pragma once
 #include <cuda_bf16.h>
 
@@ -135,6 +136,71 @@ struct GemmRing {
   }
 };
 
+// A stage of K-major operands (gemm_tc.cu, conv1d_tc.cu): 128B-swizzled boxes of 64 k, laid out as A hi [128 rows] |
+// B hi [kBTileBytes] and, with kSplit (bf16x3: A_hi*B_hi + A_lo*B_hi + A_hi*B_lo), A lo | B lo behind them.  A bf16x3
+// stage is twice as large, so its ring has half as many stages.
+template <bool kSplit, int kBTileBytes>
+struct KMajorStage {
+  static constexpr int kStages = kSplit ? 2 : 4;
+  static constexpr int kBHi = A_TILE_BYTES;  // offsets in the stage; A hi is at 0
+  static constexpr int kALo = A_TILE_BYTES + kBTileBytes;
+  static constexpr int kBLo = kALo + A_TILE_BYTES;
+  using Ring = GemmRing<kStages, (kSplit ? 2 : 1) * kALo>;
+
+  // TMA bytes of a stage whose B boxes hold block_n rows
+  __host__ __device__ static constexpr uint32_t tx_bytes(int block_n) {
+    return (kSplit ? 2u : 1u) * (uint32_t)(A_TILE_BYTES + block_n * GEMM_BK * 2);
+  }
+
+  // producer: the next stage holds k block kglob of the weights (B boxes at (kglob * 64, n0) of w_hi / w_lo) and the
+  // matching A boxes, which load_a(a_hi or a_lo, full barrier, destination) issues.  kglob is taken by reference: by value,
+  // the compiler assigns the producer loop's uniform registers differently.
+  template <class LoadA>
+  __device__ __forceinline__ static void produce(Ring& ring, bool leader, uint32_t tx, const CUtensorMap* a_hi, const CUtensorMap* a_lo,
+                                                 const CUtensorMap* w_hi, const CUtensorMap* w_lo, const int& kglob, int n0,
+                                                 LoadA&& load_a) {
+    ring.produce(leader, tx, [&](uint64_t* bar, uint8_t* st) {
+      load_a(a_hi, bar, st);
+      tma_load_2d(w_hi, bar, st + kBHi, kglob * GEMM_BK, n0);
+      if (kSplit) {
+        load_a(a_lo, bar, st + kALo);
+        tma_load_2d(w_lo, bar, st + kBLo, kglob * GEMM_BK, n0);
+      }
+    });
+  }
+
+  // consumers: the products of k block kb in the stage at shared address st for warpgroup wg (A rows [64 * wg, +64)) and
+  // the n64 blocks c < nch.  k16 steps outer, n64 blocks inner; bf16x3 then adds the A_lo*B_hi and A_hi*B_lo products of
+  // each k16 step.  The first products of k block 0 overwrite the accumulators.
+  template <int NCH>
+  __device__ __forceinline__ static void mma(float (&acc)[NCH][32], uint32_t st, int wg, int nch, int kb) {
+    const uint32_t a_hi = st + wg * (64 * 128);
+    const uint32_t b_hi = st + kBHi;
+#pragma unroll
+    for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
+      const uint64_t da = make_smem_desc_sw128(a_hi) + 2 * kk;
+#pragma unroll
+      for (int c = 0; c < NCH; ++c)
+        if (c < nch) wgmma_ss_m64n64_bf16<0, 0>(acc[c], da, make_smem_desc_sw128(b_hi + c * (64 * 128)) + 2 * kk, (kb | kk) != 0);
+    }
+    if (kSplit) {
+      const uint32_t a_lo = st + kALo + wg * (64 * 128);
+      const uint32_t b_lo = st + kBLo;
+#pragma unroll
+      for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
+        const uint64_t da_lo = make_smem_desc_sw128(a_lo) + 2 * kk, da_hi = make_smem_desc_sw128(a_hi) + 2 * kk;
+#pragma unroll
+        for (int c = 0; c < NCH; ++c) {
+          if (c < nch) {
+            wgmma_ss_m64n64_bf16<0, 0>(acc[c], da_lo, make_smem_desc_sw128(b_hi + c * (64 * 128)) + 2 * kk, 1);
+            wgmma_ss_m64n64_bf16<0, 0>(acc[c], da_hi, make_smem_desc_sw128(b_lo + c * (64 * 128)) + 2 * kk, 1);
+          }
+        }
+      }
+    }
+  }
+};
+
 // consumers: both warpgroups are done reading the ring; park the tile in it (n64 blocks c < nmma; the rest was not computed)
 template <int NCH>
 __device__ __forceinline__ void park_tile(float* img, int pitch, int wg, int nmma, const float (&acc)[NCH][32]) {
@@ -143,6 +209,16 @@ __device__ __forceinline__ void park_tile(float* img, int pitch, int wg, int nmm
   for (int c = 0; c < NCH; ++c)
     if (c < nmma) acc_store_fragment(img, pitch, wg * 64, c * 64, acc[c]);
   consumer_sync();
+}
+
+// 16 floats of a per-column vector (bias, gamma, beta) as warp-uniform float4 loads; p is 16-byte aligned
+__device__ __forceinline__ void ldg16(const float* __restrict__ p, float (&v)[16]) {
+  const float4* q = reinterpret_cast<const float4*>(p);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float4 f = __ldg(q + j);
+    v[4 * j] = f.x; v[4 * j + 1] = f.y; v[4 * j + 2] = f.z; v[4 * j + 3] = f.w;
+  }
 }
 
 // bf16 of 16 floats, packed pairwise with cvt.rn.bf16x2; pack_hi_lo adds lo = bf16(y - hi)

@@ -47,11 +47,9 @@ struct GemmKParams {
 constexpr int PAIR_MAX_BN = 192;
 template <bool kSplit, bool kPair>
 struct GemmCfg {
-  static constexpr int kStages = kSplit ? 2 : 4;
-  static constexpr int kBTile = kPair ? PAIR_MAX_BN * GEMM_BK * 2 : B_TILE_BYTES;
-  static constexpr int kStageBytes = (kSplit ? 2 : 1) * (A_TILE_BYTES + kBTile);
-  using Ring = GemmRing<kStages, kStageBytes>;
   static constexpr int kMaxBn = kPair ? PAIR_MAX_BN : GEMM_MAX_BN;
+  using Stage = KMajorStage<kSplit, kMaxBn * GEMM_BK * 2>;
+  using Ring = typename Stage::Ring;
   static constexpr int kPitch = acc_pitch(kMaxBn);
   // the plain (non-LayerNorm) epilogue stages two planes; pair mode is LayerNorm-only
   static constexpr int kStageOutOffset = stage_out_offset(kMaxBn);
@@ -99,17 +97,8 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
 // Epilogue for one 128 x block_n accumulator tile (image rows in shared memory).  8 epilogue warps: warp (quarter, half)
 // owns rows [32*quarter, +32) (thread = one output row) and the lower / upper half of the tile's 16-column chunks, so
 // two warps per SM sub-partition interleave and hide each other's latencies.  Per-column vectors (bias, gamma, beta) are read
-// as warp-uniform float4 loads (buffers are padded to n_pad by the host).
+// with ldg16 (buffers are padded to n_pad by the host).
 // ----------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void ldg16(const float* __restrict__ p, float (&v)[16]) {
-  const float4* q = reinterpret_cast<const float4*>(p);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float4 f = __ldg(q + j);
-    v[4 * j] = f.x; v[4 * j + 1] = f.y; v[4 * j + 2] = f.z; v[4 * j + 3] = f.w;
-  }
-}
-
 __device__ __forceinline__ void store_chunk(const GemmKParams& p, size_t orow, int col0, const float (&y)[16]) {
   const size_t o = orow * (size_t)p.ld_out + col0;
   if (p.out_f32) {
@@ -145,6 +134,34 @@ __device__ __forceinline__ void apply_dropout16(float (&y)[16], float p, uint32_
     const uint32_t h = dropout_mix((x0 + (uint32_t)(j >> 1) * DROPOUT_C1) ^ hterm);
     y[j] = (h & 0xffffu) >= t16 ? y[j] * ks : 0.f;
     y[j + 1] = (h >> 16) >= t16 ? y[j + 1] * ks : 0.f;
+  }
+}
+
+// the first steps of every epilogue on the accumulator chunk y (columns n0 + c0 of output row orow): + bias, ReLU, dropout
+// before the residual add.  The bias goes through the caller's scratch chunk aux, and its load and add sit under separate
+// tests: a local array or one test changes how the epilogues' registers are allocated.
+__device__ __forceinline__ void bias_relu_dropout16(const GemmKParams& p, size_t orow, int n0, int c0, float (&aux)[16], float (&y)[16]) {
+  if (p.bias) ldg16(p.bias + n0 + c0, aux);
+  if (p.bias) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) y[j] += aux[j];
+  }
+  if (p.relu) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) y[j] = fmaxf(y[j], 0.f);
+  }
+  if (p.drop_pre_p > 0.f) apply_dropout16(y, p.drop_pre_p, p.drop_seed, p.drop_pre_site, orow * (uint64_t)p.ld_out + n0 + c0);
+}
+
+// zero the columns of a partial tile past N (c0 + j >= ncols) and, unless row_keep, the whole chunk
+__device__ __forceinline__ void zero_outside16(float (&y)[16], bool partial, int c0, int ncols, bool row_keep) {
+  if (partial) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) y[j] = (c0 + j < ncols) ? y[j] : 0.f;
+  }
+  if (!row_keep) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) y[j] = 0.f;
   }
 }
 
@@ -198,26 +215,10 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
 #pragma unroll
         for (int u = 0; u < 2; ++u) {
           const int c0 = (u ? cb : ca) << 4;
-          if (p.bias) ldg16(p.bias + n0 + c0, aux);
 #pragma unroll
           for (int j = 0; j < 16; ++j) y[j] = __uint_as_float(u ? qb[j] : qa[j]);
-          if (p.bias) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) y[j] += aux[j];
-          }
-          if (p.relu) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) y[j] = fmaxf(y[j], 0.f);
-          }
-          if (p.drop_pre_p > 0.f) apply_dropout16(y, p.drop_pre_p, p.drop_seed, p.drop_pre_site, orow * (uint64_t)p.ld_out + n0 + c0);
-          if (partial) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) y[j] = (c0 + j < ncols) ? y[j] : 0.f;
-          }
-          if (!row_keep) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) y[j] = 0.f;
-          }
+          bias_relu_dropout16(p, orow, n0, c0, aux, y);
+          zero_outside16(y, partial, c0, ncols, row_keep);
           uint32_t h[8], l[8];
           if (p.h16) {
 #pragma unroll
@@ -250,32 +251,16 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
       for (int i = 0; i < IN_FLIGHT; ++i) {
         if (g0 + i < ch_end) {   // warp-uniform
           const int c0 = (g0 + i) << 4;
-          if (p.bias) ldg16(p.bias + n0 + c0, aux);
 #pragma unroll
           for (int j = 0; j < 16; ++j) y[j] = __uint_as_float(q[i][j]);
-          if (p.bias) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) y[j] += aux[j];
-          }
-          if (p.relu) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) y[j] = fmaxf(y[j], 0.f);
-          }
-          if (p.drop_pre_p > 0.f) apply_dropout16(y, p.drop_pre_p, p.drop_seed, p.drop_pre_site, orow * (uint64_t)p.ld_out + n0 + c0);
+          bias_relu_dropout16(p, orow, n0, c0, aux, y);
           if (p.residual && row_ok) {
             ld_global_nc_v8f(p.residual + orow * (size_t)p.ld_res + n0 + c0, aux);
             ld_global_nc_v8f(p.residual + orow * (size_t)p.ld_res + n0 + c0 + 8, aux + 8);
 #pragma unroll
             for (int j = 0; j < 16; ++j) y[j] += aux[j];
           }
-          if (partial) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) y[j] = (c0 + j < ncols) ? y[j] : 0.f;
-          }
-          if (!row_keep) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) y[j] = 0.f;
-          }
+          zero_outside16(y, partial, c0, ncols, row_keep);
           if (row_ok) store_chunk(p, orow, n0 + c0, y);
         }
       }
@@ -322,26 +307,14 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
   bool have_k = false;
   auto pass1_chunk = [&](int ch, uint32_t (&rr)[16], float (&rs)[16]) {
     const int c0 = ch << 4;
-    if (p.bias) ldg16(p.bias + n0 + c0, aux);
 #pragma unroll
     for (int j = 0; j < 16; ++j) y[j] = __uint_as_float(rr[j]);
-    if (p.bias) {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) y[j] += aux[j];
-    }
-    if (p.relu) {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) y[j] = fmaxf(y[j], 0.f);
-    }
-    if (p.drop_pre_p > 0.f) apply_dropout16(y, p.drop_pre_p, p.drop_seed, p.drop_pre_site, orow * (uint64_t)p.ld_out + n0 + c0);
+    bias_relu_dropout16(p, orow, n0, c0, aux, y);
     if (has_res) {
 #pragma unroll
       for (int j = 0; j < 16; ++j) y[j] += rs[j];
     }
-    if (partial) {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) y[j] = (c0 + j < ncols) ? y[j] : 0.f;
-    }
+    zero_outside16(y, partial, c0, ncols, true);  // a masked row is zeroed in pass 2
     if (!have_k) { shiftK = y[0]; have_k = true; }   // column c0 of the first chunk is always a logical column when n_h > 0
     if (partial) {
 #pragma unroll
@@ -426,14 +399,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
 #pragma unroll
     for (int j = 0; j < 16; ++j) y[j] = (__uint_as_float(rr[j]) - mean) * rstd * aux[j] + bt[j];
     if (p.drop_post_p > 0.f) apply_dropout16(y, p.drop_post_p, p.drop_seed, p.drop_post_site, orow * (uint64_t)p.ld_out + n0 + c0);
-    if (partial) {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) y[j] = (c0 + j < ncols) ? y[j] : 0.f;
-    }
-    if (!row_keep) {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) y[j] = 0.f;
-    }
+    zero_outside16(y, partial, c0, ncols, row_keep);
     if (row_ok) store_chunk(p, orow, n0 + c0, y);
   };
   __syncwarp();
@@ -482,7 +448,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
   __syncthreads();
   if (kPair) cluster_sync_all();  // the peer's exchange barriers are initialised before anyone arrives on them
 
-  const uint32_t stage_tx = (kSplit ? 2u : 1u) * (uint32_t)(A_TILE_BYTES + p.block_n * GEMM_BK * 2);
+  const uint32_t stage_tx = Cfg::Stage::tx_bytes(p.block_n);
 
   if (warp >= GEMM_EPI_WARPS) {
     setmaxnreg_dec<40>();
@@ -501,14 +467,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
         const CUtensorMap* mh = p.seg_src[s] == 0 ? &tmA0h : &tmA1h;
         const CUtensorMap* ml = p.seg_src[s] == 0 ? &tmA0l : &tmA1l;
         for (int kb = 0; kb < p.seg_kblocks[s]; ++kb, ++kglob) {
-          ring.produce(leader, stage_tx, [&](uint64_t* bar, uint8_t* st) {
-            tma_load_3d(mh, bar, st, kb * GEMM_BK, t0 + p.seg_shift[s], b);
-            tma_load_2d(&tmWh, bar, st + A_TILE_BYTES, kglob * GEMM_BK, n0);
-            if (kSplit) {
-              uint8_t* st2 = st + A_TILE_BYTES + Cfg::kBTile;
-              tma_load_3d(ml, bar, st2, kb * GEMM_BK, t0 + p.seg_shift[s], b);
-              tma_load_2d(&tmWl, bar, st2 + A_TILE_BYTES, kglob * GEMM_BK, n0);
-            }
+          Cfg::Stage::produce(ring, leader, stage_tx, mh, ml, &tmWh, &tmWl, kglob, n0, [&](const CUtensorMap* m, uint64_t* bar, uint8_t* dst) {
+            tma_load_3d(m, bar, dst, kb * GEMM_BK, t0 + p.seg_shift[s], b);
           });
         }
       }
@@ -533,32 +493,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
       const int b = m_tile / p.tiles_per_row;
       const int t0 = (m_tile % p.tiles_per_row) * GEMM_BM;
       float acc[GEMM_NCH][32];
-      ring.mma_tile(total_kb, acc, [&](uint32_t st, int kb) {
-        const uint32_t a_hi = st + wg * (64 * 128);
-        const uint32_t b_hi = st + A_TILE_BYTES;
-#pragma unroll
-        for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
-          const uint64_t da = make_smem_desc_sw128(a_hi) + 2 * kk;
-#pragma unroll
-          for (int c = 0; c < GEMM_NCH; ++c)
-            if (c < nch) wgmma_ss_m64n64_bf16<0, 0>(acc[c], da, make_smem_desc_sw128(b_hi + c * (64 * 128)) + 2 * kk, (kb | kk) != 0);
-        }
-        if (kSplit) {
-          const uint32_t a_lo = st + A_TILE_BYTES + Cfg::kBTile + wg * (64 * 128);
-          const uint32_t b_lo = st + 2 * A_TILE_BYTES + Cfg::kBTile;
-#pragma unroll
-          for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
-            const uint64_t da_lo = make_smem_desc_sw128(a_lo) + 2 * kk, da_hi = make_smem_desc_sw128(a_hi) + 2 * kk;
-#pragma unroll
-            for (int c = 0; c < GEMM_NCH; ++c) {
-              if (c < nch) {
-                wgmma_ss_m64n64_bf16<0, 0>(acc[c], da_lo, make_smem_desc_sw128(b_hi + c * (64 * 128)) + 2 * kk, 1);
-                wgmma_ss_m64n64_bf16<0, 0>(acc[c], da_hi, make_smem_desc_sw128(b_lo + c * (64 * 128)) + 2 * kk, 1);
-              }
-            }
-          }
-        }
-      });
+      ring.mma_tile(total_kb, acc, [&](uint32_t st, int kb) { Cfg::Stage::mma(acc, st, wg, nch, kb); });
       park_tile(img, Cfg::kPitch, wg, nch, acc);
       PairCtx px{};
       if (kPair) {

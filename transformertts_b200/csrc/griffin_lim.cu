@@ -247,16 +247,6 @@ __global__ void gl_batch_table_kernel(const int32_t* __restrict__ off, int n_cli
   }
 }
 
-// largest c in [0, n) with tab[c] <= x, for a non-decreasing tab with tab[0] <= x < tab[n]
-__device__ __forceinline__ int find_clip(const int32_t* __restrict__ tab, int n, int x) {
-  int lo = 0, hi = n;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (__ldg(tab + mid) <= x) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
 __global__ void __launch_bounds__(WARPS * 32)
 istft_frames_batch_kernel(GlProjLoad load, const int32_t* __restrict__ tab, int n_clips, float* __restrict__ frames) {
   __shared__ float sre[WARPS][32 * 33], sim[WARPS][32 * 33];

@@ -362,15 +362,6 @@ stft_mel_v2_kernel(const float* __restrict__ wav, int n_samples, int n_frames, i
 
 // ---- packed ragged batch (ttsb_stft_mel_log_batch).  The clip table (uploaded by the entry point) holds three (n_clips + 1)
 // prefix arrays: so[c] first sample, fo[c] first output frame, po[c] first frame PAIR of clip c.  A pair never spans two clips.
-__device__ __forceinline__ int find_clip(const int32_t* __restrict__ tab, int n, int x) {
-  int lo = 0, hi = n;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (__ldg(tab + mid) <= x) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
 __device__ __forceinline__ void load_batch_pair(const float* __restrict__ wav, const int32_t* __restrict__ tab, int n_clips, int item,
                                                 int lane, float (&re)[32], float (&im)[32]) {
   const int32_t* so = tab;

@@ -35,6 +35,17 @@ __device__ __forceinline__ uint32_t pack_bf16(__nv_bfloat16 a, __nv_bfloat16 b) 
   return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
 }
 
+// The clip of a packed ragged batch that holds item x: the largest c in [0, n) with tab[c] <= x, for a non-decreasing
+// prefix table tab (device memory) with tab[0] <= x
+__device__ __forceinline__ int find_clip(const int32_t* __restrict__ tab, int n, int x) {
+  int lo = 0, hi = n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(tab + mid) <= x) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
 // Stateless dropout decision shared by forward and backward kernels: keep element `idx` of dropout site `site` when the
 // 32-bit mix of (seed, site, idx) is >= thresh = p * 2^32 (keras Dropout semantics: kept values are scaled by 1/(1-p)).
 // c_drop_salt (one copy per translation unit, zero unless a host sets it with ttsb_set_dropout_salt) is XORed into the seed:
