@@ -562,7 +562,8 @@ int ttsb_griffinlim_batch(const float* magnitude, const float* init_angles, cons
                           float* wav_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
- * Ragged-batch Conv1D on the tensor cores (the MelGAN generator, transformertts_b200/model/melgan.py).
+ * Ragged-batch Conv1D on the tensor cores (the MelGAN generator, transformertts_b200/model/melgan.py; the extended form below
+ * serves the HiFi-GAN generator).
  * Layout: a packed ragged batch of n_clips clips, channels-last 16-bit (rows, ld).  Clip c has L_c rows, given as the int32
  * prefix sums clip_offsets[0..n_clips] (HOST memory, clip_offsets[0] = 0), framed by TTSB_CONV1D_HALO halo rows on each
  * side: its rows are clip_offsets[c] + (2c + 1) HALO + [0, L_c), and the buffer holds clip_offsets[n_clips] + 2 HALO n_clips
@@ -619,6 +620,68 @@ int ttsb_conv1d_tc(const ttsb_conv1d_args* a, void* stream);
 int ttsb_conv1d_out_tanh(const void* in_hi, const void* in_lo, int ld_in, int channels, const int32_t* clip_offsets, int n_clips,
                          int drop_tail, const float* weight, float bias, void* workspace, int64_t workspace_bytes, float* wav_out,
                          void* stream);
+
+/* The same conv in its extended form (the HiFi-GAN generator, transformertts_b200/model/hifigan.py).  Differences from
+ * ttsb_conv1d_tc:
+ *   halo       halo rows on each side of every clip, 0..TTSB_CONV1D_EX_MAX_HALO, for the inputs and the outputs alike;
+ *              |tap_shift| <= halo, and up to TTSB_CONV1D_EX_MAX_TAPS taps.
+ *   slope      act = LeakyReLU_slope(y), slope in [0, 1].
+ *   res_hi/lo  optional residual in the output layout (ld_out columns, res_lo only in bf16x3): y = bias + conv + (res_hi + res_lo).
+ *              It must not alias out_hi or act_hi.
+ *   sum        optional fp32 plane in the output layout, for the multi-receptive-field average of HiFi-GAN's resblocks, in torch's
+ *              order (xs = rb_0(x); xs += rb_1(x); ...; x = xs / nk), after the residual:
+ *                TTSB_CONV1D_SUM_WRITE  sum = y                 (resblock 0)
+ *                TTSB_CONV1D_SUM_ADD    sum = sum + y           (the middle resblocks)
+ *                TTSB_CONV1D_SUM_FINISH y = (sum + y) / sum_div (the last one; then out / act are written from this y)
+ *              WRITE and ADD count as an output, so out and act may both be NULL.
+ *   out_rows   rows of the output layout, sum up L_c + 2 halo n_clips: the shape of the outputs, the residual and the sum.
+ * res_hi, res_lo and sum are 16-byte aligned.  With TTSB_HALO_NONE and zero-initialised planes the halos stay zero (no
+ * computed row is ever stored into a halo), which is every zero-padded conv's padding, and clips of any length >= 1 work.
+ * ttsb_conv1d_out_tanh_ex is ttsb_conv1d_out_tanh over a layout of `halo` (3..TTSB_CONV1D_EX_MAX_HALO) rows, whose halos hold
+ * the padding (zeros for HiFi-GAN); it needs only L_c > drop_tail.  The refusals are those of ttsb_conv1d_tc, plus any
+ * inconsistent halo, slope, residual, sum or out_rows, all before any CUDA call. */
+#define TTSB_CONV1D_EX_MAX_TAPS 16
+#define TTSB_CONV1D_EX_MAX_HALO 64
+#define TTSB_CONV1D_SUM_NONE 0
+#define TTSB_CONV1D_SUM_WRITE 1
+#define TTSB_CONV1D_SUM_ADD 2
+#define TTSB_CONV1D_SUM_FINISH 3
+typedef struct ttsb_conv1d_ex_args {
+  int n_clips;
+  const int32_t* clip_offsets; /* HOST, int32 (n_clips + 1) */
+  int halo;
+  int num_taps;
+  int tap_src[TTSB_CONV1D_EX_MAX_TAPS];
+  int tap_shift[TTSB_CONV1D_EX_MAX_TAPS];
+  const void* in_hi[2];
+  const void* in_lo[2];
+  int ld_in[2];
+  const void* w_hi;
+  const void* w_lo;
+  const float* bias; /* fp32 (N), or NULL */
+  int N;
+  int up;
+  const void* res_hi; /* or NULL */
+  const void* res_lo;
+  float* sum; /* fp32 (out_rows, ld_out), or NULL */
+  int sum_mode;
+  float sum_div;
+  void* out_hi;
+  void* out_lo;
+  void* act_hi;
+  void* act_lo;
+  int ld_out;
+  int64_t out_rows;
+  float slope;
+  int halo_mode;
+  int precision; /* TTSB_PREC_BF16 or TTSB_PREC_BF16X3 */
+  void* workspace;
+  int64_t workspace_bytes;
+} ttsb_conv1d_ex_args;
+int ttsb_conv1d_ex_tc(const ttsb_conv1d_ex_args* a, void* stream);
+int ttsb_conv1d_out_tanh_ex(const void* in_hi, const void* in_lo, int ld_in, int channels, int halo, const int32_t* clip_offsets,
+                            int n_clips, int drop_tail, const float* weight, float bias, void* workspace, int64_t workspace_bytes,
+                            float* wav_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Data-parallel gradient exchange (BASELINE.json: "NCCL allreduce over NVLink on gradient buckets only"; the reference has

@@ -4,13 +4,17 @@
     python predict_tts.py -f lines.txt [-p MODEL_DIR | --step 95000] [-o OUTDIR] [-m] [-s] [-v]
     python predict_tts.py -t "phoneme string" ...
     python predict_tts.py -f lines.txt --vocoder melgan --vocoder_checkpoint melgan.pt ...
+    python predict_tts.py -f lines.txt --vocoder hifigan --vocoder_checkpoint g_02500000 [--vocoder_config v1|config.json] ...
 
 Every input line is tokenised, turned into a mel by ``ForwardTransformer.predict`` (one line per call, as the reference does)
 and vocoded on the GPU with ``Audio.reconstruct_waveform_batch`` (mel inversion + 32 Griffin-Lim iterations), in chunks of
 ``VOCODE_CHUNK`` lines so that device memory stays bounded however long the file is.  With ``--vocoder melgan`` the chunks
 go through a MelGAN generator instead (``MelGANGenerator.vocode_batch``, weights from ``--vocoder_checkpoint``), as the
 reference's synthesis notebook does one line at a time; a line of T frames then gives 256 T samples (Griffin-Lim:
-256 (T - 1)).  Output:
+256 (T - 1)).  With ``--vocoder hifigan`` they go through a HiFi-GAN generator (``HiFiGANGenerator.vocode_batch``, a
+jik876/hifi-gan checkpoint; its config is ``--vocoder_config``, a config.json path or v1 / v2 / v3, by default the
+config.json beside the checkpoint), also 256 T samples per line; HiFi-GAN takes the MelGAN normaliser's log-mels, so a
+model with another ``normalizer`` is refused.  Output:
 ``<outdir>/outputs/<fname>/<fname>_<data_name>_<git_hash>_<step>.wav``, the concatenation of all lines; with ``--single`` also
 ``..._<i>.wav`` per line, with ``--store_mel`` ``..._<i>.mel.npy`` (the (T, n_mels) mel of line i).
 
@@ -44,11 +48,15 @@ def parse_args(argv=None):
     parser.add_argument('--store_mel', '-m', dest='store_mel', action='store_true')
     parser.add_argument('--verbose', '-v', dest='verbose', action='store_true')
     parser.add_argument('--single', '-s', dest='single', action='store_true')
-    parser.add_argument('--vocoder', dest='vocoder', default='griffinlim', choices=('griffinlim', 'melgan'))
+    parser.add_argument('--vocoder', dest='vocoder', default='griffinlim', choices=('griffinlim', 'melgan', 'hifigan'))
     parser.add_argument('--vocoder_checkpoint', dest='vocoder_checkpoint', default=None, type=str)
+    parser.add_argument('--vocoder_config', dest='vocoder_config', default=None, type=str,
+                        help='HiFi-GAN config: a config.json path or v1 / v2 / v3 (default: config.json beside the checkpoint)')
     args = parser.parse_args(argv)
-    if args.vocoder == 'melgan' and args.vocoder_checkpoint is None:
-        parser.error('--vocoder melgan needs --vocoder_checkpoint PATH')
+    if args.vocoder in ('melgan', 'hifigan') and args.vocoder_checkpoint is None:
+        parser.error(f'--vocoder {args.vocoder} needs --vocoder_checkpoint PATH')
+    if args.vocoder_config is not None and args.vocoder != 'hifigan':
+        parser.error('--vocoder_config applies to --vocoder hifigan only')
     return args
 
 
@@ -118,6 +126,13 @@ def main(argv=None):
     if args.vocoder == 'melgan':
         from transformertts_b200.model.melgan import MelGANGenerator
         vocoder = MelGANGenerator.from_checkpoint(args.vocoder_checkpoint, device=model.device)
+    elif args.vocoder == 'hifigan':
+        normalizer = model.config.get('normalizer')
+        if normalizer != 'MelGAN':
+            raise SystemExit(f'--vocoder hifigan takes the MelGAN normaliser\'s log-mels (ln(max(S, 1e-5))); this model\'s normalizer '
+                             f'is {normalizer!r}, whose mels HiFi-GAN would misread')
+        from transformertts_b200.model.hifigan import HiFiGANGenerator
+        vocoder = HiFiGANGenerator.from_checkpoint(args.vocoder_checkpoint, config=args.vocoder_config, device=model.device)
     print(f'Output wav under {output_path.parent}')
     wavs = []
     for start in range(0, len(text), VOCODE_CHUNK):

@@ -1,6 +1,7 @@
-"""Mel -> waveform with the MelGAN generator for a file's worth of utterances.
+"""Mel -> waveform with the MelGAN or HiFi-GAN generator for a file's worth of utterances.
 
     python tools/vocoder_bench.py [--clips 64] [--reps 3] [--out DIR]
+    python tools/vocoder_bench.py --vocoder hifigan [--config v1|v2|v3] [--clips 64] [--reps 3] [--out DIR]
 
 Workload: that of tools/synth_bench.py -- `--clips` seeded ragged clips of 2-10 s (T_c uniform in 173..862 frames), mels from
 the CUDA front end (Audio.mel_spectrogram) -- and a seeded generator checkpoint (oracle/melgan_oracle.py, seed 0).  Paths:
@@ -13,7 +14,12 @@ Every path runs once before timing; a timing is the host clock around whole call
 averaged over `--reps` calls.  FLOPs are counted from the layer shapes (multiply-adds x 2, the useful products only: the
 zero-padded columns of the 32-channel stage are not counted).  Prints one JSON line: seconds per call, seconds of audio per
 second, library launches per call, achieved TFLOP/s, the largest |difference| of each vocode_batch mode from the notebook
-path, and the card name and power limit read in the same run.  `--out` also writes it to DIR/vocoder_bench.json."""
+path, and the card name and power limit read in the same run.  `--out` also writes it to DIR/vocoder_bench.json.
+
+With `--vocoder hifigan` the same clips go through a seeded HiFi-GAN generator of `--config` (oracle/hifigan_oracle.py,
+seed 0), without pad frames.  Paths: `module`, jik876's generator as a torch module in fp32 on the GPU (cuDNN, TF32 off), one
+clip per call as its inference.py runs it; `bf16x3` and `bf16`, HiFiGANGenerator.vocode_batch with all clips in one call.
+FLOPs count the useful products of every conv (a transposed conv's output row sums 2 of its k taps per input channel)."""
 import argparse
 import json
 import subprocess
@@ -26,9 +32,11 @@ import torch
 
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 from oracle import audio_oracle as ao  # noqa: E402
+from oracle import hifigan_oracle as ho  # noqa: E402
 from oracle import melgan_oracle as mo  # noqa: E402
 from transformertts_b200 import lib  # noqa: E402
 from transformertts_b200.data.audio import Audio  # noqa: E402
+from transformertts_b200.model import hifigan as hg  # noqa: E402
 from transformertts_b200.model import melgan as mg  # noqa: E402
 
 
@@ -66,11 +74,59 @@ def generator_flops(frames) -> float:
     return total
 
 
+def hifigan_flops(h: dict, frames) -> float:
+    """FLOPs of one HiFi-GAN forward over clips of frames[c] frames, from the layer shapes."""
+    shapes = hg.layer_shapes(h)
+    rates = h['upsample_rates']
+    total = 0.0
+    for L in frames:
+        total += 2.0 * L * int(np.prod(shapes['conv_pre'][1]))
+        rows = L
+        for i, u in enumerate(rates):
+            cin, cout, _ = shapes[f'ups.{i}'][1]
+            rows *= u
+            total += 2.0 * rows * cout * cin * 2
+            ch = cout
+            total += sum(2.0 * rows * int(np.prod(s)) for n, (_, s) in shapes.items() if n.startswith('resblocks.') and s[0] == ch)
+        total += 2.0 * rows * int(np.prod(shapes['conv_post'][1]))
+    return total
+
+
+def hifigan_main(args, mels, lengths):
+    h = hg.load_config(args.config)
+    sd = ho.init_state_dict(h, seed=0)
+    module = ho.build(h, sd, dtype=torch.float32).cuda()
+
+    def per_clip():
+        with torch.no_grad():
+            return [module(torch.from_numpy(m).cuda()[None])[0, 0].cpu().numpy() for m in mels]
+
+    res = dict(workload='hifigan_vocode', config=args.config, clips=args.clips, frames=int(lengths.sum()), min_frames=int(lengths.min()),
+               max_frames=int(lengths.max()), reps=args.reps, audio_s=round(float(256 * lengths.sum() / 22050), 1))
+    flops = hifigan_flops(h, [int(T) for T in lengths])
+    res['gflop_per_call'] = round(flops / 1e9, 1)
+    res['gflop_per_audio_s'] = round(flops / 1e9 / res['audio_s'], 2)
+    t, launches, w_ref = timed(per_clip, args.reps)
+    res.update(module_s=round(t, 5), module_audio_s_per_s=round(res['audio_s'] / t, 1), module_tflops=round(flops / t / 1e12, 2))
+    del module
+    for prec in ('bf16x3', 'bf16'):
+        g = hg.HiFiGANGenerator(h, device='cuda', precision=prec).load_state_dict(sd)
+        t, launches, w = timed(lambda: g.vocode_batch(mels), args.reps)
+        res.update({f'{prec}_s': round(t, 5), f'{prec}_audio_s_per_s': round(res['audio_s'] / t, 1), f'{prec}_launches': launches,
+                    f'{prec}_tflops': round(flops / t / 1e12, 2),
+                    f'{prec}_max_abs_diff_vs_module': float(max(np.abs(a - b).max() for a, b in zip(w, w_ref)))})
+        del g
+        torch.cuda.empty_cache()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--clips', type=int, default=64)
     ap.add_argument('--reps', type=int, default=3)
     ap.add_argument('--out', default=None)
+    ap.add_argument('--vocoder', choices=('melgan', 'hifigan'), default='melgan')
+    ap.add_argument('--config', default='v1', help='HiFi-GAN config: v1 / v2 / v3 or a config.json path')
     args = ap.parse_args()
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
@@ -78,6 +134,8 @@ def main():
                   normalizer='MelGAN')
     lengths = np.random.default_rng(2024).integers(173, 863, size=args.clips)
     mels = [audio.mel_spectrogram(ao.make_clips(1, 256 * (int(T) - 1), seed=500 + c)[0]).T for c, T in enumerate(lengths)]
+    if args.vocoder == 'hifigan':
+        return report(hifigan_main(args, mels, lengths), args)
     sd = mo.init_state_dict(seed=0)
     module = mo.build(sd, dtype=torch.float32).cuda()
     pad = torch.full((1, 80, mo.PAD_FRAMES), mo.PAD_VALUE, device='cuda')
@@ -102,6 +160,10 @@ def main():
         del g
     t, launches, _ = timed(lambda: audio.reconstruct_waveform_batch(mels, seed=0), args.reps)
     res.update(griffinlim_s=round(t, 5), griffinlim_audio_s_per_s=round(res['audio_s'] / t, 1), griffinlim_launches=launches)
+    report(res, args)
+
+
+def report(res, args):
     res['card'] = card()
     line = json.dumps(res)
     print(line)

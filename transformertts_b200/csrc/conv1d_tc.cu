@@ -1,9 +1,12 @@
-// Ragged-batch Conv1D on the pipeline of gemm_pipeline.cuh (ttsb_conv1d_tc), for the MelGAN generator: dilated 3-tap convs,
-// the ResStack's shortcut + 1x1 conv as one two-source product, transposed convs phrased over their input rows, and the
-// 7-tap input conv.  Clips are packed channels-last with TTSB_CONV1D_HALO halo rows on each side (include/ttsb.h), so a tap
-// is a row shift of a 2-D TMA load and a 128-row tile may span several clips.  The epilogue (one thread per row) maps the
-// row to its clip, skips halo rows, adds the bias, writes y and LeakyReLU(y) as bf16 hi/lo planes and mirrors the rows next
-// to each clip edge into the halos the next conv reads.  ttsb_conv1d_out_tanh is the generator's N = 1 output layer.
+// Ragged-batch Conv1D on the pipeline of gemm_pipeline.cuh, for the MelGAN and HiFi-GAN generators: dilated convs, the
+// ResStack's shortcut + 1x1 conv as one two-source product, transposed convs phrased over their input rows, and the input
+// convs.  Clips are packed channels-last with `halo` rows on each side (include/ttsb.h), so a tap is a row shift of a 2-D TMA
+// load and a 128-row tile may span several clips.  The epilogue (one thread per row) maps the row to its clip, skips halo
+// rows, adds the bias (and in the extended form a residual and the multi-receptive-field sum), writes y and LeakyReLU(y) as
+// bf16 hi/lo planes and mirrors the rows next to each clip edge into the halos the next conv reads.
+// ttsb_conv1d_tc (MelGAN: 9 halo rows, slope 0.2) and ttsb_conv1d_ex_tc (any halo up to 64, up to 16 taps, any slope, residual
+// and sum) run the same kernel template; kEx = false compiles the residual and sum steps out and fixes the halo and slope.
+// ttsb_conv1d_out_tanh / ttsb_conv1d_out_tanh_ex are the generators' N = 1 output layer.
 #include <vector>
 
 #include "../../include/ttsb.h"
@@ -12,18 +15,25 @@
 namespace ttsb {
 
 constexpr int CONV_HALO = TTSB_CONV1D_HALO;
-constexpr float LRELU_SLOPE = 0.2f;
+constexpr float LRELU_SLOPE = 0.2f;  // ttsb_conv1d_tc's LeakyReLU
 
 struct ConvKParams {
   int rows;  // GEMM rows: every row of the packed input layout, halos included
   int N, block_n, n_tiles, num_tiles;
   int num_taps;
-  int tap_src[TTSB_CONV1D_MAX_TAPS], tap_shift[TTSB_CONV1D_MAX_TAPS];
+  int tap_src[TTSB_CONV1D_EX_MAX_TAPS], tap_shift[TTSB_CONV1D_EX_MAX_TAPS];
   int kblocks[2];
   int n_clips;
   const int32_t* tab;  // device: region start rows [n_clips + 1], then the clip_offsets prefix sums [n_clips + 1]
   int up, halo_mode, ld_out;
+  int halo;     // kEx only (else CONV_HALO)
+  float slope;  // kEx only (else LRELU_SLOPE)
   const float* bias;
+  const __nv_bfloat16* res_hi;  // kEx only: residual planes, output layout
+  const __nv_bfloat16* res_lo;
+  float* sum;                   // kEx only: fp32 multi-receptive-field sum, output layout
+  int sum_mode;
+  float sum_div;
   __nv_bfloat16* out_hi;
   __nv_bfloat16* out_lo;
   __nv_bfloat16* act_hi;
@@ -40,7 +50,7 @@ struct ConvCfg {
 };
 
 // 16 columns of output row orow: y (and LeakyReLU(y)) as bf16 hi/lo, or zeros
-__device__ __forceinline__ void conv_store16(const ConvKParams& p, size_t orow, int col, const float (&y)[16], bool zero) {
+__device__ __forceinline__ void conv_store16(const ConvKParams& p, size_t orow, int col, const float (&y)[16], bool zero, float slope) {
   const size_t o = orow * (size_t)p.ld_out + col;
   uint32_t h[8], l[8];
   float v[16];
@@ -53,24 +63,61 @@ __device__ __forceinline__ void conv_store16(const ConvKParams& p, size_t orow, 
   }
   if (p.act_hi) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j) v[j] = zero ? 0.f : (y[j] > 0.f ? y[j] : LRELU_SLOPE * y[j]);
+    for (int j = 0; j < 16; ++j) v[j] = zero ? 0.f : (y[j] > 0.f ? y[j] : slope * y[j]);
     pack_hi_lo(v, h, l, p.act_lo != nullptr);
     st_global_v8(p.act_hi + o, h);
     if (p.act_lo) st_global_v8(p.act_lo + o, l);
   }
 }
 
+// residual (hi + lo) and multi-receptive-field sum steps of ttsb_conv1d_ex_tc on 16 columns of output row orow
+__device__ __forceinline__ void conv_res_sum16(const ConvKParams& p, size_t orow, int col, float (&y)[16]) {
+  const size_t o = orow * (size_t)p.ld_out + col;
+  if (p.res_hi) {
+    uint32_t h[8], l[8];
+    ld_global_nc_v8(p.res_hi + o, h);
+    if (p.res_lo) ld_global_nc_v8(p.res_lo + o, l);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      float r0 = __uint_as_float(h[k] << 16), r1 = __uint_as_float(h[k] & 0xffff0000u);
+      if (p.res_lo) { r0 += __uint_as_float(l[k] << 16); r1 += __uint_as_float(l[k] & 0xffff0000u); }
+      y[2 * k] += r0;
+      y[2 * k + 1] += r1;
+    }
+  }
+  if (p.sum_mode == TTSB_CONV1D_SUM_WRITE) {
+    st_global_v8f(p.sum + o, y);
+    st_global_v8f(p.sum + o + 8, y + 8);
+  } else if (p.sum_mode != TTSB_CONV1D_SUM_NONE) {  // torch's order: sum = sum + y; the last add is followed by / nk
+    float s[16];
+#pragma unroll
+    for (int k = 0; k < 16; k += 4) *reinterpret_cast<float4*>(s + k) = *reinterpret_cast<const float4*>(p.sum + o + k);
+#pragma unroll
+    for (int k = 0; k < 16; ++k) s[k] += y[k];
+    if (p.sum_mode == TTSB_CONV1D_SUM_ADD) {
+      st_global_v8f(p.sum + o, s);
+      st_global_v8f(p.sum + o + 8, s + 8);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 16; ++k) y[k] = s[k] / p.sum_div;
+    }
+  }
+}
+
+template <bool kEx>
 __device__ __forceinline__ void conv_epilogue(const ConvKParams& p, const float* arow, int g, int n0, int half) {
   if (g >= p.rows) return;
+  const int H = kEx ? p.halo : CONV_HALO;
+  const float slope = kEx ? p.slope : LRELU_SLOPE;
   const int32_t* reg = p.tab;
   const int32_t* off = p.tab + p.n_clips + 1;
   const int c = find_clip(reg, p.n_clips, g);
   const int off_c = __ldg(off + c);
   const int L = __ldg(off + c + 1) - off_c;
-  const int j = g - __ldg(reg + c) - CONV_HALO;
+  const int j = g - __ldg(reg + c) - H;
   if (j < 0 || j >= L) return;  // a halo row: written only by the mirror stores of the rows it copies
   const int Lo = L * p.up;
-  const long long base = (long long)off_c * p.up + (long long)(2 * c + 1) * CONV_HALO;  // output row of clip position 0
+  const long long base = (long long)off_c * p.up + (long long)(2 * c + 1) * H;  // output row of clip position 0
   const int nch = p.block_n >> 4;
   const int ch_begin = half ? (nch + 1) >> 1 : 0;
   const int ch_end = half ? nch : (nch + 1) >> 1;
@@ -88,19 +135,20 @@ __device__ __forceinline__ void conv_epilogue(const ConvKParams& p, const float*
     }
     const int phase = col / p.ld_out, cc = col - phase * p.ld_out;
     const int pos = j * p.up + phase;  // position in the output clip
-    conv_store16(p, (size_t)(base + pos), cc, y, false);
+    if (kEx) conv_res_sum16(p, (size_t)(base + pos), cc, y);
+    conv_store16(p, (size_t)(base + pos), cc, y, false, slope);
     if (p.halo_mode == TTSB_HALO_REFLECT) {
-      if (pos >= 1 && pos <= CONV_HALO) conv_store16(p, (size_t)(base - pos), cc, y, false);
-      if (pos >= Lo - 1 - CONV_HALO && pos <= Lo - 2) conv_store16(p, (size_t)(base + 2 * (Lo - 1) - pos), cc, y, false);
+      if (pos >= 1 && pos <= H) conv_store16(p, (size_t)(base - pos), cc, y, false, slope);
+      if (pos >= Lo - 1 - H && pos <= Lo - 2) conv_store16(p, (size_t)(base + 2 * (Lo - 1) - pos), cc, y, false, slope);
     } else if (p.halo_mode == TTSB_HALO_ZERO) {
-      if (pos < CONV_HALO) conv_store16(p, (size_t)(base - 1 - pos), cc, y, true);
-      if (pos >= Lo - CONV_HALO) conv_store16(p, (size_t)(base + 2 * Lo - 1 - pos), cc, y, true);
+      if (pos < H) conv_store16(p, (size_t)(base - 1 - pos), cc, y, true, slope);
+      if (pos >= Lo - H) conv_store16(p, (size_t)(base + 2 * Lo - 1 - pos), cc, y, true, slope);
     }
   }
 }
 
 // tensor maps: A[src][hi/lo] (ld_in[src], rows) boxes (64, 128); W[hi/lo] (K_total, N) boxes (64, block_n)
-template <bool kSplit>
+template <bool kSplit, bool kEx>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant__ CUtensorMap tmA0l,
                  const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUtensorMap tmA1l,
@@ -160,7 +208,7 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constan
       park_tile(img, Cfg::kPitch, wg, nch, acc);
       const int row = quarter * 32 + lane;
       __syncwarp();
-      conv_epilogue(p, img + (size_t)row * Cfg::kPitch, m0 + row, n0, half);
+      conv_epilogue<kEx>(p, img + (size_t)row * Cfg::kPitch, m0 + row, n0, half);
       ring.release_tile(false);
     }
   }
@@ -168,9 +216,10 @@ done:
   __syncthreads();
 }
 
-// one thread per output sample: tanh(bias + 7-tap dot product over the reflect-padded channels), fixed summation order
+// one thread per output sample: tanh(bias + 7-tap dot product over the padded channels), fixed summation order; the 3 rows of
+// padding on each side are the clip's halo rows (reflected for MelGAN, zeros for HiFi-GAN)
 __global__ void __launch_bounds__(256)
-conv1d_out_tanh_kernel(const __nv_bfloat16* __restrict__ in_hi, const __nv_bfloat16* __restrict__ in_lo, int ld_in, int channels,
+conv1d_out_tanh_kernel(const __nv_bfloat16* __restrict__ in_hi, const __nv_bfloat16* __restrict__ in_lo, int ld_in, int channels, int halo,
                        const int32_t* __restrict__ tab, int n_clips, int drop_tail, const float* __restrict__ weight, float bias,
                        int total, float* __restrict__ wav_out) {
   extern __shared__ float sw[];  // (7, channels)
@@ -182,7 +231,7 @@ conv1d_out_tanh_kernel(const __nv_bfloat16* __restrict__ in_hi, const __nv_bfloa
     const int off_c = __ldg(off + c);
     const int j = i - off_c;
     if (j >= __ldg(off + c + 1) - off_c - drop_tail) continue;
-    const size_t row = (size_t)__ldg(tab + c) + CONV_HALO + j;
+    const size_t row = (size_t)__ldg(tab + c) + halo + j;
     float acc = bias;
     for (int k = 0; k < 7; ++k) {
       const __nv_bfloat16* h = in_hi + (row + k - 3) * (size_t)ld_in;
@@ -197,9 +246,10 @@ conv1d_out_tanh_kernel(const __nv_bfloat16* __restrict__ in_hi, const __nv_bfloa
   }
 }
 
-// checks the host offset table and fills tab (region starts, prefix sums); min_out_len: the least up * L_c; 0 on success
-static int conv_table(const char* what, const int32_t* clip_offsets, int n_clips, int up, int min_out_len, std::vector<int32_t>& tab,
-                      long long* rows) {
+// checks the host offset table and fills tab (region starts, prefix sums); min_out_len: the least up * L_c; *rows: input
+// rows, *out_rows: output rows of the layout; 0 on success
+static int conv_table(const char* what, const int32_t* clip_offsets, int n_clips, int up, int halo, int min_out_len, std::vector<int32_t>& tab,
+                      long long* rows, long long* out_rows) {
   if (!clip_offsets) { set_last_error("%s: clip_offsets is NULL", what); return TTSB_ERR_INVALID_ARGUMENT; }
   if (n_clips < 1) { set_last_error("%s: n_clips must be >= 1", what); return TTSB_ERR_INVALID_ARGUMENT; }
   if (clip_offsets[0] != 0) { set_last_error("%s: clip_offsets[0] must be 0", what); return TTSB_ERR_INVALID_ARGUMENT; }
@@ -212,13 +262,17 @@ static int conv_table(const char* what, const int32_t* clip_offsets, int n_clips
       return TTSB_ERR_INVALID_ARGUMENT;
     }
   }
-  const long long total = (long long)clip_offsets[n_clips] * up + 2LL * CONV_HALO * n_clips;
-  if (total > INT32_MAX) { set_last_error("%s: too many rows", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  const long long total = (long long)clip_offsets[n_clips] * up + 2LL * halo * n_clips;
+  if (total > INT32_MAX || (long long)clip_offsets[n_clips] + 2LL * halo * n_clips > INT32_MAX) {
+    set_last_error("%s: too many rows", what);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
   for (int c = 0; c <= n_clips; ++c) {
-    tab[c] = clip_offsets[c] + 2 * CONV_HALO * c;
+    tab[c] = clip_offsets[c] + 2 * halo * c;
     tab[n_clips + 1 + c] = clip_offsets[c];
   }
-  *rows = (long long)clip_offsets[n_clips] + 2LL * CONV_HALO * n_clips;
+  *rows = (long long)clip_offsets[n_clips] + 2LL * halo * n_clips;
+  *out_rows = total;
   return 0;
 }
 
@@ -230,45 +284,56 @@ static int check_workspace(const char* what, const void* ws, int64_t bytes, int 
   return 0;
 }
 
-}  // namespace ttsb
-
-using namespace ttsb;
-
-extern "C" int64_t ttsb_conv1d_workspace_bytes(int n_clips) {
-  if (n_clips < 1) {
-    set_last_error("ttsb_conv1d_workspace_bytes: n_clips < 1");
-    return -1;
-  }
-  return 2 * (int64_t)(n_clips + 1) * (int64_t)sizeof(int32_t);
-}
-
-extern "C" int ttsb_conv1d_tc(const ttsb_conv1d_args* a, void* stream_v) {
-  const char* what = "ttsb_conv1d_tc";
-  if (!a) { set_last_error("ttsb_conv1d_tc: args is NULL"); return TTSB_ERR_INVALID_ARGUMENT; }
-  if (a->precision != TTSB_PREC_BF16 && a->precision != TTSB_PREC_BF16X3) { set_last_error("ttsb_conv1d_tc: unknown precision"); return TTSB_ERR_INVALID_ARGUMENT; }
+// the shared host side of ttsb_conv1d_tc (ex = false: no residual or sum, out_rows unchecked) and ttsb_conv1d_ex_tc
+static int conv1d_launch(const char* what, const ttsb_conv1d_ex_args* a, bool ex, int max_taps, void* stream_v) {
+  if (a->precision != TTSB_PREC_BF16 && a->precision != TTSB_PREC_BF16X3) { set_last_error("%s: unknown precision", what); return TTSB_ERR_INVALID_ARGUMENT; }
   const bool split = a->precision == TTSB_PREC_BF16X3;
-  if (a->num_taps < 1 || a->num_taps > TTSB_CONV1D_MAX_TAPS) { set_last_error("ttsb_conv1d_tc: num_taps must be in [1, 7]"); return TTSB_ERR_INVALID_ARGUMENT; }
+  const int H = a->halo;
+  if (H < 0 || H > TTSB_CONV1D_EX_MAX_HALO) { set_last_error("%s: halo = %d must be in [0, %d]", what, H, TTSB_CONV1D_EX_MAX_HALO); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (a->num_taps < 1 || a->num_taps > max_taps) { set_last_error("%s: num_taps must be in [1, %d]", what, max_taps); return TTSB_ERR_INVALID_ARGUMENT; }
   int k_total = 0;
   for (int s = 0; s < a->num_taps; ++s) {
     const int src = a->tap_src[s];
     if (src < 0 || src > 1 || !a->in_hi[src] || (split && !a->in_lo[src])) {
-      set_last_error("ttsb_conv1d_tc: tap %d reads source %d, which is missing (bf16x3 needs in_lo too)", s, src);
+      set_last_error("%s: tap %d reads source %d, which is missing (bf16x3 needs in_lo too)", what, s, src);
       return TTSB_ERR_INVALID_ARGUMENT;
     }
-    if (a->ld_in[src] < GEMM_BK || a->ld_in[src] % GEMM_BK) { set_last_error("ttsb_conv1d_tc: ld_in[%d] = %d must be a positive multiple of 64", src, a->ld_in[src]); return TTSB_ERR_INVALID_ARGUMENT; }
-    if (a->tap_shift[s] < -CONV_HALO || a->tap_shift[s] > CONV_HALO) { set_last_error("ttsb_conv1d_tc: |tap_shift| must be <= %d", CONV_HALO); return TTSB_ERR_INVALID_ARGUMENT; }
+    if (a->ld_in[src] < GEMM_BK || a->ld_in[src] % GEMM_BK) { set_last_error("%s: ld_in[%d] = %d must be a positive multiple of 64", what, src, a->ld_in[src]); return TTSB_ERR_INVALID_ARGUMENT; }
+    if (a->tap_shift[s] < -H || a->tap_shift[s] > H) { set_last_error("%s: |tap_shift| must be <= %d (the halo)", what, H); return TTSB_ERR_INVALID_ARGUMENT; }
     k_total += a->ld_in[src];
   }
-  if (!a->w_hi || (split && !a->w_lo)) { set_last_error("ttsb_conv1d_tc: missing packed weights"); return TTSB_ERR_INVALID_ARGUMENT; }
-  if (a->N < 64 || a->N % 64 || (a->N > GEMM_MAX_BN && a->N % GEMM_MAX_BN)) { set_last_error("ttsb_conv1d_tc: N = %d must be a multiple of 64, at most 256 or a multiple of 256", a->N); return TTSB_ERR_INVALID_ARGUMENT; }
-  if (a->up < 1 || a->N % a->up || a->N / a->up != a->ld_out || a->ld_out % 16) { set_last_error("ttsb_conv1d_tc: need N = up * ld_out with ld_out a multiple of 16"); return TTSB_ERR_INVALID_ARGUMENT; }
-  if (a->halo_mode < TTSB_HALO_NONE || a->halo_mode > TTSB_HALO_ZERO) { set_last_error("ttsb_conv1d_tc: unknown halo_mode"); return TTSB_ERR_INVALID_ARGUMENT; }
-  if (!a->out_hi && !a->act_hi) { set_last_error("ttsb_conv1d_tc: no output"); return TTSB_ERR_INVALID_ARGUMENT; }
-  const int min_len = a->halo_mode == TTSB_HALO_REFLECT ? CONV_HALO + 1 : (a->halo_mode == TTSB_HALO_ZERO ? CONV_HALO : 1);
+  if (!a->w_hi || (split && !a->w_lo)) { set_last_error("%s: missing packed weights", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (a->N < 64 || a->N % 64 || (a->N > GEMM_MAX_BN && a->N % GEMM_MAX_BN)) { set_last_error("%s: N = %d must be a multiple of 64, at most 256 or a multiple of 256", what, a->N); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (a->up < 1 || a->N % a->up || a->N / a->up != a->ld_out || a->ld_out % 16) { set_last_error("%s: need N = up * ld_out with ld_out a multiple of 16", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (a->halo_mode < TTSB_HALO_NONE || a->halo_mode > TTSB_HALO_ZERO) { set_last_error("%s: unknown halo_mode", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (ex) {
+    if (!(a->slope == a->slope) || a->slope < 0.f || a->slope > 1.f) { set_last_error("%s: slope must be in [0, 1]", what); return TTSB_ERR_INVALID_ARGUMENT; }
+    if (a->res_hi && split != (a->res_lo != nullptr)) { set_last_error("%s: the residual needs res_lo in bf16x3 and only there", what); return TTSB_ERR_INVALID_ARGUMENT; }
+    if (!a->res_hi && a->res_lo) { set_last_error("%s: res_lo without res_hi", what); return TTSB_ERR_INVALID_ARGUMENT; }
+    if (a->res_hi && (a->res_hi == a->out_hi || a->res_hi == a->act_hi)) { set_last_error("%s: the residual must not alias an output", what); return TTSB_ERR_INVALID_ARGUMENT; }
+    if ((reinterpret_cast<uintptr_t>(a->res_hi) | reinterpret_cast<uintptr_t>(a->res_lo) | reinterpret_cast<uintptr_t>(a->sum)) % 16) {
+      set_last_error("%s: res_hi, res_lo and sum must be 16-byte aligned", what);
+      return TTSB_ERR_INVALID_ARGUMENT;
+    }
+    if (a->sum_mode < TTSB_CONV1D_SUM_NONE || a->sum_mode > TTSB_CONV1D_SUM_FINISH) { set_last_error("%s: unknown sum_mode", what); return TTSB_ERR_INVALID_ARGUMENT; }
+    if ((a->sum_mode != TTSB_CONV1D_SUM_NONE) != (a->sum != nullptr)) { set_last_error("%s: sum must be given exactly when sum_mode is not NONE", what); return TTSB_ERR_INVALID_ARGUMENT; }
+    if (a->sum_mode == TTSB_CONV1D_SUM_FINISH && !(a->sum_div >= 1.f && a->sum_div < 1e6f)) { set_last_error("%s: sum_div must be in [1, 1e6)", what); return TTSB_ERR_INVALID_ARGUMENT; }
+    const bool stores = a->sum_mode == TTSB_CONV1D_SUM_WRITE || a->sum_mode == TTSB_CONV1D_SUM_ADD;
+    if (!a->out_hi && !a->act_hi && !stores) { set_last_error("%s: no output", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  } else if (!a->out_hi && !a->act_hi) {
+    set_last_error("%s: no output", what);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  const int min_len = a->halo_mode == TTSB_HALO_REFLECT ? H + 1 : (a->halo_mode == TTSB_HALO_ZERO ? H : 1);
   std::vector<int32_t> tab;
-  long long rows = 0;
-  int rc = conv_table(what, a->clip_offsets, a->n_clips, a->up, min_len, tab, &rows);
+  long long rows = 0, out_rows = 0;
+  int rc = conv_table(what, a->clip_offsets, a->n_clips, a->up, H, min_len, tab, &rows, &out_rows);
   if (rc) return rc;
+  if (ex && a->out_rows != out_rows) {
+    set_last_error("%s: out_rows = %lld, but the output layout of these clips has %lld rows (residual, sum and outputs all have that shape)",
+                   what, (long long)a->out_rows, out_rows);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
   rc = check_workspace(what, a->workspace, a->workspace_bytes, a->n_clips);
   if (rc) return rc;
 
@@ -287,7 +352,14 @@ extern "C" int ttsb_conv1d_tc(const ttsb_conv1d_args* a, void* stream_v) {
   p.up = a->up;
   p.halo_mode = a->halo_mode;
   p.ld_out = a->ld_out;
+  p.halo = H;
+  p.slope = a->slope;
   p.bias = a->bias;
+  p.res_hi = static_cast<const __nv_bfloat16*>(a->res_hi);
+  p.res_lo = static_cast<const __nv_bfloat16*>(a->res_lo);
+  p.sum = a->sum;
+  p.sum_mode = a->sum_mode;
+  p.sum_div = a->sum_div;
   p.out_hi = static_cast<__nv_bfloat16*>(a->out_hi);
   p.out_lo = split && a->out_hi ? static_cast<__nv_bfloat16*>(a->out_lo) : nullptr;
   p.act_hi = static_cast<__nv_bfloat16*>(a->act_hi);
@@ -307,24 +379,23 @@ extern "C" int ttsb_conv1d_tc(const ttsb_conv1d_args* a, void* stream_v) {
     if (rc) return rc;
   }
   TTSB_CUDA_OK(cudaMemcpyAsync(a->workspace, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
-  if (split)
-    return launch_pipeline<conv1d_tc_kernel<true>>(ConvCfg<true>::kSmemBytes, p.num_tiles, false, stream, "conv1d_tc_kernel launch",
-                                                   tmA[0][0], tmA[0][1], tmA[1][0], tmA[1][1], tmW[0], tmW[1], p);
-  return launch_pipeline<conv1d_tc_kernel<false>>(ConvCfg<false>::kSmemBytes, p.num_tiles, false, stream, "conv1d_tc_kernel launch",
-                                                  tmA[0][0], tmA[0][1], tmA[1][0], tmA[1][1], tmW[0], tmW[1], p);
+#define TTSB_CONV_LAUNCH(S, E)                                                                                                         \
+  launch_pipeline<conv1d_tc_kernel<S, E>>(ConvCfg<S>::kSmemBytes, p.num_tiles, false, stream, "conv1d_tc_kernel launch", tmA[0][0], \
+                                          tmA[0][1], tmA[1][0], tmA[1][1], tmW[0], tmW[1], p)
+  if (ex) return split ? TTSB_CONV_LAUNCH(true, true) : TTSB_CONV_LAUNCH(false, true);
+  return split ? TTSB_CONV_LAUNCH(true, false) : TTSB_CONV_LAUNCH(false, false);
+#undef TTSB_CONV_LAUNCH
 }
 
-extern "C" int ttsb_conv1d_out_tanh(const void* in_hi, const void* in_lo, int ld_in, int channels, const int32_t* clip_offsets, int n_clips,
-                                    int drop_tail, const float* weight, float bias, void* workspace, int64_t workspace_bytes, float* wav_out,
-                                    void* stream_v) {
-  const char* what = "ttsb_conv1d_out_tanh";
-  if (!in_hi || !weight || !wav_out) { set_last_error("ttsb_conv1d_out_tanh: NULL pointer"); return TTSB_ERR_INVALID_ARGUMENT; }
-  if (channels < 1 || ld_in < channels || ld_in > 256 || ld_in % 8) { set_last_error("ttsb_conv1d_out_tanh: need 1 <= channels <= ld_in <= 256, ld_in % 8 == 0"); return TTSB_ERR_INVALID_ARGUMENT; }
-  if (drop_tail < 0) { set_last_error("ttsb_conv1d_out_tanh: drop_tail < 0"); return TTSB_ERR_INVALID_ARGUMENT; }
+static int out_tanh_launch(const char* what, const void* in_hi, const void* in_lo, int ld_in, int channels, int halo, int min_len,
+                           const int32_t* clip_offsets, int n_clips, int drop_tail, const float* weight, float bias, void* workspace,
+                           int64_t workspace_bytes, float* wav_out, void* stream_v) {
+  if (!in_hi || !weight || !wav_out) { set_last_error("%s: NULL pointer", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (channels < 1 || ld_in < channels || ld_in > 256 || ld_in % 8) { set_last_error("%s: need 1 <= channels <= ld_in <= 256, ld_in %% 8 == 0", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (drop_tail < 0) { set_last_error("%s: drop_tail < 0", what); return TTSB_ERR_INVALID_ARGUMENT; }
   std::vector<int32_t> tab;
-  long long rows = 0;
-  // the 3-row reflect padding lies in the halos: the clip needs rows 1..3 and must outlast drop_tail
-  int rc = conv_table(what, clip_offsets, n_clips, 1, (drop_tail + 1 > 4 ? drop_tail + 1 : 4), tab, &rows);
+  long long rows = 0, out_rows = 0;
+  int rc = conv_table(what, clip_offsets, n_clips, 1, halo, min_len, tab, &rows, &out_rows);
   if (rc) return rc;
   rc = check_workspace(what, workspace, workspace_bytes, n_clips);
   if (rc) return rc;
@@ -333,8 +404,72 @@ extern "C" int ttsb_conv1d_out_tanh(const void* in_hi, const void* in_lo, int ld
   const int total = clip_offsets[n_clips];
   const int grid = min((total + 255) / 256, 8 * num_sms());
   conv1d_out_tanh_kernel<<<grid, 256, 7 * channels * sizeof(float), stream>>>(
-      static_cast<const __nv_bfloat16*>(in_hi), static_cast<const __nv_bfloat16*>(in_lo), ld_in, channels, static_cast<const int32_t*>(workspace),
-      n_clips, drop_tail, weight, bias, total, wav_out);
+      static_cast<const __nv_bfloat16*>(in_hi), static_cast<const __nv_bfloat16*>(in_lo), ld_in, channels, halo,
+      static_cast<const int32_t*>(workspace), n_clips, drop_tail, weight, bias, total, wav_out);
   count_launch();
   return check_cuda(cudaGetLastError(), "conv1d_out_tanh_kernel launch");
+}
+
+}  // namespace ttsb
+
+using namespace ttsb;
+
+extern "C" int64_t ttsb_conv1d_workspace_bytes(int n_clips) {
+  if (n_clips < 1) {
+    set_last_error("ttsb_conv1d_workspace_bytes: n_clips < 1");
+    return -1;
+  }
+  return 2 * (int64_t)(n_clips + 1) * (int64_t)sizeof(int32_t);
+}
+
+extern "C" int ttsb_conv1d_tc(const ttsb_conv1d_args* a, void* stream_v) {
+  if (!a) { set_last_error("ttsb_conv1d_tc: args is NULL"); return TTSB_ERR_INVALID_ARGUMENT; }
+  ttsb_conv1d_ex_args e{};
+  e.n_clips = a->n_clips;
+  e.clip_offsets = a->clip_offsets;
+  e.halo = CONV_HALO;
+  e.num_taps = a->num_taps;
+  for (int s = 0; s < TTSB_CONV1D_MAX_TAPS; ++s) { e.tap_src[s] = a->tap_src[s]; e.tap_shift[s] = a->tap_shift[s]; }
+  for (int i = 0; i < 2; ++i) { e.in_hi[i] = a->in_hi[i]; e.in_lo[i] = a->in_lo[i]; e.ld_in[i] = a->ld_in[i]; }
+  e.w_hi = a->w_hi;
+  e.w_lo = a->w_lo;
+  e.bias = a->bias;
+  e.N = a->N;
+  e.up = a->up;
+  e.out_hi = a->out_hi;
+  e.out_lo = a->out_lo;
+  e.act_hi = a->act_hi;
+  e.act_lo = a->act_lo;
+  e.ld_out = a->ld_out;
+  e.slope = LRELU_SLOPE;
+  e.halo_mode = a->halo_mode;
+  e.precision = a->precision;
+  e.workspace = a->workspace;
+  e.workspace_bytes = a->workspace_bytes;
+  return conv1d_launch("ttsb_conv1d_tc", &e, false, TTSB_CONV1D_MAX_TAPS, stream_v);
+}
+
+extern "C" int ttsb_conv1d_ex_tc(const ttsb_conv1d_ex_args* a, void* stream_v) {
+  if (!a) { set_last_error("ttsb_conv1d_ex_tc: args is NULL"); return TTSB_ERR_INVALID_ARGUMENT; }
+  return conv1d_launch("ttsb_conv1d_ex_tc", a, true, TTSB_CONV1D_EX_MAX_TAPS, stream_v);
+}
+
+extern "C" int ttsb_conv1d_out_tanh(const void* in_hi, const void* in_lo, int ld_in, int channels, const int32_t* clip_offsets, int n_clips,
+                                    int drop_tail, const float* weight, float bias, void* workspace, int64_t workspace_bytes, float* wav_out,
+                                    void* stream_v) {
+  // the 3-row reflect padding lies in the halos: the clip needs rows 1..3 and must outlast drop_tail
+  return out_tanh_launch("ttsb_conv1d_out_tanh", in_hi, in_lo, ld_in, channels, CONV_HALO, drop_tail + 1 > 4 ? drop_tail + 1 : 4,
+                         clip_offsets, n_clips, drop_tail, weight, bias, workspace, workspace_bytes, wav_out, stream_v);
+}
+
+extern "C" int ttsb_conv1d_out_tanh_ex(const void* in_hi, const void* in_lo, int ld_in, int channels, int halo, const int32_t* clip_offsets,
+                                       int n_clips, int drop_tail, const float* weight, float bias, void* workspace, int64_t workspace_bytes,
+                                       float* wav_out, void* stream_v) {
+  if (halo < 3 || halo > TTSB_CONV1D_EX_MAX_HALO) {
+    set_last_error("ttsb_conv1d_out_tanh_ex: halo = %d must be in [3, %d]", halo, TTSB_CONV1D_EX_MAX_HALO);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  // the 3-row padding lies in the halos, so any clip that outlasts drop_tail works
+  return out_tanh_launch("ttsb_conv1d_out_tanh_ex", in_hi, in_lo, ld_in, channels, halo, drop_tail + 1, clip_offsets, n_clips, drop_tail,
+                         weight, bias, workspace, workspace_bytes, wav_out, stream_v);
 }

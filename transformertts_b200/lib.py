@@ -33,7 +33,7 @@ EXPORTS = [
     'ttsb_stft_mel_log_batch_workspace_bytes', 'ttsb_stft_mel_log_batch', 'ttsb_pitch_workspace_bytes', 'ttsb_pitch_dio_stonemask',
     'ttsb_dp_unique_id', 'ttsb_dp_init', 'ttsb_dp_allreduce_bucket', 'ttsb_dp_destroy',
     'ttsb_decode_attn_workspace_bytes', 'ttsb_decode_attn', 'ttsb_decode_prologue', 'ttsb_decode_commit',
-    'ttsb_conv1d_workspace_bytes', 'ttsb_conv1d_tc', 'ttsb_conv1d_out_tanh',
+    'ttsb_conv1d_workspace_bytes', 'ttsb_conv1d_tc', 'ttsb_conv1d_out_tanh', 'ttsb_conv1d_ex_tc', 'ttsb_conv1d_out_tanh_ex',
     'ttsb_resample_batch_workspace_bytes', 'ttsb_resample_batch',
 ]
 
@@ -136,6 +136,8 @@ def load() -> C.CDLL:
     lib.ttsb_conv1d_workspace_bytes.restype = C.c_int64
     lib.ttsb_conv1d_out_tanh.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_float,
                                          C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.ttsb_conv1d_out_tanh_ex.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                            C.c_float, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     lib.ttsb_pitch_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double]
     lib.ttsb_pitch_dio_stonemask.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double,
                                              C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
@@ -636,11 +638,14 @@ def decode_commit(post, B, r, mel, stop_col, stop_index, max_iters, mel_out, sto
 
 
 # ------------------------------------------------------------------------------------------------------------
-# ragged-batch Conv1D (the MelGAN generator)
+# ragged-batch Conv1D (the MelGAN and HiFi-GAN generators)
 # ------------------------------------------------------------------------------------------------------------
 CONV1D_HALO = 9
 CONV1D_MAX_TAPS = 7
 HALO_NONE, HALO_REFLECT, HALO_ZERO = 0, 1, 2
+CONV1D_EX_MAX_TAPS = 16
+CONV1D_EX_MAX_HALO = 64
+SUM_NONE, SUM_WRITE, SUM_ADD, SUM_FINISH = 0, 1, 2, 3
 
 
 class Conv1dArgs(C.Structure):
@@ -672,3 +677,30 @@ def conv1d_out_tanh(in_hi, in_lo, channels, clip_offsets, drop_tail, weight, bia
     _check(load().ttsb_conv1d_out_tanh(ptr(in_hi), ptr(in_lo), in_hi.shape[-1], int(channels), co, n, int(drop_tail), ptr(weight),
                                        C.c_float(bias), ptr(workspace), C.c_int64(workspace.numel() * workspace.element_size()),
                                        ptr(wav_out), _stream()), 'ttsb_conv1d_out_tanh')
+
+
+class Conv1dExArgs(C.Structure):
+    _fields_ = [
+        ('n_clips', C.c_int), ('clip_offsets', C.c_void_p), ('halo', C.c_int), ('num_taps', C.c_int),
+        ('tap_src', C.c_int * CONV1D_EX_MAX_TAPS), ('tap_shift', C.c_int * CONV1D_EX_MAX_TAPS),
+        ('in_hi', C.c_void_p * 2), ('in_lo', C.c_void_p * 2), ('ld_in', C.c_int * 2),
+        ('w_hi', C.c_void_p), ('w_lo', C.c_void_p), ('bias', C.c_void_p), ('N', C.c_int), ('up', C.c_int),
+        ('res_hi', C.c_void_p), ('res_lo', C.c_void_p), ('sum', C.c_void_p), ('sum_mode', C.c_int), ('sum_div', C.c_float),
+        ('out_hi', C.c_void_p), ('out_lo', C.c_void_p), ('act_hi', C.c_void_p), ('act_lo', C.c_void_p), ('ld_out', C.c_int),
+        ('out_rows', C.c_int64), ('slope', C.c_float), ('halo_mode', C.c_int), ('precision', C.c_int),
+        ('workspace', C.c_void_p), ('workspace_bytes', C.c_int64),
+    ]
+
+
+def conv1d_ex_tc(args: Conv1dExArgs):
+    """One ragged-batch conv in the extended form (include/ttsb.h: ttsb_conv1d_ex_tc)."""
+    _check(load().ttsb_conv1d_ex_tc(C.byref(args), _stream()), 'ttsb_conv1d_ex_tc')
+
+
+def conv1d_out_tanh_ex(in_hi, in_lo, channels, halo, clip_offsets, drop_tail, weight, bias, workspace, wav_out):
+    """The output layer over a layout of `halo` rows (include/ttsb.h: ttsb_conv1d_out_tanh_ex)."""
+    co, n = _host_offsets(clip_offsets)
+    _check(load().ttsb_conv1d_out_tanh_ex(ptr(in_hi), ptr(in_lo), in_hi.shape[-1], int(channels), int(halo), co, n, int(drop_tail),
+                                          ptr(weight), C.c_float(bias), ptr(workspace),
+                                          C.c_int64(workspace.numel() * workspace.element_size()), ptr(wav_out), _stream()),
+           'ttsb_conv1d_out_tanh_ex')

@@ -110,15 +110,15 @@ def ragged_offsets(counts: Sequence[int], rate: int = 1) -> np.ndarray:
     return np.concatenate([[0], np.cumsum(np.asarray(counts, dtype=np.int64) * rate)]).astype(np.int64)
 
 
-def layout_rows(counts: Sequence[int], rate: int = 1) -> int:
-    """Rows of the packed layout of clips with counts[c] * rate rows each."""
-    return int(np.sum(counts) * rate) + 2 * lib.CONV1D_HALO * len(counts)
+def layout_rows(counts: Sequence[int], rate: int = 1, halo: int = lib.CONV1D_HALO) -> int:
+    """Rows of the packed layout of clips with counts[c] * rate rows each and `halo` rows on each side."""
+    return int(np.sum(counts) * rate) + 2 * halo * len(counts)
 
 
-def pack_clips(clips: Sequence[np.ndarray], cols: int, mode: int) -> np.ndarray:
+def pack_clips(clips: Sequence[np.ndarray], cols: int, mode: int, halo: int = lib.CONV1D_HALO) -> np.ndarray:
     """Host packing of (L_c, C) clips into the halo layout (rows, cols) float32, halos filled by `mode`."""
-    H = lib.CONV1D_HALO
-    out = np.zeros((layout_rows([len(x) for x in clips]), cols), dtype=np.float32)
+    H = halo
+    out = np.zeros((layout_rows([len(x) for x in clips], halo=H), cols), dtype=np.float32)
     r = 0
     for x in clips:
         L, Cc = x.shape
@@ -129,9 +129,9 @@ def pack_clips(clips: Sequence[np.ndarray], cols: int, mode: int) -> np.ndarray:
     return out
 
 
-def unpack_clips(buf: np.ndarray, counts: Sequence[int], channels: int) -> List[np.ndarray]:
+def unpack_clips(buf: np.ndarray, counts: Sequence[int], channels: int, halo: int = lib.CONV1D_HALO) -> List[np.ndarray]:
     """The clip rows (L_c, channels) of a packed layout."""
-    H, r, out = lib.CONV1D_HALO, 0, []
+    H, r, out = halo, 0, []
     for L in counts:
         out.append(buf[r + H:r + H + L, :channels])
         r += L + 2 * H
@@ -147,6 +147,45 @@ class _Conv:
         w = torch.from_numpy(np.ascontiguousarray(mat, dtype=np.float32)).to(device)
         self.w_hi, self.w_lo = lib.pack_weight(w, self.N, split)
         self.bias = torch.from_numpy(np.ascontiguousarray(bias, dtype=np.float32)).to(device)
+
+
+def run_conv(conv: _Conv, counts_in, srcs, up: int, split: bool, out=None, act=None, halo=lib.HALO_NONE, ws=None,
+             rows_halo: int = lib.CONV1D_HALO, slope=None, res=None, sum_plane=None, sum_mode: int = lib.SUM_NONE, sum_div: float = 1.0):
+    """One conv launch: srcs = [(hi, lo)] per source, out / act / res = (hi, lo) planes or None.  With the defaults this is
+    ttsb_conv1d_tc (9 halo rows, LeakyReLU slope 0.2); a halo of `rows_halo` rows, another `slope`, a residual or a sum plane
+    (fp32, the output layout) make it ttsb_conv1d_ex_tc."""
+    ex = rows_halo != lib.CONV1D_HALO or slope is not None or res is not None or sum_plane is not None
+    a = lib.Conv1dExArgs() if ex else lib.Conv1dArgs()
+    off = ragged_offsets(counts_in)
+    tab = (lib.C.c_int32 * len(off))(*off.tolist())
+    a.n_clips = len(counts_in)
+    a.clip_offsets = lib.C.cast(tab, lib.C.c_void_p)
+    a.num_taps = len(conv.taps)
+    for s, (src, shift) in enumerate(conv.taps):
+        a.tap_src[s], a.tap_shift[s] = src, shift
+    for i, (hi, lo) in enumerate(srcs):
+        a.in_hi[i], a.in_lo[i], a.ld_in[i] = lib.ptr(hi), lib.ptr(lo), hi.shape[1]
+    a.w_hi, a.w_lo, a.bias = lib.ptr(conv.w_hi), lib.ptr(conv.w_lo), lib.ptr(conv.bias)
+    a.N, a.up, a.ld_out = conv.N, up, conv.N // up
+    if out is not None:
+        a.out_hi, a.out_lo = lib.ptr(out[0]), lib.ptr(out[1])
+    if act is not None:
+        a.act_hi, a.act_lo = lib.ptr(act[0]), lib.ptr(act[1])
+    a.halo_mode = halo
+    a.precision = lib.PREC_BF16X3 if split else lib.PREC_BF16
+    a.workspace, a.workspace_bytes = lib.ptr(ws), ws.numel()
+    if not ex:
+        lib.conv1d_tc(a)
+        return
+    a.halo = rows_halo
+    a.slope = 0.2 if slope is None else slope
+    if res is not None:
+        a.res_hi, a.res_lo = lib.ptr(res[0]), lib.ptr(res[1])
+    if sum_plane is not None:
+        a.sum = lib.ptr(sum_plane)
+    a.sum_mode, a.sum_div = sum_mode, sum_div
+    a.out_rows = layout_rows([c * up for c in counts_in], halo=rows_halo)
+    lib.conv1d_ex_tc(a)
 
 
 class MelGANGenerator:
@@ -230,26 +269,7 @@ class MelGANGenerator:
 
     def _run(self, conv: _Conv, counts_in, srcs, up: int, out=None, act=None, halo=lib.HALO_NONE, ws=None):
         """One ttsb_conv1d_tc launch: srcs = [(hi, lo)] per source, out / act = (hi, lo) planes or None."""
-        a = lib.Conv1dArgs()
-        off = ragged_offsets(counts_in)
-        tab = (lib.C.c_int32 * len(off))(*off.tolist())
-        a.n_clips = len(counts_in)
-        a.clip_offsets = lib.C.cast(tab, lib.C.c_void_p)
-        a.num_taps = len(conv.taps)
-        for s, (src, shift) in enumerate(conv.taps):
-            a.tap_src[s], a.tap_shift[s] = src, shift
-        for i, (hi, lo) in enumerate(srcs):
-            a.in_hi[i], a.in_lo[i], a.ld_in[i] = lib.ptr(hi), lib.ptr(lo), hi.shape[1]
-        a.w_hi, a.w_lo, a.bias = lib.ptr(conv.w_hi), lib.ptr(conv.w_lo), lib.ptr(conv.bias)
-        a.N, a.up, a.ld_out = conv.N, up, conv.N // up
-        if out is not None:
-            a.out_hi, a.out_lo = lib.ptr(out[0]), lib.ptr(out[1])
-        if act is not None:
-            a.act_hi, a.act_lo = lib.ptr(act[0]), lib.ptr(act[1])
-        a.halo_mode = halo
-        a.precision = lib.PREC_BF16X3 if self.split else lib.PREC_BF16
-        a.workspace, a.workspace_bytes = lib.ptr(ws), ws.numel()
-        lib.conv1d_tc(a)
+        run_conv(conv, counts_in, srcs, up, self.split, out=out, act=act, halo=halo, ws=ws)
 
     def vocode_device(self, mels: Sequence[np.ndarray]) -> torch.Tensor:
         """vocode_batch, leaving the packed float32 waveform (256 sum T_c samples, clip after clip) on the device."""
