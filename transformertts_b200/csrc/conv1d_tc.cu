@@ -147,13 +147,15 @@ __device__ __forceinline__ void conv_epilogue(const ConvKParams& p, const float*
   }
 }
 
-// tensor maps: A[src][hi/lo] (ld_in[src], rows) boxes (64, 128); W[hi/lo] (K_total, N) boxes (64, block_n)
-template <bool kSplit, bool kEx>
+// tensor maps: A[src][hi/lo] (ld_in[src], rows) boxes (64, 128); W[hi/lo] (K_total, N) boxes (64, block_n).  kNch: block_n / 64
+// (the wgmma width)
+template <bool kSplit, bool kEx, int kNch>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant__ CUtensorMap tmA0l,
                  const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUtensorMap tmA1l,
                  const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const ConvKParams p) {
   using Cfg = ConvCfg<kSplit>;
+  static_assert(kNch >= 1 && kNch <= GEMM_NCH, "tile width");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);
   typename Cfg::Ring ring(smem);
@@ -199,13 +201,10 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constan
     float* img = reinterpret_cast<float*>(smem);
     int total_kb = 0;
     for (int s = 0; s < p.num_taps; ++s) total_kb += p.kblocks[p.tap_src[s]];
-    const int nch = p.block_n >> 6;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       const int m0 = (tile / p.n_tiles) * GEMM_BM;
       const int n0 = (tile % p.n_tiles) * p.block_n;
-      float acc[GEMM_NCH][32];
-      ring.mma_tile(total_kb, acc, [&](uint32_t st, int kb) { Cfg::Stage::mma(acc, st, wg, nch, kb); });
-      park_tile(img, Cfg::kPitch, wg, nch, acc);
+      Cfg::Stage::template mma_park_tile<kNch>(ring, total_kb, img, Cfg::kPitch, wg);
       const int row = quarter * 32 + lane;
       __syncwarp();
       conv_epilogue<kEx>(p, img + (size_t)row * Cfg::kPitch, m0 + row, n0, half);
@@ -282,6 +281,16 @@ static int check_workspace(const char* what, const void* ws, int64_t bytes, int 
     return TTSB_ERR_INVALID_ARGUMENT;
   }
   return 0;
+}
+
+// launches the instantiation whose wgmma width kNch * 64 is p.block_n
+template <bool kSplit, bool kEx, int kNch = 1>
+static int conv_launch_tc(const CUtensorMap (&tmA)[2][2], const CUtensorMap (&tmW)[2], const ConvKParams& p, cudaStream_t stream) {
+  if constexpr (kNch < GEMM_NCH) {
+    if (p.block_n > kNch * 64) return conv_launch_tc<kSplit, kEx, kNch + 1>(tmA, tmW, p, stream);
+  }
+  return launch_pipeline<conv1d_tc_kernel<kSplit, kEx, kNch>>(ConvCfg<kSplit>::kSmemBytes, p.num_tiles, false, stream, "conv1d_tc_kernel launch",
+                                                              tmA[0][0], tmA[0][1], tmA[1][0], tmA[1][1], tmW[0], tmW[1], p);
 }
 
 // the shared host side of ttsb_conv1d_tc (ex = false: no residual or sum, out_rows unchecked) and ttsb_conv1d_ex_tc
@@ -379,12 +388,8 @@ static int conv1d_launch(const char* what, const ttsb_conv1d_ex_args* a, bool ex
     if (rc) return rc;
   }
   TTSB_CUDA_OK(cudaMemcpyAsync(a->workspace, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
-#define TTSB_CONV_LAUNCH(S, E)                                                                                                         \
-  launch_pipeline<conv1d_tc_kernel<S, E>>(ConvCfg<S>::kSmemBytes, p.num_tiles, false, stream, "conv1d_tc_kernel launch", tmA[0][0], \
-                                          tmA[0][1], tmA[1][0], tmA[1][1], tmW[0], tmW[1], p)
-  if (ex) return split ? TTSB_CONV_LAUNCH(true, true) : TTSB_CONV_LAUNCH(false, true);
-  return split ? TTSB_CONV_LAUNCH(true, false) : TTSB_CONV_LAUNCH(false, false);
-#undef TTSB_CONV_LAUNCH
+  if (ex) return split ? conv_launch_tc<true, true>(tmA, tmW, p, stream) : conv_launch_tc<false, true>(tmA, tmW, p, stream);
+  return split ? conv_launch_tc<true, false>(tmA, tmW, p, stream) : conv_launch_tc<false, false>(tmA, tmW, p, stream);
 }
 
 static int out_tanh_launch(const char* what, const void* in_hi, const void* in_lo, int ld_in, int channels, int halo, int min_len,

@@ -26,7 +26,7 @@ constexpr int GEMM_BK = 64;
 constexpr int GEMM_MAX_BN = 256;
 constexpr int GEMM_THREADS = 384;
 constexpr int GEMM_EPI_WARPS = 8;                        // the consumer / epilogue warps
-constexpr int GEMM_NCH = GEMM_MAX_BN / 64;               // wgmma n64 products per k step (the tile width rounded up to 64)
+constexpr int GEMM_NCH = GEMM_MAX_BN / 64;               // the widest tile in n64 blocks
 constexpr int A_TILE_BYTES = GEMM_BM * GEMM_BK * 2;      // 16 KiB
 constexpr int B_TILE_BYTES = GEMM_MAX_BN * GEMM_BK * 2;  // 32 KiB
 constexpr int MN_BOX_BYTES = 64 * 128;                   // one [64 k x 64 mn] TMA box of an MN-major operand
@@ -42,6 +42,24 @@ __device__ __forceinline__ uint8_t* align_smem_1024(uint8_t* p) {
 // named barriers: 5 = the 256 consumer threads, 1 + quarter = the two warps of a row quarter
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 5, 256;" ::: "memory"); }
 __device__ __forceinline__ void quarter_sync(int quarter) { asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory"); }
+
+// wgmma_fence_regs over accumulators kept as C n64 fragments
+template <int C>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[C][32]) {
+#pragma unroll
+  for (int c = 0; c < C; ++c) wgmma_fence_regs(d[c]);
+}
+
+// one m64n(64 * NCH)k16 product of K-major bf16 operands: register 32c + j of d is register j of the n64 fragment of
+// columns [64c, +64), so d is the same accumulator image as NCH n64 products
+template <int NCH>
+__device__ __forceinline__ void wgmma_ss_kmajor_bf16(float (&d)[NCH * 32], uint64_t da, uint64_t db, uint32_t acc) {
+  static_assert(NCH >= 1 && NCH <= GEMM_NCH, "wgmma width");
+  if constexpr (NCH == 1) wgmma_ss_m64n64_bf16<0, 0>(d, da, db, acc);
+  else if constexpr (NCH == 2) wgmma_ss_m64n128_bf16<0, 0>(d, da, db, acc);
+  else if constexpr (NCH == 3) wgmma_ss_m64n192_bf16<0, 0>(d, da, db, acc);
+  else wgmma_ss_m64n256_bf16<0, 0>(d, da, db, acc);
+}
 
 // Ring of kStages stages at the (1024-aligned) shared-memory base, followed by GEMM_RING_BAR_BYTES of barriers: full[s]
 // completes when stage s has landed (one arrival + the TMA bytes), empty[s] when the 8 consumer warps are done reading it,
@@ -95,9 +113,10 @@ struct GemmRing {
 
   // consumers: the kbs k blocks of a tile.  issue(stage shared address, kb) issues the wgmma products of k block kb
   // (accumulate flag off for the first products of kb 0).  A stage is released once the products of the next k block are
-  // in flight (their predecessors have finished reading it), the last one after the drain.
-  template <int NCH, class Issue>
-  __device__ __forceinline__ void mma_tile(int kbs, float (&acc)[NCH][32], Issue&& issue) {
+  // in flight (their predecessors have finished reading it), the last one after the drain.  acc is the accumulator array
+  // the products write (float[R], or float[C][32] of n64 fragments).
+  template <class Acc, class Issue>
+  __device__ __forceinline__ void mma_tile(int kbs, Acc& acc, Issue&& issue) {
     const bool lane0 = (threadIdx.x & 31) == 0;
     int prev_stage = -1;
     for (int kb = 0; kb < kbs; ++kb) {
@@ -114,8 +133,7 @@ struct GemmRing {
       advance();
     }
     wgmma_wait<0>();
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) wgmma_fence_regs(acc[c]);
+    wgmma_fence_regs(acc);
     if (prev_stage >= 0) {
       __syncwarp();
       if (lane0) mbar_arrive(empty() + prev_stage);
@@ -135,6 +153,23 @@ struct GemmRing {
     if (store_issuer) tma_store_wait_all();
   }
 };
+
+// consumers: both warpgroups are done reading the ring; park the tile in it.  acc is one m64n(R / 2) fragment (K-major
+// stages), or C n64 fragments of which the first nmma were computed (bgemm_tc.cu)
+template <int R>
+__device__ __forceinline__ void park_tile(float* img, int pitch, int wg, const float (&acc)[R]) {
+  consumer_sync();
+  acc_store_fragment(img, pitch, wg * 64, 0, acc);
+  consumer_sync();
+}
+template <int C>
+__device__ __forceinline__ void park_tile(float* img, int pitch, int wg, int nmma, const float (&acc)[C][32]) {
+  consumer_sync();
+#pragma unroll
+  for (int c = 0; c < C; ++c)
+    if (c < nmma) acc_store_fragment(img, pitch, wg * 64, c * 64, acc[c]);
+  consumer_sync();
+}
 
 // A stage of K-major operands (gemm_tc.cu, conv1d_tc.cu): 128B-swizzled boxes of 64 k, laid out as A hi [128 rows] |
 // B hi [kBTileBytes] and, with kSplit (bf16x3: A_hi*B_hi + A_lo*B_hi + A_hi*B_lo), A lo | B lo behind them.  A bf16x3
@@ -169,47 +204,37 @@ struct KMajorStage {
     });
   }
 
-  // consumers: the products of k block kb in the stage at shared address st for warpgroup wg (A rows [64 * wg, +64)) and
-  // the n64 blocks c < nch.  k16 steps outer, n64 blocks inner; bf16x3 then adds the A_lo*B_hi and A_hi*B_lo products of
-  // each k16 step.  The first products of k block 0 overwrite the accumulators.
+  // consumers: the products of k block kb in the stage at shared address st for warpgroup wg (A rows [64 * wg, +64)) into
+  // the first NCH * 64 columns, one m64n(64 * NCH)k16 wgmma per operand pair and k16 step: A_hi*B_hi for the four k16
+  // steps, then bf16x3 adds A_lo*B_hi and A_hi*B_lo per k16 step.  The first products of k block 0 overwrite the
+  // accumulators.
   template <int NCH>
-  __device__ __forceinline__ static void mma(float (&acc)[NCH][32], uint32_t st, int wg, int nch, int kb) {
-    const uint32_t a_hi = st + wg * (64 * 128);
-    const uint32_t b_hi = st + kBHi;
+  __device__ __forceinline__ static void mma(float (&acc)[NCH * 32], uint32_t st, int wg, int kb) {
+    const uint64_t da_hi = make_smem_desc_sw128(st + wg * (64 * 128));
+    const uint64_t db_hi = make_smem_desc_sw128(st + kBHi);
 #pragma unroll
-    for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
-      const uint64_t da = make_smem_desc_sw128(a_hi) + 2 * kk;
-#pragma unroll
-      for (int c = 0; c < NCH; ++c)
-        if (c < nch) wgmma_ss_m64n64_bf16<0, 0>(acc[c], da, make_smem_desc_sw128(b_hi + c * (64 * 128)) + 2 * kk, (kb | kk) != 0);
-    }
+    for (int kk = 0; kk < GEMM_BK / 16; ++kk) wgmma_ss_kmajor_bf16<NCH>(acc, da_hi + 2 * kk, db_hi + 2 * kk, (kb | kk) != 0);
     if (kSplit) {
-      const uint32_t a_lo = st + kALo + wg * (64 * 128);
-      const uint32_t b_lo = st + kBLo;
+      const uint64_t da_lo = make_smem_desc_sw128(st + kALo + wg * (64 * 128));
+      const uint64_t db_lo = make_smem_desc_sw128(st + kBLo);
 #pragma unroll
       for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
-        const uint64_t da_lo = make_smem_desc_sw128(a_lo) + 2 * kk, da_hi = make_smem_desc_sw128(a_hi) + 2 * kk;
-#pragma unroll
-        for (int c = 0; c < NCH; ++c) {
-          if (c < nch) {
-            wgmma_ss_m64n64_bf16<0, 0>(acc[c], da_lo, make_smem_desc_sw128(b_hi + c * (64 * 128)) + 2 * kk, 1);
-            wgmma_ss_m64n64_bf16<0, 0>(acc[c], da_hi, make_smem_desc_sw128(b_lo + c * (64 * 128)) + 2 * kk, 1);
-          }
-        }
+        wgmma_ss_kmajor_bf16<NCH>(acc, da_lo + 2 * kk, db_hi + 2 * kk, 1);
+        wgmma_ss_kmajor_bf16<NCH>(acc, da_hi + 2 * kk, db_lo + 2 * kk, 1);
       }
     }
   }
-};
 
-// consumers: both warpgroups are done reading the ring; park the tile in it (n64 blocks c < nmma; the rest was not computed)
-template <int NCH>
-__device__ __forceinline__ void park_tile(float* img, int pitch, int wg, int nmma, const float (&acc)[NCH][32]) {
-  consumer_sync();
-#pragma unroll
-  for (int c = 0; c < NCH; ++c)
-    if (c < nmma) acc_store_fragment(img, pitch, wg * 64, c * 64, acc[c]);
-  consumer_sync();
-}
+  // consumers: a tile of kbs k blocks into the first NCH * 64 columns, parked in the ring as the tile's image.  A kernel
+  // instantiates this for one NCH only: ptxas gives the accumulators of each wgmma width their own registers, and with
+  // several widths in one kernel it runs out of them, serialises the wgmma and spills.
+  template <int NCH>
+  __device__ __forceinline__ static void mma_park_tile(Ring& ring, int kbs, float* img, int pitch, int wg) {
+    float acc[NCH * 32];
+    ring.mma_tile(kbs, acc, [&](uint32_t st, int kb) { mma<NCH>(acc, st, wg, kb); });
+    park_tile(img, pitch, wg, acc);
+  }
+};
 
 // 16 floats of a per-column vector (bias, gamma, beta) as warp-uniform float4 loads; p is 16-byte aligned
 __device__ __forceinline__ void ldg16(const float* __restrict__ p, float (&v)[16]) {

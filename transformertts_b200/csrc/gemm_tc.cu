@@ -418,13 +418,15 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
 // ----------------------------------------------------------------------------------------------------
 // kernel
 // ----------------------------------------------------------------------------------------------------
-template <bool kSplit, bool kPair, bool kLN>
+// kNch: the tile width block_n in n64 blocks, rounded up (the wgmma width; the columns past block_n are computed and ignored)
+template <bool kSplit, bool kPair, bool kLN, int kNch>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant__ CUtensorMap tmA0l,
                const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUtensorMap tmA1l,
                const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl,
                const __grid_constant__ CUtensorMap tmOh, const __grid_constant__ CUtensorMap tmOl, const GemmKParams p) {
   using Cfg = GemmCfg<kSplit, kPair>;
+  static_assert(kNch >= 1 && kNch * 64 <= Cfg::kMaxBn, "tile width");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);
   typename Cfg::Ring ring(smem);
@@ -486,15 +488,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
     uint32_t slab_ctr = 0;  // staged epilogue: slabs stored so far (selects the staging box of single-plane outputs)
     int total_kb = 0;
     for (int s = 0; s < p.num_seg; ++s) total_kb += p.seg_kblocks[s];
-    const int nch = (p.block_n + 63) >> 6;   // n64 products per k step; columns past block_n are computed and ignored
     for (int tile = p.tile_begin + work_id; tile < p.num_tiles; tile += work_stride, ++iter) {
       const int n_tile = kPair ? cta_rank : tile % p.n_tiles;
       const int m_tile = kPair ? tile : tile / p.n_tiles;
       const int b = m_tile / p.tiles_per_row;
       const int t0 = (m_tile % p.tiles_per_row) * GEMM_BM;
-      float acc[GEMM_NCH][32];
-      ring.mma_tile(total_kb, acc, [&](uint32_t st, int kb) { Cfg::Stage::mma(acc, st, wg, nch, kb); });
-      park_tile(img, Cfg::kPitch, wg, nch, acc);
+      Cfg::Stage::template mma_park_tile<kNch>(ring, total_kb, img, Cfg::kPitch, wg);
       PairCtx px{};
       if (kPair) {
         const int slot = iter & 1;
@@ -604,12 +603,16 @@ __global__ void gemm_simt_kernel(const GemmKParams p, const GemmSimtPtrs q) {
 // ----------------------------------------------------------------------------------------------------
 // host
 // ----------------------------------------------------------------------------------------------------
-template <bool kSplit, bool kPair, bool kLN>
+// launches the instantiation whose wgmma width kNch * 64 is q.block_n rounded up to a multiple of 64
+template <bool kSplit, bool kPair, bool kLN, int kNch = 1>
 static int launch_tc(const CUtensorMap (&tmA)[2][2], const CUtensorMap (&tmW)[2], const CUtensorMap (&tmO)[2], const GemmKParams& q,
                      int work, cudaStream_t stream) {
-  return launch_pipeline<gemm_tc_kernel<kSplit, kPair, kLN>>(GemmCfg<kSplit, kPair>::kSmemBytes, work, kPair, stream,
-                                                             kPair ? "gemm_tc_kernel<pair> launch" : "gemm_tc_kernel launch", tmA[0][0], tmA[0][1], tmA[1][0],
-                                                             tmA[1][1], tmW[0], tmW[1], tmO[0], tmO[1], q);
+  if constexpr (kNch * 64 < GemmCfg<kSplit, kPair>::kMaxBn) {
+    if (q.block_n > kNch * 64) return launch_tc<kSplit, kPair, kLN, kNch + 1>(tmA, tmW, tmO, q, work, stream);
+  }
+  return launch_pipeline<gemm_tc_kernel<kSplit, kPair, kLN, kNch>>(GemmCfg<kSplit, kPair>::kSmemBytes, work, kPair, stream,
+                                                                   kPair ? "gemm_tc_kernel<pair> launch" : "gemm_tc_kernel launch", tmA[0][0], tmA[0][1],
+                                                                   tmA[1][0], tmA[1][1], tmW[0], tmW[1], tmO[0], tmO[1], q);
 }
 
 static int validate(const ttsb_gemm_args* a, int* k_total_out) {
