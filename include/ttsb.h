@@ -268,6 +268,11 @@ int ttsb_decode_commit(const float* post, int ld_post, int B, int r, int mel, in
  *   (x_mn_major = 1): dim0 is the M (or N) axis, dim1 the contraction axis -- so a transposed operand (P^T, dS^T, dO^T,
  *   V^T, K^T) is the SAME tensor read MN-major and no transposed copies exist.  The tile origin of problem z = (b,h) is
  *   (c0 + h*h_col, c1 + h*h_row, z_batch ? z : b).
+ *   The contraction runs in k blocks of 64 and relies on the tensor map's zero fill past its extent for the tail
+ *   [K, round_up(K, 64)).  So when K % 64 != 0 each operand's contraction axis (dim0 if K-major, dim1 if MN-major) must
+ *   have extent exactly K, and with H > 1 no per-head offset along it (h_col if K-major, h_row if MN-major) -- otherwise
+ *   the tail would be the next head's data; such a call returns TTSB_ERR_INVALID_ARGUMENT.  Head sizes 64, 128, 192, 256
+ *   and every T / Tk of the attention products satisfy this; several heads of size 32 or 96 do not.
  * ttsb_wgrad: weight gradients  dW[seg*Cin + c][n] += sum_{b,t} X_seg[b][t + shift_seg][c] * G[b][t][n]  for Dense
  *   (1 segment), concat-Dense (2 sources) and Conv1D (k segments with the tap shifts); X and G are the row-major bf16
  *   activations / output gradients (B, T, ld) read MN-major; dW is fp32 in the Keras (K, N) layout and is ACCUMULATED

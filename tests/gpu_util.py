@@ -326,3 +326,42 @@ def ref_mha_general(q, k, v, kv_len, H, precision, causal=False):
     w = torch.softmax(logits, -1)
     out = (w @ sp(v)).permute(0, 2, 1, 3).reshape(B, T, d)
     return out, w
+
+
+# ----------------------------------------------------------------------------------------------------------
+# ttsb_bgemm evaluated literally from its argument description (include/ttsb.h: ttsb_bgemm_args), in float64 on the host
+# ----------------------------------------------------------------------------------------------------------
+def bgemm_operand(x, dims, strides, off, B: int, H: int, n_mn: int, K: int) -> np.ndarray:
+    """float64 (B*H, n_mn, K) operand of every problem z = (b, h), read element by element as the tensor map addresses it:
+    x is the whole bf16 buffer, off = (h_col, h_row, z_batch, pointer offset in elements[, mn_major]) as TrainEngine._bgemm
+    takes it.  Coordinates outside (dim0, dim1, dim2) read as zero (the TMA fill); NaN inside them stays NaN."""
+    flat = x.detach().cpu().double().reshape(-1).numpy()
+    h_col, h_row, z_batch, ptr_off = off[:4]
+    mn_major = off[4] if len(off) > 4 else 0
+    z = np.arange(B * H)
+    b, h = z // H, z % H
+    i_mn, i_k = np.arange(n_mn)[None, :, None], np.arange(K)[None, None, :]
+    c0 = (i_mn if mn_major else i_k) + (h * h_col)[:, None, None]
+    c1 = (i_k if mn_major else i_mn) + (h * h_row)[:, None, None]
+    c2 = (z if z_batch else b)[:, None, None]
+    c0, c1, c2 = np.broadcast_arrays(c0, c1, c2)
+    inside = (c0 < dims[0]) & (c1 < dims[1]) & (c2 < dims[2])
+    idx = ptr_off + c0 + c1 * strides[0] + c2 * strides[1]
+    out = np.zeros(c0.shape)
+    out[inside] = flat[idx[inside]]
+    return out
+
+
+def ref_bgemm(B, H, M, N, K, a, a_dims, a_strides, a_off, b, b_dims, b_strides, b_off):
+    """(sum_k A_z[m][k] * B_z[n][k], sum_k |A_z[m][k] * B_z[n][k]|), each float64 (B*H, M, N), alpha not applied."""
+    A = bgemm_operand(a, a_dims, a_strides, a_off, B, H, M, K)
+    Bm = bgemm_operand(b, b_dims, b_strides, b_off, B, H, N, K)
+    return A @ Bm.transpose(0, 2, 1), np.abs(A) @ np.abs(Bm).transpose(0, 2, 1)
+
+
+def bgemm_out_index(B, H, M, out_cols, ld_out, out_batch_stride, out_h_col=0, out_by_b=0, out_ptr_off=0) -> np.ndarray:
+    """int64 (B*H, M, out_cols): the element of the output buffer that holds column n of row m of problem z."""
+    z = np.arange(B * H)
+    batch = (z // H if out_by_b else z)[:, None, None]
+    return (out_ptr_off + batch * out_batch_stride + np.arange(M)[None, :, None] * ld_out + ((z % H) * out_h_col)[:, None, None]
+            + np.arange(out_cols)[None, None, :])

@@ -468,6 +468,19 @@ extern "C" int ttsb_bgemm(const ttsb_bgemm_args* a, void* stream_v) {
     set_last_error("ttsb_bgemm: ld_out, out_cols and out_h_col must be multiples of 16 (32-byte stores)");
     return TTSB_ERR_INVALID_ARGUMENT;
   }
+  // A k block is 64 wide whatever K is.  The tail [K, round_up(K, 64)) of a problem's last block contributes nothing only
+  // where the tensor map zero-fills it, i.e. where the contraction axis of the map ends with the problem: otherwise it is
+  // the next head's data (head size 32 or 96 in a (d, T, B) tensor) and would be added to this head's products.
+  if (a->K % GEMM_BK != 0) {
+    const bool a_ok = (a->a_mn_major ? a->a_dim1 : a->a_dim0) == a->K && (a->H == 1 || (a->a_mn_major ? a->a_h_row : a->a_h_col) == 0);
+    const bool b_ok = (a->b_mn_major ? a->b_dim1 : a->b_dim0) == a->K && (a->H == 1 || (a->b_mn_major ? a->b_h_row : a->b_h_col) == 0);
+    if (!a_ok || !b_ok) {
+      set_last_error("ttsb_bgemm: K = %d is not a multiple of 64 and the contraction axis of operand %s does not end at K for every "
+                     "head (its last k block would read the next head's data); use a head size that is a multiple of 64",
+                     a->K, !a_ok ? "A" : "B");
+      return TTSB_ERR_INVALID_ARGUMENT;
+    }
+  }
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   BgParams p{};
   p.mode = 0;

@@ -21,6 +21,20 @@ from .models import (LN_EPS, _capture_graphs, _fill_inputs, _lru_get, _lru_make_
 from .transformer_utils import mask_from_lengths
 
 
+def check_head_sizes(stacks) -> None:
+    """The attention products of the training step contract over the head's columns in 64-wide k blocks (ttsb_bgemm,
+    include/ttsb.h): a head size that is not a multiple of 64 would add the next head's columns to this head's scores, so
+    only a block with a single head (whose columns end where the tensor ends) may have one, as a multiple of 16."""
+    for name, st in stacks.items():
+        for i, H in enumerate(st['heads']):
+            dh = int(st['d']) // int(H)
+            if dh % 64 != 0 and (int(H) != 1 or dh % 16 != 0):
+                raise ValueError(
+                    f"{name} block {i}: {H} heads at model dimension {st['d']} give a head size of {dh}, which the training step "
+                    f'does not support (inference does).  Head sizes that train: multiples of 64 (64, 128, 192, 256), or a '
+                    f'multiple of 16 in a block with a single head; choose {name}_num_heads accordingly.')
+
+
 class Adam:
     """Optimizer state in the reference's terms: lr (assignable), iterations, Keras hyper-parameters."""
 
@@ -34,6 +48,7 @@ class Adam:
 
 class TrainEngine:
     def __init__(self, model):
+        check_head_sizes(model._stacks)
         self.model = model
         self.dev = model.device
         names = list(model._param_shapes().keys())
