@@ -31,7 +31,7 @@ extern "C" {
 #define TTSB_ERR_CUDA (-2)
 #define TTSB_ERR_UNSUPPORTED (-3)
 
-#define TTSB_ABI_VERSION 3
+#define TTSB_ABI_VERSION 4
 
 /* precision of the tensor-core products */
 #define TTSB_PREC_BF16 0   /* single bf16 pass, fp32 accumulate */
@@ -567,70 +567,17 @@ int ttsb_griffinlim_batch(const float* magnitude, const float* init_angles, cons
                           float* wav_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
- * Ragged-batch Conv1D on the tensor cores (the MelGAN generator, transformertts_b200/model/melgan.py; the extended form below
- * serves the HiFi-GAN generator).
+ * Ragged-batch Conv1D on the tensor cores (the MelGAN and HiFi-GAN generators, transformertts_b200/model/melgan.py and
+ * hifigan.py).
  * Layout: a packed ragged batch of n_clips clips, channels-last 16-bit (rows, ld).  Clip c has L_c rows, given as the int32
- * prefix sums clip_offsets[0..n_clips] (HOST memory, clip_offsets[0] = 0), framed by TTSB_CONV1D_HALO halo rows on each
- * side: its rows are clip_offsets[c] + (2c + 1) HALO + [0, L_c), and the buffer holds clip_offsets[n_clips] + 2 HALO n_clips
- * rows.  Each call computes, for every clip row t in [0, L_c),
- *   y[c, t, :] = bias + sum_s  in_{tap_src[s]}[c, t + tap_shift[s], :] @ W[koff_s : koff_s + ld_in[tap_src[s]], :]
- * (|tap_shift| <= HALO, so a tap reads the clip's own halos; koff_s = the ld_in of the earlier taps).  W is the (K_total, N)
- * matrix packed by ttsb_pack_weight (n_pad = N); ld_in[src] is a multiple of 64 and every input column is read.
- * With up > 1 (a transposed conv phrased over its input rows), column n of y[c, t] is channel n % ld_out of output row
- * t up + n / ld_out: the outputs use the same layout with up L_c rows per clip, and N = up ld_out.
- * Outputs (bf16; the lo planes only in bf16x3; any may be NULL): out_hi/out_lo = y, act_hi/act_lo = LeakyReLU_0.2(y).
- * halo_mode: TTSB_HALO_NONE leaves the outputs' halos alone; TTSB_HALO_REFLECT writes output row L-1+k of a clip as a copy of
- * row L-1-k and row -k as a copy of row k (k = 1..HALO, needs up L_c > HALO); TTSB_HALO_ZERO writes zeros there (needs
- * up L_c >= HALO).  A halo row is written only by the store of the row it mirrors, never by a computed row.
- * N is a multiple of 64, and at most 256 or a multiple of 256; ld_out (= N / up) is a multiple of 16.  No atomics: a clip's
- * output is bit-identical wherever it sits in the batch.  workspace: ttsb_conv1d_workspace_bytes(n_clips) bytes of device
- * memory, 4-byte aligned; the entry points copy the clip table there.  Malformed offsets, clips too short for the halo
- * mode and a short workspace give TTSB_ERR_INVALID_ARGUMENT before any CUDA call.
- * ------------------------------------------------------------------------------------------------------- */
-#define TTSB_CONV1D_HALO 9
-#define TTSB_CONV1D_MAX_TAPS 7
-#define TTSB_HALO_NONE 0
-#define TTSB_HALO_REFLECT 1
-#define TTSB_HALO_ZERO 2
-typedef struct ttsb_conv1d_args {
-  int n_clips;
-  const int32_t* clip_offsets; /* HOST, int32 (n_clips + 1) */
-  int num_taps;
-  int tap_src[TTSB_CONV1D_MAX_TAPS];
-  int tap_shift[TTSB_CONV1D_MAX_TAPS];
-  const void* in_hi[2];
-  const void* in_lo[2];
-  int ld_in[2];
-  const void* w_hi;
-  const void* w_lo;
-  const float* bias; /* fp32 (N), or NULL */
-  int N;
-  int up;
-  void* out_hi;
-  void* out_lo;
-  void* act_hi;
-  void* act_lo;
-  int ld_out;
-  int halo_mode;
-  int precision; /* TTSB_PREC_BF16 or TTSB_PREC_BF16X3 */
-  void* workspace;
-  int64_t workspace_bytes;
-} ttsb_conv1d_args;
-int64_t ttsb_conv1d_workspace_bytes(int n_clips); /* -1 for n_clips < 1 */
-int ttsb_conv1d_tc(const ttsb_conv1d_args* a, void* stream);
-/* The generator's output layer: wav = tanh(bias + sum_{k=-3..3} in[t + k, :channels] . weight[k + 3, :]) for every clip row t
- * in [0, L_c - drop_tail), in = hi (+ lo) planes in the layout above (ld_in columns; the halos hold the reflect padding).
- * Clip c's samples go to wav_out[clip_offsets[c] - c drop_tail ...].  weight: fp32 (7, channels) on the device,
- * channels <= ld_in <= 256, every L_c > drop_tail >= 0. */
-int ttsb_conv1d_out_tanh(const void* in_hi, const void* in_lo, int ld_in, int channels, const int32_t* clip_offsets, int n_clips,
-                         int drop_tail, const float* weight, float bias, void* workspace, int64_t workspace_bytes, float* wav_out,
-                         void* stream);
-
-/* The same conv in its extended form (the HiFi-GAN generator, transformertts_b200/model/hifigan.py).  Differences from
- * ttsb_conv1d_tc:
- *   halo       halo rows on each side of every clip, 0..TTSB_CONV1D_EX_MAX_HALO, for the inputs and the outputs alike;
- *              |tap_shift| <= halo, and up to TTSB_CONV1D_EX_MAX_TAPS taps.
- *   slope      act = LeakyReLU_slope(y), slope in [0, 1].
+ * prefix sums clip_offsets[0..n_clips] (HOST memory, clip_offsets[0] = 0), framed by `halo` rows on each side (0..
+ * TTSB_CONV1D_EX_MAX_HALO, for the inputs and the outputs alike): its rows are clip_offsets[c] + (2c + 1) halo + [0, L_c), and
+ * the buffer holds clip_offsets[n_clips] + 2 halo n_clips rows.  Each call computes, for every clip row t in [0, L_c),
+ *   y[c, t, :] = bias + sum_s  in_{tap_src[s]}[c, t + tap_shift[s], :] @ W[koff_s : koff_s + ld_in[tap_src[s]], :]  (+ residual)
+ * (up to TTSB_CONV1D_EX_MAX_TAPS taps with |tap_shift| <= halo, so a tap reads the clip's own halos; koff_s = the ld_in of the
+ * earlier taps).  W is the (K_total, N) matrix packed by ttsb_pack_weight (n_pad = N); ld_in[src] is a multiple of 64 and every
+ * input column is read.  With up > 1 (a transposed conv phrased over its input rows), column n of y[c, t] is channel n % ld_out
+ * of output row t up + n / ld_out: the outputs use the same layout with up L_c rows per clip, and N = up ld_out.
  *   res_hi/lo  optional residual in the output layout (ld_out columns, res_lo only in bf16x3): y = bias + conv + (res_hi + res_lo).
  *              It must not alias out_hi or act_hi.
  *   sum        optional fp32 plane in the output layout, for the multi-receptive-field average of HiFi-GAN's resblocks, in torch's
@@ -640,11 +587,22 @@ int ttsb_conv1d_out_tanh(const void* in_hi, const void* in_lo, int ld_in, int ch
  *                TTSB_CONV1D_SUM_FINISH y = (sum + y) / sum_div (the last one; then out / act are written from this y)
  *              WRITE and ADD count as an output, so out and act may both be NULL.
  *   out_rows   rows of the output layout, sum up L_c + 2 halo n_clips: the shape of the outputs, the residual and the sum.
- * res_hi, res_lo and sum are 16-byte aligned.  With TTSB_HALO_NONE and zero-initialised planes the halos stay zero (no
- * computed row is ever stored into a halo), which is every zero-padded conv's padding, and clips of any length >= 1 work.
- * ttsb_conv1d_out_tanh_ex is ttsb_conv1d_out_tanh over a layout of `halo` (3..TTSB_CONV1D_EX_MAX_HALO) rows, whose halos hold
- * the padding (zeros for HiFi-GAN); it needs only L_c > drop_tail.  The refusals are those of ttsb_conv1d_tc, plus any
- * inconsistent halo, slope, residual, sum or out_rows, all before any CUDA call. */
+ * Outputs (bf16; the lo planes only in bf16x3; any may be NULL): out_hi/out_lo = y, act_hi/act_lo = LeakyReLU_slope(y), slope
+ * in [0, 1].
+ * halo_mode: TTSB_HALO_NONE leaves the outputs' halos alone; TTSB_HALO_REFLECT writes output row L-1+k of a clip as a copy of
+ * row L-1-k and row -k as a copy of row k (k = 1..halo, needs up L_c > halo); TTSB_HALO_ZERO writes zeros there (needs
+ * up L_c >= halo).  A halo row is written only by the store of the row it mirrors, never by a computed row.  So with
+ * TTSB_HALO_NONE and zero-initialised planes the halos stay zero, which is every zero-padded conv's padding, and clips of any
+ * length >= 1 work.
+ * N is a multiple of 64, and at most 256 or a multiple of 256; ld_out (= N / up) is a multiple of 16; res_hi, res_lo and sum
+ * are 16-byte aligned.  No atomics: a clip's output is bit-identical wherever it sits in the batch.  workspace:
+ * ttsb_conv1d_workspace_bytes(n_clips) bytes of device memory, 4-byte aligned; the entry points copy the clip table there.
+ * Malformed offsets, clips too short for the halo mode, a short workspace and any inconsistent halo, taps, slope, residual,
+ * sum or out_rows give TTSB_ERR_INVALID_ARGUMENT before any CUDA call.
+ * ------------------------------------------------------------------------------------------------------- */
+#define TTSB_HALO_NONE 0
+#define TTSB_HALO_REFLECT 1
+#define TTSB_HALO_ZERO 2
 #define TTSB_CONV1D_EX_MAX_TAPS 16
 #define TTSB_CONV1D_EX_MAX_HALO 64
 #define TTSB_CONV1D_SUM_NONE 0
@@ -683,7 +641,13 @@ typedef struct ttsb_conv1d_ex_args {
   void* workspace;
   int64_t workspace_bytes;
 } ttsb_conv1d_ex_args;
+int64_t ttsb_conv1d_workspace_bytes(int n_clips); /* -1 for n_clips < 1 */
 int ttsb_conv1d_ex_tc(const ttsb_conv1d_ex_args* a, void* stream);
+/* The generators' output layer: wav = tanh(bias + sum_{k=-3..3} in[t + k, :channels] . weight[k + 3, :]) for every clip row t
+ * in [0, L_c - drop_tail), in = hi (+ lo) planes in the layout above with `halo` rows (3..TTSB_CONV1D_EX_MAX_HALO) and ld_in
+ * columns; the halos hold the padding (reflected for MelGAN, zeros for HiFi-GAN).  Clip c's samples go to
+ * wav_out[clip_offsets[c] - c drop_tail ...].  weight: fp32 (7, channels) on the device, channels <= ld_in <= 256, every
+ * L_c > drop_tail >= 0. */
 int ttsb_conv1d_out_tanh_ex(const void* in_hi, const void* in_lo, int ld_in, int channels, int halo, const int32_t* clip_offsets,
                             int n_clips, int drop_tail, const float* weight, float bias, void* workspace, int64_t workspace_bytes,
                             float* wav_out, void* stream);

@@ -28,28 +28,64 @@ def test_header_symbols_are_all_exported(cdll):
 
 
 def test_abi_version_and_error_text(cdll):
-    assert cdll.ttsb_abi_version() == 3
+    assert cdll.ttsb_abi_version() == 4
     rc = cdll.ttsb_linear_fwd(None, None)
     assert rc == -1
     assert b'NULL' in cdll.ttsb_last_error()
 
 
+def _header_structs(header: str) -> dict:
+    """{struct name: [(field, C type, array length)]} of every `typedef struct name { ... } name;` in the header."""
+    macros = {m: int(v) for m, v in re.findall(r'#define (\w+) (\d+)', header)}
+    structs = {}
+    for name, body in re.findall(r'typedef struct (\w+) \{(.*?)\} \1;', header, re.S):
+        fields = []
+        for decl in re.sub(r'/\*.*?\*/', '', body, flags=re.S).split(';'):
+            if not decl.strip():
+                continue
+            ctype, first = re.match(r'\s*(.*?[\s*])(\w+(?:\[\w+\])?)$', decl.split(',')[0].rstrip()).groups()
+            for part in [first] + [d.strip() for d in decl.split(',')[1:]]:
+                fname, n = re.fullmatch(r'(\w+)(?:\[(\w+)\])?', part).groups()
+                fields.append((fname, ctype.strip(), None if n is None else int(macros.get(n, n))))
+        structs[name] = fields
+    return structs
+
+
 def test_struct_layout_matches_header():
-    """ctypes mirrors of ttsb_gemm_args / ttsb_mha_args: field order and names follow the header."""
+    """Every ctypes mirror in lib.py against its typedef struct: field names and order, C types, array lengths, offsets and
+    size; and the constants lib.py mirrors of the header's #defines."""
     from transformertts_b200 import lib
     header = (ROOT / 'include' / 'ttsb.h').read_text()
-    for struct, cls in (('ttsb_gemm_args', lib.GemmArgs), ('ttsb_mha_args', lib.MhaArgs)):
-        body = re.search(r'typedef struct %s \{(.*?)\} %s;' % (struct, struct), header, re.S).group(1)
-        body = re.sub(r'/\*.*?\*/', '', body, flags=re.S)
-        fields = []
-        for decl in body.split(';'):
-            decl = decl.strip()
-            if not decl:
-                continue
-            for part in decl.split(','):
-                name = re.findall(r'([A-Za-z_][A-Za-z0-9_]*)\s*(?:\[\d+\])?\s*$', part.strip())[0]
-                fields.append(name)
-        assert fields == [f[0] for f in cls._fields_], struct
+    structs = _header_structs(header)
+    mirrors = {'ttsb_pack_desc': lib.PackDesc, 'ttsb_gemm_args': lib.GemmArgs, 'ttsb_mha_args': lib.MhaArgs,
+               'ttsb_decode_attn_args': lib.DecodeAttnArgs, 'ttsb_bgemm_args': lib.BgemmArgs, 'ttsb_wgrad_args': lib.WgradArgs,
+               'ttsb_conv1d_ex_args': lib.Conv1dExArgs}
+    assert set(structs) == set(mirrors)
+    assert set(mirrors.values()) == {v for v in vars(lib).values() if isinstance(v, type) and issubclass(v, C.Structure)}
+    scalars = {'int': C.c_int, 'int64_t': C.c_int64, 'long long': C.c_longlong, 'uint32_t': C.c_uint32, 'float': C.c_float}
+    for struct, cls in mirrors.items():
+        fields = structs[struct]
+        assert [f[0] for f in fields] == [f[0] for f in cls._fields_], struct
+        offset = align = 0
+        for (name, ctype, n), (_, ptype) in zip(fields, cls._fields_):
+            base = C.c_void_p if ctype.endswith('*') else scalars[ctype]
+            if n is None:
+                assert ptype is base, (struct, name)
+            else:
+                assert issubclass(ptype, C.Array) and ptype._type_ is base and ptype._length_ == n, (struct, name)
+            size = C.sizeof(base)
+            offset = -(-offset // size) * size
+            assert getattr(cls, name).offset == offset, (struct, name)
+            offset += size * (n or 1)
+            align = max(align, size)
+        assert C.sizeof(cls) == -(-offset // align) * align, struct
+    for macro, value in (('TTSB_PREC_BF16', lib.PREC_BF16), ('TTSB_PREC_BF16X3', lib.PREC_BF16X3), ('TTSB_PREC_FP16', lib.PREC_FP16),
+                         ('TTSB_IMPL_TCGEN05', lib.IMPL_TCGEN05), ('TTSB_IMPL_SIMT', lib.IMPL_SIMT),
+                         ('TTSB_HALO_NONE', lib.HALO_NONE), ('TTSB_HALO_REFLECT', lib.HALO_REFLECT), ('TTSB_HALO_ZERO', lib.HALO_ZERO),
+                         ('TTSB_CONV1D_EX_MAX_TAPS', lib.CONV1D_EX_MAX_TAPS), ('TTSB_CONV1D_EX_MAX_HALO', lib.CONV1D_EX_MAX_HALO),
+                         ('TTSB_CONV1D_SUM_NONE', lib.SUM_NONE), ('TTSB_CONV1D_SUM_WRITE', lib.SUM_WRITE),
+                         ('TTSB_CONV1D_SUM_ADD', lib.SUM_ADD), ('TTSB_CONV1D_SUM_FINISH', lib.SUM_FINISH)):
+        assert re.search(r'#define %s (\d+)' % macro, header).group(1) == str(value), macro
 
 
 def test_argument_validation_without_gpu(cdll):

@@ -1,6 +1,6 @@
-"""The MelGAN vocoder on the GPU: each conv kind of ttsb_conv1d_tc against float64 torch convs (halos included), the whole
-generator against the float64 oracle (oracle/melgan_oracle.py), clip independence bit for bit, inference()'s int16 output,
-the launch count, and predict_tts.py --vocoder melgan end to end."""
+"""The MelGAN vocoder on the GPU: each conv kind of ttsb_conv1d_ex_tc with MelGAN's arguments against float64 torch convs
+(halos included), the whole generator against the float64 oracle (oracle/melgan_oracle.py), clip independence bit for bit,
+inference()'s int16 output, the launch count, and predict_tts.py --vocoder melgan end to end."""
 import subprocess
 import sys
 from pathlib import Path
@@ -48,7 +48,7 @@ def _oracle_wav(g, mel):
 
 # ---------------------------------------------------------------------------------------------------- one conv at a time
 def _run_conv(prec, conv_mat, bias, taps, srcs, counts, up, cout_cols, halo):
-    """One ttsb_conv1d_tc call on host-packed float64 sources -> (out, act) packed float64 (rows, cout_cols)."""
+    """One ttsb_conv1d_ex_tc call on host-packed float64 sources -> (out, act) packed float64 (rows, cout_cols)."""
     from transformertts_b200 import lib
     from transformertts_b200.model import melgan as mg
     gen = mg.MelGANGenerator(device=DEV, precision=prec)

@@ -1,8 +1,7 @@
 """CPU tests of the MelGAN vocoder's host side: the checkpoint specification and loader, weight-norm folding, the transposed-
-conv phase layout, the halo rule, the C-ABI refusals of ttsb_conv1d_tc / ttsb_conv1d_out_tanh and predict_tts's flags."""
+conv phase layout, the halo rule, the C-ABI refusals of ttsb_conv1d_ex_tc / ttsb_conv1d_out_tanh_ex with MelGAN's
+arguments and predict_tts's flags."""
 import ctypes as C
-import re
-from pathlib import Path
 
 import numpy as np
 import pytest
@@ -12,8 +11,6 @@ import torch.nn.functional as F
 from oracle import melgan_oracle as mo
 from transformertts_b200 import lib
 from transformertts_b200.model import melgan as mg
-
-ROOT = Path(__file__).resolve().parent.parent
 
 
 @pytest.fixture(scope='module')
@@ -146,28 +143,6 @@ def test_pack_clips_layout():
     assert (buf[:lib.CONV1D_HALO] == 0).all() and (buf[:, 3:] == 0).all()
 
 
-def test_conv1d_struct_matches_header():
-    header = (ROOT / 'include' / 'ttsb.h').read_text()
-    body = re.search(r'typedef struct ttsb_conv1d_args \{(.*?)\} ttsb_conv1d_args;', header, re.S).group(1)
-    body = re.sub(r'/\*.*?\*/', '', body, flags=re.S)
-    fields = []
-    for decl in body.split(';'):
-        decl = decl.strip()
-        if decl:
-            name, arr = re.findall(r'([A-Za-z_][A-Za-z0-9_]*)\s*(\[[A-Z0-9_]+\])?\s*$', decl)[0]
-            ctype = decl[:decl.rfind(name)].strip()
-            fields.append((name, ctype, arr))
-    assert [f[0] for f in fields] == [f[0] for f in lib.Conv1dArgs._fields_]
-    kinds = {'int': C.c_int, 'int64_t': C.c_int64}
-    for (name, ctype, arr), (pname, ptype) in zip(fields, lib.Conv1dArgs._fields_):
-        n = {'[TTSB_CONV1D_MAX_TAPS]': lib.CONV1D_MAX_TAPS, '[2]': 2, '': 1}[arr]
-        base = C.c_void_p if '*' in ctype else kinds[ctype]
-        assert C.sizeof(ptype) == n * C.sizeof(base) and (ptype == base if n == 1 else ptype._type_ == base), name
-    for macro, value in (('TTSB_CONV1D_HALO', lib.CONV1D_HALO), ('TTSB_CONV1D_MAX_TAPS', lib.CONV1D_MAX_TAPS),
-                         ('TTSB_HALO_NONE', lib.HALO_NONE), ('TTSB_HALO_REFLECT', lib.HALO_REFLECT), ('TTSB_HALO_ZERO', lib.HALO_ZERO)):
-        assert re.search(r'#define %s (\d+)' % macro, header).group(1) == str(value)
-
-
 @pytest.fixture(scope='module')
 def cdll():
     from transformertts_b200 import build
@@ -176,27 +151,30 @@ def cdll():
 
 
 def _valid_args(lengths, ws_bytes=None, up=1, halo=lib.HALO_REFLECT):
-    """Arguments that pass validation; the pointers are dummies (never dereferenced: every call below is refused)."""
+    """MelGAN's arguments (9 halo rows, three taps, slope 0.2) that pass validation; the pointers are dummies (never
+    dereferenced: every call below is refused)."""
     off = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int32)
     tab = (C.c_int32 * len(off))(*off.tolist())
-    a = lib.Conv1dArgs()
-    a.n_clips, a.clip_offsets, a.num_taps = len(lengths), C.cast(tab, C.c_void_p), 3
+    a = lib.Conv1dExArgs()
+    a.n_clips, a.clip_offsets, a.halo, a.num_taps = len(lengths), C.cast(tab, C.c_void_p), lib.CONV1D_HALO, 3
     for s, d in enumerate((-1, 0, 1)):
         a.tap_src[s], a.tap_shift[s] = 0, d
     a.in_hi[0] = a.in_lo[0] = a.w_hi = a.w_lo = a.act_hi = a.act_lo = 256
     a.ld_in[0], a.N, a.up, a.ld_out, a.halo_mode, a.precision = 64, 64 * up, up, 64, halo, lib.PREC_BF16X3
+    a.slope, a.sum_mode = 0.2, lib.SUM_NONE
+    a.out_rows = mg.layout_rows(lengths, up)
     a.workspace = 256
     a.workspace_bytes = ws_bytes if ws_bytes is not None else 8 * (len(lengths) + 1)
     return a, tab
 
 
 def _refused(cdll, a, text):
-    assert cdll.ttsb_conv1d_tc(C.byref(a), None) == -1
-    assert text in cdll.ttsb_last_error().decode()
+    assert cdll.ttsb_conv1d_ex_tc(C.byref(a), None) == -1
+    assert text in cdll.ttsb_last_error().decode(), cdll.ttsb_last_error().decode()
 
 
 def test_conv1d_refusals_without_gpu(cdll):
-    assert cdll.ttsb_conv1d_tc(None, None) == -1 and b'NULL' in cdll.ttsb_last_error()
+    assert cdll.ttsb_conv1d_ex_tc(None, None) == -1 and b'NULL' in cdll.ttsb_last_error()
     assert cdll.ttsb_conv1d_workspace_bytes(0) == -1 and cdll.ttsb_conv1d_workspace_bytes(3) == 32
     a, keep = _valid_args([12, 10]); a.clip_offsets = None; _refused(cdll, a, 'clip_offsets is NULL')
     a, keep = _valid_args([12, 10]); a.in_lo[0] = None; _refused(cdll, a, 'source 0')
@@ -204,26 +182,28 @@ def test_conv1d_refusals_without_gpu(cdll):
     a, keep = _valid_args([12, 10]); a.act_hi = None; _refused(cdll, a, 'no output')
     a, keep = _valid_args([12, 10]); a.workspace = None; _refused(cdll, a, 'workspace')
     a, keep = _valid_args([12, 10], ws_bytes=16); _refused(cdll, a, 'workspace')
-    a, keep = _valid_args([12, 10]); a.tap_shift[0] = -10; _refused(cdll, a, 'tap_shift')
+    a, keep = _valid_args([12, 10]); a.tap_shift[0] = -10; _refused(cdll, a, '|tap_shift| must be <= 9')
     a, keep = _valid_args([12, 10]); a.ld_in[0] = 80; _refused(cdll, a, 'ld_in')
     a, keep = _valid_args([12, 10]); a.N = 96; a.ld_out = 96; _refused(cdll, a, 'N = 96')
-    a, keep = _valid_args([12, 10]); a.num_taps = 8; _refused(cdll, a, 'num_taps')
+    a, keep = _valid_args([12, 10]); a.num_taps = 17; _refused(cdll, a, 'num_taps must be in [1, 16]')
     a, keep = _valid_args([12, 10]); a.precision = 2; _refused(cdll, a, 'precision')
     a, keep = _valid_args([12, 12, 9]); _refused(cdll, a, 'clip 2 has 9 output rows')        # reflect halos need 10
     a, keep = _valid_args([2, 3], up=8, halo=lib.HALO_ZERO); a.ld_out = 48; _refused(cdll, a, 'ld_out')
     a, keep = _valid_args([12, 10]); keep[1], keep[2] = 12, 11; _refused(cdll, a, 'increasing')   # non-monotonic
     a, keep = _valid_args([12, 10]); keep[0] = 1; _refused(cdll, a, 'clip_offsets[0]')
     a, keep = _valid_args([12, 10]); a.n_clips = 0; _refused(cdll, a, 'n_clips')
-    # the output layer
+    # the output layer over MelGAN's halo
     off = (C.c_int32 * 3)(0, 3000, 6000)
     p = C.c_void_p(256)
-    f = cdll.ttsb_conv1d_out_tanh
-    assert f(None, None, 64, 32, off, 2, 2560, p, C.c_float(0), p, C.c_int64(24), p, None) == -1
-    assert f(p, None, 64, 32, off, 2, 2560, p, C.c_float(0), p, C.c_int64(4), p, None) == -1
+    f = cdll.ttsb_conv1d_out_tanh_ex
+    H = lib.CONV1D_HALO
+    assert f(None, None, 64, 32, H, off, 2, 2560, p, C.c_float(0), p, C.c_int64(24), p, None) == -1
+    assert b'NULL' in cdll.ttsb_last_error()
+    assert f(p, None, 64, 32, H, off, 2, 2560, p, C.c_float(0), p, C.c_int64(4), p, None) == -1
     assert b'workspace' in cdll.ttsb_last_error()
-    assert f(p, None, 64, 65, off, 2, 2560, p, C.c_float(0), p, C.c_int64(24), p, None) == -1
+    assert f(p, None, 64, 65, H, off, 2, 2560, p, C.c_float(0), p, C.c_int64(24), p, None) == -1
     short = (C.c_int32 * 3)(0, 3000, 5000)
-    assert f(p, None, 64, 32, short, 2, 2560, p, C.c_float(0), p, C.c_int64(24), p, None) == -1
+    assert f(p, None, 64, 32, H, short, 2, 2560, p, C.c_float(0), p, C.c_int64(24), p, None) == -1
     assert b'clip 1' in cdll.ttsb_last_error()
 
 

@@ -2,20 +2,15 @@
 // ResStack's shortcut + 1x1 conv as one two-source product, transposed convs phrased over their input rows, and the input
 // convs.  Clips are packed channels-last with `halo` rows on each side (include/ttsb.h), so a tap is a row shift of a 2-D TMA
 // load and a 128-row tile may span several clips.  The epilogue (one thread per row) maps the row to its clip, skips halo
-// rows, adds the bias (and in the extended form a residual and the multi-receptive-field sum), writes y and LeakyReLU(y) as
-// bf16 hi/lo planes and mirrors the rows next to each clip edge into the halos the next conv reads.
-// ttsb_conv1d_tc (MelGAN: 9 halo rows, slope 0.2) and ttsb_conv1d_ex_tc (any halo up to 64, up to 16 taps, any slope, residual
-// and sum) run the same kernel template; kEx = false compiles the residual and sum steps out and fixes the halo and slope.
-// ttsb_conv1d_out_tanh / ttsb_conv1d_out_tanh_ex are the generators' N = 1 output layer.
+// rows, adds the bias, an optional residual and the multi-receptive-field sum, writes y and LeakyReLU(y) as bf16 hi/lo planes
+// and mirrors the rows next to each clip edge into the halos the next conv reads.  ttsb_conv1d_ex_tc takes the halo (up to 64
+// rows), up to 16 taps and the slope per call; ttsb_conv1d_out_tanh_ex is the generators' N = 1 output layer.
 #include <vector>
 
 #include "../../include/ttsb.h"
 #include "gemm_pipeline.cuh"
 
 namespace ttsb {
-
-constexpr int CONV_HALO = TTSB_CONV1D_HALO;
-constexpr float LRELU_SLOPE = 0.2f;  // ttsb_conv1d_tc's LeakyReLU
 
 struct ConvKParams {
   int rows;  // GEMM rows: every row of the packed input layout, halos included
@@ -26,12 +21,12 @@ struct ConvKParams {
   int n_clips;
   const int32_t* tab;  // device: region start rows [n_clips + 1], then the clip_offsets prefix sums [n_clips + 1]
   int up, halo_mode, ld_out;
-  int halo;     // kEx only (else CONV_HALO)
-  float slope;  // kEx only (else LRELU_SLOPE)
+  int halo;
+  float slope;
   const float* bias;
-  const __nv_bfloat16* res_hi;  // kEx only: residual planes, output layout
+  const __nv_bfloat16* res_hi;  // residual planes, output layout
   const __nv_bfloat16* res_lo;
-  float* sum;                   // kEx only: fp32 multi-receptive-field sum, output layout
+  float* sum;                   // fp32 multi-receptive-field sum, output layout
   int sum_mode;
   float sum_div;
   __nv_bfloat16* out_hi;
@@ -70,7 +65,7 @@ __device__ __forceinline__ void conv_store16(const ConvKParams& p, size_t orow, 
   }
 }
 
-// residual (hi + lo) and multi-receptive-field sum steps of ttsb_conv1d_ex_tc on 16 columns of output row orow
+// residual (hi + lo) and multi-receptive-field sum steps on 16 columns of output row orow
 __device__ __forceinline__ void conv_res_sum16(const ConvKParams& p, size_t orow, int col, float (&y)[16]) {
   const size_t o = orow * (size_t)p.ld_out + col;
   if (p.res_hi) {
@@ -104,11 +99,10 @@ __device__ __forceinline__ void conv_res_sum16(const ConvKParams& p, size_t orow
   }
 }
 
-template <bool kEx>
 __device__ __forceinline__ void conv_epilogue(const ConvKParams& p, const float* arow, int g, int n0, int half) {
   if (g >= p.rows) return;
-  const int H = kEx ? p.halo : CONV_HALO;
-  const float slope = kEx ? p.slope : LRELU_SLOPE;
+  const int H = p.halo;
+  const float slope = p.slope;
   const int32_t* reg = p.tab;
   const int32_t* off = p.tab + p.n_clips + 1;
   const int c = find_clip(reg, p.n_clips, g);
@@ -135,7 +129,7 @@ __device__ __forceinline__ void conv_epilogue(const ConvKParams& p, const float*
     }
     const int phase = col / p.ld_out, cc = col - phase * p.ld_out;
     const int pos = j * p.up + phase;  // position in the output clip
-    if (kEx) conv_res_sum16(p, (size_t)(base + pos), cc, y);
+    conv_res_sum16(p, (size_t)(base + pos), cc, y);
     conv_store16(p, (size_t)(base + pos), cc, y, false, slope);
     if (p.halo_mode == TTSB_HALO_REFLECT) {
       if (pos >= 1 && pos <= H) conv_store16(p, (size_t)(base - pos), cc, y, false, slope);
@@ -149,7 +143,7 @@ __device__ __forceinline__ void conv_epilogue(const ConvKParams& p, const float*
 
 // tensor maps: A[src][hi/lo] (ld_in[src], rows) boxes (64, 128); W[hi/lo] (K_total, N) boxes (64, block_n).  kNch: block_n / 64
 // (the wgmma width)
-template <bool kSplit, bool kEx, int kNch>
+template <bool kSplit, int kNch>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant__ CUtensorMap tmA0l,
                  const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUtensorMap tmA1l,
@@ -207,7 +201,7 @@ conv1d_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constan
       Cfg::Stage::template mma_park_tile<kNch>(ring, total_kb, img, Cfg::kPitch, wg);
       const int row = quarter * 32 + lane;
       __syncwarp();
-      conv_epilogue<kEx>(p, img + (size_t)row * Cfg::kPitch, m0 + row, n0, half);
+      conv_epilogue(p, img + (size_t)row * Cfg::kPitch, m0 + row, n0, half);
       ring.release_tile(false);
     }
   }
@@ -284,22 +278,22 @@ static int check_workspace(const char* what, const void* ws, int64_t bytes, int 
 }
 
 // launches the instantiation whose wgmma width kNch * 64 is p.block_n
-template <bool kSplit, bool kEx, int kNch = 1>
+template <bool kSplit, int kNch = 1>
 static int conv_launch_tc(const CUtensorMap (&tmA)[2][2], const CUtensorMap (&tmW)[2], const ConvKParams& p, cudaStream_t stream) {
   if constexpr (kNch < GEMM_NCH) {
-    if (p.block_n > kNch * 64) return conv_launch_tc<kSplit, kEx, kNch + 1>(tmA, tmW, p, stream);
+    if (p.block_n > kNch * 64) return conv_launch_tc<kSplit, kNch + 1>(tmA, tmW, p, stream);
   }
-  return launch_pipeline<conv1d_tc_kernel<kSplit, kEx, kNch>>(ConvCfg<kSplit>::kSmemBytes, p.num_tiles, false, stream, "conv1d_tc_kernel launch",
-                                                              tmA[0][0], tmA[0][1], tmA[1][0], tmA[1][1], tmW[0], tmW[1], p);
+  return launch_pipeline<conv1d_tc_kernel<kSplit, kNch>>(ConvCfg<kSplit>::kSmemBytes, p.num_tiles, false, stream, "conv1d_tc_kernel launch",
+                                                         tmA[0][0], tmA[0][1], tmA[1][0], tmA[1][1], tmW[0], tmW[1], p);
 }
 
-// the shared host side of ttsb_conv1d_tc (ex = false: no residual or sum, out_rows unchecked) and ttsb_conv1d_ex_tc
-static int conv1d_launch(const char* what, const ttsb_conv1d_ex_args* a, bool ex, int max_taps, void* stream_v) {
+// the host side of ttsb_conv1d_ex_tc: every refusal before any CUDA call
+static int conv1d_launch(const char* what, const ttsb_conv1d_ex_args* a, void* stream_v) {
   if (a->precision != TTSB_PREC_BF16 && a->precision != TTSB_PREC_BF16X3) { set_last_error("%s: unknown precision", what); return TTSB_ERR_INVALID_ARGUMENT; }
   const bool split = a->precision == TTSB_PREC_BF16X3;
   const int H = a->halo;
   if (H < 0 || H > TTSB_CONV1D_EX_MAX_HALO) { set_last_error("%s: halo = %d must be in [0, %d]", what, H, TTSB_CONV1D_EX_MAX_HALO); return TTSB_ERR_INVALID_ARGUMENT; }
-  if (a->num_taps < 1 || a->num_taps > max_taps) { set_last_error("%s: num_taps must be in [1, %d]", what, max_taps); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (a->num_taps < 1 || a->num_taps > TTSB_CONV1D_EX_MAX_TAPS) { set_last_error("%s: num_taps must be in [1, %d]", what, TTSB_CONV1D_EX_MAX_TAPS); return TTSB_ERR_INVALID_ARGUMENT; }
   int k_total = 0;
   for (int s = 0; s < a->num_taps; ++s) {
     const int src = a->tap_src[s];
@@ -315,30 +309,25 @@ static int conv1d_launch(const char* what, const ttsb_conv1d_ex_args* a, bool ex
   if (a->N < 64 || a->N % 64 || (a->N > GEMM_MAX_BN && a->N % GEMM_MAX_BN)) { set_last_error("%s: N = %d must be a multiple of 64, at most 256 or a multiple of 256", what, a->N); return TTSB_ERR_INVALID_ARGUMENT; }
   if (a->up < 1 || a->N % a->up || a->N / a->up != a->ld_out || a->ld_out % 16) { set_last_error("%s: need N = up * ld_out with ld_out a multiple of 16", what); return TTSB_ERR_INVALID_ARGUMENT; }
   if (a->halo_mode < TTSB_HALO_NONE || a->halo_mode > TTSB_HALO_ZERO) { set_last_error("%s: unknown halo_mode", what); return TTSB_ERR_INVALID_ARGUMENT; }
-  if (ex) {
-    if (!(a->slope == a->slope) || a->slope < 0.f || a->slope > 1.f) { set_last_error("%s: slope must be in [0, 1]", what); return TTSB_ERR_INVALID_ARGUMENT; }
-    if (a->res_hi && split != (a->res_lo != nullptr)) { set_last_error("%s: the residual needs res_lo in bf16x3 and only there", what); return TTSB_ERR_INVALID_ARGUMENT; }
-    if (!a->res_hi && a->res_lo) { set_last_error("%s: res_lo without res_hi", what); return TTSB_ERR_INVALID_ARGUMENT; }
-    if (a->res_hi && (a->res_hi == a->out_hi || a->res_hi == a->act_hi)) { set_last_error("%s: the residual must not alias an output", what); return TTSB_ERR_INVALID_ARGUMENT; }
-    if ((reinterpret_cast<uintptr_t>(a->res_hi) | reinterpret_cast<uintptr_t>(a->res_lo) | reinterpret_cast<uintptr_t>(a->sum)) % 16) {
-      set_last_error("%s: res_hi, res_lo and sum must be 16-byte aligned", what);
-      return TTSB_ERR_INVALID_ARGUMENT;
-    }
-    if (a->sum_mode < TTSB_CONV1D_SUM_NONE || a->sum_mode > TTSB_CONV1D_SUM_FINISH) { set_last_error("%s: unknown sum_mode", what); return TTSB_ERR_INVALID_ARGUMENT; }
-    if ((a->sum_mode != TTSB_CONV1D_SUM_NONE) != (a->sum != nullptr)) { set_last_error("%s: sum must be given exactly when sum_mode is not NONE", what); return TTSB_ERR_INVALID_ARGUMENT; }
-    if (a->sum_mode == TTSB_CONV1D_SUM_FINISH && !(a->sum_div >= 1.f && a->sum_div < 1e6f)) { set_last_error("%s: sum_div must be in [1, 1e6)", what); return TTSB_ERR_INVALID_ARGUMENT; }
-    const bool stores = a->sum_mode == TTSB_CONV1D_SUM_WRITE || a->sum_mode == TTSB_CONV1D_SUM_ADD;
-    if (!a->out_hi && !a->act_hi && !stores) { set_last_error("%s: no output", what); return TTSB_ERR_INVALID_ARGUMENT; }
-  } else if (!a->out_hi && !a->act_hi) {
-    set_last_error("%s: no output", what);
+  if (!(a->slope == a->slope) || a->slope < 0.f || a->slope > 1.f) { set_last_error("%s: slope must be in [0, 1]", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (a->res_hi && split != (a->res_lo != nullptr)) { set_last_error("%s: the residual needs res_lo in bf16x3 and only there", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (!a->res_hi && a->res_lo) { set_last_error("%s: res_lo without res_hi", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (a->res_hi && (a->res_hi == a->out_hi || a->res_hi == a->act_hi)) { set_last_error("%s: the residual must not alias an output", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if ((reinterpret_cast<uintptr_t>(a->res_hi) | reinterpret_cast<uintptr_t>(a->res_lo) | reinterpret_cast<uintptr_t>(a->sum)) % 16) {
+    set_last_error("%s: res_hi, res_lo and sum must be 16-byte aligned", what);
     return TTSB_ERR_INVALID_ARGUMENT;
   }
+  if (a->sum_mode < TTSB_CONV1D_SUM_NONE || a->sum_mode > TTSB_CONV1D_SUM_FINISH) { set_last_error("%s: unknown sum_mode", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if ((a->sum_mode != TTSB_CONV1D_SUM_NONE) != (a->sum != nullptr)) { set_last_error("%s: sum must be given exactly when sum_mode is not NONE", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (a->sum_mode == TTSB_CONV1D_SUM_FINISH && !(a->sum_div >= 1.f && a->sum_div < 1e6f)) { set_last_error("%s: sum_div must be in [1, 1e6)", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  const bool stores = a->sum_mode == TTSB_CONV1D_SUM_WRITE || a->sum_mode == TTSB_CONV1D_SUM_ADD;
+  if (!a->out_hi && !a->act_hi && !stores) { set_last_error("%s: no output", what); return TTSB_ERR_INVALID_ARGUMENT; }
   const int min_len = a->halo_mode == TTSB_HALO_REFLECT ? H + 1 : (a->halo_mode == TTSB_HALO_ZERO ? H : 1);
   std::vector<int32_t> tab;
   long long rows = 0, out_rows = 0;
   int rc = conv_table(what, a->clip_offsets, a->n_clips, a->up, H, min_len, tab, &rows, &out_rows);
   if (rc) return rc;
-  if (ex && a->out_rows != out_rows) {
+  if (a->out_rows != out_rows) {
     set_last_error("%s: out_rows = %lld, but the output layout of these clips has %lld rows (residual, sum and outputs all have that shape)",
                    what, (long long)a->out_rows, out_rows);
     return TTSB_ERR_INVALID_ARGUMENT;
@@ -388,11 +377,10 @@ static int conv1d_launch(const char* what, const ttsb_conv1d_ex_args* a, bool ex
     if (rc) return rc;
   }
   TTSB_CUDA_OK(cudaMemcpyAsync(a->workspace, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
-  if (ex) return split ? conv_launch_tc<true, true>(tmA, tmW, p, stream) : conv_launch_tc<false, true>(tmA, tmW, p, stream);
-  return split ? conv_launch_tc<true, false>(tmA, tmW, p, stream) : conv_launch_tc<false, false>(tmA, tmW, p, stream);
+  return split ? conv_launch_tc<true>(tmA, tmW, p, stream) : conv_launch_tc<false>(tmA, tmW, p, stream);
 }
 
-static int out_tanh_launch(const char* what, const void* in_hi, const void* in_lo, int ld_in, int channels, int halo, int min_len,
+static int out_tanh_launch(const char* what, const void* in_hi, const void* in_lo, int ld_in, int channels, int halo,
                            const int32_t* clip_offsets, int n_clips, int drop_tail, const float* weight, float bias, void* workspace,
                            int64_t workspace_bytes, float* wav_out, void* stream_v) {
   if (!in_hi || !weight || !wav_out) { set_last_error("%s: NULL pointer", what); return TTSB_ERR_INVALID_ARGUMENT; }
@@ -400,7 +388,8 @@ static int out_tanh_launch(const char* what, const void* in_hi, const void* in_l
   if (drop_tail < 0) { set_last_error("%s: drop_tail < 0", what); return TTSB_ERR_INVALID_ARGUMENT; }
   std::vector<int32_t> tab;
   long long rows = 0, out_rows = 0;
-  int rc = conv_table(what, clip_offsets, n_clips, 1, halo, min_len, tab, &rows, &out_rows);
+  // the 3-row padding lies in the halos, so any clip that outlasts drop_tail works
+  int rc = conv_table(what, clip_offsets, n_clips, 1, halo, drop_tail + 1, tab, &rows, &out_rows);
   if (rc) return rc;
   rc = check_workspace(what, workspace, workspace_bytes, n_clips);
   if (rc) return rc;
@@ -427,44 +416,9 @@ extern "C" int64_t ttsb_conv1d_workspace_bytes(int n_clips) {
   return 2 * (int64_t)(n_clips + 1) * (int64_t)sizeof(int32_t);
 }
 
-extern "C" int ttsb_conv1d_tc(const ttsb_conv1d_args* a, void* stream_v) {
-  if (!a) { set_last_error("ttsb_conv1d_tc: args is NULL"); return TTSB_ERR_INVALID_ARGUMENT; }
-  ttsb_conv1d_ex_args e{};
-  e.n_clips = a->n_clips;
-  e.clip_offsets = a->clip_offsets;
-  e.halo = CONV_HALO;
-  e.num_taps = a->num_taps;
-  for (int s = 0; s < TTSB_CONV1D_MAX_TAPS; ++s) { e.tap_src[s] = a->tap_src[s]; e.tap_shift[s] = a->tap_shift[s]; }
-  for (int i = 0; i < 2; ++i) { e.in_hi[i] = a->in_hi[i]; e.in_lo[i] = a->in_lo[i]; e.ld_in[i] = a->ld_in[i]; }
-  e.w_hi = a->w_hi;
-  e.w_lo = a->w_lo;
-  e.bias = a->bias;
-  e.N = a->N;
-  e.up = a->up;
-  e.out_hi = a->out_hi;
-  e.out_lo = a->out_lo;
-  e.act_hi = a->act_hi;
-  e.act_lo = a->act_lo;
-  e.ld_out = a->ld_out;
-  e.slope = LRELU_SLOPE;
-  e.halo_mode = a->halo_mode;
-  e.precision = a->precision;
-  e.workspace = a->workspace;
-  e.workspace_bytes = a->workspace_bytes;
-  return conv1d_launch("ttsb_conv1d_tc", &e, false, TTSB_CONV1D_MAX_TAPS, stream_v);
-}
-
 extern "C" int ttsb_conv1d_ex_tc(const ttsb_conv1d_ex_args* a, void* stream_v) {
   if (!a) { set_last_error("ttsb_conv1d_ex_tc: args is NULL"); return TTSB_ERR_INVALID_ARGUMENT; }
-  return conv1d_launch("ttsb_conv1d_ex_tc", a, true, TTSB_CONV1D_EX_MAX_TAPS, stream_v);
-}
-
-extern "C" int ttsb_conv1d_out_tanh(const void* in_hi, const void* in_lo, int ld_in, int channels, const int32_t* clip_offsets, int n_clips,
-                                    int drop_tail, const float* weight, float bias, void* workspace, int64_t workspace_bytes, float* wav_out,
-                                    void* stream_v) {
-  // the 3-row reflect padding lies in the halos: the clip needs rows 1..3 and must outlast drop_tail
-  return out_tanh_launch("ttsb_conv1d_out_tanh", in_hi, in_lo, ld_in, channels, CONV_HALO, drop_tail + 1 > 4 ? drop_tail + 1 : 4,
-                         clip_offsets, n_clips, drop_tail, weight, bias, workspace, workspace_bytes, wav_out, stream_v);
+  return conv1d_launch("ttsb_conv1d_ex_tc", a, stream_v);
 }
 
 extern "C" int ttsb_conv1d_out_tanh_ex(const void* in_hi, const void* in_lo, int ld_in, int channels, int halo, const int32_t* clip_offsets,
@@ -474,7 +428,6 @@ extern "C" int ttsb_conv1d_out_tanh_ex(const void* in_hi, const void* in_lo, int
     set_last_error("ttsb_conv1d_out_tanh_ex: halo = %d must be in [3, %d]", halo, TTSB_CONV1D_EX_MAX_HALO);
     return TTSB_ERR_INVALID_ARGUMENT;
   }
-  // the 3-row padding lies in the halos, so any clip that outlasts drop_tail works
-  return out_tanh_launch("ttsb_conv1d_out_tanh_ex", in_hi, in_lo, ld_in, channels, halo, drop_tail + 1, clip_offsets, n_clips, drop_tail,
-                         weight, bias, workspace, workspace_bytes, wav_out, stream_v);
+  return out_tanh_launch("ttsb_conv1d_out_tanh_ex", in_hi, in_lo, ld_in, channels, halo, clip_offsets, n_clips, drop_tail, weight, bias,
+                         workspace, workspace_bytes, wav_out, stream_v);
 }

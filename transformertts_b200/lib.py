@@ -33,7 +33,7 @@ EXPORTS = [
     'ttsb_stft_mel_log_batch_workspace_bytes', 'ttsb_stft_mel_log_batch', 'ttsb_pitch_workspace_bytes', 'ttsb_pitch_dio_stonemask',
     'ttsb_dp_unique_id', 'ttsb_dp_init', 'ttsb_dp_allreduce_bucket', 'ttsb_dp_destroy',
     'ttsb_decode_attn_workspace_bytes', 'ttsb_decode_attn', 'ttsb_decode_prologue', 'ttsb_decode_commit',
-    'ttsb_conv1d_workspace_bytes', 'ttsb_conv1d_tc', 'ttsb_conv1d_out_tanh', 'ttsb_conv1d_ex_tc', 'ttsb_conv1d_out_tanh_ex',
+    'ttsb_conv1d_workspace_bytes', 'ttsb_conv1d_ex_tc', 'ttsb_conv1d_out_tanh_ex',
     'ttsb_resample_batch_workspace_bytes', 'ttsb_resample_batch',
 ]
 
@@ -134,8 +134,6 @@ def load() -> C.CDLL:
     lib.ttsb_stft_mel_log_batch_workspace_bytes.restype = C.c_int64
     lib.ttsb_pitch_workspace_bytes.restype = C.c_int64
     lib.ttsb_conv1d_workspace_bytes.restype = C.c_int64
-    lib.ttsb_conv1d_out_tanh.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_float,
-                                         C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     lib.ttsb_conv1d_out_tanh_ex.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                             C.c_float, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     lib.ttsb_pitch_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double]
@@ -640,23 +638,13 @@ def decode_commit(post, B, r, mel, stop_col, stop_index, max_iters, mel_out, sto
 # ------------------------------------------------------------------------------------------------------------
 # ragged-batch Conv1D (the MelGAN and HiFi-GAN generators)
 # ------------------------------------------------------------------------------------------------------------
+# MelGAN's halo rows on each side of a clip (model/melgan.py): the largest tap shift of its convs, that of the ResStacks'
+# dilation-9 convs.  Not a header constant: every call passes its halo (HiFi-GAN's depends on the config).
 CONV1D_HALO = 9
-CONV1D_MAX_TAPS = 7
 HALO_NONE, HALO_REFLECT, HALO_ZERO = 0, 1, 2
 CONV1D_EX_MAX_TAPS = 16
 CONV1D_EX_MAX_HALO = 64
 SUM_NONE, SUM_WRITE, SUM_ADD, SUM_FINISH = 0, 1, 2, 3
-
-
-class Conv1dArgs(C.Structure):
-    _fields_ = [
-        ('n_clips', C.c_int), ('clip_offsets', C.c_void_p), ('num_taps', C.c_int),
-        ('tap_src', C.c_int * CONV1D_MAX_TAPS), ('tap_shift', C.c_int * CONV1D_MAX_TAPS),
-        ('in_hi', C.c_void_p * 2), ('in_lo', C.c_void_p * 2), ('ld_in', C.c_int * 2),
-        ('w_hi', C.c_void_p), ('w_lo', C.c_void_p), ('bias', C.c_void_p), ('N', C.c_int), ('up', C.c_int),
-        ('out_hi', C.c_void_p), ('out_lo', C.c_void_p), ('act_hi', C.c_void_p), ('act_lo', C.c_void_p), ('ld_out', C.c_int),
-        ('halo_mode', C.c_int), ('precision', C.c_int), ('workspace', C.c_void_p), ('workspace_bytes', C.c_int64),
-    ]
 
 
 def conv1d_workspace_bytes(n_clips: int) -> int:
@@ -664,19 +652,6 @@ def conv1d_workspace_bytes(n_clips: int) -> int:
     if n < 0:
         raise TtsbError(load().ttsb_last_error().decode())
     return n
-
-
-def conv1d_tc(args: Conv1dArgs):
-    """One ragged-batch conv (include/ttsb.h: ttsb_conv1d_tc).  args.clip_offsets points at a host int32 table."""
-    _check(load().ttsb_conv1d_tc(C.byref(args), _stream()), 'ttsb_conv1d_tc')
-
-
-def conv1d_out_tanh(in_hi, in_lo, channels, clip_offsets, drop_tail, weight, bias, workspace, wav_out):
-    """The generator's output layer (include/ttsb.h: ttsb_conv1d_out_tanh); clip_offsets: host sequence (n_clips + 1)."""
-    co, n = _host_offsets(clip_offsets)
-    _check(load().ttsb_conv1d_out_tanh(ptr(in_hi), ptr(in_lo), in_hi.shape[-1], int(channels), co, n, int(drop_tail), ptr(weight),
-                                       C.c_float(bias), ptr(workspace), C.c_int64(workspace.numel() * workspace.element_size()),
-                                       ptr(wav_out), _stream()), 'ttsb_conv1d_out_tanh')
 
 
 class Conv1dExArgs(C.Structure):
@@ -693,12 +668,13 @@ class Conv1dExArgs(C.Structure):
 
 
 def conv1d_ex_tc(args: Conv1dExArgs):
-    """One ragged-batch conv in the extended form (include/ttsb.h: ttsb_conv1d_ex_tc)."""
+    """One ragged-batch conv (include/ttsb.h: ttsb_conv1d_ex_tc).  args.clip_offsets points at a host int32 table."""
     _check(load().ttsb_conv1d_ex_tc(C.byref(args), _stream()), 'ttsb_conv1d_ex_tc')
 
 
 def conv1d_out_tanh_ex(in_hi, in_lo, channels, halo, clip_offsets, drop_tail, weight, bias, workspace, wav_out):
-    """The output layer over a layout of `halo` rows (include/ttsb.h: ttsb_conv1d_out_tanh_ex)."""
+    """The generators' output layer over a layout of `halo` rows (include/ttsb.h: ttsb_conv1d_out_tanh_ex); clip_offsets: host
+    sequence (n_clips + 1)."""
     co, n = _host_offsets(clip_offsets)
     _check(load().ttsb_conv1d_out_tanh_ex(ptr(in_hi), ptr(in_lo), in_hi.shape[-1], int(channels), int(halo), co, n, int(drop_tail),
                                           ptr(weight), C.c_float(bias), ptr(workspace),

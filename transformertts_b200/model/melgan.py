@@ -1,7 +1,7 @@
 """MelGAN generator (the vocoder of the reference's synthesis notebook: seungwonpark/melgan via torch.hub) on the GPU, a
 packed ragged batch of clips per call.
 
-Every conv of the generator is one ``ttsb_conv1d_tc`` launch over all clips (csrc/conv1d_tc.cu): clips are packed
+Every conv of the generator is one ``ttsb_conv1d_ex_tc`` launch over all clips (csrc/conv1d_tc.cu): clips are packed
 channels-last with ``lib.CONV1D_HALO`` halo rows on each side, which hold each clip's own reflect (or zero) padding, so a tap
 is a row shift and no clip sees another.  Per call: the input conv, then per upsampling stage the transposed conv plus two
 products per ResStack block (the dilated conv; the shortcut and the block's 1x1 conv as one two-source product), then the
@@ -150,16 +150,15 @@ class _Conv:
 
 
 def run_conv(conv: _Conv, counts_in, srcs, up: int, split: bool, out=None, act=None, halo=lib.HALO_NONE, ws=None,
-             rows_halo: int = lib.CONV1D_HALO, slope=None, res=None, sum_plane=None, sum_mode: int = lib.SUM_NONE, sum_div: float = 1.0):
-    """One conv launch: srcs = [(hi, lo)] per source, out / act / res = (hi, lo) planes or None.  With the defaults this is
-    ttsb_conv1d_tc (9 halo rows, LeakyReLU slope 0.2); a halo of `rows_halo` rows, another `slope`, a residual or a sum plane
-    (fp32, the output layout) make it ttsb_conv1d_ex_tc."""
-    ex = rows_halo != lib.CONV1D_HALO or slope is not None or res is not None or sum_plane is not None
-    a = lib.Conv1dExArgs() if ex else lib.Conv1dArgs()
+             rows_halo: int = lib.CONV1D_HALO, slope: float = 0.2, res=None, sum_plane=None, sum_mode: int = lib.SUM_NONE, sum_div: float = 1.0):
+    """One ttsb_conv1d_ex_tc launch: srcs = [(hi, lo)] per source, out / act / res = (hi, lo) planes or None, over a layout of
+    `rows_halo` halo rows; act is LeakyReLU_slope; sum_plane is fp32 in the output layout.  The defaults are MelGAN's."""
+    a = lib.Conv1dExArgs()
     off = ragged_offsets(counts_in)
     tab = (lib.C.c_int32 * len(off))(*off.tolist())
     a.n_clips = len(counts_in)
     a.clip_offsets = lib.C.cast(tab, lib.C.c_void_p)
+    a.halo = rows_halo
     a.num_taps = len(conv.taps)
     for s, (src, shift) in enumerate(conv.taps):
         a.tap_src[s], a.tap_shift[s] = src, shift
@@ -174,11 +173,7 @@ def run_conv(conv: _Conv, counts_in, srcs, up: int, split: bool, out=None, act=N
     a.halo_mode = halo
     a.precision = lib.PREC_BF16X3 if split else lib.PREC_BF16
     a.workspace, a.workspace_bytes = lib.ptr(ws), ws.numel()
-    if not ex:
-        lib.conv1d_tc(a)
-        return
-    a.halo = rows_halo
-    a.slope = 0.2 if slope is None else slope
+    a.slope = slope
     if res is not None:
         a.res_hi, a.res_lo = lib.ptr(res[0]), lib.ptr(res[1])
     if sum_plane is not None:
@@ -268,7 +263,7 @@ class MelGANGenerator:
         return hi, (torch.empty_like(hi) if self.split else None)
 
     def _run(self, conv: _Conv, counts_in, srcs, up: int, out=None, act=None, halo=lib.HALO_NONE, ws=None):
-        """One ttsb_conv1d_tc launch: srcs = [(hi, lo)] per source, out / act = (hi, lo) planes or None."""
+        """One conv launch: srcs = [(hi, lo)] per source, out / act = (hi, lo) planes or None."""
         run_conv(conv, counts_in, srcs, up, self.split, out=out, act=act, halo=halo, ws=ws)
 
     def vocode_device(self, mels: Sequence[np.ndarray]) -> torch.Tensor:
@@ -306,7 +301,8 @@ class MelGANGenerator:
                     xa, xb = xb, xa
                 counts = counts_out
             wav = torch.empty(HOP * sum(m.shape[1] for m in ms), dtype=torch.float32, device=self.device)
-            lib.conv1d_out_tanh(act[0], act[1], 32, ragged_offsets(counts), HOP * PAD_FRAMES, self._out_w, self._out_b, ws, wav)
+            lib.conv1d_out_tanh_ex(act[0], act[1], 32, lib.CONV1D_HALO, ragged_offsets(counts), HOP * PAD_FRAMES, self._out_w,
+                                   self._out_b, ws, wav)
         return wav
 
     def vocode_batch(self, mels: Sequence[np.ndarray]) -> List[np.ndarray]:
