@@ -6,8 +6,9 @@
     python predict_tts.py -f lines.txt --vocoder melgan --vocoder_checkpoint melgan.pt ...
     python predict_tts.py -f lines.txt --vocoder hifigan --vocoder_checkpoint g_02500000 [--vocoder_config v1|config.json] ...
 
-Every input line is tokenised, turned into a mel by ``ForwardTransformer.predict`` (one line per call, as the reference does)
-and vocoded on the GPU with ``Audio.reconstruct_waveform_batch`` (mel inversion + 32 Griffin-Lim iterations), in chunks of
+Every input line is tokenised and the lines are turned into mels by ``ForwardTransformer.predict_batch`` (sorted by length,
+a padded batch per forward pass; each mel is bit for bit what ``predict`` gives the line alone, which is how the reference
+predicts, one line per call).  The mels are vocoded on the GPU with ``Audio.reconstruct_waveform_batch`` (mel inversion + 32 Griffin-Lim iterations), in chunks of
 ``VOCODE_CHUNK`` lines so that device memory stays bounded however long the file is.  With ``--vocoder melgan`` the chunks
 go through a MelGAN generator instead (``MelGANGenerator.vocode_batch``, weights from ``--vocoder_checkpoint``), as the
 reference's synthesis notebook does one line at a time; a line of T frames then gives 256 T samples (Griffin-Lim:
@@ -134,17 +135,19 @@ def main(argv=None):
         from transformertts_b200.model.hifigan import HiFiGANGenerator
         vocoder = HiFiGANGenerator.from_checkpoint(args.vocoder_checkpoint, config=args.vocoder_config, device=model.device)
     print(f'Output wav under {output_path.parent}')
+    tokens = []
+    for line in text:
+        tokens.append(tokenizer(line))
+        if args.verbose:
+            print(f'Predicting {line}')
+            print(f'Tokens: "{tokens[-1]}"')
+    outs = model.predict_batch(tokens, encode=False, phoneme_max_duration=None)
     wavs = []
     for start in range(0, len(text), VOCODE_CHUNK):
         mels = []
         for i in range(start, min(start + VOCODE_CHUNK, len(text))):
-            tokens = tokenizer(text[i])
-            if args.verbose:
-                print(f'Predicting {text[i]}')
-                print(f'Tokens: "{tokens}"')
-            out = model.predict(tokens, encode=False, phoneme_max_duration=None)
-            mel = out['mel'].cpu().numpy()                      # (T, n_mels)
-            if mel.ndim != 2 or mel.shape[0] < 4:
+            mel = outs[i]['mel'].cpu().numpy()                  # (T, n_mels)
+            if mel.shape[0] < 4:
                 raise ValueError(f'line {i} gives a mel of shape {mel.shape}; the vocoder needs at least 4 frames')
             mels.append(mel)
             if args.store_mel:

@@ -181,7 +181,9 @@ struct PairCtx {
   uint32_t parity;
 };
 
-template <bool kLN>
+// kPairOrder (single-CTA LayerNorm tiles of a row that could also run as a CTA pair): the row statistics are formed in the
+// pair's order of operations, so the row's output is bit-identical whichever schedule runs its tile (see the LayerNorm part)
+template <bool kLN, bool kPairOrder>
 __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow, int b, int t0, int n0, int row, int half,
                                               int quarter, float* red /* [2][2][128] */,
                                               const PairCtx& px, uint8_t* stage_out, const CUtensorMap* tmOh, const CUtensorMap* tmOl,
@@ -315,6 +317,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
       for (int j = 0; j < 16; ++j) y[j] += rs[j];
     }
     zero_outside16(y, partial, c0, ncols, true);  // a masked row is zeroed in pass 2
+    if constexpr (!kPairOrder) {
     if (!have_k) { shiftK = y[0]; have_k = true; }   // column c0 of the first chunk is always a logical column when n_h > 0
     if (partial) {
 #pragma unroll
@@ -330,6 +333,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
         s_sh += dv;
         q_sh = fmaf(dv, dv, q_sh);
       }
+    }
     }
 #pragma unroll
     for (int j = 0; j < 16; ++j) rr[j] = __float_as_uint(y[j]);
@@ -350,6 +354,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
       pass1_chunk(ch + 1, r2, res2);
     }
   }
+  float mean, m2, n_total;
+  if constexpr (!kPairOrder) {
   // (mean, M2, n) of this thread's column range, then of the CTA's columns (half 0 is always operand 'a': both warps of
   // the pair evaluate the same expression and get bit-identical statistics)
   const int n_mine = max(0, min(ncols, ch_end << 4) - (ch_begin << 4));
@@ -367,7 +373,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
   const float n_a = half == 0 ? nf : (float)(ncols - n_mine), n_b = (float)ncols - n_a;
   const float mean_a = half == 0 ? mean_h : mean_o, mean_b = half == 0 ? mean_o : mean_h;
   const float m2_a = half == 0 ? m2_h : m2_o, m2_b = half == 0 ? m2_o : m2_h;
-  float mean, m2;
   if (n_b > 0.f && n_a > 0.f) {
     const float delta = mean_b - mean_a;
     mean = mean_a + delta * (n_b * inv_n);
@@ -376,7 +381,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
     mean = n_a > 0.f ? mean_a : mean_b;
     m2 = n_a > 0.f ? m2_a : m2_b;
   }
-  float n_total = (float)ncols;
+  n_total = (float)ncols;
   if (px.active) {
     // combine with the peer CTA's half of the row (Chan et al.): exact two-pass statistics with ONE exchange
     if (half == 0) st_cluster_v2(px.peer_slot + (uint32_t)row * 8u, mean, m2);
@@ -389,6 +394,47 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
     m2 = m2 + pr.y + delta * delta * (0.5f * (float)ncols);
     mean = 0.5f * (mean + pr.x);
     n_total = 2.f * (float)ncols;
+  }
+  } else {
+    // The pair's order of operations in one CTA.  N is a multiple of 32, so warp half h holds exactly pair CTA h's
+    // columns; the pair sums them as two ranges, one per warp, each shifted by its first value.  Those sums are formed
+    // again from the values pass 1 parked, and each step restates the pair path's expression above term for term: the
+    // two ranges' (mean, M2), Chan's merge of the ranges, then the equal-count merge of the halves.
+    const int ncols_h = ncols >> 1;
+    const int ch_mid = ch_begin + (((nch >> 1) + 1) >> 1);
+    const float inv_h = 1.f / (float)ncols_h;
+    float mean_r[2], m2_r[2];
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      const int lo = k ? ch_mid : ch_begin, hi = k ? ch_end : ch_mid;
+      const float kk = arow[lo << 4];
+      float s = 0.f, q = 0.f;
+      for (int ch = lo; ch < hi; ++ch) {
+        acc_ld16(arow + (ch << 4), r);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float dv = __uint_as_float(r[j]) - kk;
+          s += dv;
+          q = fmaf(dv, dv, q);
+        }
+      }
+      const float nr = (float)((hi - lo) << 4);
+      mean_r[k] = kk + s / nr;
+      m2_r[k] = fmaxf(q - s * s / nr, 0.f);
+    }
+    const float n_a = (float)((ch_mid - ch_begin) << 4), n_b = (float)ncols_h - n_a;
+    const float delta_r = mean_r[1] - mean_r[0];
+    const float mean_h = mean_r[0] + delta_r * (n_b * inv_h);
+    const float m2_h = m2_r[0] + m2_r[1] + delta_r * delta_r * (n_a * n_b * inv_h);
+    float* red_m2 = red + 2 * GEMM_BM;
+    red[half * GEMM_BM + row] = mean_h;
+    red_m2[half * GEMM_BM + row] = m2_h;
+    quarter_sync(quarter);
+    const float mean_o = red[(half ^ 1) * GEMM_BM + row], m2_o = red_m2[(half ^ 1) * GEMM_BM + row];
+    const float delta = mean_h - mean_o;
+    m2 = m2_h + m2_o + delta * delta * (0.5f * (float)ncols_h);
+    mean = 0.5f * (mean_h + mean_o);
+    n_total = 2.f * (float)ncols_h;
   }
   const float rstd = rsqrtf(m2 / n_total + p.eps);
   auto pass2_chunk = [&](int ch, uint32_t (&rr)[16]) {
@@ -418,8 +464,9 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
 // ----------------------------------------------------------------------------------------------------
 // kernel
 // ----------------------------------------------------------------------------------------------------
-// kNch: the tile width block_n in n64 blocks, rounded up (the wgmma width; the columns past block_n are computed and ignored)
-template <bool kSplit, bool kPair, bool kLN, int kNch>
+// kNch: the tile width block_n in n64 blocks, rounded up (the wgmma width; the columns past block_n are computed and ignored).
+// kPairOrder: see epilogue_tile
+template <bool kSplit, bool kPair, bool kLN, int kNch, bool kPairOrder = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant__ CUtensorMap tmA0l,
                const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUtensorMap tmA1l,
@@ -505,7 +552,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
         px.parity = (uint32_t)((iter >> 1) & 1);
       }
       const int row = quarter * 32 + lane;
-      epilogue_tile<kLN>(p, img + (size_t)row * Cfg::kPitch, b, t0, n_tile * p.block_n, row, half, quarter, red_all, px,
+      epilogue_tile<kLN, kPairOrder>(p, img + (size_t)row * Cfg::kPitch, b, t0, n_tile * p.block_n, row, half, quarter, red_all, px,
                          smem + Cfg::kStageOutOffset, &tmOh, &tmOl, slab_ctr);
       ring.release_tile(!kLN && p.staged && half == 0 && lane == 0);
     }
@@ -604,13 +651,13 @@ __global__ void gemm_simt_kernel(const GemmKParams p, const GemmSimtPtrs q) {
 // host
 // ----------------------------------------------------------------------------------------------------
 // launches the instantiation whose wgmma width kNch * 64 is q.block_n rounded up to a multiple of 64
-template <bool kSplit, bool kPair, bool kLN, int kNch = 1>
+template <bool kSplit, bool kPair, bool kLN, bool kPairOrder = false, int kNch = 1>
 static int launch_tc(const CUtensorMap (&tmA)[2][2], const CUtensorMap (&tmW)[2], const CUtensorMap (&tmO)[2], const GemmKParams& q,
                      int work, cudaStream_t stream) {
   if constexpr (kNch * 64 < GemmCfg<kSplit, kPair>::kMaxBn) {
-    if (q.block_n > kNch * 64) return launch_tc<kSplit, kPair, kLN, kNch + 1>(tmA, tmW, tmO, q, work, stream);
+    if (q.block_n > kNch * 64) return launch_tc<kSplit, kPair, kLN, kPairOrder, kNch + 1>(tmA, tmW, tmO, q, work, stream);
   }
-  return launch_pipeline<gemm_tc_kernel<kSplit, kPair, kLN, kNch>>(GemmCfg<kSplit, kPair>::kSmemBytes, work, kPair, stream,
+  return launch_pipeline<gemm_tc_kernel<kSplit, kPair, kLN, kNch, kPairOrder>>(GemmCfg<kSplit, kPair>::kSmemBytes, work, kPair, stream,
                                                                    kPair ? "gemm_tc_kernel<pair> launch" : "gemm_tc_kernel launch", tmA[0][0], tmA[0][1],
                                                                    tmA[1][0], tmA[1][1], tmW[0], tmW[1], tmO[0], tmO[1], q);
 }
@@ -784,6 +831,8 @@ extern "C" int ttsb_linear_fwd(const ttsb_gemm_args* a, void* stream_v) {
     // pair mode: a cluster of two CTAs per 128-row tile.  Separate instantiations for the LayerNorm and the plain epilogue:
     // each gets its own register allocation
     if (as_pair) return split ? launch_tc<true, true, true>(tmA, tmW, tmO, q, work, stream) : launch_tc<false, true, true>(tmA, tmW, tmO, q, work, stream);
+    if (q.gamma != nullptr && pair_ok)  // a row the pair schedule could also run: its arithmetic in a single CTA
+      return split ? launch_tc<true, false, true, true>(tmA, tmW, tmO, q, work, stream) : launch_tc<false, false, true, true>(tmA, tmW, tmO, q, work, stream);
     if (q.gamma != nullptr)
       return split ? launch_tc<true, false, true>(tmA, tmW, tmO, q, work, stream) : launch_tc<false, false, true>(tmA, tmW, tmO, q, work, stream);
     return split ? launch_tc<true, false, false>(tmA, tmW, tmO, q, work, stream) : launch_tc<false, false, false>(tmA, tmW, tmO, q, work, stream);

@@ -41,6 +41,30 @@ def _round_up(x: int, m: int) -> int:
     return (x + m - 1) // m * m
 
 
+# predict_batch with CUDA graphs pads phonemes and frames to these multiples, so that batches reuse captured graphs
+GRAPH_TP_MULTIPLE = 16
+GRAPH_TM_MULTIPLE = 64
+
+
+def _round_len(n: int, multiple: int, limit: int) -> int:
+    """n rounded up to a multiple, but not past `limit` (the positional-encoding table) unless n itself is."""
+    return max(n, min(_round_up(n, multiple), limit))
+
+
+def plan_batches(lengths, batch_size: int) -> List[List[int]]:
+    """predict_batch's plan: line indices sorted by length (ties in input order), in consecutive groups of batch_size."""
+    order = sorted(range(len(lengths)), key=lambda i: lengths[i])
+    return [order[i:i + batch_size] for i in range(0, len(order), batch_size)]
+
+
+def padded_batch(lines, idx, Tp: int, dtype=np.int32) -> np.ndarray:
+    """The lines `idx` as a (len(idx), Tp) array, each padded with zeros at the end."""
+    out = np.zeros((len(idx), Tp), dtype=dtype)
+    for r, i in enumerate(idx):
+        out[r, :len(lines[i])] = lines[i]
+    return out
+
+
 def _pick_block_n(N: int, need_single_tile: bool) -> int:
     n16 = _round_up(N, 16)
     if n16 <= 256:
@@ -531,9 +555,12 @@ class ForwardTransformer:
         return (at_hi, at_lo), wts
 
     def _block(self, P, name: str, i: int, x, lens, B: int, T: int, attn_out: Optional[dict], key: str, need_f32: bool = True,
-               maps: str = 'first'):
+               maps: str = 'first', isolate: bool = False):
         """One SelfAttentionDenseBlock / SelfAttentionConvBlock (reference: model/layers.py:214-264).  With
         `return_attention_weights` the probabilities (`maps` rows, see _mha) are stored in attn_out[key].
+
+        isolate: zero the padded frames of the intermediate conv outputs too, so every row computes what it computes
+        alone (the reference leaves them unmasked, and the next conv reads them as the frame after a row's last).
 
         In bf16x3 mode the hi/lo pair of an activation carries 16 mantissa bits and serves as the residual stream itself:
         the LayerNorm GEMMs then write no fp32 copy (x[0] / the returned z[0] are None unless `need_f32`) -- 4 instead of
@@ -584,15 +611,16 @@ class ForwardTransformer:
                 pl = P[pre + f'conv{j}']
                 _, o_hi, o_lo = self._act(B, T, pl.n_pad, f32=False)
                 self._gemm(pl, B, T, [(h_hi, h_lo, ld, 0)], [0] * k, shifts, relu=True, out_hi=o_hi, out_lo=o_lo,
-                           tag=f'{name}.conv{j}')
+                           row_len=lens if isolate else None, tag=f'{name}.conv{j}')
                 h_hi, h_lo, ld = o_hi, o_lo, pl.n_pad
             self._gemm(P[pre + f'conv{n - 1}'], B, T, [(h_hi, h_lo, ld, 0)], [0] * k, shifts, **res(y),
                        ln=(W[pre + 'ln2.gamma'], W[pre + 'ln2.beta']), row_len=lens, out_f32=z[0], out_hi=z[1], out_lo=z[2],
                        tag=f'{name}.conv{n - 1}')
         return z
 
-    def _stat_predictor(self, P, name: str, x, lens, B: int, T: int, relu_head: bool):
-        """StatPredictor (reference: model/layers.py:463-524).  The input is already zero at padded rows."""
+    def _stat_predictor(self, P, name: str, x, lens, B: int, T: int, relu_head: bool, isolate: bool = False):
+        """StatPredictor (reference: model/layers.py:463-524).  The input is already zero at padded rows; `isolate` zeroes
+        them in every conv + LayerNorm output as well (see _block)."""
         W = self.weights
         filt = self.config['duration_conv_filters' if name == 'dur_pred' else 'pitch_conv_filters']
         k = int(self.config['duration_kernel_size' if name == 'dur_pred' else 'pitch_kernel_size'])
@@ -604,7 +632,7 @@ class ForwardTransformer:
             pl = P[f'{name}.conv{j}']
             h_f, o_hi, o_lo = self._act(B, T, pl.n_pad)
             self._gemm(pl, B, T, [(h_hi, h_lo, ld, 0)], [0] * k, shifts, relu=True,
-                       ln=P[f'{name}.ln{j}'], out_f32=h_f, out_hi=o_hi, out_lo=o_lo)
+                       ln=P[f'{name}.ln{j}'], row_len=lens if isolate else None, out_f32=h_f, out_hi=o_hi, out_lo=o_lo)
             h_hi, h_lo, ld = o_hi, o_lo, pl.n_pad
         out = torch.empty((B, T), dtype=torch.float32, device=self.device)
         lib.statpred_head_fwd(h_f, int(filt[-1]), W[f'{name}.out.w'].reshape(-1).contiguous(), W[f'{name}.out.b'], relu_head, lens, out)
@@ -616,7 +644,7 @@ class ForwardTransformer:
     # ---- the two halves of call(): everything up to the integer durations, and the length regulator + decoder.  The
     # output length Tm = max_b sum_i durations[b,i] is data dependent (as in the reference), so the host reads the row
     # totals once between the two (one device->host copy + sync per call; it also carries the negative-duration flag).
-    def _stage_encoder(self, P, x, tgt_dur, tgt_pitch, scalar: float, mx, mn):
+    def _stage_encoder(self, P, x, tgt_dur, tgt_pitch, scalar: float, mx, mn, isolate: bool = False):
         W = self.weights
         dev = self.device
         B, Tp = x.shape
@@ -630,9 +658,10 @@ class ForwardTransformer:
         enc_attn = {}
         n_enc = len(self._stacks['encoder']['heads'])
         for i in range(n_enc):   # the pitch embedding below reads the fp32 plane of the last block
-            h = self._block(P, 'encoder', i, h, enc_len, B, Tp, enc_attn, self._attn_key('encoder', i), need_f32=(i == n_enc - 1))
-        durations = self._stat_predictor(P, 'dur_pred', h, enc_len, B, Tp, relu_head=True)
-        pitch = self._stat_predictor(P, 'pitch_pred', h, enc_len, B, Tp, relu_head=False)
+            h = self._block(P, 'encoder', i, h, enc_len, B, Tp, enc_attn, self._attn_key('encoder', i), need_f32=(i == n_enc - 1),
+                            isolate=isolate)
+        durations = self._stat_predictor(P, 'dur_pred', h, enc_len, B, Tp, relu_head=True, isolate=isolate)
+        pitch = self._stat_predictor(P, 'pitch_pred', h, enc_len, B, Tp, relu_head=False, isolate=isolate)
         src_pitch = tgt_pitch if tgt_pitch is not None else pitch
         h_pe = torch.empty((B, Tp, d), dtype=torch.float32, device=dev)
         lib.pitch_embed_add_fwd(h[0], src_pitch, P['pitch_embed.w'], W['pitch_embed.b'], h_pe)
@@ -643,7 +672,7 @@ class ForwardTransformer:
         return {'h_pe': h_pe, 'durations': durations, 'pitch': pitch, 'dur_int': dur_int, 'dec_len': dec_len,
                 'encoder_attention': enc_attn}
 
-    def _stage_decoder(self, P, st, B: int, Tm: int):
+    def _stage_decoder(self, P, st, B: int, Tm: int, isolate: bool = False):
         W = self.weights
         dev = self.device
         dd = self._stacks['decoder']['d']
@@ -654,7 +683,8 @@ class ForwardTransformer:
         lib.expand_ln_pe_fwd(st['h_pe'], idx, W['decoder.ln.gamma'], W['decoder.ln.beta'], P['decoder.pe'],
                              W['decoder.pos_scalar'].reshape(1), LN_EPS, m[0], m[1], m[2])
         for i in range(len(self._stacks['decoder']['heads'])):
-            m = self._block(P, 'decoder', i, m, st['dec_len'], B, Tm, dec_attn, self._attn_key('decoder', i), need_f32=False)
+            m = self._block(P, 'decoder', i, m, st['dec_len'], B, Tm, dec_attn, self._attn_key('decoder', i), need_f32=False,
+                            isolate=isolate)
         mel = torch.empty((B, Tm, self.mel_channels), dtype=torch.float32, device=dev)
         self._gemm(P['out'], B, Tm, [(m[1], m[2], dd, 0)], [0], [0], out_f32=mel, ld_out=self.mel_channels)
         return mel, dec_attn
@@ -693,20 +723,27 @@ class ForwardTransformer:
         tgt_dur, tgt_pitch = prep(target_durations, torch.float32), prep(target_pitch, torch.float32)
         mx, mn = prep(max_durations_mask, torch.float32), prep(min_durations_mask, torch.float32)
         scalar = 1.0 if tgt_dur is not None else float(durations_scalar)
+        return self._forward(P, x, tgt_dur, tgt_pitch, scalar, mx, mn)
+
+    def _forward(self, P, x, tgt_dur, tgt_pitch, scalar: float, mx, mn, isolate: bool = False):
+        """The two halves of call() on host (B,Tp) inputs, eager or as CUDA graphs.  isolate: each row computes exactly what it
+        computes alone (see _block); call() keeps the reference's padded-batch semantics and never sets it."""
+        dev = self.device
+        B = x.shape[0]
         use_graphs = self.cuda_graphs and not self.return_attention_weights and self._prof is None and self.impl != 'simt'
         if use_graphs:
-            return self._call_graphed(P, x, tgt_dur, tgt_pitch, scalar, mx, mn)
+            return self._call_graphed(P, x, tgt_dur, tgt_pitch, scalar, mx, mn, isolate)
 
         def dev_t(t, dtype):
             return None if t is None else t.to(device=dev, dtype=dtype).contiguous()
 
         st = self._stage_encoder(P, dev_t(x, torch.int32), dev_t(tgt_dur, torch.float32), dev_t(tgt_pitch, torch.float32), scalar,
-                                 dev_t(mx, torch.float32), dev_t(mn, torch.float32))
+                                 dev_t(mx, torch.float32), dev_t(mn, torch.float32), isolate=isolate)
         Tm = self._read_lengths(st['dec_len'])
         if Tm == 0:
             mel, dec_attn = torch.zeros((B, 0, self.mel_channels), dtype=torch.float32, device=dev), {}
         else:
-            mel, dec_attn = self._stage_decoder(P, st, B, Tm)
+            mel, dec_attn = self._stage_decoder(P, st, B, Tm, isolate=isolate)
         return self._outputs(st, mel, dec_attn, Tm)
 
     def _outputs(self, st, mel, dec_attn, Tm, clone: bool = False):
@@ -726,11 +763,11 @@ class ForwardTransformer:
         [(g, out)] = _capture_graphs(self, self.device, fn, fn)
         return g, out
 
-    def _call_graphed(self, P, x, tgt_dur, tgt_pitch, scalar, mx, mn):
+    def _call_graphed(self, P, x, tgt_dur, tgt_pitch, scalar, mx, mn, isolate: bool = False):
         dev = self.device
         B, Tp = x.shape
         key = (B, Tp, tgt_dur is not None, tgt_pitch is not None, mx is not None, mn is not None, scalar, self.precision,
-               self.attention_precision, id(P))
+               self.attention_precision, isolate, id(P))
         ent = _lru_get(self._enc_graphs, key)
         if ent is None:
             _lru_make_room(self._enc_graphs, self.max_cached_graphs)
@@ -738,7 +775,8 @@ class ForwardTransformer:
             ins = {'x': torch.empty((B, Tp), dtype=torch.int32, device=dev), 'dur': f32(tgt_dur), 'pitch': f32(tgt_pitch),
                    'mx': f32(mx), 'mn': f32(mn)}
             self._fill(ins, x, tgt_dur, tgt_pitch, mx, mn)
-            g, st = self._capture(lambda: self._stage_encoder(P, ins['x'], ins['dur'], ins['pitch'], scalar, ins['mx'], ins['mn']))
+            g, st = self._capture(lambda: self._stage_encoder(P, ins['x'], ins['dur'], ins['pitch'], scalar, ins['mx'], ins['mn'],
+                                                              isolate=isolate))
             ent = {'ins': ins, 'graph': g, 'st': st, 'dec': {}}
             self._enc_graphs[key] = ent
         else:
@@ -748,10 +786,12 @@ class ForwardTransformer:
         Tm = self._read_lengths(st['dec_len'])
         if Tm == 0:
             return self._outputs(st, torch.zeros((B, 0, self.mel_channels), dtype=torch.float32, device=dev), {}, 0, clone=True)
+        if isolate:  # the padding does not reach any row: run at a rounded length, so that batches share decoder graphs
+            Tm = _round_len(Tm, GRAPH_TM_MULTIPLE, self._stacks['decoder']['max_pos'])
         dec = _lru_get(ent['dec'], Tm)
         if dec is None:
             _lru_make_room(ent['dec'], self.max_cached_graphs)
-            g, (mel, dec_attn) = self._capture(lambda: self._stage_decoder(P, st, B, Tm))
+            g, (mel, dec_attn) = self._capture(lambda: self._stage_decoder(P, st, B, Tm, isolate=isolate))
             dec = {'graph': g, 'mel': mel}
             ent['dec'][Tm] = dec
         _replay(dec['graph'])
@@ -815,6 +855,80 @@ class ForwardTransformer:
                         durations_scalar=duration_scalar, max_durations_mask=max_mask, min_durations_mask=min_mask)
         out['mel'] = out['mel'].squeeze()
         return out
+
+    def predict_batch(self, inputs, encode=False, speed_regulator=1., phoneme_max_duration=None, phoneme_min_duration=None,
+                      phoneme_durations=None, phoneme_pitch=None, batch_size: int = 64) -> List[dict]:
+        """predict() for many lines, a padded batch per forward pass; no reference counterpart.
+
+        Line i's result equals predict(inputs[i]) bit for bit, whatever the other lines, the batch size or the line's place
+        in its batch: unlike a padded call(), which keeps the reference's batch semantics, the batch runs the forward with
+        isolated rows (every padded frame of every intermediate is zero, as Keras' 'same' padding gives a line alone).
+
+        inputs: 1-D token sequences without pad ids (or strings, with encode=True).  phoneme_durations / phoneme_pitch: None
+        or one array per line, as long as the line.  Speed and the max / min duration tables apply to every line.  Lines are
+        sorted by length and run batch_size at a time; with cuda_graphs=True the phoneme and frame axes are padded to
+        multiples of 16 and 64, so that captured graphs are reused across batches.
+
+        Returns one dict per line, in input order: 'mel' (T_i, n_mels), 'duration' and 'pitch' (Tp_i, 1), 'int_durations'
+        (Tp_i,) -- device tensors, as predict() returns -- and 'mel_lengths' T_i (int)."""
+        if self.return_attention_weights:
+            raise ValueError('predict_batch returns no attention weights: construct the model with return_attention_weights=False')
+        if batch_size < 1:
+            raise ValueError(f'batch_size must be positive, got {batch_size}')
+        if isinstance(inputs, (str, bytes)) or len(inputs) == 0:
+            raise ValueError('inputs must be a non-empty list of lines')
+        lines = []
+        for i, inp in enumerate(inputs):
+            if encode:
+                inp = self.encode_text(inp)
+            t = torch.as_tensor(inp).detach().cpu()
+            if t.dim() != 1 or t.numel() == 0:
+                raise ValueError(f'line {i}: expected a non-empty 1-D token sequence, got shape {tuple(t.shape)}')
+            t = t.to(torch.int32).numpy()
+            if (t == 0).any():
+                raise ValueError(f'line {i}: pad id 0 inside a line')
+            lines.append(t)
+        durs = self._per_line(phoneme_durations, lines, 'phoneme_durations')
+        pits = self._per_line(phoneme_pitch, lines, 'phoneme_pitch')
+        return self._predict_lines(lines, durs, pits, float(np.float32(1. / speed_regulator)), phoneme_max_duration,
+                                   phoneme_min_duration, int(batch_size))
+
+    @staticmethod
+    def _per_line(values, lines, name: str):
+        if values is None:
+            return None
+        if len(values) != len(lines):
+            raise ValueError(f'{name}: {len(values)} arrays for {len(lines)} lines')
+        out = []
+        for i, v in enumerate(values):
+            v = torch.as_tensor(v).detach().cpu().to(torch.float32).reshape(-1).numpy()
+            if v.shape[0] != len(lines[i]):
+                raise ValueError(f'{name}[{i}]: {v.shape[0]} values for a line of {len(lines[i])} tokens')
+            out.append(v)
+        return out
+
+    @_on_device
+    def _predict_lines(self, lines, durs, pits, duration_scalar: float, max_table, min_table, batch_size: int) -> List[dict]:
+        P = self._prepare()
+        graphs = self.cuda_graphs and self._prof is None and self.impl != 'simt'
+        results = [None] * len(lines)
+        for idx in plan_batches([len(t) for t in lines], batch_size):
+            Tp = max(len(lines[i]) for i in idx)
+            if graphs:
+                Tp = _round_len(Tp, GRAPH_TP_MULTIPLE, self._stacks['encoder']['max_pos'])
+            tok = padded_batch(lines, idx, Tp)
+            tgt_dur = None if durs is None else torch.from_numpy(padded_batch(durs, idx, Tp, np.float32))
+            tgt_pitch = None if pits is None else torch.from_numpy(padded_batch(pits, idx, Tp, np.float32))
+            mx = self._duration_mask(tok, max_table, float('inf'))
+            mn = self._duration_mask(tok, min_table, 0.0)
+            scalar = 1.0 if tgt_dur is not None else duration_scalar  # as call() does
+            out = self._forward(P, torch.from_numpy(tok), tgt_dur, tgt_pitch, scalar, mx, mn, isolate=True)
+            mel_len = self._len_host[:len(idx)].tolist()  # the row totals _forward read back
+            for r, i in enumerate(idx):
+                n, T = len(lines[i]), mel_len[r]
+                results[i] = {'mel': out['mel'][r, :T], 'duration': out['duration'][r, :n], 'pitch': out['pitch'][r, :n],
+                              'int_durations': out['int_durations'][r, :n], 'mel_lengths': T}
+        return results
 
     # ------------------------------------------------------------------------------------------------
     # persistence (reference: model/models.py:600-638 -- config.yaml + weights file in one directory)
