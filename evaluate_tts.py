@@ -1,0 +1,103 @@
+#!/usr/bin/env python
+"""Objective scores of ForwardTransformer checkpoints on the validation split (no reference counterpart).
+
+    python evaluate_tts.py --config CFG -p MODEL_DIR [-o OUTDIR]
+    python evaluate_tts.py --config CFG -p WEIGHTS_DIR --weights_glob 'step_*'          # every checkpoint, in step order
+    python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder melgan --vocoder_checkpoint melgan.pt
+    python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder hifigan --vocoder_checkpoint g_02500000 [--vocoder_config v1]
+
+The validation split is read as train_tts.py reads it (``valid_metadata``, ``mels``, ``durations`` and ``char_pitch`` of the
+config's data directory; ``pitch_stats.pkl`` for pitch errors in Hz when it exists).  For every checkpoint:
+
+* free running (``predict_batch`` of the phonemes alone): MCD-DTW against the recorded mel, duration MAE in frames per phoneme,
+  the exact-match rate and the ratio of predicted to recorded frames, pitch RMSE over the phonemes with a target pitch != 0;
+* teacher forced (``predict_batch`` with the target durations and pitch): MCD-DTW;
+* with ``--vocoder``: the free-running mels and the recorded mels (copy synthesis: the vocoder's own floor) are vocoded, their
+  log-mels re-extracted on the GPU and scored against the recorded mel.
+
+MCD is the DCT of the 80-bin natural-log mel (coefficients 1..24), not the SPTK / WORLD mel-cepstrum: compare its numbers
+with each other, not with papers (see transformertts_b200/utils/evaluation.py).  Per-line and corpus-mean values go to
+``<OUTDIR>/evaluation.json`` (default OUTDIR: MODEL_DIR), one entry per checkpoint; one summary line per checkpoint is printed.
+"""
+from __future__ import annotations
+
+import re
+from argparse import ArgumentParser
+from pathlib import Path
+
+
+def parse_args(argv=None):
+    parser = ArgumentParser()
+    parser.add_argument('--config', required=True, type=str)
+    parser.add_argument('--path', '-p', dest='path', required=True, type=str)
+    parser.add_argument('--weights_glob', default=None, type=str, help="checkpoint directories under --path, e.g. 'step_*'")
+    parser.add_argument('--outdir', '-o', dest='outdir', default=None, type=str)
+    parser.add_argument('--n_ceps', default=24, type=int)
+    parser.add_argument('--vocoder', default=None, choices=('griffinlim', 'melgan', 'hifigan'))
+    parser.add_argument('--vocoder_checkpoint', default=None, type=str)
+    parser.add_argument('--vocoder_config', default=None, type=str,
+                        help='HiFi-GAN config: a config.json path or v1 / v2 / v3 (default: config.json beside the checkpoint)')
+    args = parser.parse_args(argv)
+    if args.vocoder in ('melgan', 'hifigan') and args.vocoder_checkpoint is None:
+        parser.error(f'--vocoder {args.vocoder} needs --vocoder_checkpoint PATH')
+    if args.vocoder_config is not None and args.vocoder != 'hifigan':
+        parser.error('--vocoder_config applies to --vocoder hifigan only')
+    return args
+
+
+def checkpoints(path: Path, pattern):
+    """The model directories to score: `path` itself, or its sub-directories matching `pattern` in step order."""
+    if pattern is None:
+        return [path]
+    found = [p for p in path.glob(pattern) if (p / 'config.yaml').exists()]
+    if not found:
+        raise SystemExit(f'no checkpoint directory matches {path / pattern}')
+    step = lambda p: int(m.group(1)) if (m := re.search(r'(\d+)$', p.name)) else -1
+    return sorted(found, key=lambda p: (step(p), p.name))
+
+
+def main(argv=None):
+    args = parse_args(argv)
+    import yaml
+    from predict_tts import VOCODE_CHUNK, load_vocoder
+    from transformertts_b200.data.audio import Audio
+    from transformertts_b200.model.models import ForwardTransformer
+    from transformertts_b200.utils import evaluation as ev
+    from transformertts_b200.utils.training_config_manager import TrainingConfigManager
+
+    cm = TrainingConfigManager(args.config)
+    ev.check_normalizer(cm.config, 'config')
+    vs = ev.load_validation_set(cm)
+    root = Path(args.path)
+    results = []
+    vocoder = None
+    for ckpt in checkpoints(root, args.weights_glob):
+        model = ForwardTransformer.load_model(ckpt)
+        with open(ckpt / 'config.yaml') as f:
+            step = yaml.safe_load(f).get('step', model.step)
+        ev.check_normalizer(model.config)
+        audio = vocode = None
+        if args.vocoder is not None:
+            audio = Audio.from_config(model.config)
+            if vocoder is None:
+                vocoder = load_vocoder(args.vocoder, args.vocoder_checkpoint, args.vocoder_config, model)
+
+            def vocode(mels, audio=audio):
+                wavs = []
+                for start in range(0, len(mels), VOCODE_CHUNK):
+                    part = [m.T for m in mels[start:start + VOCODE_CHUNK]]
+                    wavs.extend(audio.reconstruct_waveform_batch(part, seed=start) if vocoder is None else vocoder.vocode_batch(part))
+                return wavs
+        res = ev.evaluate_model(model, vs, n_ceps=args.n_ceps, vocode=vocode, audio=audio)
+        res = dict(checkpoint=str(ckpt), step=int(step), **res)
+        results.append(res)
+        print(ev.summary_line(f'{ckpt.name} (step {step})', res), flush=True)
+    out = Path(args.outdir) if args.outdir is not None else root
+    ev.write_json({'config': str(args.config), 'n_ceps': args.n_ceps, 'vocoder': args.vocoder, 'lines': len(vs.names),
+                   'checkpoints': results}, out / 'evaluation.json')
+    print(f'wrote {out / "evaluation.json"}')
+    return 0
+
+
+if __name__ == '__main__':
+    raise SystemExit(main())

@@ -567,6 +567,32 @@ int ttsb_griffinlim_batch(const float* magnitude, const float* init_angles, cons
                           float* wav_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Mel-cepstral distortion after dynamic time warping  (evaluate_tts.py; no reference counterpart;
+ * tests/evaluation_oracle.py restates the definition in float64)
+ *   A packed ragged batch of n_pairs pairs of fp32 log-mel sequences (frames, n_mels) on the device: pair p compares frames
+ *   x_offsets[p] .. x_offsets[p+1] - 1 of x with frames y_offsets[p] .. y_offsets[p+1] - 1 of y (both tables int32
+ *   (n_pairs + 1) in HOST memory, from 0, every sequence >= 1 frame).  With K = n_ceps (1 <= K < n_mels):
+ *     cepstra   c_k[t] = sum_m dct[k-1][m] x[t][m], k = 1..K, summed in float64 in increasing m; dct fp64 (K, n_mels) on the
+ *               device, rows 1..K of the orthonormal DCT-II (c0, the energy, is left out);
+ *     distance  d(i, j) = kappa sqrt(2 sum_k (c_k[i] - c'_k[j])^2), summed in increasing k; kappa = 10 / ln 10 from the host;
+ *     DTW       steps (1,1), (1,0), (0,1): C[0][0] = d(0,0), C[i][j] = d(i,j) + min(C[i-1][j-1], C[i-1][j], C[i][j-1]),
+ *               ties to the diagonal unless another predecessor is strictly smaller, then (i-1, j) before (i, j-1); the
+ *               path length L (cells on the path) is that of the chosen predecessor + 1.
+ *   Outputs (device): cost_out fp64 (n_pairs) = C[Tx-1][Ty-1], path_len_out int32 (n_pairs) = L[Tx-1][Ty-1]; the pair's MCD is
+ *   cost / L.  Every product and sum is rounded on its own (no FMA contraction), so the result equals the float64 restatement
+ *   bit for bit and does not depend on the other pairs or the pair's position.  min(Tx, Ty) may be at most
+ *   TTSB_MCD_DTW_MAX_FRAMES: one CTA per pair keeps three anti-diagonals of (C, L) in shared memory.
+ *   workspace: ttsb_mcd_dtw_workspace_bytes(...) bytes of device memory, 8-byte aligned (the cepstra of every frame and the
+ *   pair table).  NULL pointers, malformed offsets, an empty sequence, K out of range, a pair past the frame limit, kappa not
+ *   finite and positive and a short workspace give TTSB_ERR_INVALID_ARGUMENT before any CUDA call.
+ * ------------------------------------------------------------------------------------------------------- */
+#define TTSB_MCD_DTW_MAX_FRAMES 4096
+int64_t ttsb_mcd_dtw_workspace_bytes(const int32_t* x_offsets, const int32_t* y_offsets, int n_pairs, int n_ceps); /* -1: invalid */
+int ttsb_mcd_dtw(const float* x, const int32_t* x_offsets, const float* y, const int32_t* y_offsets, int n_pairs, int n_mels,
+                 const double* dct, int n_ceps, double kappa, void* workspace, int64_t workspace_bytes, double* cost_out,
+                 int32_t* path_len_out, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Ragged-batch Conv1D on the tensor cores (the MelGAN and HiFi-GAN generators, transformertts_b200/model/melgan.py and
  * hifigan.py).
  * Layout: a packed ragged batch of n_clips clips, channels-last 16-bit (rows, ld).  Clip c has L_c rows, given as the int32

@@ -111,6 +111,22 @@ def load_model(args):
     return model, dict(model.config), args.step
 
 
+def load_vocoder(name: str, checkpoint, config, model):
+    """The generator --vocoder names (weights from checkpoint, HiFi-GAN's config from config) on the model's device, or None
+    for Griffin-Lim, which Audio.reconstruct_waveform_batch runs."""
+    if name == 'melgan':
+        from transformertts_b200.model.melgan import MelGANGenerator
+        return MelGANGenerator.from_checkpoint(checkpoint, device=model.device)
+    if name == 'hifigan':
+        normalizer = model.config.get('normalizer')
+        if normalizer != 'MelGAN':
+            raise SystemExit(f'--vocoder hifigan takes the MelGAN normaliser\'s log-mels (ln(max(S, 1e-5))); this model\'s normalizer '
+                             f'is {normalizer!r}, whose mels HiFi-GAN would misread')
+        from transformertts_b200.model.hifigan import HiFiGANGenerator
+        return HiFiGANGenerator.from_checkpoint(checkpoint, config=config, device=model.device)
+    return None
+
+
 def main(argv=None):
     args = parse_args(argv)
     fname, text = read_input(args)
@@ -123,17 +139,7 @@ def main(argv=None):
     from transformertts_b200.data.audio import Audio
     audio = Audio.from_config(model.config)
     tokenizer = make_tokenizer(model)
-    vocoder = None
-    if args.vocoder == 'melgan':
-        from transformertts_b200.model.melgan import MelGANGenerator
-        vocoder = MelGANGenerator.from_checkpoint(args.vocoder_checkpoint, device=model.device)
-    elif args.vocoder == 'hifigan':
-        normalizer = model.config.get('normalizer')
-        if normalizer != 'MelGAN':
-            raise SystemExit(f'--vocoder hifigan takes the MelGAN normaliser\'s log-mels (ln(max(S, 1e-5))); this model\'s normalizer '
-                             f'is {normalizer!r}, whose mels HiFi-GAN would misread')
-        from transformertts_b200.model.hifigan import HiFiGANGenerator
-        vocoder = HiFiGANGenerator.from_checkpoint(args.vocoder_checkpoint, config=args.vocoder_config, device=model.device)
+    vocoder = load_vocoder(args.vocoder, args.vocoder_checkpoint, args.vocoder_config, model)
     print(f'Output wav under {output_path.parent}')
     tokens = []
     for line in text:

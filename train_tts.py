@@ -15,7 +15,9 @@ durations and per-character pitch can be produced here with ``train_aligner.py``
 ``transformertts_b200/data/datasets.py`` with the bucket boundaries / batch sizes of the config (yaml :22-24), shuffled with
 the reference's seed, assembled in pinned memory and copied to the GPU on a side stream (``PrefetchLoader``).  Under
 torchrun every rank takes its row slice of each global batch (bucket batch sizes rounded down to a multiple of the world
-size).  TensorBoard logging, audio rendering and the espeak phonemizer are outside the hot path.
+size).  TensorBoard logging, audio rendering and the espeak phonemizer are outside the hot path.  With ``--evaluate``, every
+validation also scores free-running predictions of the validation split on rank 0 (MCD-DTW, duration and pitch errors; see
+evaluate_tts.py) and writes them to ``<log_dir>/evaluation_step_N.json``.
 """
 from __future__ import annotations
 
@@ -104,7 +106,12 @@ def main():
     ap.add_argument('--batch_size', type=int, default=32)
     ap.add_argument('--weights_dir', default=None)
     ap.add_argument('--checkpoint_frequency', type=int, default=1000, help="steps between rewrites of weights/latest (reference: 1000)")
+    ap.add_argument('--evaluate', action='store_true',
+                    help='at every validation, also score free-running predictions of the validation split (rank 0; '
+                         'writes evaluation_step_N.json under the log directory, see evaluate_tts.py)')
     args = ap.parse_args()
+    if args.evaluate and (args.synthetic or args.batches):
+        ap.error('--evaluate scores the on-disk validation split; it does not apply to --synthetic or --batches')
 
     local_rank = int(os.environ.get('LOCAL_RANK', '0'))
     torch.cuda.set_device(local_rank)
@@ -147,6 +154,11 @@ def main():
             next(data)
     else:
         data, valid = make_datasets(cm, cfg, rank, world, device)
+    eval_set = None
+    if args.evaluate and rank == 0:
+        from transformertts_b200.utils import evaluation as ev
+        ev.check_normalizer(cfg, 'config')
+        eval_set = ev.load_validation_set(cm)
     max_steps = args.max_steps or int(cfg['max_steps'])
     save_freq, save_start = int(cfg.get('weights_save_frequency', 5000)), int(cfg.get('weights_save_starting_step', 0))
     val_freq = int(cfg.get('validation_frequency', 0) or 0)
@@ -169,6 +181,10 @@ def main():
             v = validate(model, valid, device, world > 1)
             if rank == 0:
                 print(f'validation loss at step {model.step}: {v:.4f}', flush=True)
+            if eval_set is not None:
+                res = dict(step=model.step, **ev.evaluate_model(model, eval_set, teacher_forced=False))
+                print(ev.summary_line(f'evaluation at step {model.step}', res), flush=True)
+                ev.write_json(res, cm.log_dir / f'evaluation_step_{model.step}.json')
     if rank == 0:
         model.save_model(cm.weights_dir / f'step_{model.step}')
         model.save_model(cm.weights_dir / 'latest')

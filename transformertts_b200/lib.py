@@ -35,6 +35,7 @@ EXPORTS = [
     'ttsb_decode_attn_workspace_bytes', 'ttsb_decode_attn', 'ttsb_decode_prologue', 'ttsb_decode_commit',
     'ttsb_conv1d_workspace_bytes', 'ttsb_conv1d_ex_tc', 'ttsb_conv1d_out_tanh_ex',
     'ttsb_resample_batch_workspace_bytes', 'ttsb_resample_batch',
+    'ttsb_mcd_dtw_workspace_bytes', 'ttsb_mcd_dtw',
 ]
 
 
@@ -143,6 +144,10 @@ def load() -> C.CDLL:
     lib.ttsb_resample_batch_workspace_bytes.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
     lib.ttsb_resample_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
                                         C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.ttsb_mcd_dtw_workspace_bytes.restype = C.c_int64
+    lib.ttsb_mcd_dtw_workspace_bytes.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    lib.ttsb_mcd_dtw.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_double,
+                                 C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
     for name in EXPORTS:
         if not hasattr(lib, name):
             raise TtsbError(f'libttsb.so does not export {name}')
@@ -384,6 +389,36 @@ def resample_batch(wav, sample_offsets, src_rates, dst_rate, half_window, out_of
     ws = torch.empty(nb, dtype=torch.uint8, device=wav.device)
     _check(load().ttsb_resample_batch(ptr(wav), so, rates, n, int(dst_rate), ptr(half_window), half_window.numel(), oo, ptr(ws),
                                       C.c_int64(nb), ptr(out), _stream()), 'ttsb_resample_batch')
+
+
+# the longest shorter side of a pair ttsb_mcd_dtw takes (include/ttsb.h: TTSB_MCD_DTW_MAX_FRAMES)
+MCD_DTW_MAX_FRAMES = 4096
+
+
+def mcd_dtw_workspace_bytes(x_offsets, y_offsets, n_ceps: int) -> int:
+    xo, n = _host_offsets(x_offsets)
+    yo, n_y = _host_offsets(y_offsets)
+    if n_y != n:
+        raise TtsbError(f'{n} pairs in x_offsets, {n_y} in y_offsets')
+    nb = int(load().ttsb_mcd_dtw_workspace_bytes(xo, yo, n, int(n_ceps)))
+    if nb < 0:
+        raise TtsbError(load().ttsb_last_error().decode())
+    return nb
+
+
+def mcd_dtw(x, x_offsets, y, y_offsets, dct, kappa, cost_out, path_len_out):
+    """DTW cost and path length of every pair of a packed ragged batch of log-mel sequences (include/ttsb.h: ttsb_mcd_dtw).
+    x, y fp32 (frames, n_mels), dct fp64 (n_ceps, n_mels), cost_out fp64 (n_pairs,) and path_len_out int32 (n_pairs,) on the
+    device; the offset tables (n_pairs + 1) are host sequences."""
+    xo, n = _host_offsets(x_offsets)
+    yo, n_y = _host_offsets(y_offsets)
+    if n_y != n:
+        raise TtsbError(f'{n} pairs in x_offsets, {n_y} in y_offsets')
+    n_ceps, n_mels = dct.shape
+    nb = mcd_dtw_workspace_bytes(x_offsets, y_offsets, n_ceps)
+    ws = torch.empty(nb, dtype=torch.uint8, device=x.device)
+    _check(load().ttsb_mcd_dtw(ptr(x), xo, ptr(y), yo, n, int(n_mels), ptr(dct), int(n_ceps), float(kappa), ptr(ws), C.c_int64(nb),
+                               ptr(cost_out), ptr(path_len_out), _stream()), 'ttsb_mcd_dtw')
 
 
 # ------------------------------------------------------------------------------------------------------------
