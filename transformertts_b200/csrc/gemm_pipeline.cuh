@@ -7,11 +7,14 @@
 //               output row: warp (quarter = warp & 3, half = warp >> 2) owns rows [32*quarter, +32) and one half of the
 //               tile's 16-column chunks, so two warps per SM sub-partition hide each other's latencies
 //   warps 9-11  idle: the producer warpgroup hands its registers to the others with setmaxnreg
-// The producer refills the ring only after the epilogue has released the previous tile's image (no double buffering).
+// With an image epilogue the producer refills the ring only after the epilogue has released the previous tile's image
+// (wait_image_free / release_tile: no double buffering).  An epilogue that runs from the accumulator registers and stages
+// its stores outside the ring (gemm_tc.cu, the plain 16-bit epilogue) skips both, and the producer loads the next tile
+// while it runs.
 // A kernel supplies the TMA loads of a stage, the wgmma products of a k block (KMajorStage for K-major A and B tiles) and
-// its epilogue.  16-bit outputs leave through staging boxes in the ring (stage_out_offset, staged_slab_begin / _end) as
-// TMA tile stores: a thread owns one output ROW, so direct stores are 32-byte pieces of 32 different rows per warp
-// instruction (request-rate bound).
+// its epilogue.  16-bit outputs of an image epilogue leave through staging boxes in the ring (stage_out_offset,
+// staged_slab_begin / _end) as TMA tile stores: a thread owns one output ROW, so direct stores are 32-byte pieces of 32
+// different rows per warp instruction (request-rate bound).
 #pragma once
 #include <cuda_bf16.h>
 
@@ -63,7 +66,7 @@ __device__ __forceinline__ void wgmma_ss_kmajor_bf16(float (&d)[NCH * 32], uint6
 
 // Ring of kStages stages at the (1024-aligned) shared-memory base, followed by GEMM_RING_BAR_BYTES of barriers: full[s]
 // completes when stage s has landed (one arrival + the TMA bytes), empty[s] when the 8 consumer warps are done reading it,
-// img_free when the epilogue has released the previous tile's image.  Every thread constructs its own GemmRing: the producer
+// img_free when an image epilogue has released the previous tile's image.  Every thread constructs its own GemmRing: the producer
 // and the consumers each advance their own copy of the position (img_phase / first are the producer's only).
 constexpr int GEMM_RING_BAR_BYTES = 256;
 template <int kStages, int kStageBytes>

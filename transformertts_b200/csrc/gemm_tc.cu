@@ -1,7 +1,8 @@
 // Tensor-core GEMM family for the ForwardTransformer blocks (Dense / concat-projection / Conv1D 'same') on the pipeline of
 // gemm_pipeline.cuh: the producer reads activations through 3-D maps over (C,T,B) (OOB rows = 'same' zero padding), and
 // the thread-per-row epilogue fuses bias / ReLU / residual / LayerNorm / row mask and writes fp32 + bf16 hi/lo (or fp16)
-// copies for the next GEMM / the attention kernel.
+// copies for the next GEMM / the attention kernel.  A plain epilogue with 16-bit outputs only runs from the accumulator
+// registers instead (epilogue_regs), and the producer loads the next tile meanwhile.
 //
 // Replaces, in the reference (TF2/Keras ops): model/layers.py:134-136,149 (q/k/v + concat projection),
 // :93-94 (FFN), :19-26,36-40 (Conv1D stack + residual LayerNorm), :498-524 (predictor convs), model/models.py:422.
@@ -38,26 +39,31 @@ struct GemmKParams {
   float drop_pre_p, drop_post_p;  // training dropout: on the GEMM output before the residual add / on the LayerNorm output
   uint32_t drop_pre_site, drop_post_site, drop_seed;
   int h16;  // 1: out_hi receives IEEE fp16 instead of bf16 (single plane; operands of the fp16 attention)
-  int staged;  // 1: 16-bit outputs go through shared memory and TMA tile stores (plain epilogue, block_n % 64 == 0)
 };
 
 // kPair: the LayerNorm GEMMs run as a cluster of two CTAs that split the N (row) dimension of one 128-row tile in halves
 // (twice as many work items -> no wave-quantisation tail, small-M encoder GEMMs fill the chip) and exchange per-row
 // (mean, M2) through distributed shared memory before normalising.
 constexpr int PAIR_MAX_BN = 192;
+constexpr int REG_BOX_ROWS = 16;                  // register epilogue: one warp's rows of the tile
+constexpr int REG_BOX_COLS = 32;
+constexpr int REG_BOX_BYTES = REG_BOX_ROWS * 64;  // a [16 rows x 32 cols] 16-bit staging box, 64B-swizzled
 template <bool kSplit, bool kPair>
 struct GemmCfg {
   static constexpr int kMaxBn = kPair ? PAIR_MAX_BN : GEMM_MAX_BN;
   using Stage = KMajorStage<kSplit, kMaxBn * GEMM_BK * 2>;
   using Ring = typename Stage::Ring;
   static constexpr int kPitch = acc_pitch(kMaxBn);
-  // the plain (non-LayerNorm) epilogue stages two planes; pair mode is LayerNorm-only
-  static constexpr int kStageOutOffset = stage_out_offset(kMaxBn);
-  static_assert(img_bytes(kMaxBn) <= Ring::kBytes && (kPair || kStageOutOffset + STAGE_OUT_BYTES <= Ring::kBytes), "image must fit the ring");
+  static_assert(img_bytes(kMaxBn) <= Ring::kBytes, "image must fit the ring");
   static constexpr int kRedOffset = Ring::kBytes + GEMM_RING_BAR_BYTES;  // [2][2][128] floats of intra-CTA exchange
   static constexpr int kXchgOffset = kRedOffset + 2048;         // pair mode: [2 slots][128] float2 written by the peer CTA
   static constexpr int kXbarOffset = kXchgOffset + 2048;        // pair mode: 2 mbarriers
   static constexpr int kSmemBytes = kXbarOffset + 64 + 1024;    // + alignment slack
+  // the register epilogue (plain, 16-bit outputs only): no image and no LayerNorm exchange, but two staging buffers (a hi and
+  // a lo box each) per consumer warp behind the ring, so that the producer may refill the ring while they are in use
+  static constexpr int kRegBoxOffset = (Ring::kBytes + GEMM_RING_BAR_BYTES + 1023) / 1024 * 1024;
+  static constexpr int kRegSmemBytes = kRegBoxOffset + GEMM_EPI_WARPS * 4 * REG_BOX_BYTES + 1024;
+  static_assert(kRegSmemBytes <= 232448, "register-epilogue staging must fit shared memory");
 };
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
@@ -185,9 +191,7 @@ struct PairCtx {
 // pair's order of operations, so the row's output is bit-identical whichever schedule runs its tile (see the LayerNorm part)
 template <bool kLN, bool kPairOrder>
 __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow, int b, int t0, int n0, int row, int half,
-                                              int quarter, float* red /* [2][2][128] */,
-                                              const PairCtx& px, uint8_t* stage_out, const CUtensorMap* tmOh, const CUtensorMap* tmOl,
-                                              uint32_t& slab_ctr) {
+                                              int quarter, float* red /* [2][2][128] */, const PairCtx& px) {
   const int t = t0 + row;
   const bool row_ok = t < p.T;
   const bool row_keep = row_ok && (p.row_len == nullptr || t < __ldg(p.row_len + b));
@@ -201,47 +205,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
   float y[16], aux[16];
 
   if constexpr (!kLN) {
-    if (p.staged) {
-      // 16-bit outputs as TMA tile stores (staged_slab_begin / _end); rows >= T and columns >= N are clipped by the tensor map
-      const bool issuer = half == 0 && (threadIdx.x & 31) == 0;
-      const int lrow = row & 31;
-      const bool two = p.out_lo != nullptr && !p.h16;
-      uint8_t* box_lo = staged_slab_lo_box(stage_out, quarter);
-      uint32_t qa[16], qb[16];
-      for (int s0 = 0; s0 < nch; s0 += 4) {   // 64-column slab: this warp handles chunks s0 + 2*half, +1
-        const int ca = s0 + 2 * half, cb = ca + 1;
-        __syncwarp();
-        acc_ld16(arow + (ca << 4), qa);
-        acc_ld16(arow + (cb << 4), qb);
-        uint8_t* box_hi = staged_slab_begin(stage_out, quarter, issuer, two, slab_ctr);
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const int c0 = (u ? cb : ca) << 4;
-#pragma unroll
-          for (int j = 0; j < 16; ++j) y[j] = __uint_as_float(u ? qb[j] : qa[j]);
-          bias_relu_dropout16(p, orow, n0, c0, aux, y);
-          zero_outside16(y, partial, c0, ncols, row_keep);
-          uint32_t h[8], l[8];
-          if (p.h16) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const __half2 hh = __floats2half2_rn(y[2 * j], y[2 * j + 1]);
-              h[j] = *reinterpret_cast<const uint32_t*>(&hh);
-            }
-          } else {
-            pack_hi_lo(y, h, l, two);
-          }
-          st_box_chunk(box_hi, lrow, 2 * (2 * half + u), h);
-          if (two) st_box_chunk(box_lo, lrow, 2 * (2 * half + u), l);
-        }
-        staged_slab_end(quarter, issuer, [&] {
-          tma_store_3d(tmOh, box_hi, n0 + (s0 << 4), t0 + quarter * 32, b);
-          if (two) tma_store_3d(tmOl, box_lo, n0 + (s0 << 4), t0 + quarter * 32, b);
-        });
-      }
-      return;
-    }
-    // direct stores (fp32 outputs, residual adds, odd tile widths)
+    // direct stores (fp32 outputs, residual adds, odd tile widths); 16-bit outputs alone take epilogue_regs
     constexpr int IN_FLIGHT = 2;
     uint32_t q[IN_FLIGHT][16];
     for (int g0 = ch_begin; g0 < ch_end; g0 += IN_FLIGHT) {
@@ -462,11 +426,124 @@ __device__ __forceinline__ void epilogue_tile(const GemmKParams& p, float* arow,
 }
 
 // ----------------------------------------------------------------------------------------------------
+// Register epilogue: the plain epilogue with 16-bit outputs only, run on the accumulators of the finished tile, with no
+// image.  Consumer warp w holds rows [16w, +16) of the tile (the wgmma fragment, wgmma_sm90.cuh: rows lane/4 and lane/4 + 8,
+// column pairs 8i + 2 * (lane & 3)).  Each element pair takes the steps and the operations of bias_relu_dropout16 ->
+// zero_outside16 -> pack_hi_lo / __floats2half2_rn, with the same dropout pair index, so the bits are those of the
+// image epilogue.  A 32-column half slab leaves as one [16 rows x 32 cols] TMA tile store per plane from one of the warp's
+// two staging buffers, which alternate, so a buffer is only waited for when the store two half slabs back still reads
+// it; rows >= T are clipped by the tensor map.  The buffers lie outside the ring: the producer fills the ring with the next
+// tile meanwhile.  Half slabs rather than 64-column slabs keep the packed values of a store within the registers the
+// accumulators leave (ptxas gives a 384-thread CTA 168 per thread; 128 hold the accumulators).
+// ----------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+
+template <int NCH>
+__device__ __forceinline__ void epilogue_regs(const GemmKParams& p, const float (&acc)[NCH * 32], int b, int t0, int n0, int warp,
+                                              uint8_t* bufs, const CUtensorMap* tmOh, const CUtensorMap* tmOl, uint32_t& half_ctr) {
+  const int lane = threadIdx.x & 31;
+  const bool two = p.out_lo != nullptr && !p.h16;
+  const int ncols = min(p.block_n, p.N - n0);  // logical columns in this tile
+  const bool partial = ncols < p.block_n;
+  const int row0 = t0 + REG_BOX_ROWS * warp;
+  uint64_t elem0[2];  // dropout element index of the tile's column 0 in the fragment's two rows
+  bool row_keep[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int t = row0 + (lane >> 2) + 8 * hh;
+    const bool row_ok = t < p.T;
+    row_keep[hh] = row_ok && (p.row_len == nullptr || t < __ldg(p.row_len + b));
+    elem0[hh] = ((size_t)b * p.T + (row_ok ? t : 0)) * (uint64_t)p.ld_out + n0;
+  }
+  const uint32_t t16 = dropout_thresh(p.drop_pre_p) >> 16;
+  const float ks = 1.f / (1.f - p.drop_pre_p);
+  // lane l writes the 4 bytes of its column pair in rows l/4 and l/4 + 8 of a 64B-swizzled box (64-byte rows, 16-byte chunk
+  // index ^= (row >> 1) & 3): the eight rows of one store fill the 32 banks once
+  const uint32_t st_row = (uint32_t)((lane >> 2) * 64 + 4 * (lane & 3));
+  const uint32_t sw = (uint32_t)((lane >> 3) & 3);
+
+#pragma unroll
+  for (int s = 0; s < 2 * NCH; ++s) {
+    uint32_t h[8], l[8];  // [2 * chunk + row half] of the half slab's four 8-column chunks
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int col = 32 * s + 8 * i + 2 * (lane & 3);
+      float2 bias = make_float2(0.f, 0.f);
+      if (p.bias) bias = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + col));
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        float y0 = acc[16 * s + 4 * i + 2 * hh], y1 = acc[16 * s + 4 * i + 2 * hh + 1];
+        if (p.bias) {
+          y0 += bias.x;
+          y1 += bias.y;
+        }
+        if (p.relu) {
+          y0 = fmaxf(y0, 0.f);
+          y1 = fmaxf(y1, 0.f);
+        }
+        if (p.drop_pre_p > 0.f) {
+          const uint32_t hs = dropout_hash(p.drop_seed, p.drop_pre_site, (elem0[hh] + col) >> 1);
+          y0 = (hs & 0xffffu) >= t16 ? y0 * ks : 0.f;
+          y1 = (hs >> 16) >= t16 ? y1 * ks : 0.f;
+        }
+        if (partial) {
+          y0 = col < ncols ? y0 : 0.f;
+          y1 = col + 1 < ncols ? y1 : 0.f;
+        }
+        if (!row_keep[hh]) {
+          y0 = 0.f;
+          y1 = 0.f;
+        }
+        if (p.h16) {
+          const __half2 v = __floats2half2_rn(y0, y1);
+          h[2 * i + hh] = *reinterpret_cast<const uint32_t*>(&v);
+        } else {
+          const __nv_bfloat162 v = __floats2bfloat162_rn(y0, y1);
+          const uint32_t hv = *reinterpret_cast<const uint32_t*>(&v);
+          h[2 * i + hh] = hv;
+          if (two) {
+            const __nv_bfloat162 w = __floats2bfloat162_rn(y0 - __uint_as_float(hv << 16), y1 - __uint_as_float(hv & 0xffff0000u));
+            l[2 * i + hh] = *reinterpret_cast<const uint32_t*>(&w);
+          }
+        }
+      }
+    }
+    // the values are ready: only now wait until the store issued from this buffer two half slabs back has read it
+    uint8_t* box_hi = bufs + (half_ctr & 1u) * 2 * REG_BOX_BYTES;
+    uint8_t* box_lo = box_hi + REG_BOX_BYTES;
+    ++half_ctr;
+    if (lane == 0) tma_store_wait_read_but_one();
+    __syncwarp();
+    const uint32_t a_hi = smem_u32(box_hi) + st_row, a_lo = smem_u32(box_lo) + st_row;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      // rows l/4 and l/4 + 8 have the same (row >> 1) & 3
+      const uint32_t o = (((uint32_t)i ^ sw) << 4);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        st_shared_b32(a_hi + o + hh * 8 * 64, h[2 * i + hh]);
+        if (two) st_shared_b32(a_lo + o + hh * 8 * 64, l[2 * i + hh]);
+      }
+    }
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+      tma_store_3d(tmOh, box_hi, n0 + 32 * s, row0, b);
+      if (two) tma_store_3d(tmOl, box_lo, n0 + 32 * s, row0, b);
+      tma_store_commit();
+    }
+  }
+}
+
+// ----------------------------------------------------------------------------------------------------
 // kernel
 // ----------------------------------------------------------------------------------------------------
 // kNch: the tile width block_n in n64 blocks, rounded up (the wgmma width; the columns past block_n are computed and ignored).
-// kPairOrder: see epilogue_tile
-template <bool kSplit, bool kPair, bool kLN, int kNch, bool kPairOrder = false>
+// kPairOrder: see epilogue_tile.  kRegEpi: the plain epilogue with 16-bit outputs only, from the accumulators
+// (epilogue_regs, block_n = 64 * kNch); the tile is not parked and the producer does not wait for the epilogue.
+template <bool kSplit, bool kPair, bool kLN, int kNch, bool kPairOrder = false, bool kRegEpi = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant__ CUtensorMap tmA0l,
                const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUtensorMap tmA1l,
@@ -474,6 +551,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
                const __grid_constant__ CUtensorMap tmOh, const __grid_constant__ CUtensorMap tmOl, const GemmKParams p) {
   using Cfg = GemmCfg<kSplit, kPair>;
   static_assert(kNch >= 1 && kNch * 64 <= Cfg::kMaxBn, "tile width");
+  static_assert(!kRegEpi || (!kLN && !kPair), "the register epilogue is the plain single-CTA one");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);
   typename Cfg::Ring ring(smem);
@@ -510,7 +588,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
       const int b = m_tile / p.tiles_per_row;
       const int t0 = (m_tile % p.tiles_per_row) * GEMM_BM;
       const int n0 = n_tile * p.block_n;
-      ring.wait_image_free();
+      if constexpr (!kRegEpi) ring.wait_image_free();
       int kglob = 0;
       for (int s = 0; s < p.num_seg; ++s) {
         const CUtensorMap* mh = p.seg_src[s] == 0 ? &tmA0h : &tmA1h;
@@ -532,7 +610,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
     float* img = reinterpret_cast<float*>(smem);
     int iter = 0;
     float2* xslots = reinterpret_cast<float2*>(smem + Cfg::kXchgOffset);
-    uint32_t slab_ctr = 0;  // staged epilogue: slabs stored so far (selects the staging box of single-plane outputs)
+    uint8_t* reg_bufs = smem + Cfg::kRegBoxOffset + warp * 4 * REG_BOX_BYTES;
+    uint32_t half_ctr = 0;  // register epilogue: half slabs stored so far (selects the staging buffer)
     int total_kb = 0;
     for (int s = 0; s < p.num_seg; ++s) total_kb += p.seg_kblocks[s];
     for (int tile = p.tile_begin + work_id; tile < p.num_tiles; tile += work_stride, ++iter) {
@@ -540,23 +619,28 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0h, const __grid_constant_
       const int m_tile = kPair ? tile : tile / p.n_tiles;
       const int b = m_tile / p.tiles_per_row;
       const int t0 = (m_tile % p.tiles_per_row) * GEMM_BM;
-      Cfg::Stage::template mma_park_tile<kNch>(ring, total_kb, img, Cfg::kPitch, wg);
-      PairCtx px{};
-      if (kPair) {
-        const int slot = iter & 1;
-        px.active = 1;
-        px.my_slot = xslots + slot * GEMM_BM;
-        px.my_bar = xbar + slot;
-        px.peer_slot = map_to_peer(smem_u32(px.my_slot), (uint32_t)(cta_rank ^ 1));
-        px.peer_bar = map_to_peer(smem_u32(px.my_bar), (uint32_t)(cta_rank ^ 1));
-        px.parity = (uint32_t)((iter >> 1) & 1);
+      if constexpr (kRegEpi) {
+        float acc[kNch * 32];
+        ring.mma_tile(total_kb, acc, [&](uint32_t st, int kb) { Cfg::Stage::template mma<kNch>(acc, st, wg, kb); });
+        epilogue_regs<kNch>(p, acc, b, t0, n_tile * p.block_n, warp, reg_bufs, &tmOh, &tmOl, half_ctr);
+      } else {
+        Cfg::Stage::template mma_park_tile<kNch>(ring, total_kb, img, Cfg::kPitch, wg);
+        PairCtx px{};
+        if (kPair) {
+          const int slot = iter & 1;
+          px.active = 1;
+          px.my_slot = xslots + slot * GEMM_BM;
+          px.my_bar = xbar + slot;
+          px.peer_slot = map_to_peer(smem_u32(px.my_slot), (uint32_t)(cta_rank ^ 1));
+          px.peer_bar = map_to_peer(smem_u32(px.my_bar), (uint32_t)(cta_rank ^ 1));
+          px.parity = (uint32_t)((iter >> 1) & 1);
+        }
+        const int row = quarter * 32 + lane;
+        epilogue_tile<kLN, kPairOrder>(p, img + (size_t)row * Cfg::kPitch, b, t0, n_tile * p.block_n, row, half, quarter, red_all, px);
+        ring.release_tile(false);
       }
-      const int row = quarter * 32 + lane;
-      epilogue_tile<kLN, kPairOrder>(p, img + (size_t)row * Cfg::kPitch, b, t0, n_tile * p.block_n, row, half, quarter, red_all, px,
-                         smem + Cfg::kStageOutOffset, &tmOh, &tmOl, slab_ctr);
-      ring.release_tile(!kLN && p.staged && half == 0 && lane == 0);
     }
-    Cfg::Ring::finish(!kLN && p.staged && half == 0 && lane == 0);
+    Cfg::Ring::finish(kRegEpi && lane == 0);
   }
 done:
   __syncthreads();
@@ -651,15 +735,16 @@ __global__ void gemm_simt_kernel(const GemmKParams p, const GemmSimtPtrs q) {
 // host
 // ----------------------------------------------------------------------------------------------------
 // launches the instantiation whose wgmma width kNch * 64 is q.block_n rounded up to a multiple of 64
-template <bool kSplit, bool kPair, bool kLN, bool kPairOrder = false, int kNch = 1>
+template <bool kSplit, bool kPair, bool kLN, bool kPairOrder = false, bool kRegEpi = false, int kNch = 1>
 static int launch_tc(const CUtensorMap (&tmA)[2][2], const CUtensorMap (&tmW)[2], const CUtensorMap (&tmO)[2], const GemmKParams& q,
                      int work, cudaStream_t stream) {
-  if constexpr (kNch * 64 < GemmCfg<kSplit, kPair>::kMaxBn) {
-    if (q.block_n > kNch * 64) return launch_tc<kSplit, kPair, kLN, kPairOrder, kNch + 1>(tmA, tmW, tmO, q, work, stream);
+  using Cfg = GemmCfg<kSplit, kPair>;
+  if constexpr (kNch * 64 < Cfg::kMaxBn) {
+    if (q.block_n > kNch * 64) return launch_tc<kSplit, kPair, kLN, kPairOrder, kRegEpi, kNch + 1>(tmA, tmW, tmO, q, work, stream);
   }
-  return launch_pipeline<gemm_tc_kernel<kSplit, kPair, kLN, kNch, kPairOrder>>(GemmCfg<kSplit, kPair>::kSmemBytes, work, kPair, stream,
-                                                                   kPair ? "gemm_tc_kernel<pair> launch" : "gemm_tc_kernel launch", tmA[0][0], tmA[0][1],
-                                                                   tmA[1][0], tmA[1][1], tmW[0], tmW[1], tmO[0], tmO[1], q);
+  return launch_pipeline<gemm_tc_kernel<kSplit, kPair, kLN, kNch, kPairOrder, kRegEpi>>(
+      kRegEpi ? Cfg::kRegSmemBytes : Cfg::kSmemBytes, work, kPair, stream, kPair ? "gemm_tc_kernel<pair> launch" : "gemm_tc_kernel launch",
+      tmA[0][0], tmA[0][1], tmA[1][0], tmA[1][1], tmW[0], tmW[1], tmO[0], tmO[1], q);
 }
 
 static int validate(const ttsb_gemm_args* a, int* k_total_out) {
@@ -812,21 +897,20 @@ extern "C" int ttsb_linear_fwd(const ttsb_gemm_args* a, void* stream_v) {
       int rc2 = make_tmap_bf16_2d(&tmW[h], base, k_total, as_pair ? a->N : q.n_tiles * q.block_n, (uint64_t)k_total, GEMM_BK, q.block_n);
       if (rc2) return rc2;
     }
-    // plain epilogue with 16-bit outputs only: tile stores through shared memory
-    CUtensorMap tmO[2] = {tmW[0], tmW[1]};  // placeholders when the staged path is off
-    q.staged = 0;
-    if (!as_pair && q.gamma == nullptr && q.out_hi != nullptr && q.out_f32 == nullptr && q.out_preln == nullptr &&
-        q.residual == nullptr && q.block_n % 64 == 0 && q.ld_out % 8 == 0) {
+    // plain epilogue with 16-bit outputs only: from the accumulators, as tile stores of [16 rows x 32 cols] boxes
+    CUtensorMap tmO[2] = {tmW[0], tmW[1]};  // placeholders when the register epilogue is off
+    const bool reg_epi = !as_pair && q.gamma == nullptr && q.out_hi != nullptr && q.out_f32 == nullptr && q.out_preln == nullptr &&
+                         q.residual == nullptr && q.block_n % 64 == 0 && q.ld_out % 8 == 0;
+    if (reg_epi) {
       const int width = q.n_tiles * q.block_n;
-      int rc3 = make_tmap_bf16_3d(&tmO[0], q.out_hi, (uint64_t)width, (uint64_t)a->T, (uint64_t)a->B, (uint64_t)q.ld_out,
-                                  (uint64_t)q.ld_out * a->T, 64, 32);
+      int rc3 = make_tmap_bf16_3d_sw64(&tmO[0], q.out_hi, (uint64_t)width, (uint64_t)a->T, (uint64_t)a->B, (uint64_t)q.ld_out,
+                                       (uint64_t)q.ld_out * a->T, REG_BOX_COLS, REG_BOX_ROWS);
       if (rc3) return rc3;
       if (q.out_lo) {
-        rc3 = make_tmap_bf16_3d(&tmO[1], q.out_lo, (uint64_t)width, (uint64_t)a->T, (uint64_t)a->B, (uint64_t)q.ld_out,
-                                (uint64_t)q.ld_out * a->T, 64, 32);
+        rc3 = make_tmap_bf16_3d_sw64(&tmO[1], q.out_lo, (uint64_t)width, (uint64_t)a->T, (uint64_t)a->B, (uint64_t)q.ld_out,
+                                     (uint64_t)q.ld_out * a->T, REG_BOX_COLS, REG_BOX_ROWS);
         if (rc3) return rc3;
       }
-      q.staged = 1;
     }
     // pair mode: a cluster of two CTAs per 128-row tile.  Separate instantiations for the LayerNorm and the plain epilogue:
     // each gets its own register allocation
@@ -835,6 +919,9 @@ extern "C" int ttsb_linear_fwd(const ttsb_gemm_args* a, void* stream_v) {
       return split ? launch_tc<true, false, true, true>(tmA, tmW, tmO, q, work, stream) : launch_tc<false, false, true, true>(tmA, tmW, tmO, q, work, stream);
     if (q.gamma != nullptr)
       return split ? launch_tc<true, false, true>(tmA, tmW, tmO, q, work, stream) : launch_tc<false, false, true>(tmA, tmW, tmO, q, work, stream);
+    if (reg_epi)
+      return split ? launch_tc<true, false, false, false, true>(tmA, tmW, tmO, q, work, stream)
+                   : launch_tc<false, false, false, false, true>(tmA, tmW, tmO, q, work, stream);
     return split ? launch_tc<true, false, false>(tmA, tmW, tmO, q, work, stream) : launch_tc<false, false, false>(tmA, tmW, tmO, q, work, stream);
   };
   if (pair && hybrid_full > 0) {
