@@ -66,7 +66,7 @@ def main(argv=None):
     from transformertts_b200.utils.training_config_manager import TrainingConfigManager
 
     cm = TrainingConfigManager(args.config)
-    ev.check_normalizer(cm.config, 'config')
+    ev.natural_log_mels(cm.config, 'config')
     vs = ev.load_validation_set(cm)
     root = Path(args.path)
     results = []
@@ -75,7 +75,7 @@ def main(argv=None):
         model = ForwardTransformer.load_model(ckpt)
         with open(ckpt / 'config.yaml') as f:
             step = yaml.safe_load(f).get('step', model.step)
-        ev.check_normalizer(model.config)
+        ev.natural_log_mels(model.config)
         audio = vocode = None
         if args.vocoder is not None:
             audio = Audio.from_config(model.config)

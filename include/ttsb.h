@@ -567,6 +567,49 @@ int ttsb_griffinlim_batch(const float* magnitude, const float* init_angles, cons
                           float* wav_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * The STFT family at any supported configuration  (Audio at settings other than n_fft 1024 / hop 256 / win 1024, e.g. the
+ * reference's config/data_config_wavernn.yaml: n_fft 2048, hop 275, win 1100)
+ *   n_fft a power of two in [256, 4096], 1 <= hop_length <= win_length <= n_fft, win_length >= 2 (a periodic Hann of one sample
+ *   would be 0, where librosa's window is [1]); window = periodic Hann(win_length) centred in
+ *   n_fft (librosa's pad_center), centred frames with reflect padding; n_bins = n_fft / 2 + 1.  A clip of L samples has
+ *   1 + L / hop frames and needs L > n_fft / 2.  Offset tables are int32 (n_clips + 1) in HOST memory, from 0; the entry points
+ *   check them and the configuration and give TTSB_ERR_INVALID_ARGUMENT before any CUDA call, then copy the twiddles, the
+ *   window (both computed in float64 and rounded once) and a clip table into `workspace` (device memory, 256-byte aligned, of
+ *   the size the matching _workspace_bytes query returns; -1 there for invalid arguments).  Frame pairs never span two clips,
+ *   reflect padding happens at each clip's own edges and the overlap-add stays inside a clip, so a clip's output is
+ *   bit-identical wherever it sits in the batch.
+ * ------------------------------------------------------------------------------------------------------- */
+/* log-mel of a packed ragged batch, as ttsb_stft_mel_log_batch: mel_basis fp32 (n_mels, n_bins) dense, band int32 (n_mels, 2) on
+ *   the device (as ttsb_mel_to_linear's: band[2m], band[2m+1] = first / past-last non-zero bin of row m; bounds outside [0, n_bins]
+ *   are clamped), out fp32 (frame_offsets[n_clips], n_mels), frame_offsets[c+1] - frame_offsets[c] = 1 + L_c / hop_length. */
+int64_t ttsb_stft_mel_log_ragged_workspace_bytes(int n_clips, int n_fft);
+int ttsb_stft_mel_log_ragged(const float* wav, const int32_t* sample_offsets, const int32_t* frame_offsets, int n_clips, int n_fft,
+                             int hop_length, int win_length, const float* mel_basis, const int32_t* band, int n_mels, int normalizer,
+                             void* workspace, int64_t workspace_bytes, float* out, void* stream);
+/* ttsb_mel_to_linear at n_bins = n_fft / 2 + 1 in [129, 2049] bins: mel_basis (n_mels, n_bins), basis_pinv (n_bins, n_mels),
+ *   bin_mels (n_bins, 2), out (n_frames, n_bins). */
+int ttsb_mel_to_linear_ex(const float* mel_amp, int n_frames, int n_mels, int n_bins, const float* mel_basis, const float* basis_pinv,
+                          const int32_t* band, const int32_t* bin_mels, float step, int n_iter, float* out, void* stream);
+/* librosa.stft of every clip of a packed batch: wav (sample_offsets[n_clips]) -> complex64 (sum of 1 + L_c / hop, n_bins) as
+ *   interleaved (re, im) floats, clip c's frames after those of clips 0 .. c-1. */
+int64_t ttsb_stft_complex_ragged_workspace_bytes(int n_clips, int n_fft);
+int ttsb_stft_complex_ragged(const float* wav, const int32_t* sample_offsets, int n_clips, int n_fft, int hop_length, int win_length,
+                             void* workspace, int64_t workspace_bytes, float* spec_out, void* stream);
+/* librosa.istft of every clip of a packed batch: complex64 (total_frames, n_bins), clip c in frames frame_offsets[c] ..
+ *   frame_offsets[c+1] - 1 (>= 2 frames) -> wav_out fp32 (hop (total_frames - n_clips)), clip c's hop (T_c - 1) samples from
+ *   sample hop (frame_offsets[c] - c).  Window-sum-square normalisation and centre trim per clip. */
+int64_t ttsb_istft_ragged_workspace_bytes(int total_frames, int n_clips, int n_fft);
+int ttsb_istft_ragged(const float* spec, const int32_t* frame_offsets, int n_clips, int n_fft, int hop_length, int win_length,
+                      void* workspace, int64_t workspace_bytes, float* wav_out, void* stream);
+/* ttsb_griffinlim_batch at this configuration (1 + 3 n_iter + 2 launches): magnitude fp32 and init_angles complex64
+ *   (total_frames, n_bins), wav_out as ttsb_istft_ragged.  Every clip needs T_c >= n_fft / 2 / hop + 2 frames, so that its
+ *   hop (T_c - 1) samples are more than n_fft / 2 (4 at 1024 / 256, 5 at 2048 / 275); n_iter >= 0, momentum finite and >= 0. */
+int64_t ttsb_griffinlim_ragged_workspace_bytes(int total_frames, int n_clips, int n_fft);
+int ttsb_griffinlim_ragged(const float* magnitude, const float* init_angles, const int32_t* frame_offsets, int n_clips, int n_fft,
+                           int hop_length, int win_length, int n_iter, float momentum, void* workspace, int64_t workspace_bytes,
+                           float* wav_out, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Mel-cepstral distortion after dynamic time warping  (evaluate_tts.py; no reference counterpart;
  * tests/evaluation_oracle.py restates the definition in float64)
  *   A packed ragged batch of n_pairs pairs of fp32 log-mel sequences (frames, n_mels) on the device: pair p compares frames

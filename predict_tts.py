@@ -113,7 +113,15 @@ def load_model(args):
 
 def load_vocoder(name: str, checkpoint, config, model):
     """The generator --vocoder names (weights from checkpoint, HiFi-GAN's config from config) on the model's device, or None
-    for Griffin-Lim, which Audio.reconstruct_waveform_batch runs."""
+    for Griffin-Lim, which Audio.reconstruct_waveform_batch runs.  A generator is refused when the samples it makes per mel frame
+    differ from the model's hop_length: its audio would have the wrong length and pitch."""
+    if name in ('melgan', 'hifigan'):
+        from transformertts_b200.model import hifigan, melgan
+        upsampling = (melgan if name == 'melgan' else hifigan).HOP
+        hop = int(model.config['hop_length'])
+        if upsampling != hop:
+            raise SystemExit(f'--vocoder {name}: the generator upsamples each mel frame to {upsampling} samples, but the audio '
+                             f'settings have hop_length {hop}; use --vocoder griffinlim at this hop')
     if name == 'melgan':
         from transformertts_b200.model.melgan import MelGANGenerator
         return MelGANGenerator.from_checkpoint(checkpoint, device=model.device)
@@ -153,8 +161,9 @@ def main(argv=None):
         mels = []
         for i in range(start, min(start + VOCODE_CHUNK, len(text))):
             mel = outs[i]['mel'].cpu().numpy()                  # (T, n_mels)
-            if mel.shape[0] < 4:
-                raise ValueError(f'line {i} gives a mel of shape {mel.shape}; the vocoder needs at least 4 frames')
+            if mel.shape[0] < audio.min_griffinlim_frames:
+                raise ValueError(f'line {i} gives a mel of shape {mel.shape}; the vocoder needs at least {audio.min_griffinlim_frames} '
+                                 f'frames')
             mels.append(mel)
             if args.store_mel:
                 np.save(line_paths(outdir, file_name, i)[1], mel)

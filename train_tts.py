@@ -157,7 +157,7 @@ def main():
     eval_set = None
     if args.evaluate and rank == 0:
         from transformertts_b200.utils import evaluation as ev
-        ev.check_normalizer(cfg, 'config')
+        ev.natural_log_mels(cfg, 'config')
         eval_set = ev.load_validation_set(cm)
     max_steps = args.max_steps or int(cfg['max_steps'])
     save_freq, save_start = int(cfg.get('weights_save_frequency', 5000)), int(cfg.get('weights_save_starting_step', 0))

@@ -32,7 +32,10 @@ def _mel_to_hz_slaney(m):
 
 def slaney_mel_basis(sr: int, n_fft: int, n_mels: int, fmin: float, fmax: float) -> np.ndarray:
     """Area-normalised triangular Slaney filterbank (what librosa.filters.mel(htk=False, norm=1) returns, which the
-    reference reaches through librosa.feature.melspectrogram at data/audio.py:73-79) -> float32 (n_mels, 1+n_fft/2)."""
+    reference reaches through librosa.feature.melspectrogram at data/audio.py:73-79) -> float32 (n_mels, 1+n_fft/2).
+    fmax None means sr / 2, as librosa's fmax=None."""
+    if fmax is None:
+        fmax = sr / 2.0
     n_bins = 1 + n_fft // 2
     bin_hz = np.arange(n_bins, dtype=np.float64) * (sr / 2.0) / (n_bins - 1)
     edges = _mel_to_hz_slaney(np.linspace(_hz_to_mel_slaney(fmin), _hz_to_mel_slaney(fmax), n_mels + 2))
@@ -76,17 +79,48 @@ def _random_phase(shape, seed):
     return torch.polar(torch.ones_like(ph), ph).to(torch.complex64)
 
 
-def _clip_frame_counts(frame_offsets, total_frames: int) -> np.ndarray:
+def _clip_frame_counts(frame_offsets, total_frames: int, min_frames: int = 4) -> np.ndarray:
     """Host check of a packed batch's frame offsets (n_clips + 1, from 0 to total_frames) -> frames per clip.  Griffin-Lim needs
-    at least 4 frames per clip: the STFT of a shorter clip's 256 (T - 1) samples has no room for the 512-sample reflect padding."""
+    at least min_frames (Audio.min_griffinlim_frames: 4 at the reference configuration) frames per clip: the STFT of a shorter
+    clip's hop (T - 1) samples has no room for the n_fft / 2 samples of reflect padding."""
     off = np.asarray(frame_offsets.cpu() if torch.is_tensor(frame_offsets) else frame_offsets, dtype=np.int64)
     if off.ndim != 1 or len(off) < 2 or off[0] != 0 or off[-1] != total_frames:
         raise ValueError(f'frame offsets must run from 0 to {total_frames} over n_clips + 1 entries, got {off.tolist()}')
     counts = np.diff(off)
     for c, t in enumerate(counts):
-        if t < 4:
-            raise ValueError(f'clip {c} has {t} frames; Griffin-Lim needs at least 4 frames per clip')
+        if t < min_frames:
+            raise ValueError(f'clip {c} has {t} frames; Griffin-Lim needs at least {min_frames} frames per clip')
     return counts
+
+
+# the configuration the fused kernels of stft_mel.cu and griffin_lim.cu implement; every other supported one runs through the
+# general entry points of stft_general.cu
+REFERENCE_STFT = (1024, 256, 1024)
+MAX_MEL_CHANNELS = 128
+
+
+def check_audio_settings(sampling_rate, n_fft, mel_channels, hop_length, win_length, f_min, f_max) -> float:
+    """Refuse audio settings outside the supported set, naming the setting and its allowed range -> f_max in Hz (None: sr / 2)."""
+    def whole(v):
+        return isinstance(v, (int, np.integer)) and not isinstance(v, bool)
+    if not whole(sampling_rate) or sampling_rate <= 0:
+        raise ValueError(f'sampling_rate must be a positive integer, got {sampling_rate!r}')
+    if not whole(n_fft) or not 256 <= n_fft <= 4096 or n_fft & (n_fft - 1):
+        raise ValueError(f'n_fft must be a power of two in [256, 4096], got {n_fft!r}')
+    # a periodic Hann of one sample is 0.5 - 0.5 cos 0 = 0 (scipy's get_window, which librosa calls, returns [1.0] instead): a
+    # window of one sample is refused rather than computed differently from the reference
+    if not whole(win_length) or not 2 <= win_length <= n_fft:
+        raise ValueError(f'win_length must be an integer in [2, n_fft = {n_fft}], got {win_length!r}')
+    if not whole(hop_length) or not 1 <= hop_length <= win_length:
+        raise ValueError(f'hop_length must be an integer in [1, win_length = {win_length}], got {hop_length!r}')
+    if not whole(mel_channels) or not 1 <= mel_channels <= MAX_MEL_CHANNELS:
+        raise ValueError(f'mel_channels must be an integer in [1, {MAX_MEL_CHANNELS}], got {mel_channels!r}')
+    nyquist = sampling_rate / 2.0
+    fmax = nyquist if f_max is None else f_max
+    if not 0 <= f_min < fmax <= nyquist:
+        raise ValueError(f'need 0 <= f_min < f_max <= sampling_rate / 2 = {nyquist:g} Hz (f_max None means sampling_rate / 2), got '
+                         f'f_min {f_min!r}, f_max {f_max!r}')
+    return fmax
 
 
 class Normalizer:
@@ -115,8 +149,8 @@ class Audio:
                  f_max: int, normalizer: str, device: str = 'cuda:0', **kwargs):
         self.config = dict(sampling_rate=sampling_rate, n_fft=n_fft, mel_channels=mel_channels, hop_length=hop_length,
                            win_length=win_length, f_min=f_min, f_max=f_max, normalizer=normalizer, **kwargs)
-        if (n_fft, hop_length, win_length) != (1024, 256, 1024):
-            raise lib.TtsbError('the fused STFT kernel implements the reference configuration n_fft=1024, hop=256, win=1024')
+        f_max = check_audio_settings(sampling_rate, n_fft, mel_channels, hop_length, win_length, f_min, f_max)
+        self._reference_stft = (n_fft, hop_length, win_length) == REFERENCE_STFT
         self.sampling_rate, self.n_fft, self.mel_channels = sampling_rate, n_fft, mel_channels
         self.hop_length, self.win_length, self.f_min, self.f_max = hop_length, win_length, f_min, f_max
         self.normalizer = {'MelGAN': MelGAN, 'WaveRNN': WaveRNN}[normalizer]()
@@ -129,6 +163,16 @@ class Audio:
     @classmethod
     def from_config(cls, config: dict):
         return cls(**config)
+
+    @property
+    def min_mel_samples(self) -> int:
+        """Shortest clip the log-mel front end takes: reflect padding needs more than n_fft / 2 samples."""
+        return self.n_fft // 2 + 1
+
+    @property
+    def min_griffinlim_frames(self) -> int:
+        """Fewest frames per clip Griffin-Lim takes: its hop (T - 1) samples must be more than n_fft / 2 (4 at 1024 / 256)."""
+        return self.n_fft // 2 // self.hop_length + 2
 
     def _mel_basis(self) -> torch.Tensor:
         if self._basis is None:
@@ -144,7 +188,13 @@ class Audio:
         """wav fp32 CUDA (n_clips, n_samples) -> fp32 CUDA (n_clips, 1 + n_samples//hop, n_mels)."""
         n_clips, n_samples = wav.shape
         out = torch.empty((n_clips, 1 + n_samples // self.hop_length, self.mel_channels), dtype=torch.float32, device=wav.device)
-        lib.stft_mel_log(wav.contiguous(), self._mel_basis(), self.normalizer.code, out)
+        if self._reference_stft:
+            lib.stft_mel_log(wav.contiguous(), self._mel_basis(), self.normalizer.code, out)
+        else:
+            so = np.arange(n_clips + 1, dtype=np.int64) * n_samples
+            fo = np.arange(n_clips + 1, dtype=np.int64) * out.shape[1]
+            lib.stft_mel_log_ragged(wav.contiguous().reshape(-1), so, fo, self.n_fft, self.hop_length, self.win_length, self._mel_basis(),
+                                    self._inverse_tables()['band'], self.normalizer.code, out)
         return out
 
     # ---- mel -> waveform (data/audio.py:94-110)
@@ -169,17 +219,21 @@ class Audio:
         return self._inv
 
     def mel_to_linear_device(self, mel_amp: torch.Tensor, n_iter: int = 64) -> torch.Tensor:
-        """mel amplitudes (T, n_mels) CUDA -> linear magnitudes (T, 513) CUDA (librosa mel_to_stft(power=1), see ttsb.h)."""
+        """mel amplitudes (T, n_mels) CUDA -> linear magnitudes (T, n_fft/2 + 1) CUDA (librosa mel_to_stft(power=1), see ttsb.h)."""
         with torch.cuda.device(self.device):
             inv = self._inverse_tables()
             out = torch.empty((mel_amp.shape[0], self.n_fft // 2 + 1), dtype=torch.float32, device=self.device)
-            lib.mel_to_linear(mel_amp.contiguous(), self._mel_basis(), inv['pinv'], inv['band'], inv['bins'], inv['step'], n_iter, out)
+            to_linear = lib.mel_to_linear if self._reference_stft else lib.mel_to_linear_ex
+            to_linear(mel_amp.contiguous(), self._mel_basis(), inv['pinv'], inv['band'], inv['bins'], inv['step'], n_iter, out)
             return out
 
     def griffinlim_device(self, S: torch.Tensor, n_iter: int = 32, momentum: float = 0.99, init_angles: torch.Tensor = None,
                           seed: int = None) -> torch.Tensor:
-        """librosa.griffinlim on the GPU: S (T, 513) magnitudes -> waveform (256 (T-1)).  init_angles: unit-modulus complex64
-        (T, 513); default: exp(2 pi i u), u uniform (the reference draws it from numpy's global RNG)."""
+        """librosa.griffinlim on the GPU: S (T, n_fft/2 + 1) magnitudes -> waveform (hop (T-1)).  init_angles: unit-modulus
+        complex64 (T, n_fft/2 + 1); default: exp(2 pi i u), u uniform (the reference draws it from numpy's global RNG)."""
+        if not self._reference_stft:
+            return self.griffinlim_batch_device(S, [0, S.shape[0]], n_iter=n_iter, momentum=momentum, init_angles=init_angles,
+                                                seeds=[seed])
         with torch.cuda.device(self.device):
             dev = self.device
             T = S.shape[0]
@@ -210,14 +264,14 @@ class Audio:
     def griffinlim_batch_device(self, S: torch.Tensor, frame_offsets, n_iter: int = 32, momentum: float = 0.99,
                                 init_angles: torch.Tensor = None, seeds=None) -> torch.Tensor:
         """griffinlim_device for every clip of a packed batch in one pass (ttsb_griffinlim_batch, one launch per stage and
-        iteration whatever the number of clips).  S: magnitudes (F, 513) on the device, clip c in frames
-        frame_offsets[c] .. frame_offsets[c+1] - 1 -> packed waveform (256 (F - n_clips)); clip c starts at sample
-        256 (frame_offsets[c] - c).  init_angles: unit-modulus complex64 (F, 513); default: clip c draws its phase as
+        iteration whatever the number of clips).  S: magnitudes (F, n_fft/2 + 1) on the device, clip c in frames
+        frame_offsets[c] .. frame_offsets[c+1] - 1 -> packed waveform (hop (F - n_clips)); clip c starts at sample
+        hop (frame_offsets[c] - c).  init_angles: unit-modulus complex64 (F, n_fft/2 + 1); default: clip c draws its phase as
         griffinlim_device(S_c, seed=seeds[c]) does (seeds=None: as griffinlim_device(S_c))."""
         with torch.cuda.device(self.device):
             dev = self.device
             F = S.shape[0]
-            counts = _clip_frame_counts(frame_offsets, F)
+            counts = _clip_frame_counts(frame_offsets, F, self.min_griffinlim_frames)
             n_clips = len(counts)
             if init_angles is None:
                 if seeds is not None and len(seeds) != n_clips:
@@ -225,22 +279,27 @@ class Audio:
                 init_angles = torch.cat([_random_phase((int(t), S.shape[1]), None if seeds is None else seeds[c])
                                          for c, t in enumerate(counts)])
             init_angles = init_angles.to(device=dev, dtype=torch.complex64).contiguous()
+            wav = torch.empty(self.hop_length * (F - n_clips), dtype=torch.float32, device=dev)
+            if not self._reference_stft:
+                lib.griffinlim_ragged(S.contiguous(), init_angles, np.concatenate([[0], np.cumsum(counts)]), self.n_fft, self.hop_length,
+                                      self.win_length, n_iter, momentum, wav)
+                return wav
             off = torch.from_numpy(np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)).to(dev)
             ws = torch.empty(lib.griffinlim_batch_workspace_bytes(F, n_clips) // 4, dtype=torch.float32, device=dev)
-            wav = torch.empty(self.hop_length * (F - n_clips), dtype=torch.float32, device=dev)
             lib.griffinlim_batch(S.contiguous(), init_angles, off, n_iter, momentum, ws, wav)
             return wav
 
     def reconstruct_waveform_batch(self, mels, n_iter: int = 32, nnls_iter: int = 64, init_angles=None, seed: int = None) -> list:
         """reconstruct_waveform for a list of normalised mels (n_mels, T_c) in one pass: one mel inversion over the frames of all
-        clips, one batched Griffin-Lim -> list of float32 waveforms (256 (T_c - 1)).  With seed=s, clip c gets the phase of
-        reconstruct_waveform(mels[c], seed=s + c); init_angles: a list of (513, T_c) arrays, as reconstruct_waveform takes."""
+        clips, one batched Griffin-Lim -> list of float32 waveforms (hop (T_c - 1)).  With seed=s, clip c gets the phase of
+        reconstruct_waveform(mels[c], seed=s + c); init_angles: a list of (n_fft/2 + 1, T_c) arrays, as reconstruct_waveform takes."""
         ms = [np.asarray(m, dtype=np.float32) for m in mels]
         if not ms:
             return []
         for c, m in enumerate(ms):
-            if m.ndim != 2 or m.shape[1] < 4:
-                raise ValueError(f'mel {c} has shape {m.shape}; Griffin-Lim needs (n_mels, T) with T >= 4 frames')
+            if m.ndim != 2 or m.shape[1] < self.min_griffinlim_frames:
+                raise ValueError(f'mel {c} has shape {m.shape}; Griffin-Lim needs (n_mels, T) with T >= {self.min_griffinlim_frames} '
+                                 f'frames')
         counts = [m.shape[1] for m in ms]
         amp = np.concatenate([self._denormalize(m).T.astype(np.float32) for m in ms])       # (F, n_mels)
         S = self.mel_to_linear_device(torch.from_numpy(np.ascontiguousarray(amp)).to(self.device), nnls_iter)
@@ -294,13 +353,18 @@ class Audio:
         return torch.from_numpy(np.concatenate(ws)).to(self.device), so
 
     def mel_spectrogram_ragged_device(self, wav: torch.Tensor, sample_offsets) -> tuple:
-        """ttsb_stft_mel_log_batch: packed fp32 clips on the device -> (packed log-mels (F, n_mels) on the device, frame offsets).
-        Clip c's mel is bit-identical to mel_spectrogram_device on that clip alone."""
+        """ttsb_stft_mel_log_batch (ttsb_stft_mel_log_ragged away from the reference configuration): packed fp32 clips on the
+        device -> (packed log-mels (F, n_mels) on the device, frame offsets).  Clip c's mel is bit-identical to
+        mel_spectrogram_device on that clip alone."""
         with torch.cuda.device(self.device):
             so = np.asarray(sample_offsets, dtype=np.int64)
             fo = np.concatenate([[0], np.cumsum(self._frames_per_clip(np.diff(so)))])
             out = torch.empty((int(fo[-1]), self.mel_channels), dtype=torch.float32, device=self.device)
-            lib.stft_mel_log_batch(wav.contiguous(), so, fo, self._mel_basis(), self.normalizer.code, out)
+            if self._reference_stft:
+                lib.stft_mel_log_batch(wav.contiguous(), so, fo, self._mel_basis(), self.normalizer.code, out)
+            else:
+                lib.stft_mel_log_ragged(wav.contiguous(), so, fo, self.n_fft, self.hop_length, self.win_length, self._mel_basis(),
+                                        self._inverse_tables()['band'], self.normalizer.code, out)
             return out, fo
 
     def extract_pitch_device(self, wav: torch.Tensor, sample_offsets, workspace: torch.Tensor = None) -> tuple:

@@ -36,6 +36,9 @@ EXPORTS = [
     'ttsb_conv1d_workspace_bytes', 'ttsb_conv1d_ex_tc', 'ttsb_conv1d_out_tanh_ex',
     'ttsb_resample_batch_workspace_bytes', 'ttsb_resample_batch',
     'ttsb_mcd_dtw_workspace_bytes', 'ttsb_mcd_dtw',
+    'ttsb_stft_mel_log_ragged_workspace_bytes', 'ttsb_stft_mel_log_ragged', 'ttsb_mel_to_linear_ex',
+    'ttsb_stft_complex_ragged_workspace_bytes', 'ttsb_stft_complex_ragged', 'ttsb_istft_ragged_workspace_bytes', 'ttsb_istft_ragged',
+    'ttsb_griffinlim_ragged_workspace_bytes', 'ttsb_griffinlim_ragged',
 ]
 
 
@@ -148,6 +151,19 @@ def load() -> C.CDLL:
     lib.ttsb_mcd_dtw_workspace_bytes.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
     lib.ttsb_mcd_dtw.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_double,
                                  C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
+    for name in ('ttsb_stft_mel_log_ragged_workspace_bytes', 'ttsb_stft_complex_ragged_workspace_bytes',
+                 'ttsb_istft_ragged_workspace_bytes', 'ttsb_griffinlim_ragged_workspace_bytes'):
+        getattr(lib, name).restype = C.c_int64
+    lib.ttsb_stft_mel_log_ragged.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                             C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.ttsb_mel_to_linear_ex.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float,
+                                          C.c_int, C.c_void_p, C.c_void_p]
+    lib.ttsb_stft_complex_ragged.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p,
+                                             C.c_void_p]
+    lib.ttsb_istft_ragged.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p,
+                                      C.c_void_p]
+    lib.ttsb_griffinlim_ragged.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     for name in EXPORTS:
         if not hasattr(lib, name):
             raise TtsbError(f'libttsb.so does not export {name}')
@@ -642,6 +658,65 @@ def griffinlim_batch(magnitude, init_angles, frame_offsets, n_iter, momentum, wo
     _check(load().ttsb_griffinlim_batch(ptr(magnitude), ptr(init_angles), ptr(frame_offsets), frame_offsets.numel() - 1, F, int(n_iter),
                                         C.c_float(momentum), ptr(workspace), C.c_int64(workspace.numel() * workspace.element_size()),
                                         ptr(wav_out), _stream()), 'ttsb_griffinlim_batch')
+
+
+# ------------------------------------------------------------------------------------------------------------
+# the STFT family at any supported (n_fft, hop, win_length) (csrc/stft_general.cu); offset tables are host sequences
+# ------------------------------------------------------------------------------------------------------------
+def _workspace(nb: int, device) -> torch.Tensor:
+    if nb < 0:
+        raise TtsbError(load().ttsb_last_error().decode())
+    return torch.empty(nb, dtype=torch.uint8, device=device)
+
+
+def stft_mel_log_ragged(wav, sample_offsets, frame_offsets, n_fft, hop_length, win_length, mel_basis, band, normalizer, out):
+    """Log-mel of a packed ragged batch (include/ttsb.h: ttsb_stft_mel_log_ragged).  wav fp32 (total_samples,), mel_basis fp32
+    (n_mels, n_fft/2 + 1), its row bounds band int32 (n_mels, 2) and out fp32 (total_frames, n_mels) on the device."""
+    so, n = _host_offsets(sample_offsets)
+    fo, n_f = _host_offsets(frame_offsets)
+    if n_f != n:
+        raise TtsbError(f'{n} clips in sample_offsets, {n_f} in frame_offsets')
+    n_mels = mel_basis.shape[0]
+    if tuple(band.shape) != (n_mels, 2) or band.dtype != torch.int32:
+        raise TtsbError(f'band must be int32 ({n_mels}, 2), got {band.dtype} {tuple(band.shape)}')
+    ws = _workspace(int(load().ttsb_stft_mel_log_ragged_workspace_bytes(n, int(n_fft))), wav.device)
+    _check(load().ttsb_stft_mel_log_ragged(ptr(wav), so, fo, n, int(n_fft), int(hop_length), int(win_length), ptr(mel_basis), ptr(band), n_mels,
+                                           int(normalizer), ptr(ws), ws.numel(), ptr(out), _stream()), 'ttsb_stft_mel_log_ragged')
+
+
+def mel_to_linear_ex(mel_amp, basis, pinv, band, bin_mels, step, n_iter, out):
+    """ttsb_mel_to_linear at basis.shape[1] = n_fft/2 + 1 bins (include/ttsb.h: ttsb_mel_to_linear_ex)."""
+    T, n_mels = mel_amp.shape
+    _check(load().ttsb_mel_to_linear_ex(ptr(mel_amp), T, n_mels, basis.shape[1], ptr(basis), ptr(pinv), ptr(band), ptr(bin_mels),
+                                        float(step), int(n_iter), ptr(out), _stream()), 'ttsb_mel_to_linear_ex')
+
+
+def stft_complex_ragged(wav, sample_offsets, n_fft, hop_length, win_length, spec_out):
+    """librosa.stft of every clip of a packed batch (include/ttsb.h: ttsb_stft_complex_ragged) -> spec_out fp32
+    (total_frames, n_fft/2 + 1, 2), clip c with 1 + L_c // hop frames."""
+    so, n = _host_offsets(sample_offsets)
+    ws = _workspace(int(load().ttsb_stft_complex_ragged_workspace_bytes(n, int(n_fft))), wav.device)
+    _check(load().ttsb_stft_complex_ragged(ptr(wav), so, n, int(n_fft), int(hop_length), int(win_length), ptr(ws), ws.numel(),
+                                           ptr(spec_out), _stream()), 'ttsb_stft_complex_ragged')
+
+
+def istft_ragged(spec, frame_offsets, n_fft, hop_length, win_length, wav_out):
+    """librosa.istft of every clip of a packed batch (include/ttsb.h: ttsb_istft_ragged): spec fp32 (total_frames, n_fft/2 + 1, 2)
+    -> wav_out fp32 (hop (total_frames - n_clips)), clip c at sample hop (frame_offsets[c] - c)."""
+    fo, n = _host_offsets(frame_offsets)
+    ws = _workspace(int(load().ttsb_istft_ragged_workspace_bytes(spec.shape[0], n, int(n_fft))), spec.device)
+    _check(load().ttsb_istft_ragged(ptr(spec), fo, n, int(n_fft), int(hop_length), int(win_length), ptr(ws), ws.numel(), ptr(wav_out),
+                                    _stream()), 'ttsb_istft_ragged')
+
+
+def griffinlim_ragged(magnitude, init_angles, frame_offsets, n_fft, hop_length, win_length, n_iter, momentum, wav_out):
+    """Griffin-Lim of every clip of a packed batch (include/ttsb.h: ttsb_griffinlim_ragged).  magnitude fp32 (F, n_fft/2 + 1),
+    init_angles complex64 (F, n_fft/2 + 1) and wav_out fp32 (hop (F - n_clips)) on the device."""
+    fo, n = _host_offsets(frame_offsets)
+    ws = _workspace(int(load().ttsb_griffinlim_ragged_workspace_bytes(magnitude.shape[0], n, int(n_fft))), magnitude.device)
+    _check(load().ttsb_griffinlim_ragged(ptr(magnitude), ptr(init_angles), fo, n, int(n_fft), int(hop_length), int(win_length),
+                                         int(n_iter), float(momentum), ptr(ws), ws.numel(), ptr(wav_out), _stream()),
+           'ttsb_griffinlim_ragged')
 
 
 # ------------------------------------------------------------------------------------------------------------

@@ -2,7 +2,8 @@
 reference has no counterpart: it shows validation predictions in TensorBoard).
 
 * MCD-DTW: mel-cepstral distortion after dynamic time warping, on the GPU (``ttsb_mcd_dtw``).  The cepstra are the orthonormal
-  DCT-II of the natural-log mels (the MelGAN normaliser's ln(max(S, 1e-5))), coefficients 1..K with c0 (the energy) left out;
+  DCT-II of the natural-log mels (the MelGAN normaliser's ln(max(S, 1e-5)); WaveRNN-normalised mels are mapped back to it by
+  ``natural_log_mels``), coefficients 1..K with c0 (the energy) left out;
   the frame distance is 10 / ln 10 * sqrt(2 sum_k (c_k - c'_k)^2) dB and a line's MCD is the DTW path cost over the path
   length.  This is not the all-pass warped mel-cepstrum of SPTK / WORLD, so the numbers are not comparable to MCD figures in
   papers that use those; they rank models and vocoders of this project against each other.
@@ -27,7 +28,6 @@ from .. import lib
 
 KAPPA = 10.0 / math.log(10.0)   # dB per neper-like unit of the cepstral distance: 10 / ln 10
 DEFAULT_N_CEPS = 24
-MIN_VOCODED_SAMPLES = 513       # the ragged log-mel front end needs more than n_fft / 2 samples per clip
 
 
 def dct_matrix(n_mels: int, n_ceps: int) -> np.ndarray:
@@ -43,6 +43,25 @@ def check_normalizer(config: dict, what: str = 'model'):
     if normalizer != 'MelGAN':
         raise ValueError(f'MCD is computed from the MelGAN normaliser\'s natural-log mels (ln(max(S, 1e-5))); this {what}\'s '
                          f'normalizer is {normalizer!r}, whose cepstra would not be comparable')
+
+
+LN10_OVER_20 = math.log(10.0) / 20.0
+
+
+def _wavernn_to_natural_log(m: torch.Tensor) -> torch.Tensor:
+    return ((m + 4.0) / 8.0 * 100.0 - 100.0) * LN10_OVER_20
+
+
+def natural_log_mels(config: dict, what: str = 'model') -> Callable[[torch.Tensor], torch.Tensor]:
+    """The map from this config's normalised mels to the natural-log mels ln(max(S, 1e-5)) MCD is defined on: the identity for
+    the MelGAN normaliser; for WaveRNN's clip((20 log10 max(S, 1e-5) + 100) / 100, 0, 1) * 8 - 4, whose -100 dB floor is the
+    same 1e-5, ln S = ((y + 4) / 8 * 100 - 100) ln 10 / 20, exact below 0 dB (the WaveRNN normaliser clips louder bins to 0 dB).
+    Any other normaliser is refused (check_normalizer)."""
+    normalizer = config.get('normalizer')
+    if normalizer == 'WaveRNN':
+        return _wavernn_to_natural_log
+    check_normalizer(config, what)
+    return lambda m: m
 
 
 def _offsets(counts) -> np.ndarray:
@@ -150,12 +169,14 @@ def pitch_scores(pred: np.ndarray, target: np.ndarray, stats: Optional[tuple]) -
     return out
 
 
-def _mcd_fields(prefix: str, pred_mels: list, ref_mels: list, n_ceps: int) -> List[dict]:
-    """{prefix}mcd / dtw_cost / path_len per line; None for a line whose prediction has no frame."""
+def _mcd_fields(prefix: str, pred_mels: list, ref_mels: list, n_ceps: int, to_ln=lambda m: m) -> List[dict]:
+    """{prefix}mcd / dtw_cost / path_len per line, the mels mapped to natural-log mels by to_ln; None for a line whose prediction
+    has no frame."""
     rows = [{f'{prefix}mcd': None, f'{prefix}dtw_cost': None, f'{prefix}path_len': None} for _ in pred_mels]
     keep = [i for i, m in enumerate(pred_mels) if m.shape[0] > 0]
     if keep:
-        cost, path_len, mcd = mcd_dtw([pred_mels[i] for i in keep], [ref_mels[i] for i in keep], n_ceps)
+        cost, path_len, mcd = mcd_dtw([to_ln(torch.as_tensor(pred_mels[i])) for i in keep],
+                                      [to_ln(torch.as_tensor(ref_mels[i])) for i in keep], n_ceps)
         for r, i in enumerate(keep):
             rows[i] = {f'{prefix}mcd': float(mcd[r]), f'{prefix}dtw_cost': float(cost[r]), f'{prefix}path_len': int(path_len[r])}
     return rows
@@ -164,8 +185,8 @@ def _mcd_fields(prefix: str, pred_mels: list, ref_mels: list, n_ceps: int) -> Li
 def _resynthesis_mels(audio, wavs: List[np.ndarray]) -> List[torch.Tensor]:
     """Log-mels of vocoded waveforms through the ragged front end (Audio.mel_spectrogram_ragged_device)."""
     for i, w in enumerate(wavs):
-        if len(w) < MIN_VOCODED_SAMPLES:
-            raise ValueError(f'line {i}: the vocoder gave {len(w)} samples; the log-mel front end needs at least {MIN_VOCODED_SAMPLES}')
+        if len(w) < audio.min_mel_samples:
+            raise ValueError(f'line {i}: the vocoder gave {len(w)} samples; the log-mel front end needs at least {audio.min_mel_samples}')
     packed = torch.from_numpy(np.ascontiguousarray(np.concatenate(wavs), dtype=np.float32)).to(audio.device)
     mel, fo = audio.mel_spectrogram_ragged_device(packed, _offsets([len(w) for w in wavs]))
     return [mel[int(fo[i]):int(fo[i + 1])] for i in range(len(wavs))]
@@ -190,20 +211,20 @@ def evaluate_model(model, vs: ValidationSet, n_ceps: int = DEFAULT_N_CEPS, teach
     function from a list of (T, n_mels) mels to waveforms) and audio (the model's Audio), the free-running mels and the recorded
     mels are vocoded, their log-mels re-extracted on the GPU and each scored against the recorded mel (vocoded_* and
     copy_synthesis_*; the latter is the vocoder's own floor)."""
-    check_normalizer(model.config)
+    to_ln = natural_log_mels(model.config)
     tokens = tokenize(model, vs.phonemes)
     outs = model.predict_batch(tokens, encode=False, phoneme_max_duration=None, batch_size=batch_size)
     pred_mels = [o['mel'] for o in outs]
     lines = [{'name': n, 'frames_predicted': int(o['mel_lengths']), 'frames_recorded': int(m.shape[0])}
              for n, o, m in zip(vs.names, outs, vs.mels)]
-    for i, row in enumerate(_mcd_fields('', pred_mels, vs.mels, n_ceps)):
+    for i, row in enumerate(_mcd_fields('', pred_mels, vs.mels, n_ceps, to_ln)):
         lines[i].update(row)
         lines[i].update(duration_scores(outs[i]['int_durations'].cpu().numpy(), vs.durations[i]))
         lines[i].update(pitch_scores(outs[i]['pitch'].cpu().numpy(), vs.pitch[i], vs.pitch_stats))
     if teacher_forced:
         tf = model.predict_batch(tokens, encode=False, phoneme_max_duration=None, phoneme_durations=vs.durations,
                                  phoneme_pitch=vs.pitch, batch_size=batch_size)
-        for i, row in enumerate(_mcd_fields('teacher_forced_', [o['mel'] for o in tf], vs.mels, n_ceps)):
+        for i, row in enumerate(_mcd_fields('teacher_forced_', [o['mel'] for o in tf], vs.mels, n_ceps, to_ln)):
             lines[i].update(row)
     if vocode is not None:
         if audio is None:
@@ -214,8 +235,8 @@ def evaluate_model(model, vs: ValidationSet, n_ceps: int = DEFAULT_N_CEPS, teach
             for i, m in zip(kept, _resynthesis_mels(audio, vocode([pred_mels[i].cpu().numpy() for i in kept]))):
                 vocoded[i] = m
         copy = _resynthesis_mels(audio, vocode(vs.mels))
-        for i, (row, crow) in enumerate(zip(_mcd_fields('vocoded_', vocoded, vs.mels, n_ceps),
-                                            _mcd_fields('copy_synthesis_', copy, vs.mels, n_ceps))):
+        for i, (row, crow) in enumerate(zip(_mcd_fields('vocoded_', vocoded, vs.mels, n_ceps, to_ln),
+                                            _mcd_fields('copy_synthesis_', copy, vs.mels, n_ceps, to_ln))):
             lines[i].update(row)
             lines[i].update(crow)
     return {'lines': lines, 'mean': _means(lines)}
