@@ -156,6 +156,8 @@ int ttsb_layernorm_fwd(const float* x, const float* gamma, const float* beta, in
  *   cross-attention (kv_hi != NULL; model/layers.py:315-327 CrossAttentionResnorm): q from (B,T,ld_qk) at q_col0,
  *     k and v from a second buffer (B,Tk,ld_kv) at k_col0 / v_col0 (the K|V GEMM of the encoder output).
  *   out: bf16 hi (and lo when out_lo != NULL) (B,T,ld_out), head h at columns h*dh.
+ *   The H*dh columns from each column offset (>= 0) must lie inside their row (ld_qk, ld_kv, ld_out); a call that breaks
+ *   this, or names a weights_batch_index outside [0, B), returns TTSB_ERR_INVALID_ARGUMENT and writes nothing.
  *   Masking follows the reference's additive -1e9 masks: keys t >= kv_len[b] (padding mask, transformer_utils.py:24-32)
  *   and, with causal = 1, keys t > query index (look-ahead mask, transformer_utils.py:35-37; the Aligner passes
  *   max(padding, look-ahead), models.py:136-138).

@@ -262,38 +262,73 @@ def ref_mha(q, k, v, kv_len, H, precision):
     return out, w
 
 
+def operand16(t: torch.Tensor, precision: str) -> torch.Tensor:
+    """float64 (CPU) value of what the attention kernels read for fp32 `t`: the fp16 or bf16 rounding, or in bf16x3 the sum
+    hi + lo of its split (hi = bf16(t), lo = bf16(t - hi), both round to nearest, as ttsb_split_bf16 computes them)."""
+    t = t.detach().cpu().float()
+    if precision == 'fp16':
+        return t.half().double()
+    hi = t.bfloat16()
+    if precision == 'bf16':
+        return hi.double()
+    return hi.double() + (t - hi.float()).bfloat16().double()
+
+
+def _place(B, T, ld, parts):
+    """fp32 (B, T, ld) buffer holding each (tensor, column offset) of `parts`; every other column is NaN."""
+    buf = torch.full((B, T, ld), float('nan'), device=DEV)
+    taken = torch.zeros(ld, dtype=torch.bool)
+    for x, c0 in parts:
+        C = x.shape[-1]
+        assert 0 <= c0 and c0 + C <= ld and not taken[c0:c0 + C].any()
+        taken[c0:c0 + C] = True
+        buf[..., c0:c0 + C] = x
+    return buf
+
+
 def run_mha_general(q, kv_k, kv_v, kv_len, H, *, precision='fp16', impl='tcgen05', causal=False, cross=False, full_queries=True,
-                    weights_all=False):
-    """General form of ttsb_mha_fwd: q fp32 (B,T,d); k,v fp32 (B,Tk,d).  cross=True keeps k|v in a second buffer."""
+                    weights_all=False, weights_b=None, ld_qk=None, ld_kv=None, cols=None, out=None):
+    """General form of ttsb_mha_fwd: q fp32 (B,T,d); k,v fp32 (B,Tk,d).  cross=True keeps k|v in a second buffer.
+
+    Layout: q, k and v sit at column offsets cols = (q_col0, k_col0, v_col0) of a (B,T,ld_qk) buffer (self-attention), or q at
+    q_col0 of (B,T,ld_qk) and k, v at k_col0 / v_col0 of (B,Tk,ld_kv) (cross); columns outside them hold NaN.  Defaults:
+    (0, d, 2d) and ld_qk = 3d, or (0, 0, d), ld_qk = d and ld_kv = 2d.  out: the caller's (out_hi, out_lo or None) 16-bit
+    buffers of shape (rows >= B*T, ld_out), written through the ABI as they are (out_lo None passes NULL); by default both
+    planes are (B*T, d) and NaN.  weights_b: the weights of that batch row, (H,T,Tk); weights_all: (B,H,T,Tk); NaN before.
+    Returns (hi + lo of columns [0, d) of the first B*T rows as (B,T,d), weights)."""
     split = precision == 'bf16x3'
     B, T, d = q.shape
     Tk = kv_k.shape[1]
     dh = d // H
     m = lib.MhaArgs()
     m.B, m.T, m.H, m.dh = B, T, H, dh
+    keep = []
     if cross:
-        qb_hi, qb_lo = _to16(q.contiguous(), precision, split)
-        kv = torch.cat([kv_k, kv_v], dim=-1).contiguous()
-        kv_hi, kv_lo = _to16(kv, precision, split)
+        q_col0, k_col0, v_col0 = cols or (0, 0, d)
+        qb_hi, qb_lo = _to16(_place(B, T, ld_qk or d, [(q, q_col0)]), precision, split)
+        kv_hi, kv_lo = _to16(_place(B, Tk, ld_kv or 2 * d, [(kv_k, k_col0), (kv_v, v_col0)]), precision, split)
+        keep += [qb_hi, qb_lo, kv_hi, kv_lo]
         m.qk_hi = qb_hi.data_ptr()
         m.qk_lo = qb_lo.data_ptr() if split else None
-        m.ld_qk, m.q_col0 = d, 0
+        m.ld_qk, m.q_col0 = qb_hi.shape[-1], q_col0
         m.kv_hi = kv_hi.data_ptr()
         m.kv_lo = kv_lo.data_ptr() if split else None
-        m.ld_kv, m.Tk, m.k_col0, m.v_col0 = 2 * d, Tk, 0, d
+        m.ld_kv, m.Tk, m.k_col0, m.v_col0 = kv_hi.shape[-1], Tk, k_col0, v_col0
     else:
         assert Tk == T
-        qk = torch.cat([q, kv_k, kv_v], dim=-1).contiguous()
-        qk_hi, qk_lo = _to16(qk, precision, split)
+        q_col0, k_col0, v_col0 = cols or (0, d, 2 * d)
+        qk_hi, qk_lo = _to16(_place(B, T, ld_qk or 3 * d, [(q, q_col0), (kv_k, k_col0), (kv_v, v_col0)]), precision, split)
+        keep += [qk_hi, qk_lo]
         m.qk_hi = qk_hi.data_ptr()
         m.qk_lo = qk_lo.data_ptr() if split else None
-        m.ld_qk, m.q_col0, m.k_col0, m.v_col0 = 3 * d, 0, d, 2 * d
+        m.ld_qk, m.q_col0, m.k_col0, m.v_col0 = qk_hi.shape[-1], q_col0, k_col0, v_col0
     m.kv_len = kv_len.data_ptr()
-    out_hi = torch.full((B, T, d), float('nan'), device=DEV, dtype=torch.bfloat16)
-    out_lo = torch.full((B, T, d), float('nan'), device=DEV, dtype=torch.bfloat16)
+    if out is None:
+        out = (_poison16((B * T, d)), _poison16((B * T, d)))
+    out_hi, out_lo = out
     m.out_hi = out_hi.data_ptr()
-    m.out_lo = out_lo.data_ptr()
-    m.ld_out = d
+    m.out_lo = out_lo.data_ptr() if out_lo is not None else None
+    m.ld_out = out_hi.shape[-1]
     m.causal = int(causal)
     m.full_queries = int(full_queries)
     wts = None
@@ -301,18 +336,22 @@ def run_mha_general(q, kv_k, kv_v, kv_len, H, *, precision='fp16', impl='tcgen05
         wts = torch.full((B, H, T, Tk), float('nan'), device=DEV)
         m.weights_out = wts.data_ptr()
         m.weights_all = 1
+    elif weights_b is not None:
+        wts = torch.full((H, T, Tk), float('nan'), device=DEV)
+        m.weights_out = wts.data_ptr()
+        m.weights_batch_index = weights_b
     m.precision = {'bf16x3': lib.PREC_BF16X3, 'bf16': lib.PREC_BF16, 'fp16': lib.PREC_FP16}[precision]
     m.impl = lib.IMPL_SIMT if impl == 'simt' else lib.IMPL_TCGEN05
     lib.mha_fwd(m)
     torch.cuda.synchronize()
-    return out_hi.float() + out_lo.float(), wts
+    res = out_hi[:B * T].float() + (out_lo[:B * T].float() if out_lo is not None else 0)
+    return res.reshape(B, T, -1)[..., :d], wts
 
 
-def ref_mha_general(q, k, v, kv_len, H, precision, causal=False):
-    """float64 CPU attention; additive -1e9 mask = max(key padding, look-ahead) (models.py:136-138, layers.py:186-187)."""
-    cast = {'bf16x3': lambda t: t.detach().cpu().double(), 'bf16': lambda t: t.detach().cpu().bfloat16().double(),
-            'fp16': lambda t: t.detach().cpu().half().double()}[precision]
-    q, k, v = cast(q), cast(k), cast(v)
+def ref_mha_general(q, k, v, kv_len, H, precision, causal=False, full_queries=True):
+    """float64 CPU attention on the operands the kernel reads (operand16); additive -1e9 mask = max(key padding, look-ahead)
+    (models.py:136-138, layers.py:186-187).  full_queries=False: query rows >= kv_len[b] of the output are zero."""
+    q, k, v = (operand16(t, precision) for t in (q, k, v))
     B, T, d = q.shape
     Tk = k.shape[1]
     dh = d // H
@@ -325,6 +364,8 @@ def ref_mha_general(q, k, v, kv_len, H, precision, causal=False):
     logits = (logits.float() + (mask * -1e9).float()).double()
     w = torch.softmax(logits, -1)
     out = (w @ sp(v)).permute(0, 2, 1, 3).reshape(B, T, d)
+    if not full_queries:
+        out = out.masked_fill((torch.arange(T)[None, :] >= kv_len.cpu()[:, None])[..., None], 0.0)
     return out, w
 
 

@@ -96,6 +96,30 @@ def test_argument_validation_without_gpu(cdll):
     assert b'block_n' in cdll.ttsb_last_error()
     m = lib.MhaArgs()
     assert cdll.ttsb_mha_fwd(C.byref(m), None) == -1
+    # ttsb_mha_fwd refuses column layouts whose H*dh columns leave their row, and a weights row outside the batch, before
+    # any launch (fake non-null pointers: nothing may be read or written)
+    p = C.c_void_p(256)
+
+    def mha(cross=False, **kw):
+        a = lib.MhaArgs()
+        a.B, a.T, a.H, a.dh = 2, 70, 2, 64
+        a.qk_hi, a.qk_lo, a.kv_len, a.out_hi, a.out_lo = p, p, p, p, p
+        a.ld_qk, a.q_col0, a.k_col0, a.v_col0, a.ld_out = 3 * 128, 0, 128, 256, 128
+        a.precision, a.impl, a.full_queries = lib.PREC_BF16, lib.IMPL_TCGEN05, int(cross)
+        if cross:
+            a.ld_qk, a.kv_hi, a.kv_lo, a.ld_kv, a.Tk, a.k_col0, a.v_col0 = 128, p, p, 256, 33, 0, 128
+        for k, v in kw.items():
+            setattr(a, k, v)
+        return cdll.ttsb_mha_fwd(C.byref(a), None)
+
+    for impl in (lib.IMPL_TCGEN05, lib.IMPL_SIMT):
+        for bad in ({'q_col0': -8}, {'k_col0': -8}, {'v_col0': -128}, {'q_col0': 264}, {'k_col0': 264}, {'v_col0': 264},
+                    {'ld_qk': 376}, {'ld_out': 112}, {'dh': 0}, {'weights_out': p, 'weights_batch_index': 2},
+                    {'weights_out': p, 'weights_batch_index': -1}, {'cross': True, 'k_col0': 136},
+                    {'cross': True, 'v_col0': 136}, {'cross': True, 'ld_kv': 248}, {'cross': True, 'q_col0': 8},
+                    {'cross': True, 'ld_out': 64}):
+            assert mha(impl=impl, **bad) == -1, bad
+            assert b'ttsb_mha_fwd' in cdll.ttsb_last_error(), bad
     assert cdll.ttsb_stft_mel_log(None, 1, 1000, None, 80, 0, None, None) == -1
     assert cdll.ttsb_durations_to_int(None, C.c_float(1.0), None, None, 1, 1, None, None, None) == -1
     # the training attention kernels: the support query is pure host logic; bad arguments are refused before any CUDA call

@@ -293,12 +293,14 @@ mha_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ 
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
       if (tq[rr] < p.T) {
+        // the tile holding kv_len also computed its padded query rows as full rows: those are written as (+0) zeros
+        const bool pad = !p.full_queries && tq[rr] >= len;
         const size_t ob = ((size_t)b * p.T + tq[rr]) * p.ld_out + h * DH + cq;
 #pragma unroll
         for (int i = 0; i < DH / 8; ++i) {
           __nv_bfloat16 h0, l0, h1, l1;
-          split_bf16(o[4 * i + 2 * rr] * inv[rr], h0, l0);
-          split_bf16(o[4 * i + 2 * rr + 1] * inv[rr], h1, l1);
+          split_bf16(pad ? 0.f : o[4 * i + 2 * rr] * inv[rr], h0, l0);
+          split_bf16(pad ? 0.f : o[4 * i + 2 * rr + 1] * inv[rr], h1, l1);
           *reinterpret_cast<uint32_t*>(p.out_hi + ob + 8 * i) = pack_bf16(h0, h1);
           if (p.out_lo) *reinterpret_cast<uint32_t*>(p.out_lo + ob + 8 * i) = pack_bf16(l0, l1);
         }
@@ -381,11 +383,13 @@ __global__ void mha_simt_kernel(const MhaKParams p, const MhaSimtPtrs q) {
     for (int tk = threadIdx.x; tk < p.Tk; tk += blockDim.x) wrow[tk] = logit[tk] * inv;
   }
   if (q.weights_only) return;
+  const bool pad = !p.full_queries && tq >= len;   // padded query row: zeros (its weights above are still the reference's)
   for (int c = threadIdx.x; c < q.dh; c += blockDim.x) {
     const size_t vcol = (size_t)p.v_col0 + h * q.dh + c;
     float acc = 0.f;
-    for (int tk = 0; tk < p.Tk; ++tk)
-      acc = fmaf(logit[tk], ld_split(q.kv_hi, q.kv_lo, ((size_t)b * p.Tk + tk) * q.ld_kv + vcol, q.f16), acc);
+    if (!pad)
+      for (int tk = 0; tk < p.Tk; ++tk)
+        acc = fmaf(logit[tk], ld_split(q.kv_hi, q.kv_lo, ((size_t)b * p.Tk + tk) * q.ld_kv + vcol, q.f16), acc);
     acc *= inv;
     __nv_bfloat16 hi, lo;
     split_bf16(acc, hi, lo);
@@ -526,6 +530,21 @@ extern "C" int ttsb_mha_fwd(const ttsb_mha_args* a, void* stream_v) {
     set_last_error("ttsb_mha_fwd: leading dimensions / column offsets must be multiples of 8");
     return TTSB_ERR_INVALID_ARGUMENT;
   }
+  // H*dh columns from each offset must lie inside their row: past ld the tensor maps read zeros and the SIMT kernel the
+  // next row, both without an error
+  const int64_t hd = (int64_t)a->H * a->dh;
+  const int ld_k = cross ? a->ld_kv : a->ld_qk;
+  if (a->dh <= 0 || a->q_col0 < 0 || a->k_col0 < 0 || a->v_col0 < 0 || a->q_col0 + hd > a->ld_qk || a->k_col0 + hd > ld_k ||
+      a->v_col0 + hd > ld_k || hd > a->ld_out) {
+    set_last_error("ttsb_mha_fwd: need dh > 0, column offsets >= 0, q_col0 + H*dh <= ld_qk, k_col0 / v_col0 + H*dh <= %s and H*dh <= ld_out",
+                   cross ? "ld_kv" : "ld_qk");
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  // checked before anything is launched: a refused call writes nothing
+  if (a->weights_out && !a->weights_all && (a->weights_batch_index < 0 || a->weights_batch_index >= a->B)) {
+    set_last_error("ttsb_mha_fwd: weights_batch_index out of range");
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   MhaKParams p{};
   p.B = a->B; p.T = a->T; p.H = a->H;
@@ -582,9 +601,7 @@ extern "C" int ttsb_mha_fwd(const ttsb_mha_args* a, void* stream_v) {
 #undef TTSB_MHA_DISPATCH1
   if (rc) return rc;
   if (a->weights_out) {
-    if (!a->weights_all && (a->weights_batch_index < 0 || a->weights_batch_index >= a->B)) { set_last_error("ttsb_mha_fwd: weights_batch_index out of range"); return TTSB_ERR_INVALID_ARGUMENT; }
     q.weights_only = 1;
-    if (a->dh % 4) { set_last_error("ttsb_mha_fwd: the weights kernel needs head_dim %% 4 == 0"); return TTSB_ERR_UNSUPPORTED; }
     const size_t aw_smem = (size_t)(AW_Q * a->dh + AW_K * (a->dh + 4)) * sizeof(float);
     static PerDevice<size_t> aw_attr_pd;
     size_t& aw_attr = aw_attr_pd.get();
