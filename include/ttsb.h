@@ -650,7 +650,7 @@ int ttsb_mcd_dtw(const float* x, const int32_t* x_offsets, const float* y, const
  * input column is read.  With up > 1 (a transposed conv phrased over its input rows), column n of y[c, t] is channel n % ld_out
  * of output row t up + n / ld_out: the outputs use the same layout with up L_c rows per clip, and N = up ld_out.
  *   res_hi/lo  optional residual in the output layout (ld_out columns, res_lo only in bf16x3): y = bias + conv + (res_hi + res_lo).
- *              It must not alias out_hi or act_hi.
+ *              Neither plane may be an output plane.
  *   sum        optional fp32 plane in the output layout, for the multi-receptive-field average of HiFi-GAN's resblocks, in torch's
  *              order (xs = rb_0(x); xs += rb_1(x); ...; x = xs / nk), after the residual:
  *                TTSB_CONV1D_SUM_WRITE  sum = y                 (resblock 0)
@@ -659,17 +659,18 @@ int ttsb_mcd_dtw(const float* x, const int32_t* x_offsets, const float* y, const
  *              WRITE and ADD count as an output, so out and act may both be NULL.
  *   out_rows   rows of the output layout, sum up L_c + 2 halo n_clips: the shape of the outputs, the residual and the sum.
  * Outputs (bf16; the lo planes only in bf16x3; any may be NULL): out_hi/out_lo = y, act_hi/act_lo = LeakyReLU_slope(y), slope
- * in [0, 1].
+ * in [0, 1].  The conv does not run in place: no output plane may be an input plane a tap reads (in_hi, and in bf16x3 in_lo,
+ * of its source), since other tiles' taps still load the rows a tile writes.
  * halo_mode: TTSB_HALO_NONE leaves the outputs' halos alone; TTSB_HALO_REFLECT writes output row L-1+k of a clip as a copy of
  * row L-1-k and row -k as a copy of row k (k = 1..halo, needs up L_c > halo); TTSB_HALO_ZERO writes zeros there (needs
  * up L_c >= halo).  A halo row is written only by the store of the row it mirrors, never by a computed row.  So with
  * TTSB_HALO_NONE and zero-initialised planes the halos stay zero, which is every zero-padded conv's padding, and clips of any
  * length >= 1 work.
- * N is a multiple of 64, and at most 256 or a multiple of 256; ld_out (= N / up) is a multiple of 16; res_hi, res_lo and sum
- * are 16-byte aligned.  No atomics: a clip's output is bit-identical wherever it sits in the batch.  workspace:
+ * N is a multiple of 64, and at most 256 or a multiple of 256; ld_out (= N / up) is a multiple of 16; res_hi, res_lo, sum,
+ * bias and the output planes the call writes (in bf16 the lo planes are not) are 16-byte aligned.  No atomics: a clip's output is bit-identical wherever it sits in the batch.  workspace:
  * ttsb_conv1d_workspace_bytes(n_clips) bytes of device memory, 4-byte aligned; the entry points copy the clip table there.
- * Malformed offsets, clips too short for the halo mode, a short workspace and any inconsistent halo, taps, slope, residual,
- * sum or out_rows give TTSB_ERR_INVALID_ARGUMENT before any CUDA call.
+ * Malformed offsets, clips too short for the halo mode, a short workspace, misaligned or aliased planes and any inconsistent
+ * halo, taps, slope, residual, sum or out_rows give TTSB_ERR_INVALID_ARGUMENT before any CUDA call.
  * ------------------------------------------------------------------------------------------------------- */
 #define TTSB_HALO_NONE 0
 #define TTSB_HALO_REFLECT 1

@@ -242,6 +242,30 @@ def test_conv1d_ex_refusals_without_gpu(cdll):
     assert b'workspace' in cdll.ttsb_last_error()
 
 
+def _valid_ex_apart(lengths):
+    """_valid_ex with out, act, residual and input planes at six different (aligned, dummy) addresses."""
+    a, keep = _valid_ex(lengths)
+    a.act_hi, a.act_lo = 1536, 1792
+    return a, keep
+
+
+def test_conv1d_ex_refuses_misaligned_and_in_place_planes(cdll):
+    # the epilogue's 16-byte vector stores and bias loads: a misaligned plane is refused, not faulted on
+    aligned = 'out_hi, out_lo, act_hi, act_lo and bias must be 16-byte aligned'
+    for field in ('out_hi', 'out_lo', 'act_hi', 'act_lo'):
+        a, keep = _valid_ex_apart([1, 2, 3]); setattr(a, field, getattr(a, field) + 8); _refused(cdll, a, aligned)
+    a, keep = _valid_ex_apart([1, 2, 3]); a.bias = 2052; _refused(cdll, a, aligned)
+    # no in-place conv: an output plane is never a plane a tap reads, and the residual is never an output
+    a, keep = _valid_ex_apart([1, 2, 3]); a.out_hi = 256; _refused(cdll, a, 'aliases an input plane of source 0')
+    a, keep = _valid_ex_apart([1, 2, 3]); a.in_lo[0] = a.act_lo = 2048; _refused(cdll, a, 'aliases an input plane of source 0')
+    a, keep = _valid_ex_apart([1, 2, 3])
+    a.in_hi[1], a.in_lo[1], a.ld_in[1], a.tap_src[3] = 2304, 2560, 64, 1
+    a.act_hi = 2304; _refused(cdll, a, 'aliases an input plane of source 1')
+    a, keep = _valid_ex_apart([1, 2, 3]); a.res_lo = 1280; _refused(cdll, a, 'the residual must not alias an output')
+    a, keep = _valid_ex_apart([1, 2, 3]); a.res_lo = 1792; _refused(cdll, a, 'the residual must not alias an output')
+    a, keep = _valid_ex_apart([1, 2, 3]); a.res_hi = 1536; _refused(cdll, a, 'the residual must not alias an output')
+
+
 def test_vocode_batch_refuses_bad_mels_before_the_gpu():
     g = hg.HiFiGANGenerator('v1', device='cpu')
     g._convs = {}   # loading packs on the GPU; the shape check comes first

@@ -334,6 +334,25 @@ static int conv1d_launch(const char* what, const ttsb_conv1d_ex_args* a, void* s
   }
   rc = check_workspace(what, a->workspace, a->workspace_bytes, a->n_clips);
   if (rc) return rc;
+  // last of the argument checks: the planes the epilogue writes (16-byte vector stores; in bf16 the lo planes are ignored)
+  const void* outs[4] = {a->out_hi, split && a->out_hi ? a->out_lo : nullptr, a->act_hi, split && a->act_hi ? a->act_lo : nullptr};
+  if ((reinterpret_cast<uintptr_t>(outs[0]) | reinterpret_cast<uintptr_t>(outs[1]) | reinterpret_cast<uintptr_t>(outs[2]) |
+       reinterpret_cast<uintptr_t>(outs[3]) | reinterpret_cast<uintptr_t>(a->bias)) % 16) {
+    set_last_error("%s: out_hi, out_lo, act_hi, act_lo and bias must be 16-byte aligned", what);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  for (const void* o : outs) {
+    if (!o) continue;
+    if (o == a->res_hi || o == a->res_lo) { set_last_error("%s: the residual must not alias an output", what); return TTSB_ERR_INVALID_ARGUMENT; }
+    // other tiles' taps still read the rows this tile's epilogue and mirror stores write: a conv cannot run in place
+    for (int s = 0; s < a->num_taps; ++s) {
+      const int src = a->tap_src[s];
+      if (o == a->in_hi[src] || (split && o == a->in_lo[src])) {
+        set_last_error("%s: an output plane aliases an input plane of source %d (no in-place conv)", what, src);
+        return TTSB_ERR_INVALID_ARGUMENT;
+      }
+    }
+  }
 
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   ConvKParams p{};
