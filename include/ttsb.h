@@ -31,7 +31,7 @@ extern "C" {
 #define TTSB_ERR_CUDA (-2)
 #define TTSB_ERR_UNSUPPORTED (-3)
 
-#define TTSB_ABI_VERSION 4
+#define TTSB_ABI_VERSION 5
 
 /* precision of the tensor-core products */
 #define TTSB_PREC_BF16 0   /* single bf16 pass, fp32 accumulate */
@@ -473,10 +473,15 @@ int ttsb_phoneme_lengths(const int32_t* phonemes, int B, int T, int32_t padding,
  * STFT -> mel filterbank -> log   (data/audio.py:72-92, 209-231)
  *   wav fp32 (n_clips, n_samples); out fp32 (n_clips, n_frames, n_mels), n_frames = 1 + n_samples/hop.
  *   n_fft must be 1024 (the reference's config), hop 256, window = periodic Hann(1024), reflect padding.
- *   mel_basis fp32 (n_mels, 513) dense (the kernel uses its band structure); normalizer 0 = MelGAN log(clip 1e-5),
- *   1 = WaveRNN.
+ *   mel_basis fp32 (n_mels, 513) dense on the device; band int32 (n_mels, 2) in HOST memory: band[2m], band[2m+1] = first /
+ *   past-last bin of row m that may hold a non-zero weight (0 <= first <= past-last <= 513; an empty row is (0, 0)).  Only
+ *   the weights inside each row's band are read, from mel_basis itself on every call: nothing is kept between calls, so a
+ *   basis rewritten in place is used as it now stands.  normalizer 0 = MelGAN log(clip 1e-5), 1 = WaveRNN.  Bad arguments
+ *   give TTSB_ERR_INVALID_ARGUMENT before any CUDA call, with the argument named in ttsb_last_error().  The entry point never
+ *   waits for the device (it may be captured in a CUDA graph once the library has run one call on that device).  A band table
+ *   spanning more than 2048 weights runs a slower kernel that reads the basis from global memory.
  * ------------------------------------------------------------------------------------------------------- */
-int ttsb_stft_mel_log(const float* wav, int n_clips, int n_samples, const float* mel_basis, int n_mels,
+int ttsb_stft_mel_log(const float* wav, int n_clips, int n_samples, const float* mel_basis, const int32_t* band, int n_mels,
                       int normalizer, float* out, void* stream);
 /* The same for a packed ragged batch of clips (create_training_data.py:41-47 over a corpus).  Clip c owns samples
  *   sample_offsets[c] .. sample_offsets[c+1] - 1 of wav and output frames frame_offsets[c] .. frame_offsets[c+1] - 1 of out
@@ -485,12 +490,12 @@ int ttsb_stft_mel_log(const float* wav, int n_clips, int n_samples, const float*
  *   table into `workspace` (ttsb_stft_mel_log_batch_workspace_bytes(n_clips) bytes of device memory, 4-byte aligned) before
  *   its one launch; a malformed table is refused with TTSB_ERR_INVALID_ARGUMENT before any CUDA call.  Reflect padding happens
  *   at each clip's own edges and a frame pair never spans two clips, so clip c's mel is bit-identical to ttsb_stft_mel_log on
- *   that clip alone, wherever it sits in the batch.  A basis too dense for the packed filterbank table gives
- *   TTSB_ERR_UNSUPPORTED. */
+ *   that clip alone, wherever it sits in the batch.  mel_basis and band as for ttsb_stft_mel_log; a band table spanning more
+ *   than 2048 weights gives TTSB_ERR_UNSUPPORTED. */
 int64_t ttsb_stft_mel_log_batch_workspace_bytes(int n_clips);   /* -1 for n_clips < 1 */
 int ttsb_stft_mel_log_batch(const float* wav, const int32_t* sample_offsets, const int32_t* frame_offsets, int n_clips,
-                            const float* mel_basis, int n_mels, int normalizer, void* workspace, int64_t workspace_bytes,
-                            float* out, void* stream);
+                            const float* mel_basis, const int32_t* band, int n_mels, int normalizer, void* workspace,
+                            int64_t workspace_bytes, float* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * f0 by WORLD's DIO + StoneMask  (Audio.extract_pitch, data/audio.py:146-151: pw.dio(y, fs, frame_period) then pw.stonemask;

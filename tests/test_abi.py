@@ -27,8 +27,8 @@ def test_header_symbols_are_all_exported(cdll):
     assert set(lib.EXPORTS) == names
 
 
-def test_abi_version_and_error_text(cdll):
-    assert cdll.ttsb_abi_version() == 4
+def test_abi_version_5_and_error_text(cdll):
+    assert cdll.ttsb_abi_version() == 5
     rc = cdll.ttsb_linear_fwd(None, None)
     assert rc == -1
     assert b'NULL' in cdll.ttsb_last_error()
@@ -120,7 +120,18 @@ def test_argument_validation_without_gpu(cdll):
                     {'cross': True, 'ld_out': 64}):
             assert mha(impl=impl, **bad) == -1, bad
             assert b'ttsb_mha_fwd' in cdll.ttsb_last_error(), bad
-    assert cdll.ttsb_stft_mel_log(None, 1, 1000, None, 80, 0, None, None) == -1
+    assert cdll.ttsb_stft_mel_log(None, 1, 1000, None, None, 80, 0, None, None) == -1
+    # the fused log-mel reads its band table on the host and refuses bad arguments, naming them, before any CUDA call
+    band = (C.c_int32 * 256)(*[0, 513] * 128)
+    for args, what in (((1, 512, 80, 0), b'n_samples'), ((0, 1000, 80, 0), b'n_clips'), ((1, 1000, 0, 0), b'n_mels'),
+                       ((1, 1000, 129, 0), b'n_mels'), ((1, 1000, 80, 2), b'normalizer')):
+        n_clips, n_samples, n_mels, norm = args
+        assert cdll.ttsb_stft_mel_log(p, n_clips, n_samples, p, band, n_mels, norm, p, None) == -1, args
+        assert what in cdll.ttsb_last_error(), args
+    for row in ((-1, 4), (5, 4), (0, 514)):
+        bad = (C.c_int32 * 4)(0, 513, *row)
+        assert cdll.ttsb_stft_mel_log(p, 1, 1000, p, bad, 2, 0, p, None) == -1, row
+        assert b'band row 1' in cdll.ttsb_last_error(), row
     assert cdll.ttsb_durations_to_int(None, C.c_float(1.0), None, None, 1, 1, None, None, None) == -1
     # the training attention kernels: the support query is pure host logic; bad arguments are refused before any CUDA call
     assert cdll.ttsb_attn_probs_supported(128, 1008) == 1 and cdll.ttsb_attn_probs_supported(64, 48) == 1

@@ -25,14 +25,22 @@ def _i32(*v):
     return (C.c_int32 * len(v))(*v)
 
 
-def test_ragged_mel_refuses_malformed_offsets_without_gpu(cdll):
+def test_ragged_mel_refuses_malformed_offsets_and_band_tables_without_gpu(cdll):
     dev = C.c_void_p(256)          # never dereferenced: every check below fails before any CUDA call
     ws = C.c_int64(1 << 20)
-    call = lambda so, fo, n: cdll.ttsb_stft_mel_log_batch(dev, so, fo, n, dev, 80, 0, dev, ws, dev, None)
+    band = _i32(*[0, 513] * 80)
+    call = lambda so, fo, n: cdll.ttsb_stft_mel_log_batch(dev, so, fo, n, dev, band, 80, 0, dev, ws, dev, None)
     assert call(_i32(0, 2000, 4000), _i32(0, 8, 17), 2) == -1 and b'frames' in cdll.ttsb_last_error()
     assert call(_i32(0, 500, 4000), _i32(0, 2, 17), 2) == -1 and b'512' in cdll.ttsb_last_error()
     assert call(_i32(5, 2000, 4000), _i32(0, 8, 16), 2) == -1 and b'start at 0' in cdll.ttsb_last_error()
     assert call(_i32(0, 2000), _i32(0, 8), 0) == -1
+    # a band table spanning 2049 weights (one more than the packed filterbank holds) is refused before any CUDA call
+    wide = _i32(0, 513, 0, 513, 0, 513, 0, 510)
+    assert cdll.ttsb_stft_mel_log_batch(dev, _i32(0, 2000, 4000), _i32(0, 8, 16), 2, dev, wide, 4, 0, dev, ws, dev, None) == -3
+    assert b'2048' in cdll.ttsb_last_error()
+    bad_band = _i32(0, 513, 7, 6)
+    assert cdll.ttsb_stft_mel_log_batch(dev, _i32(0, 2000, 4000), _i32(0, 8, 16), 2, dev, bad_band, 2, 0, dev, ws, dev, None) == -1
+    assert b'band row 1' in cdll.ttsb_last_error()
     assert cdll.ttsb_stft_mel_log_batch_workspace_bytes(0) == -1
 
 

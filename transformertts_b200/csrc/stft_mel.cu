@@ -28,26 +28,19 @@ constexpr int MAX_MELS = 128;
 __device__ float g_tw_re[NFFT];   // cos(2 pi i / 1024)
 __device__ float g_tw_im[NFFT];   // -sin(2 pi i / 1024)
 __device__ float g_window[NFFT];  // periodic Hann
-__device__ int g_band[2 * MAX_MELS];
+// The filterbank's band structure, computed on the host from the caller's band table for each call and passed by value:
+// row m has non-zero weights at bins [lo[m], lo[m] + len[m]) only; the packed (v2) table keeps them at off[m] ..
+// off[m] + len[m] - 1 (`taps` weights in all); kmax = 1 + the highest bin any row reads.
+struct MelBands {
+  int lo[MAX_MELS], len[MAX_MELS], off[MAX_MELS];
+  int kmax;
+  int taps;   // off[n_mels - 1] + len[n_mels - 1]: weights in the packed table
+};
 
 __device__ __forceinline__ float sample_reflect(const float* __restrict__ clip, int n, int i) {
   if (i < 0) i = -i;
   if (i >= n) i = 2 * (n - 1) - i;
   return __ldg(clip + i);
-}
-
-__global__ void mel_band_kernel(const float* __restrict__ basis, int n_mels) {
-  const int m = blockIdx.x * blockDim.x + threadIdx.x;
-  if (m >= n_mels) return;
-  int lo = NBINS, hi = 0;
-  for (int k = 0; k < NBINS; ++k)
-    if (basis[(size_t)m * NBINS + k] != 0.f) {
-      lo = min(lo, k);
-      hi = max(hi, k + 1);
-    }
-  if (lo > hi) lo = hi = 0;
-  g_band[2 * m] = lo;
-  g_band[2 * m + 1] = hi;
 }
 
 struct StftSmem {
@@ -60,7 +53,7 @@ struct StftSmem {
 
 __global__ void __launch_bounds__(STFT_WARPS * 32, 2)
 stft_mel_kernel(const float* __restrict__ wav, int n_samples, int n_frames, int pairs_per_clip, const float* __restrict__ basis,
-                int n_mels, int normalizer, float* __restrict__ out) {
+                const __grid_constant__ MelBands bands, int n_mels, int normalizer, float* __restrict__ out) {
   extern __shared__ uint8_t smem_raw[];
   StftSmem& sm = *reinterpret_cast<StftSmem*>(smem_raw);
   for (int i = threadIdx.x; i < NFFT; i += blockDim.x) {
@@ -138,7 +131,7 @@ stft_mel_kernel(const float* __restrict__ wav, int n_samples, int n_frames, int 
   __syncwarp();
   // ---- banded mel filterbank + normaliser
   for (int m = lane; m < n_mels; m += 32) {
-    const int lo = g_band[2 * m], hi = g_band[2 * m + 1];
+    const int lo = bands.lo[m], hi = lo + bands.len[m];
     float accA = 0.f, accB = 0.f;
     for (int k = lo; k < hi; ++k) {
       const float wgt = __ldg(basis + (size_t)m * NBINS + k);
@@ -161,7 +154,8 @@ stft_mel_kernel(const float* __restrict__ wav, int n_samples, int n_frames, int 
 }
 
 // ----------------------------------------------------------------------------------------------------
-// Version 2 of the fused kernel (the one ttsb_stft_mel_log launches; the kernel above is kept as TTSB_STFT_V1=1 for A/B runs).
+// Version 2 of the fused kernel (the one ttsb_stft_mel_log launches; the kernel above runs band tables wider than the packed
+// filterbank holds, and every basis under TTSB_STFT_V1=1 for A/B runs).
 // Version 1 waits on global loads of samples, window, filter weights and band bounds with nothing to hide them behind, and
 // its mel loop has shared-memory bank conflicts.  Changes:
 //   * persistent warps; the samples of the NEXT frame pair are requested into the (dead) FFT registers before the
@@ -170,48 +164,12 @@ stft_mel_kernel(const float* __restrict__ wav, int n_samples, int n_frames, int 
 //   * complex values cross shared memory as 8-byte (re, im) pairs (half the load / store instructions);
 //   * only the bins below the highest non-zero filter tap are separated (372 of 513 at f_max = 8 kHz), magnitudes with
 //     x * rsqrt(x) instead of the IEEE sqrt sequence;
-//   * the filterbank is stored banded and packed (727 weights), a lane owns bands m, m+32, m+64.
+//   * the filterbank is stored banded and packed (727 weights), a lane owns bands m, m+32, m+64.  Each block gathers the
+//     packed weights from the rows of the call's own basis, at the bands the host computed from the call's band table: no
+//     table outlives a launch, so a basis rewritten in place or a new basis at a freed address is read as it stands.
 // ----------------------------------------------------------------------------------------------------
 constexpr int V2_WARPS = 8;
 constexpr int MAX_TAPS = 2048;          // packed non-zero filter weights (a triangular basis has < 2 * 513)
-
-__device__ float g_mel_w[MAX_TAPS];     // row j: weights of bins [lo_j, lo_j + len_j) at offset off_j
-__device__ int g_mel_lo[MAX_MELS], g_mel_len[MAX_MELS], g_mel_off[MAX_MELS];
-__device__ int g_mel_kmax;              // 1 + highest bin with a non-zero weight
-__device__ int g_mel_ok;                // 0: the basis is not banded enough for the packed table
-
-__global__ void mel_pack_kernel(const float* __restrict__ basis, int n_mels) {
-  __shared__ int lo_s[MAX_MELS], len_s[MAX_MELS];
-  const int m = threadIdx.x;
-  if (m < n_mels) {
-    int lo = NBINS, hi = 0;
-    for (int k = 0; k < NBINS; ++k)
-      if (basis[(size_t)m * NBINS + k] != 0.f) {
-        lo = min(lo, k);
-        hi = max(hi, k + 1);
-      }
-    if (lo > hi) lo = hi = 0;
-    lo_s[m] = lo;
-    len_s[m] = hi - lo;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int off = 0, kmax = 0, ok = 1;
-    for (int j = 0; j < n_mels; ++j) {
-      g_mel_lo[j] = lo_s[j];
-      g_mel_len[j] = len_s[j];
-      g_mel_off[j] = off;
-      kmax = max(kmax, lo_s[j] + len_s[j]);
-      off += len_s[j];
-      if (off > MAX_TAPS) { ok = 0; break; }
-    }
-    g_mel_kmax = kmax;
-    g_mel_ok = ok;
-  }
-  __syncthreads();
-  if (m < n_mels && g_mel_ok)
-    for (int i = 0; i < len_s[m]; ++i) g_mel_w[g_mel_off[m] + i] = basis[(size_t)m * NBINS + lo_s[m] + i];
-}
 
 struct StftSmem2 {
   float2 tw[NFFT];                       // (cos, -sin)(2 pi i / 1024)
@@ -248,17 +206,24 @@ __device__ __forceinline__ void load_pair(const float* __restrict__ wav, int n_s
   load_clip_pair(wav + (size_t)clip * n_samples, n_samples, n_frames, pair, lane, re, im);
 }
 
-// shared-memory tables of the v2 kernels
-__device__ __forceinline__ void load_v2_tables(StftSmem2& sm, int n_mels) {
+// shared-memory tables of the v2 kernels; the packed filterbank is gathered from the rows of the call's own basis
+__device__ __forceinline__ void load_v2_tables(StftSmem2& sm, const float* __restrict__ basis, const MelBands& bands, int n_mels) {
   for (int i = threadIdx.x; i < NFFT; i += blockDim.x) {
     sm.tw[i] = make_float2(g_tw_re[i], g_tw_im[i]);
     sm.window[i] = g_window[i];
   }
-  for (int i = threadIdx.x; i < MAX_TAPS; i += blockDim.x) sm.mel_w[i] = g_mel_w[i];
   for (int i = threadIdx.x; i < MAX_MELS; i += blockDim.x) {
-    sm.mel_lo[i] = g_mel_lo[i];
-    sm.mel_len[i] = i < n_mels ? g_mel_len[i] : 0;
-    sm.mel_off[i] = g_mel_off[i];
+    sm.mel_lo[i] = bands.lo[i];
+    sm.mel_len[i] = i < n_mels ? bands.len[i] : 0;
+    sm.mel_off[i] = bands.off[i];
+  }
+  __syncthreads();
+  // one independent load per packed weight: weight i belongs to the last row m with off[m] <= i (rows are packed in order)
+  for (int i = threadIdx.x; i < bands.taps; i += blockDim.x) {
+    int m = 0;
+    for (int step = MAX_MELS / 2; step > 0; step >>= 1)
+      if (m + step < n_mels && sm.mel_off[m + step] <= i) m += step;
+    sm.mel_w[i] = __ldg(basis + (size_t)m * NBINS + sm.mel_lo[m] + (i - sm.mel_off[m]));
   }
   __syncthreads();
 }
@@ -338,13 +303,14 @@ __device__ __forceinline__ void mel_pair(const StftSmem2& sm, float2* buf, int l
 }
 
 __global__ void __launch_bounds__(V2_WARPS * 32, 2)
-stft_mel_v2_kernel(const float* __restrict__ wav, int n_samples, int n_frames, int pairs_per_clip, int n_items, int n_mels,
-                   int normalizer, float* __restrict__ out) {
+stft_mel_v2_kernel(const float* __restrict__ wav, int n_samples, int n_frames, int pairs_per_clip, int n_items,
+                   const float* __restrict__ basis, const __grid_constant__ MelBands bands, int n_mels, int normalizer,
+                   float* __restrict__ out) {
   extern __shared__ uint8_t smem_raw[];
   StftSmem2& sm = *reinterpret_cast<StftSmem2*>(smem_raw);
-  load_v2_tables(sm, n_mels);
+  load_v2_tables(sm, basis, bands, n_mels);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int kmax = g_mel_kmax;
+  const int kmax = bands.kmax;
   const int gw = blockIdx.x * V2_WARPS + warp, nw = gridDim.x * V2_WARPS;
   float2* buf = sm.buf[warp];
   float re[32], im[32];
@@ -373,13 +339,14 @@ __device__ __forceinline__ void load_batch_pair(const float* __restrict__ wav, c
 }
 
 __global__ void __launch_bounds__(V2_WARPS * 32, 2)
-stft_mel_batch_kernel(const float* __restrict__ wav, const int32_t* __restrict__ tab, int n_clips, int n_items, int n_mels, int normalizer,
+stft_mel_batch_kernel(const float* __restrict__ wav, const int32_t* __restrict__ tab, int n_clips, int n_items,
+                      const float* __restrict__ basis, const __grid_constant__ MelBands bands, int n_mels, int normalizer,
                       float* __restrict__ out) {
   extern __shared__ uint8_t smem_raw[];
   StftSmem2& sm = *reinterpret_cast<StftSmem2*>(smem_raw);
-  load_v2_tables(sm, n_mels);
+  load_v2_tables(sm, basis, bands, n_mels);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int kmax = g_mel_kmax;
+  const int kmax = bands.kmax;
   const int gw = blockIdx.x * V2_WARPS + warp, nw = gridDim.x * V2_WARPS;
   float2* buf = sm.buf[warp];
   const int32_t* fo = tab + (n_clips + 1);
@@ -419,18 +386,26 @@ static int init_tables() {
   return 0;
 }
 
-// the packed filterbank table is rebuilt when another basis pointer shows up (a basis is a per-Audio constant); *ok = 0 when the
-// basis is not banded enough for it
-static int pack_basis(const float* mel_basis, int n_mels, cudaStream_t stream, int* ok) {
-  static PerDevice<const float*> packed_for;
-  *ok = 1;
-  if (packed_for.get() != mel_basis) {
-    mel_pack_kernel<<<1, MAX_MELS, 0, stream>>>(mel_basis, n_mels);
-    count_launch();
-    TTSB_CUDA_OK(cudaMemcpyFromSymbolAsync(ok, g_mel_ok, sizeof(int), 0, cudaMemcpyDeviceToHost, stream));
-    TTSB_CUDA_OK(cudaStreamSynchronize(stream));
-    packed_for.get() = *ok ? mel_basis : nullptr;
+// lo / len / off / kmax of the caller's band table (n_mels, 2) int32 in host memory: band[2m], band[2m+1] = first / past-last
+// non-zero bin of row m.  Returns 0, or TTSB_ERR_INVALID_ARGUMENT for a row outside 0 <= first <= past-last <= 513.  *packed = 0
+// when the rows hold more weights than the packed table of the v2 kernels (MAX_TAPS).
+static int mel_bands(const char* who, const int32_t* band, int n_mels, MelBands* b, bool* packed) {
+  *b = MelBands{};
+  int off = 0;
+  for (int m = 0; m < n_mels; ++m) {
+    const int lo = band[2 * m], hi = band[2 * m + 1];
+    if (lo < 0 || hi < lo || hi > NBINS) {
+      set_last_error("%s: band row %d is [%d, %d); need 0 <= band[2m] <= band[2m+1] <= 513", who, m, lo, hi);
+      return TTSB_ERR_INVALID_ARGUMENT;
+    }
+    b->lo[m] = lo;
+    b->len[m] = hi - lo;
+    b->off[m] = off;
+    b->kmax = max(b->kmax, hi);
+    off += hi - lo;
   }
+  b->taps = off;
+  *packed = off <= MAX_TAPS;
   return 0;
 }
 
@@ -438,35 +413,39 @@ static int pack_basis(const float* mel_basis, int n_mels, cudaStream_t stream, i
 
 using namespace ttsb;
 
-extern "C" int ttsb_stft_mel_log(const float* wav, int n_clips, int n_samples, const float* mel_basis, int n_mels,
-                                 int normalizer, float* out, void* stream_v) {
-  if (!wav || !mel_basis || !out) { set_last_error("ttsb_stft_mel_log: NULL tensor"); return TTSB_ERR_INVALID_ARGUMENT; }
-  if (n_clips <= 0 || n_samples <= NFFT / 2 || n_mels <= 0 || n_mels > MAX_MELS || (normalizer != 0 && normalizer != 1)) {
-    set_last_error("ttsb_stft_mel_log: need n_samples > 512, 0 < n_mels <= 128, normalizer in {0,1}");
+extern "C" int ttsb_stft_mel_log(const float* wav, int n_clips, int n_samples, const float* mel_basis, const int32_t* band,
+                                 int n_mels, int normalizer, float* out, void* stream_v) {
+  if (!wav || !mel_basis || !band || !out) { set_last_error("ttsb_stft_mel_log: NULL tensor"); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (n_clips <= 0) { set_last_error("ttsb_stft_mel_log: n_clips %d; need n_clips >= 1", n_clips); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (n_samples <= NFFT / 2) {
+    set_last_error("ttsb_stft_mel_log: n_samples %d; need n_samples > 512", n_samples);
     return TTSB_ERR_INVALID_ARGUMENT;
   }
-  int rc = init_tables();
+  if (n_mels <= 0 || n_mels > MAX_MELS) { set_last_error("ttsb_stft_mel_log: n_mels %d; need 0 < n_mels <= 128", n_mels); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (normalizer != 0 && normalizer != 1) {
+    set_last_error("ttsb_stft_mel_log: normalizer %d; need normalizer in {0,1}", normalizer);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  MelBands bands;
+  bool packed;
+  int rc = mel_bands("ttsb_stft_mel_log", band, n_mels, &bands, &packed);
+  if (rc) return rc;
+  rc = init_tables();
   if (rc) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   const int n_frames = 1 + n_samples / HOP;
   const int pairs = (n_frames + 1) / 2;
   static const bool use_v1 = getenv("TTSB_STFT_V1") != nullptr;
-  if (!use_v1) {
-    int ok = 1;
-    rc = pack_basis(mel_basis, n_mels, stream, &ok);
-    if (rc) return rc;
-    if (ok) {
-      const int n_items = pairs * n_clips;
-      const int grid2 = min((n_items + V2_WARPS - 1) / V2_WARPS, 2 * num_sms());
-      stft_mel_v2_kernel<<<grid2, V2_WARPS * 32, sizeof(StftSmem2), stream>>>(wav, n_samples, n_frames, pairs, n_items, n_mels, normalizer, out);
-      count_launch();
-      return check_cuda(cudaGetLastError(), "stft_mel_v2_kernel launch");
-    }
+  if (!use_v1 && packed) {
+    const int n_items = pairs * n_clips;
+    const int grid2 = min((n_items + V2_WARPS - 1) / V2_WARPS, 2 * num_sms());
+    stft_mel_v2_kernel<<<grid2, V2_WARPS * 32, sizeof(StftSmem2), stream>>>(wav, n_samples, n_frames, pairs, n_items, mel_basis, bands,
+                                                                            n_mels, normalizer, out);
+    count_launch();
+    return check_cuda(cudaGetLastError(), "stft_mel_v2_kernel launch");
   }
-  mel_band_kernel<<<1, MAX_MELS, 0, stream>>>(mel_basis, n_mels);
-  count_launch();
   dim3 grid((pairs + STFT_WARPS - 1) / STFT_WARPS, n_clips);
-  stft_mel_kernel<<<grid, STFT_WARPS * 32, sizeof(StftSmem), stream>>>(wav, n_samples, n_frames, pairs, mel_basis, n_mels,
+  stft_mel_kernel<<<grid, STFT_WARPS * 32, sizeof(StftSmem), stream>>>(wav, n_samples, n_frames, pairs, mel_basis, bands, n_mels,
                                                                         normalizer, out);
   count_launch();
   return check_cuda(cudaGetLastError(), "stft_mel_kernel launch");
@@ -486,12 +465,14 @@ extern "C" int64_t ttsb_stft_mel_log_batch_workspace_bytes(int n_clips) {
 }
 
 extern "C" int ttsb_stft_mel_log_batch(const float* wav, const int32_t* sample_offsets, const int32_t* frame_offsets, int n_clips,
-                                       const float* mel_basis, int n_mels, int normalizer, void* workspace, int64_t workspace_bytes,
-                                       float* out, void* stream_v) {
-  if (!wav || !sample_offsets || !frame_offsets || !mel_basis || !workspace || !out)
+                                       const float* mel_basis, const int32_t* band, int n_mels, int normalizer, void* workspace,
+                                       int64_t workspace_bytes, float* out, void* stream_v) {
+  if (!wav || !sample_offsets || !frame_offsets || !mel_basis || !band || !workspace || !out)
     return mel_batch_bad("ttsb_stft_mel_log_batch: NULL pointer");
-  if (n_clips < 1 || n_mels <= 0 || n_mels > MAX_MELS || (normalizer != 0 && normalizer != 1))
-    return mel_batch_bad("ttsb_stft_mel_log_batch: need n_clips >= 1, 0 < n_mels <= 128, normalizer in {0,1}");
+  if (n_clips < 1) return mel_batch_bad("ttsb_stft_mel_log_batch: n_clips %lld; need n_clips >= 1", n_clips);
+  if (n_mels <= 0 || n_mels > MAX_MELS) return mel_batch_bad("ttsb_stft_mel_log_batch: n_mels %lld; need 0 < n_mels <= 128", n_mels);
+  if (normalizer != 0 && normalizer != 1)
+    return mel_batch_bad("ttsb_stft_mel_log_batch: normalizer %lld; need normalizer in {0,1}", normalizer);
   if (workspace_bytes < ttsb_stft_mel_log_batch_workspace_bytes(n_clips))
     return mel_batch_bad("ttsb_stft_mel_log_batch: workspace too small (ttsb_stft_mel_log_batch_workspace_bytes)");
   if (reinterpret_cast<uintptr_t>(workspace) % 4 != 0) return mel_batch_bad("ttsb_stft_mel_log_batch: workspace must be 4-byte aligned");
@@ -514,21 +495,22 @@ extern "C" int ttsb_stft_mel_log_batch(const float* wav, const int32_t* sample_o
     fo[c + 1] = frame_offsets[c + 1];
     po[c + 1] = (int32_t)p;
   }
-  int rc = init_tables();
+  MelBands bands;
+  bool packed;
+  int rc = mel_bands("ttsb_stft_mel_log_batch", band, n_mels, &bands, &packed);
   if (rc) return rc;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  int ok = 1;
-  rc = pack_basis(mel_basis, n_mels, stream, &ok);
-  if (rc) return rc;
-  if (!ok) {
-    set_last_error("ttsb_stft_mel_log_batch: the mel basis has more non-zero weights than the packed table holds (%d)", MAX_TAPS);
+  if (!packed) {
+    set_last_error("ttsb_stft_mel_log_batch: the band table spans more mel weights than the packed filterbank holds (%d)", MAX_TAPS);
     return TTSB_ERR_UNSUPPORTED;
   }
+  rc = init_tables();
+  if (rc) return rc;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   TTSB_CUDA_OK(cudaMemcpyAsync(workspace, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
   const int n_items = (int)p;
   const int grid = min((n_items + V2_WARPS - 1) / V2_WARPS, 2 * num_sms());
   stft_mel_batch_kernel<<<grid, V2_WARPS * 32, sizeof(StftSmem2), stream>>>(wav, static_cast<const int32_t*>(workspace), n_clips, n_items,
-                                                                             n_mels, normalizer, out);
+                                                                             mel_basis, bands, n_mels, normalizer, out);
   count_launch();
   return check_cuda(cudaGetLastError(), "stft_mel_batch_kernel launch");
 }

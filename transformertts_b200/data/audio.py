@@ -48,6 +48,15 @@ def slaney_mel_basis(sr: int, n_fft: int, n_mels: int, fmin: float, fmax: float)
     return basis.astype(np.float32)
 
 
+def mel_band(basis: np.ndarray) -> np.ndarray:
+    """Band table of a mel basis (n_mels, n_bins) -> int32 (n_mels, 2): first / past-last bin of each row's non-zero weights,
+    (0, 0) for a row of zeros."""
+    nz = np.asarray(basis) != 0
+    first = np.argmax(nz, axis=1)
+    past_last = nz.shape[1] - np.argmax(nz[:, ::-1], axis=1)
+    return np.where(nz.any(axis=1)[:, None], np.stack([first, past_last], axis=1), 0).astype(np.int32)
+
+
 def kaiser_best_half_window() -> np.ndarray:
     """resampy's `kaiser_best` interpolation filter (the one librosa.load(sr=...) uses at its default res_type), restated from its
     published parameters: the right half of rolloff * sinc(rolloff * z) * kaiser(2n + 1, beta), z = linspace(0, 64, n + 1),
@@ -176,9 +185,15 @@ class Audio:
 
     def _mel_basis(self) -> torch.Tensor:
         if self._basis is None:
-            self._basis = torch.from_numpy(slaney_mel_basis(self.sampling_rate, self.n_fft, self.mel_channels, self.f_min,
-                                                            self.f_max)).to(self.device).contiguous()
+            basis = slaney_mel_basis(self.sampling_rate, self.n_fft, self.mel_channels, self.f_min, self.f_max)
+            self._band = mel_band(basis)
+            self._basis = torch.from_numpy(basis).to(self.device).contiguous()
         return self._basis
+
+    def _mel_band(self) -> np.ndarray:
+        """Band table (n_mels, 2) int32 of the mel basis in host memory, as the fused log-mel kernels take it."""
+        self._mel_basis()
+        return self._band
 
     def mel_spectrogram_device(self, wav: torch.Tensor) -> torch.Tensor:
         with torch.cuda.device(self.device):
@@ -189,7 +204,7 @@ class Audio:
         n_clips, n_samples = wav.shape
         out = torch.empty((n_clips, 1 + n_samples // self.hop_length, self.mel_channels), dtype=torch.float32, device=wav.device)
         if self._reference_stft:
-            lib.stft_mel_log(wav.contiguous(), self._mel_basis(), self.normalizer.code, out)
+            lib.stft_mel_log(wav.contiguous(), self._mel_basis(), self._mel_band(), self.normalizer.code, out)
         else:
             so = np.arange(n_clips + 1, dtype=np.int64) * n_samples
             fo = np.arange(n_clips + 1, dtype=np.int64) * out.shape[1]
@@ -204,10 +219,7 @@ class Audio:
         if getattr(self, '_inv', None) is None:
             A = slaney_mel_basis(self.sampling_rate, self.n_fft, self.mel_channels, self.f_min, self.f_max).astype(np.float64)
             nz = A != 0
-            band = np.zeros((A.shape[0], 2), dtype=np.int32)
-            for j in range(A.shape[0]):
-                idx = np.nonzero(nz[j])[0]
-                band[j] = (idx[0], idx[-1] + 1) if len(idx) else (0, 0)
+            band = mel_band(A)
             bins = np.zeros((A.shape[1], 2), dtype=np.int32)
             for k in range(A.shape[1]):
                 idx = np.nonzero(nz[:, k])[0]
@@ -361,7 +373,7 @@ class Audio:
             fo = np.concatenate([[0], np.cumsum(self._frames_per_clip(np.diff(so)))])
             out = torch.empty((int(fo[-1]), self.mel_channels), dtype=torch.float32, device=self.device)
             if self._reference_stft:
-                lib.stft_mel_log_batch(wav.contiguous(), so, fo, self._mel_basis(), self.normalizer.code, out)
+                lib.stft_mel_log_batch(wav.contiguous(), so, fo, self._mel_basis(), self._mel_band(), self.normalizer.code, out)
             else:
                 lib.stft_mel_log_ragged(wav.contiguous(), so, fo, self.n_fft, self.hop_length, self.win_length, self._mel_basis(),
                                         self._inverse_tables()['band'], self.normalizer.code, out)

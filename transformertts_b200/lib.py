@@ -324,10 +324,27 @@ def phoneme_lengths(ph, padding, out):
     _check(load().ttsb_phoneme_lengths(ptr(ph), B, T, int(padding), ptr(out), _stream()), 'ttsb_phoneme_lengths')
 
 
-def stft_mel_log(wav, mel_basis, normalizer, out):
+def _host_band(band, n_mels: int):
+    """int32 (n_mels, 2) band table in host memory (numpy or a CPU tensor) -> (the array, a pointer to its data, valid for as long
+    as the array lives)."""
+    import numpy as np
+    if torch.is_tensor(band):
+        if band.is_cuda:
+            raise TtsbError('band must be a host table (numpy or a CPU tensor); a device tensor would cost a synchronisation')
+        band = band.numpy()
+    a = np.ascontiguousarray(band, dtype=np.int32)
+    if a.shape != (n_mels, 2):
+        raise TtsbError(f'band must be ({n_mels}, 2), got {a.shape}')
+    return a, C.c_void_p(a.ctypes.data)
+
+
+def stft_mel_log(wav, mel_basis, band, normalizer, out):
+    """Log-mel of equal-length clips (include/ttsb.h: ttsb_stft_mel_log).  wav fp32 (n_clips, n_samples), mel_basis fp32
+    (n_mels, 513) and out fp32 (n_clips, 1 + n_samples // 256, n_mels) on the device; band int32 (n_mels, 2) in host memory."""
     n_clips, n_samples = wav.shape
     n_mels = mel_basis.shape[0]
-    _check(load().ttsb_stft_mel_log(ptr(wav), n_clips, n_samples, ptr(mel_basis), n_mels, int(normalizer), ptr(out),
+    keep, bp = _host_band(band, n_mels)
+    _check(load().ttsb_stft_mel_log(ptr(wav), n_clips, n_samples, ptr(mel_basis), bp, n_mels, int(normalizer), ptr(out),
                                     _stream()), 'ttsb_stft_mel_log')
 
 
@@ -340,9 +357,9 @@ def _host_offsets(offsets):
     return (C.c_int32 * len(a))(*a.tolist()), len(a) - 1
 
 
-def stft_mel_log_batch(wav, sample_offsets, frame_offsets, mel_basis, normalizer, out):
+def stft_mel_log_batch(wav, sample_offsets, frame_offsets, mel_basis, band, normalizer, out):
     """Log-mel of a packed ragged batch (include/ttsb.h: ttsb_stft_mel_log_batch).  wav fp32 (total_samples,) and out fp32
-    (total_frames, n_mels) on the device; the offset tables (n_clips + 1) are host sequences."""
+    (total_frames, n_mels) on the device; the offset tables (n_clips + 1) and band int32 (n_mels, 2) are host tables."""
     so, n = _host_offsets(sample_offsets)
     fo, n_f = _host_offsets(frame_offsets)
     if n_f != n:
@@ -350,8 +367,9 @@ def stft_mel_log_batch(wav, sample_offsets, frame_offsets, mel_basis, normalizer
     nb = int(load().ttsb_stft_mel_log_batch_workspace_bytes(n))
     if nb < 0:
         raise TtsbError(load().ttsb_last_error().decode())
+    keep, bp = _host_band(band, mel_basis.shape[0])
     ws = torch.empty(nb, dtype=torch.uint8, device=wav.device)
-    _check(load().ttsb_stft_mel_log_batch(ptr(wav), so, fo, n, ptr(mel_basis), mel_basis.shape[0], int(normalizer), ptr(ws),
+    _check(load().ttsb_stft_mel_log_batch(ptr(wav), so, fo, n, ptr(mel_basis), bp, mel_basis.shape[0], int(normalizer), ptr(ws),
                                           C.c_int64(nb), ptr(out), _stream()), 'ttsb_stft_mel_log_batch')
 
 
