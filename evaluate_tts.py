@@ -5,6 +5,7 @@
     python evaluate_tts.py --config CFG -p WEIGHTS_DIR --weights_glob 'step_*'          # every checkpoint, in step order
     python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder melgan --vocoder_checkpoint melgan.pt
     python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder hifigan --vocoder_checkpoint g_02500000 [--vocoder_config v1]
+    python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder wavernn --vocoder_checkpoint latest_weights.pyt
 
 The validation split is read as train_tts.py reads it (``valid_metadata``, ``mels``, ``durations`` and ``char_pitch`` of the
 config's data directory; ``pitch_stats.pkl`` for pitch errors in Hz when it exists).  For every checkpoint:
@@ -33,12 +34,12 @@ def parse_args(argv=None):
     parser.add_argument('--weights_glob', default=None, type=str, help="checkpoint directories under --path, e.g. 'step_*'")
     parser.add_argument('--outdir', '-o', dest='outdir', default=None, type=str)
     parser.add_argument('--n_ceps', default=24, type=int)
-    parser.add_argument('--vocoder', default=None, choices=('griffinlim', 'melgan', 'hifigan'))
+    parser.add_argument('--vocoder', default=None, choices=('griffinlim', 'melgan', 'hifigan', 'wavernn'))
     parser.add_argument('--vocoder_checkpoint', default=None, type=str)
     parser.add_argument('--vocoder_config', default=None, type=str,
                         help='HiFi-GAN config: a config.json path or v1 / v2 / v3 (default: config.json beside the checkpoint)')
     args = parser.parse_args(argv)
-    if args.vocoder in ('melgan', 'hifigan') and args.vocoder_checkpoint is None:
+    if args.vocoder in ('melgan', 'hifigan', 'wavernn') and args.vocoder_checkpoint is None:
         parser.error(f'--vocoder {args.vocoder} needs --vocoder_checkpoint PATH')
     if args.vocoder_config is not None and args.vocoder != 'hifigan':
         parser.error('--vocoder_config applies to --vocoder hifigan only')
@@ -59,7 +60,7 @@ def checkpoints(path: Path, pattern):
 def main(argv=None):
     args = parse_args(argv)
     import yaml
-    from predict_tts import VOCODE_CHUNK, load_vocoder
+    from predict_tts import VOCODE_CHUNK, load_vocoder, vocode_chunk
     from transformertts_b200.data.audio import Audio
     from transformertts_b200.model.models import ForwardTransformer
     from transformertts_b200.utils import evaluation as ev
@@ -86,7 +87,7 @@ def main(argv=None):
                 wavs = []
                 for start in range(0, len(mels), VOCODE_CHUNK):
                     part = [m.T for m in mels[start:start + VOCODE_CHUNK]]
-                    wavs.extend(audio.reconstruct_waveform_batch(part, seed=start) if vocoder is None else vocoder.vocode_batch(part))
+                    wavs.extend(vocode_chunk(vocoder, audio, part, start))
                 return wavs
         res = ev.evaluate_model(model, vs, n_ceps=args.n_ceps, vocode=vocode, audio=audio)
         res = dict(checkpoint=str(ckpt), step=int(step), **res)

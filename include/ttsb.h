@@ -730,6 +730,54 @@ int ttsb_conv1d_out_tanh_ex(const void* in_hi, const void* in_lo, int ld_in, int
                             float* wav_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * WaveRNN generator (fatchord/WaveRNN, transformertts_b200/model/wavernn.py): the sample-rate recurrence of every fold of
+ * every clip in one persistent cooperative launch, then the fold crossfade, crop to (T_c - 1) hop samples and the fade-out
+ * over the last 20 hop samples (csrc/wavernn.cu).  rnn_dims = fc_dims = TTSB_WAVERNN_DIMS; aux parts of 32 columns.
+ * Folds: batched, clip c of T_c frames is cut as fatchord's fold_with_overlap cuts T_c hop samples (fold length target +
+ *   2 overlap, stride target + overlap, the last fold zero-padded); otherwise one fold per clip runs max_c T_c hop steps.
+ *   n_rows is the caller's fold count, checked against that rule.  Clip c's folds use seeds[c] (host uint32) and draw
+ *   uniforms keyed by (seeds[c], fold index, step, draw): 11 per step in MOL, 1 in RAW, as oracle/wavernn_oracle.py states.
+ * Conditioning, bf16 hi (+ lo in bf16x3) planes in the ragged layout of ttsb_conv1d_ex_tc (frames as rows, cond_halo rows on
+ *   each side of every clip, cond_rows in all; the halo rows of melp are zero):
+ *   melp (ld_melp >= 2048): per mel frame, columns [0, 512) its projection onto I's mel columns, [512, 2048) onto W_ih1 I_mel.
+ *   aux (ld_aux >= 4608): per frame, [0, 512) a1 onto I, [512, 2048) a1 onto W_ih1 I, [2048, 3584) a2 onto rnn2's input
+ *   weights, [3584, 4096) a3 onto fc1, [4096, 4608) a4 onto fc2 (no biases).
+ *   Sample n of a clip (frame f = n / hop, phase p = n % hop) adds aux[f] + sum_j taps[p][j] melp[f + j - n_taps / 2];
+ *   samples past T_c hop add nothing (the biases stay).
+ * taps: device fp32 (hop, n_taps), n_taps odd <= TTSB_WAVERNN_MAX_TAPS <= 2 cond_halo + 1.
+ * vec: device fp32, [0, 512) I's x_prev column, [512, 1024) I's bias, [1024, 2560) W_ih1 I_0, [2560, 4096) W_ih1 b_I + b_ih1,
+ *   [4096, 5632) b_hh1, [5632, 7168) b_ih2, [7168, 8704) b_hh2, [8704, 9216) fc1 bias, [9216, 9728) fc2 bias, then fc3's.
+ * weights: device, (5632 + n_classes) rows of 512, row-major, fp32 in TTSB_PREC_BF16X3 (fp32 products) and bf16 in
+ *   TTSB_PREC_BF16 (bf16 products of bf16-rounded activations, fp32 sums): rows [0, 1536) W_hh1, [1536, 3072) rnn2's
+ *   W_ih[:, :512], [3072, 4608) W_hh2, [4608, 5120) fc1[:, :512], [5120, 5632) fc2[:, :512], then fc3.
+ * mode TTSB_WAVERNN_MOL (n_classes 30) or TTSB_WAVERNN_RAW (n_classes 2^bits, 8 <= bits <= 10; mu-law decoded).
+ * wav_out: device fp32, sum_c (T_c - 1) hop samples, clip after clip.  Every T_c >= TTSB_WAVERNN_MIN_FRAMES.
+ * capture: NULL, or device fp32 (n_rows, capture_steps, n_classes): the logits of each fold's first capture_steps steps.
+ * samples_out: NULL, or device fp32 (n_rows, steps): each fold's samples before the crossfade.
+ * timings: NULL, or device int64 (TTSB_WAVERNN_CTAS, 12): per CTA, for the six segments of a step (sampling, GRU1, GRU2, fc1,
+ *   fc2, fc3), the nanoseconds summed over all steps from the segment's start to its last warp finishing, then through the
+ *   grid barrier after it (%globaltimer; the timed run adds a CTA barrier per segment).
+ * workspace: ttsb_wavernn_workspace_bytes(...) bytes, 256-byte aligned.  A row's arithmetic does not depend on the other
+ * rows, its place or the grid, so a clip's waveform is bit-identical in any batch.  Bad arguments give
+ * TTSB_ERR_INVALID_ARGUMENT before any CUDA call; a device that cannot hold the grid resident gives TTSB_ERR_UNSUPPORTED.
+ * ------------------------------------------------------------------------------------------------------- */
+#define TTSB_WAVERNN_DIMS 512
+#define TTSB_WAVERNN_MOL 0
+#define TTSB_WAVERNN_RAW 1
+#define TTSB_WAVERNN_MAX_TAPS 7
+#define TTSB_WAVERNN_MIN_FRAMES 21
+#define TTSB_WAVERNN_MAX_ROWS 8192
+#define TTSB_WAVERNN_CTAS 128
+int64_t ttsb_wavernn_workspace_bytes(const int32_t* frames, int n_clips, int hop, int batched, int target, int overlap,
+                                     int n_classes); /* -1: invalid */
+int ttsb_wavernn_generate(const int32_t* frames /* HOST (n_clips) */, const uint32_t* seeds /* HOST (n_clips) */, int n_clips, int hop,
+                          int batched, int target, int overlap, int n_rows, int n_taps, const float* taps, const void* melp_hi,
+                          const void* melp_lo, int ld_melp, const void* aux_hi, const void* aux_lo, int ld_aux, int cond_halo,
+                          int64_t cond_rows, const float* vec, const void* weights, int mode, int n_classes, int precision,
+                          float* wav_out, float* capture, int capture_steps, float* samples_out, int64_t* timings,
+                          void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Data-parallel gradient exchange (BASELINE.json: "NCCL allreduce over NVLink on gradient buckets only"; the reference has
  * no distributed code).  One communicator per process / GPU.  NCCL is loaded at run time (libnccl.so.2 of the host
  * process, or $TTSB_NCCL_LIB); without it these return TTSB_ERR_UNSUPPORTED.

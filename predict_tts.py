@@ -5,6 +5,7 @@
     python predict_tts.py -t "phoneme string" ...
     python predict_tts.py -f lines.txt --vocoder melgan --vocoder_checkpoint melgan.pt ...
     python predict_tts.py -f lines.txt --vocoder hifigan --vocoder_checkpoint g_02500000 [--vocoder_config v1|config.json] ...
+    python predict_tts.py -f lines.txt --vocoder wavernn --vocoder_checkpoint latest_weights.pyt ...
 
 Every input line is tokenised and the lines are turned into mels by ``ForwardTransformer.predict_batch`` (sorted by length,
 a padded batch per forward pass; each mel is bit for bit what ``predict`` gives the line alone, which is how the reference
@@ -15,7 +16,10 @@ reference's synthesis notebook does one line at a time; a line of T frames then 
 256 (T - 1)).  With ``--vocoder hifigan`` they go through a HiFi-GAN generator (``HiFiGANGenerator.vocode_batch``, a
 jik876/hifi-gan checkpoint; its config is ``--vocoder_config``, a config.json path or v1 / v2 / v3, by default the
 config.json beside the checkpoint), also 256 T samples per line; HiFi-GAN takes the MelGAN normaliser's log-mels, so a
-model with another ``normalizer`` is refused.  Output:
+model with another ``normalizer`` is refused.  With ``--vocoder wavernn`` they go through a fatchord/WaveRNN generator
+(``WaveRNNGenerator.vocode_batch``, batched folds of 11000 + 2 550 samples), line i sampled with seed i; its hop is the
+product of its upsample factors and must equal the model's, the model must use the ``WaveRNN`` normaliser, a line of T
+frames gives 275 (T - 1) samples at hop 275, and a line below 21 frames is refused.  Output:
 ``<outdir>/outputs/<fname>/<fname>_<data_name>_<git_hash>_<step>.wav``, the concatenation of all lines; with ``--single`` also
 ``..._<i>.wav`` per line, with ``--store_mel`` ``..._<i>.mel.npy`` (the (T, n_mels) mel of line i).
 
@@ -49,12 +53,12 @@ def parse_args(argv=None):
     parser.add_argument('--store_mel', '-m', dest='store_mel', action='store_true')
     parser.add_argument('--verbose', '-v', dest='verbose', action='store_true')
     parser.add_argument('--single', '-s', dest='single', action='store_true')
-    parser.add_argument('--vocoder', dest='vocoder', default='griffinlim', choices=('griffinlim', 'melgan', 'hifigan'))
+    parser.add_argument('--vocoder', dest='vocoder', default='griffinlim', choices=('griffinlim', 'melgan', 'hifigan', 'wavernn'))
     parser.add_argument('--vocoder_checkpoint', dest='vocoder_checkpoint', default=None, type=str)
     parser.add_argument('--vocoder_config', dest='vocoder_config', default=None, type=str,
                         help='HiFi-GAN config: a config.json path or v1 / v2 / v3 (default: config.json beside the checkpoint)')
     args = parser.parse_args(argv)
-    if args.vocoder in ('melgan', 'hifigan') and args.vocoder_checkpoint is None:
+    if args.vocoder in ('melgan', 'hifigan', 'wavernn') and args.vocoder_checkpoint is None:
         parser.error(f'--vocoder {args.vocoder} needs --vocoder_checkpoint PATH')
     if args.vocoder_config is not None and args.vocoder != 'hifigan':
         parser.error('--vocoder_config applies to --vocoder hifigan only')
@@ -132,7 +136,32 @@ def load_vocoder(name: str, checkpoint, config, model):
                              f'is {normalizer!r}, whose mels HiFi-GAN would misread')
         from transformertts_b200.model.hifigan import HiFiGANGenerator
         return HiFiGANGenerator.from_checkpoint(checkpoint, config=config, device=model.device)
+    if name == 'wavernn':
+        normalizer = model.config.get('normalizer')
+        if normalizer != 'WaveRNN':
+            raise SystemExit(f'--vocoder wavernn takes the WaveRNN normaliser\'s mels; this model\'s normalizer is {normalizer!r}')
+        from transformertts_b200.model.wavernn import WaveRNNGenerator
+        g = WaveRNNGenerator.from_checkpoint(checkpoint, device=model.device)
+        hop = int(model.config['hop_length'])
+        if g.hop != hop:
+            raise SystemExit(f'--vocoder wavernn: the generator upsamples each mel frame to {g.hop} samples, but the audio settings '
+                             f'have hop_length {hop}')
+        return g
     return None
+
+
+def vocode_chunk(vocoder, audio, mels, start: int):
+    """Waveforms of the (n_mels, T) mels of lines start, start + 1, ...: Griffin-Lim (vocoder None) and WaveRNN draw line i
+    with seed i."""
+    if vocoder is None:
+        return audio.reconstruct_waveform_batch(mels, seed=start)
+    from transformertts_b200.model.wavernn import MIN_FRAMES, WaveRNNGenerator
+    if isinstance(vocoder, WaveRNNGenerator):
+        for j, m in enumerate(mels):
+            if m.shape[1] < MIN_FRAMES:
+                raise ValueError(f'line {start + j} gives a mel of {m.shape[1]} frames; the WaveRNN vocoder needs at least {MIN_FRAMES}')
+        return vocoder.vocode_batch(mels, seeds=range(start, start + len(mels)))
+    return vocoder.vocode_batch(mels)
 
 
 def main(argv=None):
@@ -167,10 +196,7 @@ def main(argv=None):
             mels.append(mel)
             if args.store_mel:
                 np.save(line_paths(outdir, file_name, i)[1], mel)
-        if vocoder is None:
-            chunk = audio.reconstruct_waveform_batch([m.T for m in mels], seed=start)
-        else:
-            chunk = vocoder.vocode_batch([m.T for m in mels])
+        chunk = vocode_chunk(vocoder, audio, [m.T for m in mels], start)
         for j, wav in enumerate(chunk):
             if args.single:
                 audio.save_wav(wav, line_paths(outdir, file_name, start + j)[0])

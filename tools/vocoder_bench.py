@@ -2,6 +2,7 @@
 
     python tools/vocoder_bench.py [--clips 64] [--reps 3] [--out DIR]
     python tools/vocoder_bench.py --vocoder hifigan [--config v1|v2|v3] [--clips 64] [--reps 3] [--out DIR]
+    python tools/vocoder_bench.py --vocoder wavernn [--clips 64] [--reps 3] [--out DIR]
 
 Workload: that of tools/synth_bench.py -- `--clips` seeded ragged clips of 2-10 s (T_c uniform in 173..862 frames), mels from
 the CUDA front end (Audio.mel_spectrogram) -- and a seeded generator checkpoint (oracle/melgan_oracle.py, seed 0).  Paths:
@@ -19,7 +20,17 @@ path, and the card name and power limit read in the same run.  `--out` also writ
 With `--vocoder hifigan` the same clips go through a seeded HiFi-GAN generator of `--config` (oracle/hifigan_oracle.py,
 seed 0), without pad frames.  Paths: `module`, jik876's generator as a torch module in fp32 on the GPU (cuDNN, TF32 off), one
 clip per call as its inference.py runs it; `bf16x3` and `bf16`, HiFiGANGenerator.vocode_batch with all clips in one call.
-FLOPs count the useful products of every conv (a transposed conv's output row sums 2 of its k taps per input channel)."""
+FLOPs count the useful products of every conv (a transposed conv's output row sums 2 of its k taps per input channel).
+
+With `--vocoder wavernn` the workload is `--clips` seeded ragged clips of 1-10 s (T_c uniform in 81..802 frames at hop 275,
+22050 Hz) of WaveRNN-normalised mels (oracle/wavernn_oracle.make_mels), then one 10 s clip alone, through a seeded MOL
+generator at fatchord's defaults (target 11000, overlap 550, batched).  Paths: `torch`, fatchord's generate() loop (I, two
+GRU cells, fc1-fc3, the MOL draw) as a torch fp32 module on the GPU, eager, TF32 off, over the same folds as one batch (the
+folds of every clip together: fatchord runs one clip per call, which would only be slower); `bf16x3` and `bf16`,
+WaveRNNGenerator.vocode_batch.  Reported: seconds per call (each path `--reps` calls after one untimed), audio seconds per second, microseconds per step (call time over
+target + 2 overlap steps), library launches, GFLOP per second of audio from the shapes (the recurrence: 2 x 3.83 M
+multiply-adds per sample, as the generator computes every sample of every fold), and from one more call with the kernel's
+phase timers the µs per step of each segment (sampling, GRU1, GRU2, fc1, fc2, fc3): work and the grid barrier after it."""
 import argparse
 import json
 import subprocess
@@ -34,6 +45,7 @@ sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 from oracle import audio_oracle as ao  # noqa: E402
 from oracle import hifigan_oracle as ho  # noqa: E402
 from oracle import melgan_oracle as mo  # noqa: E402
+from oracle import wavernn_oracle as wo  # noqa: E402
 from transformertts_b200 import lib  # noqa: E402
 from transformertts_b200.data.audio import Audio  # noqa: E402
 from transformertts_b200.model import hifigan as hg  # noqa: E402
@@ -120,16 +132,86 @@ def hifigan_main(args, mels, lengths):
     return res
 
 
+def wavernn_torch_loop(net, fmels, target, overlap):
+    """fatchord's generate() loop in torch on the GPU, the folds of all clips as one batch (before the crossfade)."""
+    ms, auxs = [], []
+    with torch.no_grad():
+        for m in fmels:
+            m_up, aux = net.conditioning(torch.from_numpy(m).cuda()[None])
+            ms.append(wo.fold_with_overlap(m_up[None], target, overlap))
+            auxs.append(wo.fold_with_overlap(aux[None], target, overlap))
+        m_up, aux = torch.cat(ms), torch.cat(auxs)
+        cells = net._cells()
+        R, L = m_up.shape[:2]
+        h1 = torch.zeros(R, 512, device='cuda')
+        h2 = torch.zeros_like(h1)
+        x = torch.zeros(R, 1, device='cuda')
+        out = []
+        for i in range(L):
+            logits, h1, h2 = net.step_logits(cells, x, m_up[:, i], aux[:, i], h1, h2)
+            u = torch.empty(R, 10, device='cuda').uniform_(1e-5, 1 - 1e-5)
+            k = (logits[:, :10] - torch.log(-torch.log(u))).argmax(1, keepdim=True)
+            mu, ls = logits[:, 10:20].gather(1, k), logits[:, 20:30].gather(1, k).clamp(min=wo.LOG_SCALE_MIN)
+            u = torch.empty_like(mu).uniform_(1e-5, 1 - 1e-5)
+            x = (mu + torch.exp(ls) * (torch.log(u) - torch.log(1. - u))).clamp(-1, 1)
+            out.append(x)
+        return torch.cat(out, 1).cpu()
+
+
+def wavernn_phases(g, fm, steps):
+    """One more call with the kernel's phase timers on (a separate run: the timers add a CTA barrier per segment) -> per
+    segment of a step, µs per step: work (mean and slowest CTA, to the CTA's last warp) and the grid barrier after it (mean)."""
+    tim = torch.zeros((lib.WAVERNN_CTAS, 2 * len(lib.WAVERNN_SEGMENTS)), dtype=torch.int64, device='cuda')
+    g._generate(fm, None, True, wo.TARGET, wo.OVERLAP, timings=tim)
+    t = tim.cpu().numpy().astype(np.float64) / 1e3 / steps
+    out = {seg: dict(work=round(float(t[:, 2 * i].mean()), 1), work_max=round(float(t[:, 2 * i].max()), 1),
+                     barrier=round(float(t[:, 2 * i + 1].mean()), 1)) for i, seg in enumerate(lib.WAVERNN_SEGMENTS)}
+    out['total'] = round(float(t.sum(1).mean()), 1)
+    return out
+
+
+def wavernn_main(args):
+    rng = np.random.default_rng(2024)
+    sets = {'batch': [int(T) for T in rng.integers(81, 803, size=args.clips)], 'single': [802]}
+    sd = wo.init_state_dict(seed=0)
+    net = wo.build(sd).float().cuda()
+    from transformertts_b200.model import wavernn as wrn
+    res = dict(workload='wavernn_vocode', target=wo.TARGET, overlap=wo.OVERLAP, reps=args.reps)
+    steps = wo.TARGET + 2 * wo.OVERLAP
+    macs = 3.83e6   # I (rank-1 x_prev column and conditioning), rnn1, rnn2, fc1-fc3 per sample: 2 x 3.83 M FLOP
+    for name, lengths in sets.items():
+        mels = wo.make_mels(lengths, seed=7)
+        fm = [wo.to_fatchord(m).astype(np.float32) for m in mels]
+        rows, _ = wrn.fold_rows(lengths, 275, True, wo.TARGET, wo.OVERLAP)
+        audio_s = 275 * (sum(lengths) - len(lengths)) / 22050
+        r = dict(clips=len(lengths), frames=sum(lengths), folds=len(rows), audio_s=round(audio_s, 1),
+                 gflop_per_audio_s=round(2 * macs * len(rows) * steps / 1e9 / audio_s, 1))
+        t, _, _ = timed(lambda: wavernn_torch_loop(net, fm, wo.TARGET, wo.OVERLAP), args.reps)
+        r.update(torch_s=round(t, 3), torch_audio_s_per_s=round(audio_s / t, 1), torch_us_per_step=round(t / steps * 1e6, 1))
+        for prec in ('bf16x3', 'bf16'):
+            g = wrn.WaveRNNGenerator(device='cuda', precision=prec).load_state_dict(sd)
+            t, launches, _ = timed(lambda: g.vocode_batch(mels), args.reps)
+            r.update({f'{prec}_s': round(t, 3), f'{prec}_audio_s_per_s': round(audio_s / t, 1),
+                      f'{prec}_us_per_step': round(t / steps * 1e6, 1), f'{prec}_launches': launches,
+                      f'{prec}_tflops': round(2 * macs * len(rows) * steps / t / 1e12, 2)})
+            r[f'{prec}_phases_us_per_step'] = wavernn_phases(g, fm, steps)
+            del g
+        res[name] = r
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--clips', type=int, default=64)
     ap.add_argument('--reps', type=int, default=3)
     ap.add_argument('--out', default=None)
-    ap.add_argument('--vocoder', choices=('melgan', 'hifigan'), default='melgan')
+    ap.add_argument('--vocoder', choices=('melgan', 'hifigan', 'wavernn'), default='melgan')
     ap.add_argument('--config', default='v1', help='HiFi-GAN config: v1 / v2 / v3 or a config.json path')
     args = ap.parse_args()
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
+    if args.vocoder == 'wavernn':
+        return report(wavernn_main(args), args)
     audio = Audio(sampling_rate=22050, n_fft=1024, mel_channels=80, hop_length=256, win_length=1024, f_min=0, f_max=8000,
                   normalizer='MelGAN')
     lengths = np.random.default_rng(2024).integers(173, 863, size=args.clips)

@@ -39,6 +39,7 @@ EXPORTS = [
     'ttsb_stft_mel_log_ragged_workspace_bytes', 'ttsb_stft_mel_log_ragged', 'ttsb_mel_to_linear_ex',
     'ttsb_stft_complex_ragged_workspace_bytes', 'ttsb_stft_complex_ragged', 'ttsb_istft_ragged_workspace_bytes', 'ttsb_istft_ragged',
     'ttsb_griffinlim_ragged_workspace_bytes', 'ttsb_griffinlim_ragged',
+    'ttsb_wavernn_workspace_bytes', 'ttsb_wavernn_generate',
 ]
 
 
@@ -164,6 +165,9 @@ def load() -> C.CDLL:
                                       C.c_void_p]
     lib.ttsb_griffinlim_ragged.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                            C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.ttsb_wavernn_workspace_bytes.restype = C.c_int64
+    lib.ttsb_wavernn_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
+    lib.ttsb_wavernn_generate.argtypes = [t for _, t in WAVERNN_PARAMS] + [C.c_void_p]
     for name in EXPORTS:
         if not hasattr(lib, name):
             raise TtsbError(f'libttsb.so does not export {name}')
@@ -808,3 +812,47 @@ def conv1d_out_tanh_ex(in_hi, in_lo, channels, halo, clip_offsets, drop_tail, we
                                           ptr(weight), C.c_float(bias), ptr(workspace),
                                           C.c_int64(workspace.numel() * workspace.element_size()), ptr(wav_out), _stream()),
            'ttsb_conv1d_out_tanh_ex')
+
+
+# ------------------------------------------------------------------------------------------------------------
+# WaveRNN generator (include/ttsb.h: ttsb_wavernn_generate)
+# ------------------------------------------------------------------------------------------------------------
+WAVERNN_DIMS = 512
+WAVERNN_MOL, WAVERNN_RAW = 0, 1
+WAVERNN_MAX_TAPS = 7
+WAVERNN_MIN_FRAMES = 21
+WAVERNN_CTAS = 128
+WAVERNN_SEGMENTS = ('sampling', 'gru1', 'gru2', 'fc1', 'fc2', 'fc3')   # the timed segments of a step
+
+
+# ttsb_wavernn_generate's parameters in order (the stream follows)
+WAVERNN_PARAMS = (
+    ('frames', C.c_void_p), ('seeds', C.c_void_p), ('n_clips', C.c_int), ('hop', C.c_int), ('batched', C.c_int), ('target', C.c_int),
+    ('overlap', C.c_int), ('n_rows', C.c_int), ('n_taps', C.c_int), ('taps', C.c_void_p), ('melp_hi', C.c_void_p),
+    ('melp_lo', C.c_void_p), ('ld_melp', C.c_int), ('aux_hi', C.c_void_p), ('aux_lo', C.c_void_p), ('ld_aux', C.c_int),
+    ('cond_halo', C.c_int), ('cond_rows', C.c_int64), ('vec', C.c_void_p), ('weights', C.c_void_p), ('mode', C.c_int),
+    ('n_classes', C.c_int), ('precision', C.c_int), ('wav_out', C.c_void_p), ('capture', C.c_void_p), ('capture_steps', C.c_int),
+    ('samples_out', C.c_void_p), ('timings', C.c_void_p), ('workspace', C.c_void_p), ('workspace_bytes', C.c_int64),
+)
+
+
+def wavernn_workspace_bytes(frames, hop: int, batched: bool, target: int, overlap: int, n_classes: int) -> int:
+    tab = (C.c_int32 * len(frames))(*[int(f) for f in frames])
+    n = int(load().ttsb_wavernn_workspace_bytes(C.cast(tab, C.c_void_p), len(frames), int(hop), int(bool(batched)), int(target),
+                                                int(overlap), int(n_classes)))
+    if n < 0:
+        raise TtsbError(f'ttsb_wavernn_workspace_bytes: {load().ttsb_last_error().decode()}')
+    return n
+
+
+def wavernn_generate_rc(stream=None, **kw) -> int:
+    """ttsb_wavernn_generate with the parameters of WAVERNN_PARAMS by name (missing ones NULL / 0) -> its return code."""
+    unknown = set(kw) - {n for n, _ in WAVERNN_PARAMS}
+    if unknown:
+        raise TypeError(f'ttsb_wavernn_generate has no parameter {sorted(unknown)[0]}')
+    return int(load().ttsb_wavernn_generate(*[kw.get(n, None if t is C.c_void_p else 0) for n, t in WAVERNN_PARAMS], stream))
+
+
+def wavernn_generate(**kw):
+    """One WaveRNN generation (include/ttsb.h: ttsb_wavernn_generate); frames / seeds point at host tables."""
+    _check(wavernn_generate_rc(_stream(), **kw), 'ttsb_wavernn_generate')
