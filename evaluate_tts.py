@@ -6,6 +6,7 @@
     python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder melgan --vocoder_checkpoint melgan.pt
     python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder hifigan --vocoder_checkpoint g_02500000 [--vocoder_config v1]
     python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder wavernn --vocoder_checkpoint latest_weights.pyt
+    python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder melgan --vocoder_checkpoint melgan.pt --f0    # + pitch / voicing
 
 The validation split is read as train_tts.py reads it (``valid_metadata``, ``mels``, ``durations`` and ``char_pitch`` of the
 config's data directory; ``pitch_stats.pkl`` for pitch errors in Hz when it exists).  For every checkpoint:
@@ -14,7 +15,11 @@ config's data directory; ``pitch_stats.pkl`` for pitch errors in Hz when it exis
   the exact-match rate and the ratio of predicted to recorded frames, pitch RMSE over the phonemes with a target pitch != 0;
 * teacher forced (``predict_batch`` with the target durations and pitch): MCD-DTW;
 * with ``--vocoder``: the free-running mels and the recorded mels (copy synthesis: the vocoder's own floor) are vocoded, their
-  log-mels re-extracted on the GPU and scored against the recorded mel.
+  log-mels re-extracted on the GPU and scored against the recorded mel;
+* with ``--f0`` (needs ``--vocoder`` and the recorded frame pitch ``pitch.<audio>/<name>.npy`` with ``pitch_stats.pkl``): the
+  WORLD F0 of both sets of waveforms (DIO + StoneMask on the GPU, at the frame period of the training data) against the
+  recorded frame pitch along each line's MCD-DTW warping path: gross pitch error (GPE, |f / f_ref - 1| > 20 %), voicing
+  decision error (VDE), F0 frame error (FFE) and the F0 RMSE in cents.
 
 MCD is the DCT of the 80-bin natural-log mel (coefficients 1..24), not the SPTK / WORLD mel-cepstrum: compare its numbers
 with each other, not with papers (see transformertts_b200/utils/evaluation.py).  Per-line and corpus-mean values go to
@@ -38,7 +43,11 @@ def parse_args(argv=None):
     parser.add_argument('--vocoder_checkpoint', default=None, type=str)
     parser.add_argument('--vocoder_config', default=None, type=str,
                         help='HiFi-GAN config: a config.json path or v1 / v2 / v3 (default: config.json beside the checkpoint)')
+    parser.add_argument('--f0', action='store_true',
+                        help='also score the F0 and voicing of the vocoded audio against the recorded frame pitch (needs --vocoder)')
     args = parser.parse_args(argv)
+    if args.f0 and args.vocoder is None:
+        parser.error('--f0 scores vocoded audio: it needs --vocoder')
     if args.vocoder in ('melgan', 'hifigan', 'wavernn') and args.vocoder_checkpoint is None:
         parser.error(f'--vocoder {args.vocoder} needs --vocoder_checkpoint PATH')
     if args.vocoder_config is not None and args.vocoder != 'hifigan':
@@ -68,7 +77,7 @@ def main(argv=None):
 
     cm = TrainingConfigManager(args.config)
     ev.natural_log_mels(cm.config, 'config')
-    vs = ev.load_validation_set(cm)
+    vs = ev.load_validation_set(cm, frame_pitch=args.f0)
     root = Path(args.path)
     results = []
     vocoder = None
@@ -89,7 +98,7 @@ def main(argv=None):
                     part = [m.T for m in mels[start:start + VOCODE_CHUNK]]
                     wavs.extend(vocode_chunk(vocoder, audio, part, start))
                 return wavs
-        res = ev.evaluate_model(model, vs, n_ceps=args.n_ceps, vocode=vocode, audio=audio)
+        res = ev.evaluate_model(model, vs, n_ceps=args.n_ceps, vocode=vocode, audio=audio, f0=args.f0)
         res = dict(checkpoint=str(ckpt), step=int(step), **res)
         results.append(res)
         print(ev.summary_line(f'{ckpt.name} (step {step})', res), flush=True)

@@ -617,8 +617,8 @@ int ttsb_griffinlim_ragged(const float* magnitude, const float* init_angles, con
                            float* wav_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
- * Mel-cepstral distortion after dynamic time warping  (evaluate_tts.py; no reference counterpart;
- * tests/evaluation_oracle.py restates the definition in float64)
+ * Mel-cepstral distortion after dynamic time warping, and its warping path  (evaluate_tts.py, --f0 for the path; no reference
+ * counterpart; tests/evaluation_oracle.py restates the definition in float64, tests/dtw_path_oracle.py the path)
  *   A packed ragged batch of n_pairs pairs of fp32 log-mel sequences (frames, n_mels) on the device: pair p compares frames
  *   x_offsets[p] .. x_offsets[p+1] - 1 of x with frames y_offsets[p] .. y_offsets[p+1] - 1 of y (both tables int32
  *   (n_pairs + 1) in HOST memory, from 0, every sequence >= 1 frame).  With K = n_ceps (1 <= K < n_mels):
@@ -641,6 +641,22 @@ int64_t ttsb_mcd_dtw_workspace_bytes(const int32_t* x_offsets, const int32_t* y_
 int ttsb_mcd_dtw(const float* x, const int32_t* x_offsets, const float* y, const int32_t* y_offsets, int n_pairs, int n_mels,
                  const double* dct, int n_ceps, double kappa, void* workspace, int64_t workspace_bytes, double* cost_out,
                  int32_t* path_len_out, void* stream);
+/* ttsb_mcd_dtw_path: ttsb_mcd_dtw with the same arguments, definition and outputs (cost_out and path_len_out equal
+ *   ttsb_mcd_dtw's bit for bit), which also writes each pair's warping path, for frame-level scores along it (the F0 scores of
+ *   evaluate_tts.py --f0).
+ *   path_out (device) int32 (i, j) pairs: pair p's path starts at entry P_p = sum_{q<p} (Tx_q + Ty_q - 1), the longest a path of
+ *   the earlier pairs can be, and runs from (0, 0) to (Tx-1, Ty-1); its first path_len_out[p] entries are written.  Each step
+ *   goes to the predecessor the DTW recursion chose, under its tie rule (diagonal, then (i-1, j), then (i, j-1)), so consecutive
+ *   entries differ by (1,1), (1,0) or (0,1).  A pair's path does not depend on the other pairs or its position.
+ *   The sweep keeps 2 bits per cell of the predecessor it took in the workspace (ttsb_mcd_dtw_path_workspace_bytes(...) bytes,
+ *   8-byte aligned); a pair may have at most TTSB_MCD_DTW_PATH_MAX_CELLS cells (Tx * Ty; 4 MiB of bits, e.g. 4096 x 4096 or
+ *   1,200 x 13,981), and min(Tx, Ty) is at most TTSB_MCD_DTW_MAX_FRAMES as above.  Everything ttsb_mcd_dtw refuses, a NULL
+ *   path_out and a pair past the cell limit give TTSB_ERR_INVALID_ARGUMENT before any CUDA call. */
+#define TTSB_MCD_DTW_PATH_MAX_CELLS 16777216
+int64_t ttsb_mcd_dtw_path_workspace_bytes(const int32_t* x_offsets, const int32_t* y_offsets, int n_pairs, int n_ceps); /* -1: invalid */
+int ttsb_mcd_dtw_path(const float* x, const int32_t* x_offsets, const float* y, const int32_t* y_offsets, int n_pairs, int n_mels,
+                      const double* dct, int n_ceps, double kappa, void* workspace, int64_t workspace_bytes, double* cost_out,
+                      int32_t* path_len_out, int32_t* path_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Ragged-batch Conv1D on the tensor cores (the MelGAN and HiFi-GAN generators, transformertts_b200/model/melgan.py and

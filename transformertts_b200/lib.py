@@ -35,7 +35,7 @@ EXPORTS = [
     'ttsb_decode_attn_workspace_bytes', 'ttsb_decode_attn', 'ttsb_decode_prologue', 'ttsb_decode_commit',
     'ttsb_conv1d_workspace_bytes', 'ttsb_conv1d_ex_tc', 'ttsb_conv1d_out_tanh_ex',
     'ttsb_resample_batch_workspace_bytes', 'ttsb_resample_batch',
-    'ttsb_mcd_dtw_workspace_bytes', 'ttsb_mcd_dtw',
+    'ttsb_mcd_dtw_workspace_bytes', 'ttsb_mcd_dtw', 'ttsb_mcd_dtw_path_workspace_bytes', 'ttsb_mcd_dtw_path',
     'ttsb_stft_mel_log_ragged_workspace_bytes', 'ttsb_stft_mel_log_ragged', 'ttsb_mel_to_linear_ex',
     'ttsb_stft_complex_ragged_workspace_bytes', 'ttsb_stft_complex_ragged', 'ttsb_istft_ragged_workspace_bytes', 'ttsb_istft_ragged',
     'ttsb_griffinlim_ragged_workspace_bytes', 'ttsb_griffinlim_ragged',
@@ -152,6 +152,10 @@ def load() -> C.CDLL:
     lib.ttsb_mcd_dtw_workspace_bytes.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
     lib.ttsb_mcd_dtw.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_double,
                                  C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.ttsb_mcd_dtw_path_workspace_bytes.restype = C.c_int64
+    lib.ttsb_mcd_dtw_path_workspace_bytes.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    lib.ttsb_mcd_dtw_path.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_double,
+                                      C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     for name in ('ttsb_stft_mel_log_ragged_workspace_bytes', 'ttsb_stft_complex_ragged_workspace_bytes',
                  'ttsb_istft_ragged_workspace_bytes', 'ttsb_griffinlim_ragged_workspace_bytes'):
         getattr(lib, name).restype = C.c_int64
@@ -457,6 +461,35 @@ def mcd_dtw(x, x_offsets, y, y_offsets, dct, kappa, cost_out, path_len_out):
     ws = torch.empty(nb, dtype=torch.uint8, device=x.device)
     _check(load().ttsb_mcd_dtw(ptr(x), xo, ptr(y), yo, n, int(n_mels), ptr(dct), int(n_ceps), float(kappa), ptr(ws), C.c_int64(nb),
                                ptr(cost_out), ptr(path_len_out), _stream()), 'ttsb_mcd_dtw')
+
+
+# the most cells (Tx * Ty) of a pair ttsb_mcd_dtw_path takes (include/ttsb.h: TTSB_MCD_DTW_PATH_MAX_CELLS)
+MCD_DTW_PATH_MAX_CELLS = 16777216
+
+
+def mcd_dtw_path_workspace_bytes(x_offsets, y_offsets, n_ceps: int) -> int:
+    xo, n = _host_offsets(x_offsets)
+    yo, n_y = _host_offsets(y_offsets)
+    if n_y != n:
+        raise TtsbError(f'{n} pairs in x_offsets, {n_y} in y_offsets')
+    nb = int(load().ttsb_mcd_dtw_path_workspace_bytes(xo, yo, n, int(n_ceps)))
+    if nb < 0:
+        raise TtsbError(load().ttsb_last_error().decode())
+    return nb
+
+
+def mcd_dtw_path(x, x_offsets, y, y_offsets, dct, kappa, cost_out, path_len_out, path_out):
+    """mcd_dtw that also writes each pair's warping path (include/ttsb.h: ttsb_mcd_dtw_path): path_out int32 (sum of
+    Tx + Ty - 1, 2) on the device, pair p's path from row sum_{q<p} (Tx_q + Ty_q - 1)."""
+    xo, n = _host_offsets(x_offsets)
+    yo, n_y = _host_offsets(y_offsets)
+    if n_y != n:
+        raise TtsbError(f'{n} pairs in x_offsets, {n_y} in y_offsets')
+    n_ceps, n_mels = dct.shape
+    nb = mcd_dtw_path_workspace_bytes(x_offsets, y_offsets, n_ceps)
+    ws = torch.empty(nb, dtype=torch.uint8, device=x.device)
+    _check(load().ttsb_mcd_dtw_path(ptr(x), xo, ptr(y), yo, n, int(n_mels), ptr(dct), int(n_ceps), float(kappa), ptr(ws), C.c_int64(nb),
+                                    ptr(cost_out), ptr(path_len_out), ptr(path_out), _stream()), 'ttsb_mcd_dtw_path')
 
 
 # ------------------------------------------------------------------------------------------------------------

@@ -10,6 +10,9 @@ reference has no counterpart: it shows validation predictions in TensorBoard).
 * Duration errors of the integer durations against the Aligner's durations: mean absolute error in frames per phoneme, the
   rate of exact matches and the ratio of predicted to recorded frames.
 * Pitch RMSE over the phonemes whose target pitch is not 0 (unvoiced), in normalised units and, with ``pitch_stats.pkl``, in Hz.
+* F0 of vocoded audio (``f0=True``): the WORLD F0 (DIO + StoneMask on the GPU) of the vocoded waveforms against the recorded
+  frame pitch, frame by frame along the MCD-DTW warping path (``ttsb_mcd_dtw_path``): gross pitch error (GPE), voicing
+  decision error (VDE), F0 frame error (FFE) and the F0 RMSE in cents (``f0_scores``).
 
 Corpus values are means over lines."""
 from __future__ import annotations
@@ -84,6 +87,70 @@ def mcd_dtw_packed(x: torch.Tensor, x_offsets, y: torch.Tensor, y_offsets, n_cep
     return cost, path_len, cost / path_len
 
 
+MCD_DTW_PATH_BUDGET = 1 << 30   # bytes of ttsb_mcd_dtw_path workspace per call (cepstra and 2 bits per DTW cell)
+
+
+def mcd_dtw_paths(mels_a: Sequence, mels_b: Sequence, n_ceps: int = DEFAULT_N_CEPS, workspace_budget: int = MCD_DTW_PATH_BUDGET):
+    """mcd_dtw with the warping paths (``ttsb_mcd_dtw_path``): -> (cost, path_len, mcd, paths), the first three as mcd_dtw
+    returns them (bit for bit) and paths[i] int32 (path_len[i], 2), the (i, j) frame pairs of line i's optimal path from (0, 0)
+    to (Tx - 1, Ty - 1).  The pairs are split into calls whose workspaces hold at most `workspace_budget` bytes (a pair larger
+    than that runs alone); a pair's result does not depend on the others, so the split changes nothing."""
+    if len(mels_a) != len(mels_b) or len(mels_a) == 0:
+        raise ValueError(f'need two non-empty lists of the same length, got {len(mels_a)} and {len(mels_b)}')
+    device = next((m.device for m in list(mels_a) + list(mels_b) if torch.is_tensor(m) and m.is_cuda),
+                  torch.device('cuda', torch.cuda.current_device()))
+    lens = [(int(np.shape(a)[0]), int(np.shape(b)[0])) for a, b in zip(mels_a, mels_b)]
+    groups, size = [[]], 0
+    for i, (tx, ty) in enumerate(lens):
+        # a pair's workspace alone bounds its share of a batch's (the batch shares one pair table)
+        nb = lib.mcd_dtw_path_workspace_bytes([0, tx], [0, ty], n_ceps) if tx > 0 and ty > 0 else 0
+        if groups[-1] and size + nb > workspace_budget:
+            groups.append([])
+            size = 0
+        groups[-1].append(i)
+        size += nb
+    n = len(lens)
+    cost, path_len, paths = np.empty(n), np.empty(n, dtype=np.int32), [None] * n
+    for g in groups:
+        x, xo = _pack([mels_a[i] for i in g], device)
+        y, yo = _pack([mels_b[i] for i in g], device)
+        n_mels = x.shape[1]
+        if y.shape[1] != n_mels:
+            raise ValueError(f'x {tuple(x.shape)} and y {tuple(y.shape)}: need the same n_mels')
+        starts = np.concatenate([[0], np.cumsum([lens[i][0] + lens[i][1] - 1 for i in g])])
+        with torch.cuda.device(device):
+            dct = torch.from_numpy(dct_matrix(n_mels, n_ceps)).to(device)
+            c = torch.empty(len(g), dtype=torch.float64, device=device)
+            ln = torch.empty(len(g), dtype=torch.int32, device=device)
+            path = torch.empty((int(starts[-1]), 2), dtype=torch.int32, device=device)
+            lib.mcd_dtw_path(x, xo, y, yo, dct, KAPPA, c, ln, path)
+            c, ln, path = c.cpu().numpy(), ln.cpu().numpy(), path.cpu().numpy()
+        for r, i in enumerate(g):
+            cost[i], path_len[i] = c[r], ln[r]
+            paths[i] = path[starts[r]:starts[r] + ln[r]].copy()
+    return cost, path_len, cost / path_len, paths
+
+
+def f0_scores(f0_a_hz, f0_b_hz, path) -> dict:
+    """Pitch and voicing of contour a against contour b (Hz, 0 = unvoiced; voiced means f0 > 0) over the steps (i, j) of a
+    warping path, float64.  A step counts when i < len(a) and j < len(b) (a WORLD contour can be a frame shorter than the mel the
+    path aligns); f0_steps is their number.  VDE: voicing mismatches / steps; GPE: steps voiced on both sides with
+    |f_a / f_b - 1| > 0.2 / steps voiced on both sides; FFE: (gross errors + voicing mismatches) / steps; f0_rmse_cents:
+    sqrt(mean((1200 log2(f_a / f_b))^2)) over the steps voiced on both sides.  A score with an empty denominator is None."""
+    a, b = np.asarray(f0_a_hz, dtype=np.float64).reshape(-1), np.asarray(f0_b_hz, dtype=np.float64).reshape(-1)
+    path = np.asarray(path, dtype=np.int64).reshape(-1, 2)
+    scored = path[(path[:, 0] < len(a)) & (path[:, 1] < len(b))]
+    fa, fb = a[scored[:, 0]], b[scored[:, 1]]
+    va, vb = fa > 0.0, fb > 0.0
+    both = va & vb
+    n, n_both, flips = len(scored), int(both.sum()), int((va != vb).sum())
+    ratio = fa[both] / fb[both]
+    gross = int((np.abs(ratio - 1.0) > 0.2).sum())
+    cents = 1200.0 * np.log2(ratio)
+    return {'gpe': gross / n_both if n_both else None, 'vde': flips / n if n else None, 'ffe': (gross + flips) / n if n else None,
+            'f0_rmse_cents': float(np.sqrt(np.mean(cents * cents))) if n_both else None, 'f0_steps': n}
+
+
 def _pack(mels, device) -> tuple:
     ts = [torch.as_tensor(m).to(device=device, dtype=torch.float32) for m in mels]
     for i, t in enumerate(ts):
@@ -118,11 +185,14 @@ class ValidationSet:
     durations: List[np.ndarray]
     pitch: List[np.ndarray]
     pitch_stats: Optional[tuple] = None
+    frame_pitch: Optional[List[np.ndarray]] = None   # recorded F0 per mel frame in Hz (0 = unvoiced), float64
 
 
-def load_validation_set(cm) -> ValidationSet:
+def load_validation_set(cm, frame_pitch: bool = False) -> ValidationSet:
     """The config's validation split (``valid_metadata``, ``mels``, ``durations`` and ``char_pitch`` of a
-    TrainingConfigManager), plus ``pitch_stats.pkl`` when the data directory has one."""
+    TrainingConfigManager), plus ``pitch_stats.pkl`` when the data directory has one.  With frame_pitch, also the recorded
+    frame F0 ``pitch.<audio>/<name>.npy`` in Hz: create_training_data.py stores it normalised, so it is de-normalised with
+    ``pitch_stats.pkl`` (p std + mean where p != 0); a missing file or missing statistics raise FileNotFoundError."""
     from ..data.datasets import DataReader
     reader = DataReader(cm.valid_metadata_path, is_processed=True)
     names = list(reader.text_dict)
@@ -133,11 +203,24 @@ def load_validation_set(cm) -> ValidationSet:
         with open(cm.data_dir / 'pitch_stats.pkl', 'rb') as f:
             st = pickle.load(f)
         stats = (float(st['pitch_mean']), float(st['pitch_std']))
+    frames = None
+    if frame_pitch:
+        if stats is None:
+            raise FileNotFoundError(f'{cm.data_dir / "pitch_stats.pkl"} not found: the frame pitch is stored normalised and needs '
+                                    f'its statistics')
+        missing = [cm.pitch_dir / f'{n}.npy' for n in names if not (cm.pitch_dir / f'{n}.npy').exists()]
+        if missing:
+            raise FileNotFoundError(f'no frame pitch {missing[0]}' + (f' (and {len(missing) - 1} more)' if len(missing) > 1 else ''))
+        frames = []
+        for n in names:
+            p = np.load(cm.pitch_dir / f'{n}.npy').astype(np.float64).reshape(-1)
+            frames.append(np.where(p != 0.0, p * stats[1] + stats[0], 0.0))
     return ValidationSet(
         names=names, phonemes=[reader.text_dict[n] for n in names],
         mels=[np.load(cm.mel_dir / f'{n}.npy').astype(np.float32) for n in names],
         durations=[np.load(cm.duration_dir / f'{n}.npy').astype(np.int64) for n in names],
-        pitch=[np.load(cm.pitch_per_char / f'{n}.npy').astype(np.float32).reshape(-1) for n in names], pitch_stats=stats)
+        pitch=[np.load(cm.pitch_per_char / f'{n}.npy').astype(np.float32).reshape(-1) for n in names], pitch_stats=stats,
+        frame_pitch=frames)
 
 
 def tokenize(model, phonemes: Sequence[str]) -> List[List[int]]:
@@ -169,16 +252,53 @@ def pitch_scores(pred: np.ndarray, target: np.ndarray, stats: Optional[tuple]) -
     return out
 
 
-def _mcd_fields(prefix: str, pred_mels: list, ref_mels: list, n_ceps: int, to_ln=lambda m: m) -> List[dict]:
-    """{prefix}mcd / dtw_cost / path_len per line, the mels mapped to natural-log mels by to_ln; None for a line whose prediction
-    has no frame."""
+def _mcd_fields(prefix: str, pred_mels: list, ref_mels: list, n_ceps: int, to_ln=lambda m: m, with_paths: bool = False) -> tuple:
+    """({prefix}mcd / dtw_cost / path_len per line, the mels mapped to natural-log mels by to_ln, paths): None for a line whose
+    prediction has no frame.  paths[i] is line i's warping path with with_paths (mcd_dtw_paths, the same scores), else None."""
     rows = [{f'{prefix}mcd': None, f'{prefix}dtw_cost': None, f'{prefix}path_len': None} for _ in pred_mels]
+    paths = [None] * len(pred_mels)
     keep = [i for i, m in enumerate(pred_mels) if m.shape[0] > 0]
     if keep:
-        cost, path_len, mcd = mcd_dtw([to_ln(torch.as_tensor(pred_mels[i])) for i in keep],
-                                      [to_ln(torch.as_tensor(ref_mels[i])) for i in keep], n_ceps)
+        a = [to_ln(torch.as_tensor(pred_mels[i])) for i in keep]
+        b = [to_ln(torch.as_tensor(ref_mels[i])) for i in keep]
+        if with_paths:
+            cost, path_len, mcd, kept_paths = mcd_dtw_paths(a, b, n_ceps)
+            for r, i in enumerate(keep):
+                paths[i] = kept_paths[r]
+        else:
+            cost, path_len, mcd = mcd_dtw(a, b, n_ceps)
         for r, i in enumerate(keep):
             rows[i] = {f'{prefix}mcd': float(mcd[r]), f'{prefix}dtw_cost': float(cost[r]), f'{prefix}path_len': int(path_len[r])}
+    return rows, paths
+
+
+F0_KEYS = ('gpe', 'vde', 'ffe', 'f0_rmse_cents', 'f0_steps')
+F0_FLOOR = 71.0                    # pyworld's default f0_floor, which Audio.extract_pitch_device runs DIO with
+PITCH_CHUNK_SAMPLES = 1 << 24      # samples per DIO call (its workspace takes about 190 bytes per sample)
+
+
+def _dio_takes(audio, n_samples: int) -> bool:
+    """Whether ttsb_pitch_dio_stonemask takes a clip of n_samples: it needs more WORLD frames than DIO's voice_range_minimum."""
+    fp = audio.hop_length / audio.sampling_rate * 1000
+    return int(audio._pitch_frames([n_samples])[0]) > int(0.5 + 1000.0 / fp / F0_FLOOR) * 2 + 1
+
+
+def _f0_fields(prefix: str, audio, wavs: list, paths: list, frame_pitch: list) -> List[dict]:
+    """{prefix}gpe / vde / ffe / f0_rmse_cents / f0_steps per line: the F0 of wavs[i] against the recorded frame_pitch[i] along
+    paths[i] (f0_scores); None for a line without a path or too short for DIO."""
+    rows = [{prefix + k: None for k in F0_KEYS} for _ in wavs]
+    keep = [i for i, (w, p) in enumerate(zip(wavs, paths)) if p is not None and _dio_takes(audio, len(w))]
+    chunks, samples = [[]], 0
+    for i in keep:
+        if chunks[-1] and samples + len(wavs[i]) > PITCH_CHUNK_SAMPLES:
+            chunks.append([])
+            samples = 0
+        chunks[-1].append(i)
+        samples += len(wavs[i])
+    for chunk in chunks:
+        if chunk:   # a clip's F0 does not depend on the other clips of the batch
+            for i, f0 in zip(chunk, audio.extract_pitch_batch([wavs[i] for i in chunk])):
+                rows[i] = {prefix + k: v for k, v in f0_scores(f0, frame_pitch[i], paths[i]).items()}
     return rows
 
 
@@ -203,42 +323,55 @@ def _means(lines: List[dict]) -> dict:
 
 
 def evaluate_model(model, vs: ValidationSet, n_ceps: int = DEFAULT_N_CEPS, teacher_forced: bool = True,
-                   vocode: Optional[Callable[[List[np.ndarray]], List[np.ndarray]]] = None, audio=None, batch_size: int = 64) -> dict:
+                   vocode: Optional[Callable[[List[np.ndarray]], List[np.ndarray]]] = None, audio=None, batch_size: int = 64,
+                   f0: bool = False) -> dict:
     """Scores of `model` on `vs`: {'lines': [one dict per line], 'mean': {means over lines}}.
 
     Free-running (``predict_batch`` of the phonemes alone): MCD-DTW against the recorded mel, duration and pitch errors.  With
     teacher_forced, also ``predict_batch`` with the target durations and pitch, scored by MCD-DTW (tf_*).  With vocode (a
     function from a list of (T, n_mels) mels to waveforms) and audio (the model's Audio), the free-running mels and the recorded
     mels are vocoded, their log-mels re-extracted on the GPU and each scored against the recorded mel (vocoded_* and
-    copy_synthesis_*; the latter is the vocoder's own floor)."""
+    copy_synthesis_*; the latter is the vocoder's own floor).  With f0 (needs vocode and vs.frame_pitch), also the F0 scores of
+    both sets of waveforms against the recorded frame pitch along the same MCD-DTW paths (vocoded_gpe ... and
+    copy_synthesis_gpe ..., see f0_scores), with the F0 of Audio.extract_pitch_batch at WORLD's settings of the training data."""
+    if f0 and (vocode is None or vs.frame_pitch is None):
+        raise ValueError('the F0 scores need a vocoder and the recorded frame pitch (load_validation_set(cm, frame_pitch=True))')
     to_ln = natural_log_mels(model.config)
     tokens = tokenize(model, vs.phonemes)
     outs = model.predict_batch(tokens, encode=False, phoneme_max_duration=None, batch_size=batch_size)
     pred_mels = [o['mel'] for o in outs]
     lines = [{'name': n, 'frames_predicted': int(o['mel_lengths']), 'frames_recorded': int(m.shape[0])}
              for n, o, m in zip(vs.names, outs, vs.mels)]
-    for i, row in enumerate(_mcd_fields('', pred_mels, vs.mels, n_ceps, to_ln)):
+    for i, row in enumerate(_mcd_fields('', pred_mels, vs.mels, n_ceps, to_ln)[0]):
         lines[i].update(row)
         lines[i].update(duration_scores(outs[i]['int_durations'].cpu().numpy(), vs.durations[i]))
         lines[i].update(pitch_scores(outs[i]['pitch'].cpu().numpy(), vs.pitch[i], vs.pitch_stats))
     if teacher_forced:
         tf = model.predict_batch(tokens, encode=False, phoneme_max_duration=None, phoneme_durations=vs.durations,
                                  phoneme_pitch=vs.pitch, batch_size=batch_size)
-        for i, row in enumerate(_mcd_fields('teacher_forced_', [o['mel'] for o in tf], vs.mels, n_ceps, to_ln)):
+        for i, row in enumerate(_mcd_fields('teacher_forced_', [o['mel'] for o in tf], vs.mels, n_ceps, to_ln)[0]):
             lines[i].update(row)
     if vocode is not None:
         if audio is None:
             raise ValueError('vocoding needs the Audio front end of the model')
         kept = [i for i, m in enumerate(pred_mels) if m.shape[0] > 0]
         vocoded = [torch.empty(0)] * len(pred_mels)   # a line without frames has nothing to vocode: its score stays None
+        vocoded_wavs = [None] * len(pred_mels)
         if kept:
-            for i, m in zip(kept, _resynthesis_mels(audio, vocode([pred_mels[i].cpu().numpy() for i in kept]))):
-                vocoded[i] = m
-        copy = _resynthesis_mels(audio, vocode(vs.mels))
-        for i, (row, crow) in enumerate(zip(_mcd_fields('vocoded_', vocoded, vs.mels, n_ceps, to_ln),
-                                            _mcd_fields('copy_synthesis_', copy, vs.mels, n_ceps, to_ln))):
+            wavs = vocode([pred_mels[i].cpu().numpy() for i in kept])
+            for i, w, m in zip(kept, wavs, _resynthesis_mels(audio, wavs)):
+                vocoded[i], vocoded_wavs[i] = m, w
+        copy_wavs = vocode(vs.mels)
+        copy = _resynthesis_mels(audio, copy_wavs)
+        rows, paths = _mcd_fields('vocoded_', vocoded, vs.mels, n_ceps, to_ln, with_paths=f0)
+        crows, cpaths = _mcd_fields('copy_synthesis_', copy, vs.mels, n_ceps, to_ln, with_paths=f0)
+        for i, (row, crow) in enumerate(zip(rows, crows)):
             lines[i].update(row)
             lines[i].update(crow)
+        if f0:
+            for prefix, wavs, ps in (('vocoded_', vocoded_wavs, paths), ('copy_synthesis_', copy_wavs, cpaths)):
+                for i, row in enumerate(_f0_fields(prefix, audio, wavs, ps, vs.frame_pitch)):
+                    lines[i].update(row)
     return {'lines': lines, 'mean': _means(lines)}
 
 
@@ -254,6 +387,10 @@ def summary_line(label: str, result: dict) -> str:
          + f' | pitch RMSE {f("pitch_rmse")}' + (f' ({f("pitch_rmse_hz", ".2f")} Hz)' if m.get('pitch_rmse_hz') is not None else ''))
     if 'vocoded_mcd' in m:
         s += f' | vocoded MCD {f("vocoded_mcd")}, copy synthesis {f("copy_synthesis_mcd")}'
+    for label, p in (('vocoded', 'vocoded_'), ('copy synthesis', 'copy_synthesis_')):
+        if f'{p}gpe' in m:
+            s += (f' | {label} GPE {f(p + "gpe")}, VDE {f(p + "vde")}, FFE {f(p + "ffe")}, '
+                  f'F0 RMSE {f(p + "f0_rmse_cents", ".1f")} cents')
     return s
 
 
