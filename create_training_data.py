@@ -21,12 +21,23 @@ sr=sampling_rate)`` does (resampy's ``kaiser_best`` filter): the off-rate files 
 ``ttsb_resample_batch`` launch, then through the same ``Audio.preprocess`` (volume normalisation, hop padding) as every other file.
 Files already at ``sampling_rate`` take exactly the path they take without resampling.
 
+With ``trim_silence`` set (and ``trim_silence_top_db``), the leading and trailing silence of every file is trimmed as the
+reference's ``librosa.effects.trim(y, top_db, frame_length=256, hop_length=64)`` does, after the volume normalisation and before
+the hop padding: the files of a batch, at the configured rate and resampled alike, go through one ``ttsb_trim_silence_bounds``
+launch, and the loader threads do only the volume normalisation.  The mels, the pitch, ``mel_len.pkl``, the length filter and
+the pitch statistics then see the trimmed clips.  Without ``trim_silence`` the script runs exactly as before.
+
 Differences from the reference:
   * Without the ``phonemizer`` package (and espeak), the text column of the metadata is taken to BE phonemes in the model's
     alphabet, as ``predict_tts.py`` does; the script says so when it starts.  With it, the reference's arguments are used.
   * Files are processed in metadata order, so the pitch statistics and the phonemized metadata are in that order; the
     reference's process pool completes them in no fixed order, so its statistics differ in the last bits from run to run.
-  * The ``trim_silence`` / ``trim_long_silences`` settings are refused (no librosa or webrtcvad); see ``Audio.preprocess``.
+  * The ``trim_long_silences`` setting is refused (no webrtcvad), and so is ``trim_silence`` without ``trim_silence_top_db``
+    (librosa would be called with top_db=None); see ``Audio.preprocess``.
+  * A file whose trimmed clip is too short for the log-mel or pitch kernels (fewer than ``n_fft / 2 + 1`` samples, or no more
+    WORLD frames than DIO's voice_range_minimum) gets no ``.npy`` files: it is listed in ``under-over_sized_mels.pkl`` with its
+    frame count ``1 + L // hop_length`` in ``mel_len.pkl``, and its pitch does not enter the statistics.  The reference computes
+    its tiny mel and pitch, and then drops the file by ``min_mel_len`` all the same.
   * Resampling restates resampy's ``kaiser_best`` table from its published parameters rather than reading resampy's precomputed
     file, so it may differ from librosa's result in the last bits of the filter.  A file too short to resample (fewer output
     samples than one) stops the script with its name; the reference's worker would raise inside resampy.
@@ -105,15 +116,22 @@ class TooShortToResample(ValueError):
     pass
 
 
+def host_preprocess(audio):
+    """The part of Audio.preprocess done before a file joins its batch: all of it, or with trim_silence everything before the
+    trim (the trim and the hop padding then run a batch at a time in trim_batch)."""
+    return audio.preprocess_before_trim if audio.trim_silence else audio.preprocess
+
+
 def wav_loader(audio):
-    """path -> (samples, None) preprocessed as Audio.load_wav does when the file is at the configured rate, else the raw mono
-    samples and their rate, to be resampled with the rest of the batch."""
+    """path -> (samples, None) preprocessed as Audio.load_wav does when the file is at the configured rate (up to the trim with
+    trim_silence), else the raw mono samples and their rate, to be resampled with the rest of the batch."""
     from transformertts_b200.data.audio import resampled_length
+    preprocess = host_preprocess(audio)
 
     def load(path):
         y, sr = audio.read_wav(str(path))
         if sr == audio.sampling_rate:
-            return audio.preprocess(y), None
+            return preprocess(y), None
         try:
             resampled_length(len(y), sr, audio.sampling_rate)
         except ValueError as e:
@@ -140,7 +158,20 @@ def resample_batch(audio, batch, rates_seen: dict):
     for c in off:
         sr = batch[c][1][1]
         rates_seen[sr] = rates_seen.get(sr, 0) + 1
-    return [(path, audio.preprocess(done[c]) if c in done else y) for c, (path, (y, _)) in enumerate(batch)]
+    preprocess = host_preprocess(audio)
+    return [(path, preprocess(done[c]) if c in done else y) for c, (path, (y, _)) in enumerate(batch)]
+
+
+def trim_batch(audio, batch):
+    """trim_silence: trim every clip of a batch in one launch, then pad it to the hop as Audio.preprocess does."""
+    trimmed = audio.trim_silence_ragged([y for _, y in batch])
+    return [(path, audio.pad_to_hop(y)) for (path, _), y in zip(batch, trimmed)]
+
+
+def too_short(audio, n_samples: int) -> bool:
+    """Whether a trimmed clip is too short for the log-mel (reflect padding) or DIO (its contour fix) kernels."""
+    from transformertts_b200.utils.evaluation import _dio_takes
+    return n_samples < audio.min_mel_samples or not _dio_takes(audio, n_samples)
 
 
 def process_mels(cm, audio, wav_files, budget: int = BATCH_SAMPLES):
@@ -152,15 +183,27 @@ def process_mels(cm, audio, wav_files, budget: int = BATCH_SAMPLES):
     with ThreadPoolExecutor(max_workers=2) as writer:
         for raw in batches(wav_files, budget, wav_loader(audio), loaded_samples(audio)):
             batch = resample_batch(audio, raw, rates_seen)
-            wav, so = audio._pack([y for _, y in batch])
-            mel, fo_mel = audio.mel_spectrogram_ragged_device(wav, so)
-            f0, fo_f0 = audio.extract_pitch_device(wav, so)
-            mel, f0 = mel.cpu().numpy(), f0.cpu().numpy()
+            short = set()
+            if audio.trim_silence:
+                batch = trim_batch(audio, batch)
+                short = {c for c, (_, y) in enumerate(batch) if too_short(audio, len(y))}
+            kept = [item for c, item in enumerate(batch) if c not in short]
+            if kept:
+                wav, so = audio._pack([y for _, y in kept])
+                mel, fo_mel = audio.mel_spectrogram_ragged_device(wav, so)
+                f0, fo_f0 = audio.extract_pitch_device(wav, so)
+                mel, f0 = mel.cpu().numpy(), f0.cpu().numpy()
+            k = 0       # clip k of the packed batch
             for c, (path, y) in enumerate(batch):
-                m, p = mel[fo_mel[c]:fo_mel[c + 1]], f0[fo_f0[c]:fo_f0[c + 1]]
+                name = Path(path).stem
+                if c in short:
+                    len_dict[name] = 1 + len(y) // audio.hop_length
+                    remove_files.append(name)
+                    continue
+                m, p = mel[fo_mel[k]:fo_mel[k + 1]], f0[fo_f0[k]:fo_f0[k + 1]]
+                k += 1
                 assert m.shape[1] == audio.config['mel_channels'], len(m.shape) == 2
                 assert m.shape[0] == p.shape[0], f'{m.shape[0]} == {p.shape[0]} (wav {y.shape})'
-                name = Path(path).stem
                 writer.submit(np.save, (cm.mel_dir / name).with_suffix('.npy'), m)
                 pitches[(cm.pitch_dir / name).with_suffix('.npy')] = p
                 len_dict[name] = m.shape[0]

@@ -538,6 +538,24 @@ int ttsb_resample_batch(const float* wav, const int32_t* sample_offsets, const i
                         float* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Silence trimming  (Audio.trim_silence_bounds_device; data/audio.py:164-169: librosa.effects.trim(y, top_db, frame_length=256,
+ * hop_length=64); tests/trim_oracle.py restates the algorithm)
+ *   wav: fp32 clips packed end to end, clip c at samples sample_offsets[c] .. sample_offsets[c+1] - 1 (int32 (n_clips + 1), HOST
+ *   memory, from 0; every clip at least one sample).  Per clip of L samples: x is the clip reflect-padded by 128 samples on each
+ *   side as np.pad(y, 128, 'reflect') pads it (repeated reflection below 129 samples, a 1-sample clip repeated); frame
+ *   t = 0 .. L / 64 has the power p_t = (sum of x[64 t + k]^2, k = 0 .. 255, added in k order) / 256 in float64; frame t is
+ *   non-silent iff 10 log10(max(1e-10, p_t)) - 10 log10(max(1e-10, max_t p_t)) > -top_db, in float64.  bounds: int32
+ *   (n_clips, 2) in device memory receives [start, end) = [64 f, min(L, 64 (l + 1))) relative to the clip for its first and last
+ *   non-silent frames f and l ([0, 0) if there is none, which top_db > 0 rules out).  A clip's bounds do not depend on the other
+ *   clips or its position in the batch.  Three launches whatever the number of clips.
+ *   workspace: ttsb_trim_silence_workspace_bytes(...) bytes of device memory, 16-byte aligned (8 bytes per frame plus 24 per
+ *   clip).  Offsets that do not start at 0 or decrease, an empty clip, a top_db that is not finite or <= 0 and a short workspace
+ *   give TTSB_ERR_INVALID_ARGUMENT before any CUDA call. */
+int64_t ttsb_trim_silence_workspace_bytes(const int32_t* sample_offsets, int n_clips);   /* -1 for invalid arguments */
+int ttsb_trim_silence_bounds(const float* wav, const int32_t* sample_offsets, int n_clips, double top_db, void* workspace,
+                             int64_t workspace_bytes, int32_t* bounds, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * mel -> waveform  (Audio.reconstruct_waveform, data/audio.py:94-110: librosa mel_to_stft(power=1) + griffinlim(32, momentum .99))
  *   n_fft 1024, hop 256, periodic Hann, centred frames with reflect padding (the reference configuration).
  * ------------------------------------------------------------------------------------------------------- */

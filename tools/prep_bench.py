@@ -1,7 +1,7 @@
 """Training-data preparation throughput: log-mel + DIO/StoneMask pitch on the GPU, create_training_data.py end to end, and the numpy
 restatement of WORLD on the host cores.
 
-    python tools/prep_bench.py [--minutes 20] [--reps 3] [--cpu-clips 8] [--source-rate HZ] [--out DIR]
+    python tools/prep_bench.py [--minutes 20] [--reps 3] [--cpu-clips 8] [--source-rate HZ] [--trim] [--out DIR]
 
 Workload: seeded speech-like clips of 1-10 s (oracle/pitch_oracle.py speech_like_clip) until `--minutes` of audio, synthesised at
 `--source-rate` (default: the configured 22050 Hz).
@@ -14,6 +14,10 @@ Workload: seeded speech-like clips of 1-10 s (oracle/pitch_oracle.py speech_like
     per-sample wing lengths), and tests/resample_oracle.py (numpy, one core) on the first `--cpu-clips` clips beside it.
   * script: create_training_data.py run once as a subprocess on the same clips written as 16-bit WAV into a temporary directory
     (file reading, resampling, .npy writing, the phonemized metadata and the Python start-up included).
+  * trim (`--trim` only): Audio.trim_silence_bounds_device (ttsb_trim_silence_bounds at top_db 60) alone on each packed batch,
+    timed with CUDA events over `--reps` passes after a warm-up, beside the log-mel and pitch calls timed the same way on the same
+    batches.  With `--trim` the script arm runs with `trim_silence: true, trim_silence_top_db: 60` as well (the clips then carry
+    0-2 s of leading and trailing silence, tests/trim_oracle.py padded_speech).
   * cpu: oracle/pitch_oracle.extract_pitch (numpy restatement, not pyworld) on the first `--cpu-clips` clips with a process pool
     over all host cores, scaled to audio seconds per second.
 Prints one JSON line with audio seconds processed per second for each arm, the FP64 operation count of the pitch filters derived
@@ -37,6 +41,7 @@ sys.path.insert(0, str(ROOT))
 from oracle import pitch_oracle as po  # noqa: E402
 sys.path.insert(0, str(ROOT / 'tests'))
 import resample_oracle as ro  # noqa: E402  (the numpy restatement of resampling kept with the tests)
+import trim_oracle as to  # noqa: E402
 from transformertts_b200.data.audio import Audio  # noqa: E402
 
 FS, HOP = 22050, 256
@@ -51,11 +56,14 @@ def card():
         return 'unknown'
 
 
-def corpus(minutes: float, sr: int = FS):
+def corpus(minutes: float, sr: int = FS, silence: bool = False):
     clips, total, i = [], 0, 0
     rng = np.random.default_rng(11)
     while total < minutes * 60 * sr:
-        x = po.speech_like_clip(float(rng.uniform(1.0, 10.0)), 7000 + i, fs=float(sr))
+        if silence:
+            x = to.padded_speech(1, 7000 + i, fs=float(sr), min_s=1.0, max_s=10.0)[0]
+        else:
+            x = po.speech_like_clip(float(rng.uniform(1.0, 10.0)), 7000 + i, fs=float(sr))
         clips.append(po.pad_for_hop(x) if sr == FS else x)
         total += len(x)
         i += 1
@@ -126,6 +134,29 @@ def resample_arm(audio, clips, budget, sr, reps):
     return start.elapsed_time(end) / 1000 / reps, n_out
 
 
+def trim_arm(audio, clips, budget, reps):
+    """ttsb_trim_silence_bounds alone, then log-mel and pitch alone, on each packed batch (uploaded beforehand); CUDA events
+    around each set of calls -> (trim seconds, mel + pitch seconds) per pass."""
+    packed = [audio._pack(clips[i:j]) for i, j in batch_bounds(clips, budget)]
+
+    def timed(fn):
+        for p in packed:                     # warm-up
+            fn(*p)
+        torch.cuda.synchronize()
+        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        start.record()
+        for _ in range(reps):
+            for p in packed:
+                fn(*p)
+        end.record()
+        torch.cuda.synchronize()
+        return start.elapsed_time(end) / 1000 / reps
+
+    t_trim = timed(audio.trim_silence_bounds_device)
+    t_mel_pitch = timed(lambda wav, so: (audio.mel_spectrogram_ragged_device(wav, so), audio.extract_pitch_device(wav, so)))
+    return t_trim, t_mel_pitch
+
+
 def write_wav(path, x, sr):
     """16-bit PCM at sr, scaled and clipped as Audio.save_wav writes it."""
     import wave
@@ -147,16 +178,19 @@ def main():
     ap.add_argument('--reps', type=int, default=3)
     ap.add_argument('--cpu-clips', type=int, default=8)
     ap.add_argument('--source-rate', type=int, default=FS)
+    ap.add_argument('--trim', action='store_true')
     ap.add_argument('--out', default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit('prep_bench needs a CUDA device')
     import create_training_data as ctd
     sr = args.source_rate
-    clips = corpus(args.minutes, sr)
+    if args.trim and sr != FS:
+        raise SystemExit('--trim times the trim at the configured rate; leave --source-rate at its default')
+    clips = corpus(args.minutes, sr, silence=args.trim)
     seconds = sum(len(c) for c in clips) / sr
     audio = Audio(sampling_rate=FS, n_fft=1024, mel_channels=80, hop_length=HOP, win_length=1024, f_min=0, f_max=8000,
-                  normalizer='MelGAN')
+                  normalizer='MelGAN', trim_silence_top_db=60)
     gpu_pass(audio, clips, ctd.BATCH_SAMPLES, sr)
     t0 = time.perf_counter()
     for _ in range(args.reps):
@@ -175,6 +209,8 @@ def main():
         cfg['paths'].update(log_directory=str(tmp / 'logs'), train_data_directory=str(tmp / 'data'),
                             metadata_path=str(tmp / 'metadata.csv'), wav_directory=str(tmp / 'wavs'))
         cfg['training_data_settings'].update(n_test=10)
+        if args.trim:
+            cfg['audio_settings'].update(trim_silence=True, trim_silence_top_db=60)
         (tmp / 'cfg.yaml').write_text(yaml.safe_dump(cfg))
         t0 = time.perf_counter()
         r = subprocess.run([sys.executable, str(ROOT / 'create_training_data.py'), '--config', str(tmp / 'cfg.yaml')], capture_output=True,
@@ -184,6 +220,11 @@ def main():
             raise SystemExit(r.stdout[-2000:] + r.stderr[-2000:])
 
     rs = {}
+    if args.trim:
+        t_trim, t_mel_pitch = trim_arm(audio, clips, ctd.BATCH_SAMPLES, args.reps)
+        rs.update(trim_silence=True, trim_gpu_seconds=round(t_trim, 6), trim_gpu_audio_s_per_s=round(seconds / t_trim, 1),
+                  mel_pitch_gpu_seconds_same_batches=round(t_mel_pitch, 5),
+                  trim_fraction_of_mel_pitch=round(t_trim / t_mel_pitch, 5))
     if sr != FS:
         t_rs, n_out = resample_arm(audio, clips, ctd.BATCH_SAMPLES, sr, args.reps)
         taps = resample_taps([len(c) for c in clips], sr)

@@ -2,11 +2,13 @@
 data/audio.py:72-92, 196-231) by the fused CUDA kernels ``ttsb_stft_mel_log`` / ``ttsb_stft_mel_log_batch``, f0 by DIO +
 StoneMask (data/audio.py:146-151) by ``ttsb_pitch_dio_stonemask``, wav loading and preprocessing (data/audio.py:126-141,
 154-162) on the host, resampling to ``sampling_rate`` (librosa.load's ``kaiser_best`` resampy filter, data/audio.py:126-130) by
-``ttsb_resample_batch``, and mel -> waveform by Griffin-Lim.
+``ttsb_resample_batch``, the ``trim_silence`` trim of leading and trailing silence (librosa.effects.trim, data/audio.py:164-169)
+by ``ttsb_trim_silence_bounds``, and mel -> waveform by Griffin-Lim.
 
-Silence trimming (librosa, webrtcvad) is not implemented: ``preprocess`` refuses the two trim settings.  ``load_wav`` refuses a
-file whose rate differs from ``sampling_rate``; such files are read with ``read_wav`` and resampled a batch at a time with
-``resample_ragged`` / ``resample_ragged_device``, as ``create_training_data.py`` does.
+``trim_long_silences`` (webrtcvad voice-activity detection) is not implemented: ``preprocess`` refuses it, and refuses
+``trim_silence`` without ``trim_silence_top_db``.  ``load_wav`` refuses a file whose rate differs from ``sampling_rate``; such
+files are read with ``read_wav`` and resampled a batch at a time with ``resample_ragged`` / ``resample_ragged_device``, as
+``create_training_data.py`` does.
 """
 from __future__ import annotations
 
@@ -168,6 +170,7 @@ class Audio:
         # the preprocessing settings of the reference's audio section (data/audio.py:24-33); None when absent
         self.norm_wav, self.target_dBFS, self.int16_max = (kwargs.get(k) for k in ('norm_wav', 'target_dBFS', 'int16_max'))
         self.trim_silence, self.trim_long_silences = kwargs.get('trim_silence'), kwargs.get('trim_long_silences')
+        self.trim_silence_top_db = kwargs.get('trim_silence_top_db')
 
     @classmethod
     def from_config(cls, config: dict):
@@ -445,6 +448,36 @@ class Audio:
         out = out.cpu().numpy()
         return [out[a:b] for a, b in zip(oo[:-1], oo[1:])]
 
+    def trim_silence_bounds_device(self, wav: torch.Tensor, sample_offsets) -> torch.Tensor:
+        """ttsb_trim_silence_bounds at trim_silence_top_db: packed fp32 clips on the device -> int32 (n_clips, 2) on the device,
+        [start, end) of each clip's samples that librosa.effects.trim(y, top_db, frame_length=256, hop_length=64) keeps,
+        relative to the clip.  Clip c's bounds do not depend on the other clips."""
+        top_db = self._trim_top_db()
+        with torch.cuda.device(self.device):
+            so = np.asarray(sample_offsets, dtype=np.int64)
+            bounds = torch.empty((len(so) - 1, 2), dtype=torch.int32, device=self.device)
+            lib.trim_silence_bounds(wav.contiguous(), so, top_db, bounds)
+            return bounds
+
+    def trim_silence_ragged(self, wavs) -> list:
+        """trim_audio_silence of every clip of a list in one launch -> list of float32 arrays (slices of the float32 clips)."""
+        self._trim_top_db()             # refuse a missing setting before anything reaches the device
+        ws = [np.asarray(w, dtype=np.float32).reshape(-1) for w in wavs]
+        wav, so = self._pack(ws)
+        bounds = self.trim_silence_bounds_device(wav, so).cpu().numpy()
+        return [w[a:b] for w, (a, b) in zip(ws, bounds)]
+
+    def trim_audio_silence(self, wav) -> np.ndarray:
+        """reference: data/audio.py:164-169 (librosa.effects.trim(wav, top_db=trim_silence_top_db, frame_length=256,
+        hop_length=64)[0])."""
+        return self.trim_silence_ragged([wav])[0]
+
+    def _trim_top_db(self) -> float:
+        if self.trim_silence_top_db is None:
+            raise NotImplementedError('trim_silence needs librosa.effects.trim\'s top_db, and the audio settings have no '
+                                      'trim_silence_top_db; set it (the reference uses 60) or set trim_silence: false')
+        return float(self.trim_silence_top_db)
+
     def read_wav(self, wav_path):
         """The decoding half of librosa.load (data/audio.py:126-130) -> (float32 mono samples, the file's own rate).  PCM and float
         WAV, several channels averaged to mono; PCM is scaled as libsndfile reads it into float (int16 / 32768, ...)."""
@@ -473,15 +506,26 @@ class Audio:
         return y, sr
 
     def preprocess(self, y):
-        """reference: data/audio.py:132-141.  The silence trims are not implemented and are refused when set."""
+        """reference: data/audio.py:132-141.  trim_long_silences is refused; trim_silence runs on the GPU (trim_audio_silence)."""
+        y = self.preprocess_before_trim(y)
+        if self.trim_silence:
+            y = self.trim_audio_silence(y)
+        return self.pad_to_hop(y)
+
+    def preprocess_before_trim(self, y):
+        """The host part of preprocess before the silence trim: volume normalisation, and the refusal of the trims this project
+        does not implement (trim_long_silences; trim_silence without trim_silence_top_db)."""
         if self.norm_wav:
             y = self.normalize_volume(y, increase_only=True)
         if self.trim_long_silences:
             raise NotImplementedError('trim_long_silences needs webrtcvad voice-activity detection, which this project does not '
                                       'implement; set trim_long_silences: false in the audio settings')
         if self.trim_silence:
-            raise NotImplementedError('trim_silence needs librosa.effects.trim, which this project does not implement; set '
-                                      'trim_silence: false in the audio settings')
+            self._trim_top_db()
+        return y
+
+    def pad_to_hop(self, y):
+        """The last step of preprocess: one zero sample appended to a clip whose length is a multiple of hop_length."""
         if y.shape[0] % self.hop_length == 0:
             y = np.pad(y, (0, 1))
         return y

@@ -40,6 +40,7 @@ EXPORTS = [
     'ttsb_stft_complex_ragged_workspace_bytes', 'ttsb_stft_complex_ragged', 'ttsb_istft_ragged_workspace_bytes', 'ttsb_istft_ragged',
     'ttsb_griffinlim_ragged_workspace_bytes', 'ttsb_griffinlim_ragged',
     'ttsb_wavernn_workspace_bytes', 'ttsb_wavernn_generate',
+    'ttsb_trim_silence_workspace_bytes', 'ttsb_trim_silence_bounds',
 ]
 
 
@@ -172,6 +173,9 @@ def load() -> C.CDLL:
     lib.ttsb_wavernn_workspace_bytes.restype = C.c_int64
     lib.ttsb_wavernn_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
     lib.ttsb_wavernn_generate.argtypes = [t for _, t in WAVERNN_PARAMS] + [C.c_void_p]
+    lib.ttsb_trim_silence_workspace_bytes.restype = C.c_int64
+    lib.ttsb_trim_silence_workspace_bytes.argtypes = [C.c_void_p, C.c_int]
+    lib.ttsb_trim_silence_bounds.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     for name in EXPORTS:
         if not hasattr(lib, name):
             raise TtsbError(f'libttsb.so does not export {name}')
@@ -431,6 +435,24 @@ def resample_batch(wav, sample_offsets, src_rates, dst_rate, half_window, out_of
     ws = torch.empty(nb, dtype=torch.uint8, device=wav.device)
     _check(load().ttsb_resample_batch(ptr(wav), so, rates, n, int(dst_rate), ptr(half_window), half_window.numel(), oo, ptr(ws),
                                       C.c_int64(nb), ptr(out), _stream()), 'ttsb_resample_batch')
+
+
+def trim_silence_workspace_bytes(sample_offsets) -> int:
+    so, n = _host_offsets(sample_offsets)
+    nb = int(load().ttsb_trim_silence_workspace_bytes(so, n))
+    if nb < 0:
+        raise TtsbError(load().ttsb_last_error().decode())
+    return nb
+
+
+def trim_silence_bounds(wav, sample_offsets, top_db: float, bounds):
+    """[start, end) of the non-silent part of every clip of a packed ragged batch (include/ttsb.h: ttsb_trim_silence_bounds).
+    wav fp32 and bounds int32 (n_clips, 2) on the device; sample_offsets (n_clips + 1) is a host sequence."""
+    so, n = _host_offsets(sample_offsets)
+    nb = trim_silence_workspace_bytes(sample_offsets)
+    ws = torch.empty(nb, dtype=torch.uint8, device=wav.device)
+    _check(load().ttsb_trim_silence_bounds(ptr(wav), so, n, float(top_db), ptr(ws), C.c_int64(nb), ptr(bounds), _stream()),
+           'ttsb_trim_silence_bounds')
 
 
 # the longest shorter side of a pair ttsb_mcd_dtw takes (include/ttsb.h: TTSB_MCD_DTW_MAX_FRAMES)
