@@ -116,27 +116,16 @@ class TooShortToResample(ValueError):
     pass
 
 
-def host_preprocess(audio):
-    """The part of Audio.preprocess done before a file joins its batch: all of it, or with trim_silence everything before the
-    trim (the trim and the hop padding then run a batch at a time in trim_batch)."""
-    return audio.preprocess_before_trim if audio.trim_silence else audio.preprocess
-
-
 def wav_loader(audio):
-    """path -> (samples, None) preprocessed as Audio.load_wav does when the file is at the configured rate (up to the trim with
-    trim_silence), else the raw mono samples and their rate, to be resampled with the rest of the batch."""
-    from transformertts_b200.data.audio import resampled_length
-    preprocess = host_preprocess(audio)
+    """path -> Audio.read_for_batch(path): (samples, None) preprocessed as Audio.load_wav does when the file is at the configured
+    rate (up to the trim with trim_silence), else the raw mono samples and their rate, to be resampled with the rest of the batch."""
+    from transformertts_b200.data import audio as audio_module
 
     def load(path):
-        y, sr = audio.read_wav(str(path))
-        if sr == audio.sampling_rate:
-            return preprocess(y), None
         try:
-            resampled_length(len(y), sr, audio.sampling_rate)
-        except ValueError as e:
+            return audio.read_for_batch(str(path))
+        except audio_module.TooShortToResample as e:
             raise TooShortToResample(f'{path}: {e}') from None
-        return y, sr
     return load
 
 
@@ -151,21 +140,13 @@ def loaded_samples(audio):
     return size
 
 
-def resample_batch(audio, batch, rates_seen: dict):
-    """Resample the off-rate files of a batch in one launch, then preprocess them -> batch of (path, samples at the configured rate)."""
-    off = [c for c, (_, (_, sr)) in enumerate(batch) if sr is not None]
-    done = dict(zip(off, audio.resample_ragged([batch[c][1] for c in off]))) if off else {}
-    for c in off:
-        sr = batch[c][1][1]
-        rates_seen[sr] = rates_seen.get(sr, 0) + 1
-    preprocess = host_preprocess(audio)
-    return [(path, preprocess(done[c]) if c in done else y) for c, (path, (y, _)) in enumerate(batch)]
-
-
-def trim_batch(audio, batch):
-    """trim_silence: trim every clip of a batch in one launch, then pad it to the hop as Audio.preprocess does."""
-    trimmed = audio.trim_silence_ragged([y for _, y in batch])
-    return [(path, audio.pad_to_hop(y)) for (path, _), y in zip(batch, trimmed)]
+def finish_batch(audio, batch, rates_seen: dict):
+    """Audio.finish_batch on the loaded files of a batch (the off-rate ones resampled in one launch, every one trimmed in one
+    launch with trim_silence) -> batch of (path, samples at the configured rate, preprocessed)."""
+    for _, (_, sr) in batch:
+        if sr is not None:
+            rates_seen[sr] = rates_seen.get(sr, 0) + 1
+    return list(zip([path for path, _ in batch], audio.finish_batch([item for _, item in batch])))
 
 
 def too_short(audio, n_samples: int) -> bool:
@@ -182,10 +163,9 @@ def process_mels(cm, audio, wav_files, budget: int = BATCH_SAMPLES):
     len_dict, remove_files, mel_lens, pitches, rates_seen = {}, [], [], {}, {}
     with ThreadPoolExecutor(max_workers=2) as writer:
         for raw in batches(wav_files, budget, wav_loader(audio), loaded_samples(audio)):
-            batch = resample_batch(audio, raw, rates_seen)
+            batch = finish_batch(audio, raw, rates_seen)
             short = set()
             if audio.trim_silence:
-                batch = trim_batch(audio, batch)
                 short = {c for c, (_, y) in enumerate(batch) if too_short(audio, len(y))}
             kept = [item for c, item in enumerate(batch) if c not in short]
             if kept:

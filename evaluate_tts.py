@@ -7,6 +7,7 @@
     python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder hifigan --vocoder_checkpoint g_02500000 [--vocoder_config v1]
     python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder wavernn --vocoder_checkpoint latest_weights.pyt
     python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder melgan --vocoder_checkpoint melgan.pt --f0    # + pitch / voicing
+    python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder melgan --vocoder_checkpoint melgan.pt --mcep  # + WORLD MCD
 
 The validation split is read as train_tts.py reads it (``valid_metadata``, ``mels``, ``durations`` and ``char_pitch`` of the
 config's data directory; ``pitch_stats.pkl`` for pitch errors in Hz when it exists).  For every checkpoint:
@@ -19,10 +20,15 @@ config's data directory; ``pitch_stats.pkl`` for pitch errors in Hz when it exis
 * with ``--f0`` (needs ``--vocoder`` and the recorded frame pitch ``pitch.<audio>/<name>.npy`` with ``pitch_stats.pkl``): the
   WORLD F0 of both sets of waveforms (DIO + StoneMask on the GPU, at the frame period of the training data) against the
   recorded frame pitch along each line's MCD-DTW warping path: gross pitch error (GPE, |f / f_ref - 1| > 20 %), voicing
-  decision error (VDE), F0 frame error (FFE) and the F0 RMSE in cents.
+  decision error (VDE), F0 frame error (FFE) and the F0 RMSE in cents;
+* with ``--mcep`` (needs ``--vocoder`` and the recordings under the config's ``wav_directory``, rebuilt as
+  create_training_data.py prepared them): the WORLD mel-cepstral distortion of both sets of waveforms against the recordings,
+  the MCD published work reports: CheapTrick envelopes at the DIO / StoneMask F0, pysptk's sp2mc to ``--mcep_order`` (24) at
+  ``--mcep_alpha`` (default: pysptk's mcepalpha of the sampling rate, 0.455 at 22050 Hz), DTW over mc_1..mc_order.
 
-MCD is the DCT of the 80-bin natural-log mel (coefficients 1..24), not the SPTK / WORLD mel-cepstrum: compare its numbers
-with each other, not with papers (see transformertts_b200/utils/evaluation.py).  Per-line and corpus-mean values go to
+The plain MCD is the DCT of the 80-bin natural-log mel (coefficients 1..24), not the SPTK / WORLD mel-cepstrum: compare its
+numbers with each other; ``--mcep`` gives the one comparable to papers (see transformertts_b200/utils/evaluation.py).  Per-line
+and corpus-mean values go to
 ``<OUTDIR>/evaluation.json`` (default OUTDIR: MODEL_DIR), one entry per checkpoint; one summary line per checkpoint is printed.
 """
 from __future__ import annotations
@@ -45,9 +51,22 @@ def parse_args(argv=None):
                         help='HiFi-GAN config: a config.json path or v1 / v2 / v3 (default: config.json beside the checkpoint)')
     parser.add_argument('--f0', action='store_true',
                         help='also score the F0 and voicing of the vocoded audio against the recorded frame pitch (needs --vocoder)')
+    parser.add_argument('--mcep', action='store_true',
+                        help='also score the WORLD mel-cepstral distortion of the vocoded audio against the recordings (needs --vocoder '
+                             'and wav_directory)')
+    parser.add_argument('--mcep_order', default=24, type=int)
+    parser.add_argument('--mcep_alpha', default=None, type=float, help='all-pass constant (default: mcepalpha of the sampling rate)')
     args = parser.parse_args(argv)
     if args.f0 and args.vocoder is None:
         parser.error('--f0 scores vocoded audio: it needs --vocoder')
+    if args.mcep and args.vocoder is None:
+        parser.error('--mcep scores vocoded audio: it needs --vocoder')
+    if (args.mcep_alpha is not None or args.mcep_order != 24) and not args.mcep:
+        parser.error('--mcep_order and --mcep_alpha apply to --mcep only')
+    if args.mcep and args.mcep_order < 1:
+        parser.error(f'--mcep_order must be at least 1, got {args.mcep_order}')
+    if args.mcep_alpha is not None and not abs(args.mcep_alpha) < 1:
+        parser.error(f'--mcep_alpha must be in (-1, 1), got {args.mcep_alpha}')
     if args.vocoder in ('melgan', 'hifigan', 'wavernn') and args.vocoder_checkpoint is None:
         parser.error(f'--vocoder {args.vocoder} needs --vocoder_checkpoint PATH')
     if args.vocoder_config is not None and args.vocoder != 'hifigan':
@@ -77,7 +96,12 @@ def main(argv=None):
 
     cm = TrainingConfigManager(args.config)
     ev.natural_log_mels(cm.config, 'config')
-    vs = ev.load_validation_set(cm, frame_pitch=args.f0)
+    if args.mcep and cm.wav_directory is None:
+        raise SystemExit('--mcep scores against the recordings: the config\'s paths settings need a wav_directory')
+    vs = ev.load_validation_set(cm, frame_pitch=args.f0, recordings=args.mcep)
+    mcep_alpha = None
+    if args.mcep:
+        mcep_alpha = args.mcep_alpha if args.mcep_alpha is not None else ev.mcep_alpha(int(cm.config['sampling_rate']))
     root = Path(args.path)
     results = []
     vocoder = None
@@ -98,13 +122,16 @@ def main(argv=None):
                     part = [m.T for m in mels[start:start + VOCODE_CHUNK]]
                     wavs.extend(vocode_chunk(vocoder, audio, part, start))
                 return wavs
-        res = ev.evaluate_model(model, vs, n_ceps=args.n_ceps, vocode=vocode, audio=audio, f0=args.f0)
+        res = ev.evaluate_model(model, vs, n_ceps=args.n_ceps, vocode=vocode, audio=audio, f0=args.f0, mcep=args.mcep,
+                                mcep_order=args.mcep_order, mcep_alpha=mcep_alpha)
         res = dict(checkpoint=str(ckpt), step=int(step), **res)
         results.append(res)
         print(ev.summary_line(f'{ckpt.name} (step {step})', res), flush=True)
     out = Path(args.outdir) if args.outdir is not None else root
-    ev.write_json({'config': str(args.config), 'n_ceps': args.n_ceps, 'vocoder': args.vocoder, 'lines': len(vs.names),
-                   'checkpoints': results}, out / 'evaluation.json')
+    summary = {'config': str(args.config), 'n_ceps': args.n_ceps, 'vocoder': args.vocoder, 'lines': len(vs.names)}
+    if args.mcep:
+        summary.update(mcep_order=args.mcep_order, mcep_alpha=mcep_alpha)
+    ev.write_json(dict(summary, checkpoints=results), out / 'evaluation.json')
     print(f'wrote {out / "evaluation.json"}')
     return 0
 

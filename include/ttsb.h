@@ -556,6 +556,39 @@ int ttsb_trim_silence_bounds(const float* wav, const int32_t* sample_offsets, in
                              int64_t workspace_bytes, int32_t* bounds, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Spectral envelope by WORLD's CheapTrick  (Audio.spectral_envelope_device; pyworld.cheaptrick(x, f0, t, fs, q1=-0.15,
+ * f0_floor=71); tests/world_mcep_oracle.py restates the algorithm; the readings of WORLD's C++ are in DESIGN.md section 9)
+ *   wav: fp32 clips packed end to end, clip c at samples sample_offsets[c] .. sample_offsets[c+1] - 1 (int32 (n_clips + 1), HOST
+ *   memory, from 0).  The frames are those of ttsb_pitch_dio_stonemask: clip c has int(1000.0 L_c / fs / frame_period_ms) + 1
+ *   frames at t_i = i frame_period_ms / 1000, f0_offsets (int32 (n_clips + 1), HOST memory) their prefix sums and f0 (fp64, device)
+ *   the F0 of every frame in Hz (0: unvoiced).  fft_size: a power of two in [256, 4096] whose F0 floor 3 fs / (fft_size - 3) is
+ *   below 500 Hz; pyworld's is 2^(1 + int(log2(3 fs / f0_floor + 1))): 1024 at 16 to 24 kHz and 2048 at 44.1 and 48 kHz for
+ *   f0_floor 71.  A frame whose F0 is at or below that floor takes 500 Hz (WORLD's default); a frame whose F0 is above fs / 4 or
+ *   NaN gets an envelope of NaN.  envelope_out (fp64 (f0_offsets[n_clips], fft_size / 2 + 1), device) receives the power spectral
+ *   envelope of every frame, bins 0 .. fft_size / 2.  Float64 throughout, without FMA contraction.  WORLD's safeguard noise (1e-12
+ *   randn per windowed sample, |randn| eps per bin) is drawn from a counter-based hash keyed by (clip-local frame, sample or bin,
+ *   site) instead of WORLD's sequential generator, so a clip's envelope does not depend, bit for bit, on the other clips or its
+ *   position in the batch.  One CTA per frame.
+ *   workspace: ttsb_cheaptrick_workspace_bytes(...) bytes of device memory, 16-byte aligned (the offset tables and fft_size / 2
+ *   twiddles).  NULL pointers, malformed offsets, an empty clip, f0_offsets that disagree with WORLD's frame count, fs outside
+ *   [8000, 192000], a frame_period_ms or q1 that is not finite (or <= 0), an fft_size out of range and a short workspace give
+ *   TTSB_ERR_INVALID_ARGUMENT before any CUDA call. */
+int64_t ttsb_cheaptrick_workspace_bytes(const int32_t* sample_offsets, const int32_t* f0_offsets, int n_clips, int fs,
+                                        double frame_period_ms, int fft_size);   /* -1 for invalid arguments */
+int ttsb_cheaptrick(const float* wav, const int32_t* sample_offsets, int n_clips, int fs, double frame_period_ms, const double* f0,
+                    const int32_t* f0_offsets, double q1, int fft_size, void* workspace, int64_t workspace_bytes, double* envelope_out,
+                    void* stream);
+
+/* Mel-cepstrum of power spectral envelopes  (Audio.world_mcep_batch; pysptk.sp2mc(sp, order, alpha))
+ *   envelope: fp64 (n_frames, fft_size / 2 + 1) on the device, fft_size a power of two in [256, 4096]; matrix: fp64 (order + 1,
+ *   fft_size / 2 + 1) on the device, the linear map of sp2mc (irfft of log sp, c0 halved, SPTK's freqt to order at alpha) that
+ *   utils/evaluation.py's sp2mc_matrix builds on the host.  mc_out (fp64 (n_frames, order + 1), device) receives
+ *   mc[f][k] = sum_j matrix[k][j] log(envelope[f][j]), summed in a fixed order, so a frame's result does not depend on the
+ *   others.  One CTA per frame, no workspace.  NULL pointers, n_frames < 1, an fft_size out of range and an order outside
+ *   [1, fft_size / 2) give TTSB_ERR_INVALID_ARGUMENT before any CUDA call. */
+int ttsb_sp2mc(const double* envelope, int n_frames, int fft_size, const double* matrix, int order, double* mc_out, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * mel -> waveform  (Audio.reconstruct_waveform, data/audio.py:94-110: librosa mel_to_stft(power=1) + griffinlim(32, momentum .99))
  *   n_fft 1024, hop 256, periodic Hann, centred frames with reflect padding (the reference configuration).
  * ------------------------------------------------------------------------------------------------------- */
@@ -675,6 +708,22 @@ int64_t ttsb_mcd_dtw_path_workspace_bytes(const int32_t* x_offsets, const int32_
 int ttsb_mcd_dtw_path(const float* x, const int32_t* x_offsets, const float* y, const int32_t* y_offsets, int n_pairs, int n_mels,
                       const double* dct, int n_ceps, double kappa, void* workspace, int64_t workspace_bytes, double* cost_out,
                       int32_t* path_len_out, int32_t* path_out, void* stream);
+/* ttsb_mcd_dtw_ceps, ttsb_mcd_dtw_ceps_path: ttsb_mcd_dtw and ttsb_mcd_dtw_path over cepstra the caller computed (the WORLD
+ *   mel-cepstra of evaluate_tts.py --mcep).  x and y are frame-major fp64 (frames, ld) on the device, pair p's frames given by
+ *   x_offsets / y_offsets as above; c_k of a frame is its column first + k - 1, k = 1..K = n_ceps (first >= 0, first + K <= ld).
+ *   The columns are copied into the workspace ttsb_mcd_dtw reads, and the same kernels sweep them: distance, DTW, tie rule,
+ *   frame and cell limits, outputs and path are those of ttsb_mcd_dtw / ttsb_mcd_dtw_path, bit for bit for the same cepstra.
+ *   workspace: ttsb_mcd_dtw_ceps_workspace_bytes(...) / ttsb_mcd_dtw_ceps_path_workspace_bytes(...) bytes (the same sizes as
+ *   ttsb_mcd_dtw's and ttsb_mcd_dtw_path's), 8-byte aligned.  What those refuse, and first or K out of range, give
+ *   TTSB_ERR_INVALID_ARGUMENT before any CUDA call. */
+int64_t ttsb_mcd_dtw_ceps_workspace_bytes(const int32_t* x_offsets, const int32_t* y_offsets, int n_pairs, int n_ceps); /* -1: invalid */
+int ttsb_mcd_dtw_ceps(const double* x, const int32_t* x_offsets, const double* y, const int32_t* y_offsets, int n_pairs, int ld,
+                      int first, int n_ceps, double kappa, void* workspace, int64_t workspace_bytes, double* cost_out,
+                      int32_t* path_len_out, void* stream);
+int64_t ttsb_mcd_dtw_ceps_path_workspace_bytes(const int32_t* x_offsets, const int32_t* y_offsets, int n_pairs, int n_ceps); /* -1 */
+int ttsb_mcd_dtw_ceps_path(const double* x, const int32_t* x_offsets, const double* y, const int32_t* y_offsets, int n_pairs, int ld,
+                           int first, int n_ceps, double kappa, void* workspace, int64_t workspace_bytes, double* cost_out,
+                           int32_t* path_len_out, int32_t* path_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Ragged-batch Conv1D on the tensor cores (the MelGAN and HiFi-GAN generators, transformertts_b200/model/melgan.py and

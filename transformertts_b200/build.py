@@ -20,13 +20,14 @@ INCLUDE = PKG.parent / 'include'
 OUT = PKG / 'libttsb.so'
 OBJ_DIR = PKG / 'build'
 SOURCES = ['host.cu', 'gemm_tc.cu', 'attention_tc.cu', 'bgemm_tc.cu', 'attn_probs_tc.cu', 'rowops.cu', 'stft_mel.cu', 'train_ops.cu', 'alignment.cu', 'dp_nccl.cu', 'griffin_lim.cu', 'decode.cu', 'pitch.cu', 'conv1d_tc.cu',
-           'resample.cu', 'evaluate.cu', 'stft_general.cu', 'wavernn.cu', 'trim.cu']
+           'resample.cu', 'evaluate.cu', 'stft_general.cu', 'wavernn.cu', 'trim.cu', 'world_sp.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=default', '--expt-relaxed-constexpr']
 # pitch.cu restates WORLD's float64 C++, resample.cu resampy's float64 loop, evaluate.cu the float64 definition of MCD-DTW
-# and trim.cu librosa's frame powers in float64, which round every product and sum: no contraction into FMA (see the files'
-# headers)
-FILE_FLAGS = {'pitch.cu': ['-fmad=false'], 'resample.cu': ['-fmad=false'], 'evaluate.cu': ['-fmad=false'], 'trim.cu': ['-fmad=false']}
+# trim.cu librosa's frame powers and world_sp.cu WORLD's CheapTrick in float64, which round every product and sum: no contraction
+# into FMA (see the files' headers)
+FILE_FLAGS = {'pitch.cu': ['-fmad=false'], 'resample.cu': ['-fmad=false'], 'evaluate.cu': ['-fmad=false'], 'trim.cu': ['-fmad=false'],
+              'world_sp.cu': ['-fmad=false']}
 
 
 def _nvcc() -> str:

@@ -19,6 +19,10 @@
 // Each warp writes its two words from __ballot_sync, so no atomics and no byte-sized stores.  Diagonal d of a pair holds
 // 2 ceil(n_d / 32) words (n_d its cells) after those of diagonals 0 .. d - 1, from the pair's offset in the workspace.
 // After the last diagonal, thread 0 of the CTA walks back from (Tx - 1, Ty - 1) and writes the path from entry L - 1 down.
+//
+// ttsb_mcd_dtw_ceps(_path) score cepstra the caller computed (the WORLD mel-cepstra of world_sp.cu): mcd_ceps_copy_kernel
+// copies columns first .. first + K - 1 of the frame-major float64 rows into the same k-major workspace, and the same
+// mcd_dtw_kernel<false / true> sweeps it.
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -46,6 +50,17 @@ __global__ void mcd_cepstra_kernel(const float* __restrict__ x, int64_t Fx, cons
     double acc = 0.0;
     for (int m = 0; m < M; ++m) acc = __dadd_rn(acc, __dmul_rn(__ldg(d + m), (double)__ldg(row + m)));
     ceps[e] = acc;
+  }
+}
+
+// ceps[k F + f] = column first + k of row f of x (f < Fx), else of row f - Fx of y; rows of ld doubles
+__global__ void mcd_ceps_copy_kernel(const double* __restrict__ x, int64_t Fx, const double* __restrict__ y, int64_t F, int ld,
+                                     int first, int K, double* __restrict__ ceps) {
+  const int64_t n = F * K;
+  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+    const int k = (int)(e / F);
+    const int64_t f = e - (int64_t)k * F;
+    ceps[e] = f < Fx ? __ldg(x + f * ld + first + k) : __ldg(y + (f - Fx) * ld + first + k);
   }
 }
 
@@ -204,24 +219,12 @@ static int mcd_plan(const char* fn, const int32_t* xo, const int32_t* yo, int n_
   return 0;
 }
 
-template <bool kPath>
-static int mcd_dtw_run(const char* fn, const float* x, const int32_t* x_offsets, const float* y, const int32_t* y_offsets, int n_pairs,
-                       int n_mels, const double* dct, int n_ceps, double kappa, void* workspace, int64_t workspace_bytes, double* cost_out,
-                       int32_t* path_len_out, int32_t* path_out, void* stream_v) {
-  if (!x || !y || !dct || !workspace || !cost_out || !path_len_out || (kPath && !path_out)) {
-    set_last_error("%s: NULL pointer", fn);
-    return TTSB_ERR_INVALID_ARGUMENT;
-  }
-  if (n_mels < 2 || n_ceps < 1 || n_ceps >= n_mels) {
-    set_last_error("%s: need 1 <= n_ceps < n_mels (c0 is left out), got n_ceps %d, n_mels %d", fn, n_ceps, n_mels);
-    return TTSB_ERR_INVALID_ARGUMENT;
-  }
-  if (!std::isfinite(kappa) || kappa <= 0.0) {
-    set_last_error("%s: kappa must be finite and positive", fn);
-    return TTSB_ERR_INVALID_ARGUMENT;
-  }
-  McdPlan pl;
-  if (int rc = mcd_plan(fn, x_offsets, y_offsets, n_pairs, n_ceps, kPath, &pl)) return rc;
+// Checks the workspace, uploads the pair table (and the path's bit offsets), lets `fill` write the k-major cepstra into the
+// workspace and sweeps them with mcd_dtw_kernel<kPath>.
+template <bool kPath, typename Fill>
+static int mcd_dtw_launch(const char* fn, const McdPlan& pl, const int32_t* x_offsets, const int32_t* y_offsets, int n_pairs, int n_ceps,
+                          double kappa, void* workspace, int64_t workspace_bytes, double* cost_out, int32_t* path_len_out,
+                          int32_t* path_out, void* stream_v, Fill fill) {
   if (workspace_bytes < pl.bytes) {
     set_last_error("%s: workspace holds %lld bytes, needs %lld (%s_workspace_bytes)", fn, (long long)workspace_bytes,
                    (long long)pl.bytes, fn);
@@ -258,13 +261,63 @@ static int mcd_dtw_run(const char* fn, const float* x, const int32_t* x_offsets,
   }
   const int64_t n = pl.frames * n_ceps;
   const int grid = (int)std::min<int64_t>((n + 255) / 256, 8 * (int64_t)num_sms());
-  mcd_cepstra_kernel<<<grid, 256, 0, stream>>>(x, pl.fx, y, pl.frames, n_mels, dct, n_ceps, ceps);
-  count_launch();
-  if (int rc = check_cuda(cudaGetLastError(), "mcd_cepstra_kernel")) return rc;
+  if (int rc = fill(ceps, grid, stream)) return rc;
   mcd_dtw_kernel<kPath><<<n_pairs, DTW_THREADS, sm, stream>>>(ceps, pl.frames, n_ceps, tab_dev, n_pairs, kappa, cost_out, path_len_out,
                                                               bits, bit_off, reinterpret_cast<int2*>(path_out));
   count_launch();
   return check_cuda(cudaGetLastError(), "mcd_dtw_kernel");
+}
+
+template <bool kPath>
+static int mcd_dtw_run(const char* fn, const float* x, const int32_t* x_offsets, const float* y, const int32_t* y_offsets, int n_pairs,
+                       int n_mels, const double* dct, int n_ceps, double kappa, void* workspace, int64_t workspace_bytes, double* cost_out,
+                       int32_t* path_len_out, int32_t* path_out, void* stream_v) {
+  if (!x || !y || !dct || !workspace || !cost_out || !path_len_out || (kPath && !path_out)) {
+    set_last_error("%s: NULL pointer", fn);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  if (n_mels < 2 || n_ceps < 1 || n_ceps >= n_mels) {
+    set_last_error("%s: need 1 <= n_ceps < n_mels (c0 is left out), got n_ceps %d, n_mels %d", fn, n_ceps, n_mels);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  if (!std::isfinite(kappa) || kappa <= 0.0) {
+    set_last_error("%s: kappa must be finite and positive", fn);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  McdPlan pl;
+  if (int rc = mcd_plan(fn, x_offsets, y_offsets, n_pairs, n_ceps, kPath, &pl)) return rc;
+  return mcd_dtw_launch<kPath>(fn, pl, x_offsets, y_offsets, n_pairs, n_ceps, kappa, workspace, workspace_bytes, cost_out, path_len_out,
+                               path_out, stream_v, [&](double* ceps, int grid, cudaStream_t stream) {
+                                 mcd_cepstra_kernel<<<grid, 256, 0, stream>>>(x, pl.fx, y, pl.frames, n_mels, dct, n_ceps, ceps);
+                                 count_launch();
+                                 return check_cuda(cudaGetLastError(), "mcd_cepstra_kernel");
+                               });
+}
+
+template <bool kPath>
+static int mcd_dtw_ceps_run(const char* fn, const double* x, const int32_t* x_offsets, const double* y, const int32_t* y_offsets,
+                            int n_pairs, int ld, int first, int n_ceps, double kappa, void* workspace, int64_t workspace_bytes,
+                            double* cost_out, int32_t* path_len_out, int32_t* path_out, void* stream_v) {
+  if (!x || !y || !workspace || !cost_out || !path_len_out || (kPath && !path_out)) {
+    set_last_error("%s: NULL pointer", fn);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  if (n_ceps < 1 || first < 0 || (int64_t)first + n_ceps > ld) {
+    set_last_error("%s: need n_ceps >= 1, first >= 0 and first + n_ceps <= ld, got first %d, n_ceps %d, ld %d", fn, first, n_ceps, ld);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  if (!std::isfinite(kappa) || kappa <= 0.0) {
+    set_last_error("%s: kappa must be finite and positive", fn);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  McdPlan pl;
+  if (int rc = mcd_plan(fn, x_offsets, y_offsets, n_pairs, n_ceps, kPath, &pl)) return rc;
+  return mcd_dtw_launch<kPath>(fn, pl, x_offsets, y_offsets, n_pairs, n_ceps, kappa, workspace, workspace_bytes, cost_out, path_len_out,
+                               path_out, stream_v, [&](double* ceps, int grid, cudaStream_t stream) {
+                                 mcd_ceps_copy_kernel<<<grid, 256, 0, stream>>>(x, pl.fx, y, pl.frames, ld, first, n_ceps, ceps);
+                                 count_launch();
+                                 return check_cuda(cudaGetLastError(), "mcd_ceps_copy_kernel");
+                               });
 }
 
 }  // namespace ttsb
@@ -295,4 +348,30 @@ extern "C" int ttsb_mcd_dtw_path(const float* x, const int32_t* x_offsets, const
                                  double* cost_out, int32_t* path_len_out, int32_t* path_out, void* stream_v) {
   return mcd_dtw_run<true>("ttsb_mcd_dtw_path", x, x_offsets, y, y_offsets, n_pairs, n_mels, dct, n_ceps, kappa, workspace,
                            workspace_bytes, cost_out, path_len_out, path_out, stream_v);
+}
+
+extern "C" int64_t ttsb_mcd_dtw_ceps_workspace_bytes(const int32_t* x_offsets, const int32_t* y_offsets, int n_pairs, int n_ceps) {
+  McdPlan pl;
+  if (mcd_plan("ttsb_mcd_dtw_ceps_workspace_bytes", x_offsets, y_offsets, n_pairs, n_ceps, false, &pl)) return -1;
+  return pl.bytes;
+}
+
+extern "C" int ttsb_mcd_dtw_ceps(const double* x, const int32_t* x_offsets, const double* y, const int32_t* y_offsets, int n_pairs, int ld,
+                                 int first, int n_ceps, double kappa, void* workspace, int64_t workspace_bytes, double* cost_out,
+                                 int32_t* path_len_out, void* stream_v) {
+  return mcd_dtw_ceps_run<false>("ttsb_mcd_dtw_ceps", x, x_offsets, y, y_offsets, n_pairs, ld, first, n_ceps, kappa, workspace,
+                                 workspace_bytes, cost_out, path_len_out, nullptr, stream_v);
+}
+
+extern "C" int64_t ttsb_mcd_dtw_ceps_path_workspace_bytes(const int32_t* x_offsets, const int32_t* y_offsets, int n_pairs, int n_ceps) {
+  McdPlan pl;
+  if (mcd_plan("ttsb_mcd_dtw_ceps_path_workspace_bytes", x_offsets, y_offsets, n_pairs, n_ceps, true, &pl)) return -1;
+  return pl.bytes;
+}
+
+extern "C" int ttsb_mcd_dtw_ceps_path(const double* x, const int32_t* x_offsets, const double* y, const int32_t* y_offsets, int n_pairs,
+                                      int ld, int first, int n_ceps, double kappa, void* workspace, int64_t workspace_bytes,
+                                      double* cost_out, int32_t* path_len_out, int32_t* path_out, void* stream_v) {
+  return mcd_dtw_ceps_run<true>("ttsb_mcd_dtw_ceps_path", x, x_offsets, y, y_offsets, n_pairs, ld, first, n_ceps, kappa, workspace,
+                                workspace_bytes, cost_out, path_len_out, path_out, stream_v);
 }

@@ -3,7 +3,9 @@ data/audio.py:72-92, 196-231) by the fused CUDA kernels ``ttsb_stft_mel_log`` / 
 StoneMask (data/audio.py:146-151) by ``ttsb_pitch_dio_stonemask``, wav loading and preprocessing (data/audio.py:126-141,
 154-162) on the host, resampling to ``sampling_rate`` (librosa.load's ``kaiser_best`` resampy filter, data/audio.py:126-130) by
 ``ttsb_resample_batch``, the ``trim_silence`` trim of leading and trailing silence (librosa.effects.trim, data/audio.py:164-169)
-by ``ttsb_trim_silence_bounds``, and mel -> waveform by Griffin-Lim.
+by ``ttsb_trim_silence_bounds``, and mel -> waveform by Griffin-Lim.  For the WORLD mel-cepstral distortion of
+``evaluate_tts.py --mcep`` (no reference counterpart): WORLD's CheapTrick envelope by ``ttsb_cheaptrick`` and pysptk's sp2mc by
+``ttsb_sp2mc`` (``world_mcep_batch``), and ``load_wavs``, which rebuilds recordings as ``create_training_data.py`` prepares them.
 
 ``trim_long_silences`` (webrtcvad voice-activity detection) is not implemented: ``preprocess`` refuses it, and refuses
 ``trim_silence`` without ``trim_silence_top_db``.  ``load_wav`` refuses a file whose rate differs from ``sampling_rate``; such
@@ -70,14 +72,18 @@ def kaiser_best_half_window() -> np.ndarray:
     return kaiser(2 * n + 1, beta)[n:] * sinc_win
 
 
+class TooShortToResample(ValueError):
+    """A clip with no output sample to compute at the target rate."""
+
+
 def resampled_length(n_samples: int, sr_orig: int, sr_new: int) -> int:
     """Samples of a clip of `n_samples` at sr_orig after resampling to sr_new: ceil(n ratio) in float64, as librosa's fix_length.
-    Raises ValueError when int(n ratio) < 1 (resampy has no output sample to compute)."""
+    Raises TooShortToResample (a ValueError) when int(n ratio) < 1 (resampy has no output sample to compute)."""
     if sr_orig == sr_new:
         return int(n_samples)
     ratio = float(sr_new) / sr_orig
     if int(n_samples * ratio) < 1:
-        raise ValueError(f'{n_samples} samples at {sr_orig} Hz are too short to resample to {sr_new} Hz')
+        raise TooShortToResample(f'{n_samples} samples at {sr_orig} Hz are too short to resample to {sr_new} Hz')
     return int(np.ceil(n_samples * ratio))
 
 
@@ -407,6 +413,63 @@ class Audio:
         """reference: data/audio.py:146-151 (pw.dio(y, fs, frame_period=hop/fs*1000) then pw.stonemask) -> float64 (T,)."""
         return self.extract_pitch_batch([y])[0]
 
+    @property
+    def cheaptrick_fft_size(self) -> int:
+        """pyworld's CheapTrick FFT size at f0_floor 71 Hz: 2^(1 + int(log2(3 fs / 71 + 1))) (1024 at 16 to 24 kHz, 2048 at 44.1
+        and 48 kHz)."""
+        return 1 << (1 + int(np.log(3.0 * self.sampling_rate / 71.0 + 1) / np.log(2.0)))
+
+    def spectral_envelope_device(self, wav: torch.Tensor, sample_offsets, f0: torch.Tensor, f0_offsets) -> tuple:
+        """ttsb_cheaptrick (pyworld.cheaptrick with q1 -0.15, f0_floor 71): packed fp32 clips and their float64 F0 at WORLD's frames
+        (extract_pitch_device) on the device -> (packed float64 envelopes (frames, cheaptrick_fft_size / 2 + 1) on the device, frame
+        offsets).  Clip c's envelope does not depend on the other clips."""
+        with torch.cuda.device(self.device):
+            so = np.asarray(sample_offsets, dtype=np.int64)
+            fo = np.asarray(f0_offsets, dtype=np.int64)
+            n = self.cheaptrick_fft_size
+            env = torch.empty((int(fo[-1]), n // 2 + 1), dtype=torch.float64, device=self.device)
+            fp = self.hop_length / self.sampling_rate * 1000
+            lib.cheaptrick(wav.contiguous(), so, self.sampling_rate, fp, f0.contiguous(), fo, -0.15, n, env)
+            return env, fo
+
+    def world_mcep_batch(self, wavs, order: int = 24, alpha: float = None) -> list:
+        """WORLD mel-cepstra of every clip of a list: DIO + StoneMask (extract_pitch_device), CheapTrick (spectral_envelope_device)
+        and pysptk's sp2mc (ttsb_sp2mc) on one packed upload per PITCH_CHUNK_SAMPLES samples, at the frame period of the training
+        data -> list of float64 (T_c, order + 1).  alpha None: mcep_alpha(sampling_rate).  A clip too short for DIO raises
+        ValueError."""
+        from ..utils.evaluation import PITCH_CHUNK_SAMPLES, _dio_takes, mcep_alpha, sp2mc_matrix
+        ws = [np.asarray(w, dtype=np.float32).reshape(-1) for w in wavs]
+        for c, w in enumerate(ws):
+            if not _dio_takes(self, len(w)):
+                raise ValueError(f'clip {c} has {len(w)} samples; DIO needs more WORLD frames than its voice_range_minimum')
+        alpha = mcep_alpha(self.sampling_rate) if alpha is None else float(alpha)
+        n = self.cheaptrick_fft_size
+        key = (n, int(order), alpha)
+        if getattr(self, '_sp2mc', (None,))[0] != key:
+            self._sp2mc = (key, torch.from_numpy(sp2mc_matrix(n, int(order), alpha)).to(self.device).contiguous())
+        W = self._sp2mc[1]
+        chunks, samples = [[]], 0
+        for c, w in enumerate(ws):
+            if chunks[-1] and samples + len(w) > PITCH_CHUNK_SAMPLES:
+                chunks.append([])
+                samples = 0
+            chunks[-1].append(c)
+            samples += len(w)
+        out = [None] * len(ws)
+        with torch.cuda.device(self.device):
+            for chunk in chunks:
+                if not chunk:
+                    continue
+                wav, so = self._pack([ws[c] for c in chunk])
+                f0, fo = self.extract_pitch_device(wav, so)
+                env, _ = self.spectral_envelope_device(wav, so, f0, fo)
+                mc = torch.empty((env.shape[0], int(order) + 1), dtype=torch.float64, device=self.device)
+                lib.sp2mc(env, W, mc)
+                mc = mc.cpu().numpy()
+                for r, c in enumerate(chunk):
+                    out[c] = mc[fo[r]:fo[r + 1]]
+        return out
+
     def mel_spectrogram_ragged(self, wavs) -> list:
         """mel_spectrogram of every clip of a list in one launch -> list of (T_c, n_mels) float32, T_c = 1 + L_c // hop."""
         wav, so = self._pack(wavs)
@@ -492,6 +555,39 @@ class Audio:
         if y.ndim == 2:
             y = np.mean(y, axis=1)
         return y, sr
+
+    def read_for_batch(self, wav_path):
+        """The per-file half of preparing a recording as create_training_data.py does (load_wavs): -> (samples, None), read and
+        preprocessed up to the trim (all of preprocess without trim_silence), when the file is at sampling_rate; else (the raw mono
+        samples, the file's rate) for finish_batch to resample.  A file too short to resample raises TooShortToResample."""
+        y, sr = self.read_wav(wav_path)
+        if sr == self.sampling_rate:
+            return self._host_preprocess()(y), None
+        resampled_length(len(y), sr, self.sampling_rate)
+        return y, sr
+
+    def finish_batch(self, items) -> list:
+        """The batch half of load_wavs on read_for_batch items: the off-rate clips resampled in one launch (resample_ragged) and
+        preprocessed; with trim_silence, every clip trimmed in one launch (trim_silence_ragged) and padded to the hop -> list of
+        float32 arrays at sampling_rate, each what preprocess makes of the file's samples at that rate."""
+        items = list(items)
+        off = [c for c, (_, sr) in enumerate(items) if sr is not None]
+        done = dict(zip(off, self.resample_ragged([items[c] for c in off]))) if off else {}
+        preprocess = self._host_preprocess()
+        clips = [preprocess(done[c]) if c in done else y for c, (y, _) in enumerate(items)]
+        if self.trim_silence:
+            clips = [self.pad_to_hop(y) for y in self.trim_silence_ragged(clips)]
+        return clips
+
+    def load_wavs(self, wav_paths) -> list:
+        """Recordings as create_training_data.py prepares them before their mels: read_wav, GPU resampling of an off-rate file,
+        volume normalisation, trim_silence when configured, the pad to the hop -> list of float32 arrays."""
+        return self.finish_batch([self.read_for_batch(p) for p in wav_paths])
+
+    def _host_preprocess(self):
+        """The part of preprocess done per file: all of it, or with trim_silence everything before the trim (the trim and the hop
+        padding run a batch at a time in finish_batch)."""
+        return self.preprocess_before_trim if self.trim_silence else self.preprocess
 
     def load_wav(self, wav_path, preprocess: bool = True):
         """reference: data/audio.py:126-130 (librosa.load(path, sr=sampling_rate)) -> (float32 samples, rate): read_wav, then

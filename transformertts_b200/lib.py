@@ -41,6 +41,8 @@ EXPORTS = [
     'ttsb_griffinlim_ragged_workspace_bytes', 'ttsb_griffinlim_ragged',
     'ttsb_wavernn_workspace_bytes', 'ttsb_wavernn_generate',
     'ttsb_trim_silence_workspace_bytes', 'ttsb_trim_silence_bounds',
+    'ttsb_cheaptrick_workspace_bytes', 'ttsb_cheaptrick', 'ttsb_sp2mc',
+    'ttsb_mcd_dtw_ceps_workspace_bytes', 'ttsb_mcd_dtw_ceps', 'ttsb_mcd_dtw_ceps_path_workspace_bytes', 'ttsb_mcd_dtw_ceps_path',
 ]
 
 
@@ -176,6 +178,18 @@ def load() -> C.CDLL:
     lib.ttsb_trim_silence_workspace_bytes.restype = C.c_int64
     lib.ttsb_trim_silence_workspace_bytes.argtypes = [C.c_void_p, C.c_int]
     lib.ttsb_trim_silence_bounds.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.ttsb_cheaptrick_workspace_bytes.restype = C.c_int64
+    lib.ttsb_cheaptrick_workspace_bytes.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_int]
+    lib.ttsb_cheaptrick.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.c_double, C.c_int,
+                                    C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.ttsb_sp2mc.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    for name in ('ttsb_mcd_dtw_ceps_workspace_bytes', 'ttsb_mcd_dtw_ceps_path_workspace_bytes'):
+        getattr(lib, name).restype = C.c_int64
+        getattr(lib, name).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    lib.ttsb_mcd_dtw_ceps.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double,
+                                      C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.ttsb_mcd_dtw_ceps_path.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                           C.c_double, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     for name in EXPORTS:
         if not hasattr(lib, name):
             raise TtsbError(f'libttsb.so does not export {name}')
@@ -512,6 +526,70 @@ def mcd_dtw_path(x, x_offsets, y, y_offsets, dct, kappa, cost_out, path_len_out,
     ws = torch.empty(nb, dtype=torch.uint8, device=x.device)
     _check(load().ttsb_mcd_dtw_path(ptr(x), xo, ptr(y), yo, n, int(n_mels), ptr(dct), int(n_ceps), float(kappa), ptr(ws), C.c_int64(nb),
                                     ptr(cost_out), ptr(path_len_out), ptr(path_out), _stream()), 'ttsb_mcd_dtw_path')
+
+
+def cheaptrick_workspace_bytes(sample_offsets, f0_offsets, fs: int, frame_period_ms: float, fft_size: int) -> int:
+    so, n = _host_offsets(sample_offsets)
+    fo, n_f = _host_offsets(f0_offsets)
+    if n_f != n:
+        raise TtsbError(f'{n} clips in sample_offsets, {n_f} in f0_offsets')
+    nb = int(load().ttsb_cheaptrick_workspace_bytes(so, fo, n, int(fs), float(frame_period_ms), int(fft_size)))
+    if nb < 0:
+        raise TtsbError(load().ttsb_last_error().decode())
+    return nb
+
+
+def cheaptrick(wav, sample_offsets, fs, frame_period_ms, f0, f0_offsets, q1, fft_size, envelope_out):
+    """WORLD's CheapTrick spectral envelope of every frame of a packed ragged batch (include/ttsb.h: ttsb_cheaptrick).  wav fp32,
+    f0 fp64 (frames,) and envelope_out fp64 (frames, fft_size / 2 + 1) on the device; the offset tables are host sequences."""
+    so, n = _host_offsets(sample_offsets)
+    fo, _ = _host_offsets(f0_offsets)
+    nb = cheaptrick_workspace_bytes(sample_offsets, f0_offsets, fs, frame_period_ms, fft_size)
+    ws = torch.empty(nb, dtype=torch.uint8, device=wav.device)
+    _check(load().ttsb_cheaptrick(ptr(wav), so, n, int(fs), float(frame_period_ms), ptr(f0), fo, float(q1), int(fft_size), ptr(ws),
+                                  C.c_int64(nb), ptr(envelope_out), _stream()), 'ttsb_cheaptrick')
+
+
+def sp2mc(envelope, matrix, mc_out):
+    """mc = matrix . log(envelope) per frame (include/ttsb.h: ttsb_sp2mc).  envelope fp64 (frames, fft_size / 2 + 1), matrix fp64
+    (order + 1, fft_size / 2 + 1) and mc_out fp64 (frames, order + 1) on the device."""
+    n_frames, nb = envelope.shape
+    if matrix.dim() != 2 or matrix.shape[1] != nb or tuple(mc_out.shape) != (n_frames, matrix.shape[0]):
+        raise TtsbError(f'envelope {tuple(envelope.shape)}, matrix {tuple(matrix.shape)} and mc_out {tuple(mc_out.shape)}: need '
+                        f'(frames, bins), (order + 1, bins) and (frames, order + 1)')
+    _check(load().ttsb_sp2mc(ptr(envelope), int(n_frames), 2 * (nb - 1), ptr(matrix), int(matrix.shape[0]) - 1, ptr(mc_out), _stream()),
+           'ttsb_sp2mc')
+
+
+def mcd_dtw_ceps_workspace_bytes(x_offsets, y_offsets, n_ceps: int, path: bool = False) -> int:
+    xo, n = _host_offsets(x_offsets)
+    yo, n_y = _host_offsets(y_offsets)
+    if n_y != n:
+        raise TtsbError(f'{n} pairs in x_offsets, {n_y} in y_offsets')
+    fn = load().ttsb_mcd_dtw_ceps_path_workspace_bytes if path else load().ttsb_mcd_dtw_ceps_workspace_bytes
+    nb = int(fn(xo, yo, n, int(n_ceps)))
+    if nb < 0:
+        raise TtsbError(load().ttsb_last_error().decode())
+    return nb
+
+
+def mcd_dtw_ceps(x, x_offsets, y, y_offsets, first: int, n_ceps: int, kappa, cost_out, path_len_out, path_out=None):
+    """ttsb_mcd_dtw_ceps (ttsb_mcd_dtw_ceps_path when path_out is given) over caller-given cepstra: x, y fp64 (frames, ld) on the
+    device, columns first .. first + n_ceps - 1 scored; cost_out, path_len_out and path_out as mcd_dtw / mcd_dtw_path take them."""
+    xo, n = _host_offsets(x_offsets)
+    yo, n_y = _host_offsets(y_offsets)
+    if n_y != n:
+        raise TtsbError(f'{n} pairs in x_offsets, {n_y} in y_offsets')
+    if x.dim() != 2 or y.dim() != 2 or x.shape[1] != y.shape[1]:
+        raise TtsbError(f'x {tuple(x.shape)} and y {tuple(y.shape)}: need two (frames, ld) arrays of the same ld')
+    nb = mcd_dtw_ceps_workspace_bytes(x_offsets, y_offsets, n_ceps, path=path_out is not None)
+    ws = torch.empty(nb, dtype=torch.uint8, device=x.device)
+    head = (ptr(x), xo, ptr(y), yo, n, int(x.shape[1]), int(first), int(n_ceps), float(kappa), ptr(ws), C.c_int64(nb), ptr(cost_out),
+            ptr(path_len_out))
+    if path_out is None:
+        _check(load().ttsb_mcd_dtw_ceps(*head, _stream()), 'ttsb_mcd_dtw_ceps')
+    else:
+        _check(load().ttsb_mcd_dtw_ceps_path(*head, ptr(path_out), _stream()), 'ttsb_mcd_dtw_ceps_path')
 
 
 # ------------------------------------------------------------------------------------------------------------

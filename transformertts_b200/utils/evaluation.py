@@ -6,13 +6,19 @@ reference has no counterpart: it shows validation predictions in TensorBoard).
   ``natural_log_mels``), coefficients 1..K with c0 (the energy) left out;
   the frame distance is 10 / ln 10 * sqrt(2 sum_k (c_k - c'_k)^2) dB and a line's MCD is the DTW path cost over the path
   length.  This is not the all-pass warped mel-cepstrum of SPTK / WORLD, so the numbers are not comparable to MCD figures in
-  papers that use those; they rank models and vocoders of this project against each other.
+  papers that use those; they rank models and vocoders of this project against each other (``mcep=True`` below gives the
+  comparable one).
 * Duration errors of the integer durations against the Aligner's durations: mean absolute error in frames per phoneme, the
   rate of exact matches and the ratio of predicted to recorded frames.
 * Pitch RMSE over the phonemes whose target pitch is not 0 (unvoiced), in normalised units and, with ``pitch_stats.pkl``, in Hz.
 * F0 of vocoded audio (``f0=True``): the WORLD F0 (DIO + StoneMask on the GPU) of the vocoded waveforms against the recorded
   frame pitch, frame by frame along the MCD-DTW warping path (``ttsb_mcd_dtw_path``): gross pitch error (GPE), voicing
   decision error (VDE), F0 frame error (FFE) and the F0 RMSE in cents (``f0_scores``).
+* WORLD mel-cepstral distortion of vocoded audio (``mcep=True``): the MCD that published TTS and vocoder work reports.  Both
+  the vocoded waveforms and the recordings go through DIO + StoneMask, CheapTrick and pysptk's sp2mc (``Audio.world_mcep_batch``,
+  order 24 at ``mcep_alpha(fs)`` by default); mc_1..mc_order are DTW-aligned and scored by 10 / ln 10 sqrt(2 sum_k dmc_k^2) per
+  path step (``mcep_mcd_dtw``, ``ttsb_mcd_dtw_ceps``).  Its numbers are comparable to those of pyworld + pysptk pipelines (WORLD's
+  safeguard noise is drawn differently, see DESIGN.md section 7).
 
 Corpus values are means over lines."""
 from __future__ import annotations
@@ -131,6 +137,71 @@ def mcd_dtw_paths(mels_a: Sequence, mels_b: Sequence, n_ceps: int = DEFAULT_N_CE
     return cost, path_len, cost / path_len, paths
 
 
+def mcep_alpha(fs: int) -> float:
+    """pysptk.util.mcepalpha(fs): the all-pass constant alpha on the grid 0, 0.001, .. 0.999 whose frequency warping
+    arctan((1 - a^2) sin w / ((1 + a^2) cos w - 2a)) (mod pi) is closest in mean square to the mel scale 1000 / ln 2 ln(1 + f /
+    1000), both normalised to end at 1, over 1000 points up to fs / 2 (0.41 at 16 kHz, 0.455 at 22.05 kHz, 0.544 at 44.1 kHz)."""
+    n = 1000
+    f = (fs / 2.0) / n * np.arange(n)
+    mel = 1000.0 / np.log(2) * np.log(1 + f / 1000.0)
+    mel = mel / mel[-1]
+    omega = np.pi / n * np.arange(n)
+    alphas = np.arange(0.0, 1.0, 0.001)
+    a = alphas[:, None]
+    with np.errstate(divide='ignore', invalid='ignore'):
+        warp = np.arctan((1 - a * a) * np.sin(omega) / ((1 + a * a) * np.cos(omega) - 2 * a))
+    warp = np.where(warp < 0, warp + np.pi, warp)
+    warp = warp / warp[:, -1:]
+    return float(alphas[int(np.argmin(np.sum((mel - warp) ** 2, axis=1) / n))])
+
+
+def sp2mc_matrix(fft_size: int, order: int, alpha: float) -> np.ndarray:
+    """pysptk.sp2mc as a matrix: sp2mc(sp, order, alpha) = W @ log(sp) for a power spectrum sp of fft_size / 2 + 1 bins, W float64
+    (order + 1, fft_size / 2 + 1).  Built by running sp2mc's linear steps on the unit vectors: c = irfft(e_j), c[0] /= 2, then
+    SPTK's freqt recursion over all fft_size coefficients of c (g_0 = c_i + a d_0, g_1 = (1 - a^2) d_0 + a d_1,
+    g_k = d_{k-1} + a (d_k - g_{k-1}), for i = fft_size - 1 .. 0)."""
+    nb = fft_size // 2 + 1
+    c = np.fft.irfft(np.eye(nb), n=fft_size, axis=0)      # (fft_size, nb): column j is irfft(e_j)
+    c[0] /= 2.0
+    b = 1.0 - alpha * alpha
+    g = np.zeros((order + 1, nb))
+    for i in range(fft_size - 1, -1, -1):
+        d = g.copy()
+        g[0] = c[i] + alpha * d[0]
+        if order >= 1:
+            g[1] = b * d[0] + alpha * d[1]
+        for k in range(2, order + 1):
+            g[k] = d[k - 1] + alpha * (d[k] - g[k - 1])
+    return g
+
+
+def mcep_mcd_dtw(mceps_a: Sequence, mceps_b: Sequence, order: int):
+    """MCD-DTW of mel-cepstra mceps_a[i] against mceps_b[i] (float64 (T, >= order + 1), tensors or arrays) on coefficients
+    1..order (``ttsb_mcd_dtw_ceps``; mc_0, the energy, is left out) -> (cost, path_len, mcd) numpy arrays as mcd_dtw returns them."""
+    if len(mceps_a) != len(mceps_b) or len(mceps_a) == 0:
+        raise ValueError(f'need two non-empty lists of the same length, got {len(mceps_a)} and {len(mceps_b)}')
+    device = next((m.device for m in list(mceps_a) + list(mceps_b) if torch.is_tensor(m) and m.is_cuda),
+                  torch.device('cuda', torch.cuda.current_device()))
+
+    def pack(ms):
+        ts = [torch.as_tensor(m).to(device=device, dtype=torch.float64) for m in ms]
+        for i, t in enumerate(ts):
+            if t.dim() != 2 or t.shape[0] < 1 or t.shape[1] < order + 1:
+                raise ValueError(f'mel-cepstrum {i} has shape {tuple(t.shape)}; expected (T, >= {order + 1}) with T >= 1')
+        return torch.cat(ts).contiguous(), _offsets([t.shape[0] for t in ts])
+    x, xo = pack(mceps_a)
+    y, yo = pack(mceps_b)
+    if x.shape[1] != y.shape[1]:
+        raise ValueError(f'mel-cepstra of {x.shape[1]} and {y.shape[1]} coefficients')
+    n = len(xo) - 1
+    with torch.cuda.device(device):
+        cost = torch.empty(n, dtype=torch.float64, device=device)
+        path_len = torch.empty(n, dtype=torch.int32, device=device)
+        lib.mcd_dtw_ceps(x, xo, y, yo, 1, order, KAPPA, cost, path_len)
+        cost, path_len = cost.cpu().numpy(), path_len.cpu().numpy()
+    return cost, path_len, cost / path_len
+
+
 def f0_scores(f0_a_hz, f0_b_hz, path) -> dict:
     """Pitch and voicing of contour a against contour b (Hz, 0 = unvoiced; voiced means f0 > 0) over the steps (i, j) of a
     warping path, float64.  A step counts when i < len(a) and j < len(b) (a WORLD contour can be a frame shorter than the mel the
@@ -186,13 +257,38 @@ class ValidationSet:
     pitch: List[np.ndarray]
     pitch_stats: Optional[tuple] = None
     frame_pitch: Optional[List[np.ndarray]] = None   # recorded F0 per mel frame in Hz (0 = unvoiced), float64
+    recordings: Optional[List[np.ndarray]] = None    # the waveforms the mels were computed from, float32 at the data's rate
 
 
-def load_validation_set(cm, frame_pitch: bool = False) -> ValidationSet:
+def load_recordings(cm, names: Sequence[str], mels: Sequence[np.ndarray]) -> List[np.ndarray]:
+    """The waveform of every line, rebuilt from ``wav_directory`` as create_training_data.py built the one its mel came from
+    (Audio.load_wavs at the config's audio settings: read_wav, GPU resampling of an off-rate file, volume normalisation,
+    trim_silence when configured, the pad to the hop).  A line whose rebuilt waveform does not give its stored mel's frame count
+    (1 + L // hop_length) is refused with ValueError; a missing wav_directory or file raises FileNotFoundError."""
+    from ..data.audio import Audio
+    if cm.wav_directory is None:
+        raise FileNotFoundError('the recordings are read from the wav_directory of the paths settings, and the config has none')
+    wav_paths = {w.with_suffix('').name: w for w in Path(cm.wav_directory).expanduser().resolve().rglob('*.wav')}
+    missing = [n for n in names if n not in wav_paths]
+    if missing:
+        raise FileNotFoundError(f'no recording {missing[0]}.wav below {cm.wav_directory}'
+                                + (f' (and {len(missing) - 1} more)' if len(missing) > 1 else ''))
+    audio = Audio.from_config(cm.config)
+    wavs = audio.load_wavs([wav_paths[n] for n in names])
+    for n, w, m in zip(names, wavs, mels):
+        frames = 1 + len(w) // audio.hop_length
+        if frames != m.shape[0]:
+            raise ValueError(f'line {n}: the recording rebuilt from {wav_paths[n]} gives {frames} mel frames, its stored mel has '
+                             f'{m.shape[0]}; the mel was not computed from this file at these audio settings')
+    return wavs
+
+
+def load_validation_set(cm, frame_pitch: bool = False, recordings: bool = False) -> ValidationSet:
     """The config's validation split (``valid_metadata``, ``mels``, ``durations`` and ``char_pitch`` of a
     TrainingConfigManager), plus ``pitch_stats.pkl`` when the data directory has one.  With frame_pitch, also the recorded
     frame F0 ``pitch.<audio>/<name>.npy`` in Hz: create_training_data.py stores it normalised, so it is de-normalised with
-    ``pitch_stats.pkl`` (p std + mean where p != 0); a missing file or missing statistics raise FileNotFoundError."""
+    ``pitch_stats.pkl`` (p std + mean where p != 0); a missing file or missing statistics raise FileNotFoundError.  With
+    recordings, also each line's waveform (load_recordings)."""
     from ..data.datasets import DataReader
     reader = DataReader(cm.valid_metadata_path, is_processed=True)
     names = list(reader.text_dict)
@@ -215,12 +311,12 @@ def load_validation_set(cm, frame_pitch: bool = False) -> ValidationSet:
         for n in names:
             p = np.load(cm.pitch_dir / f'{n}.npy').astype(np.float64).reshape(-1)
             frames.append(np.where(p != 0.0, p * stats[1] + stats[0], 0.0))
+    mels = [np.load(cm.mel_dir / f'{n}.npy').astype(np.float32) for n in names]
     return ValidationSet(
-        names=names, phonemes=[reader.text_dict[n] for n in names],
-        mels=[np.load(cm.mel_dir / f'{n}.npy').astype(np.float32) for n in names],
+        names=names, phonemes=[reader.text_dict[n] for n in names], mels=mels,
         durations=[np.load(cm.duration_dir / f'{n}.npy').astype(np.int64) for n in names],
         pitch=[np.load(cm.pitch_per_char / f'{n}.npy').astype(np.float32).reshape(-1) for n in names], pitch_stats=stats,
-        frame_pitch=frames)
+        frame_pitch=frames, recordings=load_recordings(cm, names, mels) if recordings else None)
 
 
 def tokenize(model, phonemes: Sequence[str]) -> List[List[int]]:
@@ -302,6 +398,23 @@ def _f0_fields(prefix: str, audio, wavs: list, paths: list, frame_pitch: list) -
     return rows
 
 
+MCEP_KEYS = ('mcep_mcd', 'mcep_dtw_cost', 'mcep_path_len')
+
+
+def _mcep_fields(prefix: str, audio, wavs: list, rec_mceps: list, order: int, alpha: float) -> List[dict]:
+    """{prefix}mcep_mcd / mcep_dtw_cost / mcep_path_len per line: the WORLD mel-cepstra of wavs[i] against rec_mceps[i]
+    (mcep_mcd_dtw over mc_1..mc_order); None for a line without a waveform, or whose waveform or recording is too short for DIO."""
+    rows = [{prefix + k: None for k in MCEP_KEYS} for _ in wavs]
+    keep = [i for i, (w, r) in enumerate(zip(wavs, rec_mceps)) if w is not None and r is not None and _dio_takes(audio, len(w))]
+    if keep:
+        mceps = audio.world_mcep_batch([wavs[i] for i in keep], order=order, alpha=alpha)
+        cost, path_len, mcd = mcep_mcd_dtw(mceps, [rec_mceps[i] for i in keep], order)
+        for r, i in enumerate(keep):
+            rows[i] = {prefix + 'mcep_mcd': float(mcd[r]), prefix + 'mcep_dtw_cost': float(cost[r]),
+                       prefix + 'mcep_path_len': int(path_len[r])}
+    return rows
+
+
 def _resynthesis_mels(audio, wavs: List[np.ndarray]) -> List[torch.Tensor]:
     """Log-mels of vocoded waveforms through the ragged front end (Audio.mel_spectrogram_ragged_device)."""
     for i, w in enumerate(wavs):
@@ -324,7 +437,7 @@ def _means(lines: List[dict]) -> dict:
 
 def evaluate_model(model, vs: ValidationSet, n_ceps: int = DEFAULT_N_CEPS, teacher_forced: bool = True,
                    vocode: Optional[Callable[[List[np.ndarray]], List[np.ndarray]]] = None, audio=None, batch_size: int = 64,
-                   f0: bool = False) -> dict:
+                   f0: bool = False, mcep: bool = False, mcep_order: int = DEFAULT_N_CEPS, mcep_alpha: Optional[float] = None) -> dict:
     """Scores of `model` on `vs`: {'lines': [one dict per line], 'mean': {means over lines}}.
 
     Free-running (``predict_batch`` of the phonemes alone): MCD-DTW against the recorded mel, duration and pitch errors.  With
@@ -333,9 +446,14 @@ def evaluate_model(model, vs: ValidationSet, n_ceps: int = DEFAULT_N_CEPS, teach
     mels are vocoded, their log-mels re-extracted on the GPU and each scored against the recorded mel (vocoded_* and
     copy_synthesis_*; the latter is the vocoder's own floor).  With f0 (needs vocode and vs.frame_pitch), also the F0 scores of
     both sets of waveforms against the recorded frame pitch along the same MCD-DTW paths (vocoded_gpe ... and
-    copy_synthesis_gpe ..., see f0_scores), with the F0 of Audio.extract_pitch_batch at WORLD's settings of the training data."""
+    copy_synthesis_gpe ..., see f0_scores), with the F0 of Audio.extract_pitch_batch at WORLD's settings of the training data.
+    With mcep (needs vocode and vs.recordings), also the WORLD mel-cepstral distortion of both sets of waveforms against the
+    recordings (vocoded_mcep_mcd / _dtw_cost / _path_len and copy_synthesis_mcep_*): Audio.world_mcep_batch at mcep_order and
+    mcep_alpha (None: mcep_alpha(fs)) on each side, mcep_mcd_dtw over mc_1..mc_order."""
     if f0 and (vocode is None or vs.frame_pitch is None):
         raise ValueError('the F0 scores need a vocoder and the recorded frame pitch (load_validation_set(cm, frame_pitch=True))')
+    if mcep and (vocode is None or vs.recordings is None):
+        raise ValueError('the WORLD MCD needs a vocoder and the recordings (load_validation_set(cm, recordings=True))')
     to_ln = natural_log_mels(model.config)
     tokens = tokenize(model, vs.phonemes)
     outs = model.predict_batch(tokens, encode=False, phoneme_max_duration=None, batch_size=batch_size)
@@ -372,6 +490,15 @@ def evaluate_model(model, vs: ValidationSet, n_ceps: int = DEFAULT_N_CEPS, teach
             for prefix, wavs, ps in (('vocoded_', vocoded_wavs, paths), ('copy_synthesis_', copy_wavs, cpaths)):
                 for i, row in enumerate(_f0_fields(prefix, audio, wavs, ps, vs.frame_pitch)):
                     lines[i].update(row)
+        if mcep:
+            rec = [None] * len(vs.recordings)
+            kept = [i for i, w in enumerate(vs.recordings) if _dio_takes(audio, len(w))]
+            if kept:
+                for i, mc in zip(kept, audio.world_mcep_batch([vs.recordings[i] for i in kept], order=mcep_order, alpha=mcep_alpha)):
+                    rec[i] = mc
+            for prefix, wavs in (('vocoded_', vocoded_wavs), ('copy_synthesis_', copy_wavs)):
+                for i, row in enumerate(_mcep_fields(prefix, audio, wavs, rec, mcep_order, mcep_alpha)):
+                    lines[i].update(row)
     return {'lines': lines, 'mean': _means(lines)}
 
 
@@ -387,6 +514,8 @@ def summary_line(label: str, result: dict) -> str:
          + f' | pitch RMSE {f("pitch_rmse")}' + (f' ({f("pitch_rmse_hz", ".2f")} Hz)' if m.get('pitch_rmse_hz') is not None else ''))
     if 'vocoded_mcd' in m:
         s += f' | vocoded MCD {f("vocoded_mcd")}, copy synthesis {f("copy_synthesis_mcd")}'
+    if 'vocoded_mcep_mcd' in m:
+        s += f' | WORLD MCD vocoded {f("vocoded_mcep_mcd")}, copy synthesis {f("copy_synthesis_mcep_mcd")}'
     for label, p in (('vocoded', 'vocoded_'), ('copy synthesis', 'copy_synthesis_')):
         if f'{p}gpe' in m:
             s += (f' | {label} GPE {f(p + "gpe")}, VDE {f(p + "vde")}, FFE {f(p + "ffe")}, '
