@@ -3,7 +3,8 @@
 
     python create_training_data.py --config config/training_config.yaml [--skip_mels] [--skip_phonemes]
 
-It reads ``metadata_path`` (LJSpeech ``name|...|text`` lines) and the ``*.wav`` files below ``wav_directory``, and writes under
+It reads ``metadata_path`` (LJSpeech ``name|...|text`` lines) and the ``*.wav`` and ``*.flac`` files below ``wav_directory`` (a
+name that exists as both is refused), and writes under
 ``<train_data_directory>.<data_name>/``, as the reference does:
   * ``mels.<audio>/<name>.npy``: log-mel, float32 (T, mel_channels);
   * ``pitch.<audio>/<name>.npy``: per-frame f0 by DIO + StoneMask, float64 (T,), normalised by the corpus statistics;
@@ -15,6 +16,10 @@ It reads ``metadata_path`` (LJSpeech ``name|...|text`` lines) and the ``*.wav`` 
 The wavs are processed in batches of about ``BATCH_SAMPLES`` samples: a thread pool reads and preprocesses the files ahead of the
 GPU, each batch is uploaded once, its log-mels (``ttsb_stft_mel_log_batch``) and pitch (``ttsb_pitch_dio_stonemask``) are
 computed on the same packed buffer, and another thread pool writes the ``.npy`` files.
+
+FLAC files are read by the loader threads but decoded on the GPU, every FLAC file of a batch in one ``ttsb_flac_decode_batch``
+call; from then on their samples take exactly the path a WAV file's samples take, so a corpus stored as FLAC gives the same
+``.npy``, ``.pkl`` and metadata files, byte for byte, as the same corpus stored as WAV.
 
 Wavs at another rate than the audio settings' ``sampling_rate`` are resampled to it as the reference's ``librosa.load(path,
 sr=sampling_rate)`` does (resampy's ``kaiser_best`` filter): the off-rate files of a batch go through one
@@ -118,7 +123,8 @@ class TooShortToResample(ValueError):
 
 def wav_loader(audio):
     """path -> Audio.read_for_batch(path): (samples, None) preprocessed as Audio.load_wav does when the file is at the configured
-    rate (up to the trim with trim_silence), else the raw mono samples and their rate, to be resampled with the rest of the batch."""
+    rate (up to the trim with trim_silence), else the raw mono samples and their rate, to be resampled with the rest of the batch;
+    a FLAC file undecoded, to be decoded with the rest of the batch."""
     from transformertts_b200.data import audio as audio_module
 
     def load(path):
@@ -131,19 +137,24 @@ def wav_loader(audio):
 
 def loaded_samples(audio):
     """Size of a wav_loader item in the batch budget: its samples at the configured rate, so a batch of resampled files packs
-    about as many samples for the mel and pitch kernels as a batch of files already at that rate."""
-    from transformertts_b200.data.audio import resampled_length
+    about as many samples for the mel and pitch kernels as a batch of files already at that rate.  An undecoded FLAC file counts
+    its STREAMINFO total (resampled when the file is at another rate)."""
+    from transformertts_b200.data.audio import FlacStream, resampled_length
 
     def size(item):
         y, sr = item
+        if isinstance(y, FlacStream):
+            return resampled_length(y.total_samples, y.sample_rate, audio.sampling_rate)
         return len(y) if sr is None else resampled_length(len(y), sr, audio.sampling_rate)
     return size
 
 
 def finish_batch(audio, batch, rates_seen: dict):
-    """Audio.finish_batch on the loaded files of a batch (the off-rate ones resampled in one launch, every one trimmed in one
-    launch with trim_silence) -> batch of (path, samples at the configured rate, preprocessed)."""
-    for _, (_, sr) in batch:
+    """Audio.finish_batch on the loaded files of a batch (the FLAC ones decoded in one call, the off-rate ones resampled in one
+    launch, every one trimmed in one launch with trim_silence) -> batch of (path, samples at the configured rate, preprocessed)."""
+    from transformertts_b200.data.audio import FlacStream
+    for _, (y, sr) in batch:
+        sr = y.sample_rate if isinstance(y, FlacStream) and y.sample_rate != audio.sampling_rate else sr
         if sr is not None:
             rates_seen[sr] = rates_seen.get(sr, 0) + 1
     return list(zip([path for path, _ in batch], audio.finish_batch([item for _, item in batch])))

@@ -556,6 +556,40 @@ int ttsb_trim_silence_bounds(const float* wav, const int32_t* sample_offsets, in
                              int64_t workspace_bytes, int32_t* bounds, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * FLAC decoding  (Audio.read_flac_batch; data/audio.py:126-130: librosa.load(path) reads a .flac file through libsndfile;
+ * RFC 9639; tests/flac_oracle.py restates the format as an encoder and a plain decoder)
+ *   data: the frame bytes of every file (each file's bytes after its metadata blocks) concatenated in device memory; file f is
+ *   data[byte_offsets[f] .. byte_offsets[f+1]) (int64 (n_files + 1), HOST memory, from 0, at most 2^31 - 1 bytes per file).
+ *   stream_info: int64 (n_files, TTSB_FLAC_INFO_FIELDS) in HOST memory, each file's STREAMINFO as (channels, bits_per_sample,
+ *   sample_rate, min_block_size, max_block_size, total_samples).  Supported: 1 to 8 channels, 4 to 24 bits per sample, block sizes
+ *   16 <= min <= max <= 65535 (the last frame may be shorter), fixed and variable blocking, every frame-header code form.
+ *   mono_out: fp32 (sum of total_samples) on the device; file f's samples start at the sum of the totals of files < f and are what
+ *   libsndfile's float read gives (sample x 2^-(bits_per_sample - 1), exact) averaged over the channels as np.mean(y, axis=1) does
+ *   on float32 ((x0 + x1) + x2 ... for up to 7 channels, pairwise for 8, then an IEEE division).  pcm_out (optional, NULL for
+ *   none): int32 on the device, file f's samples interleaved (sample i channel c at P_f + i channels_f + c, P_f the sum of
+ *   total_samples x channels of files < f).  status_out: int32 (n_files, 2) on the device, (TTSB_FLAC_OK, frames) or (reason,
+ *   index of the frame where decoding stopped) per file; a file that fails gets zeros in its outputs and the others decode
+ *   normally.  The MD5 signature of STREAMINFO is not checked (libsndfile does not check it either).  Five launches whatever the
+ *   number of files; a file's output does not depend on the other files of the call.
+ *   workspace: ttsb_flac_decode_workspace_bytes(...) bytes of device memory, 16-byte aligned (about 2.4 bytes per frame byte, 24 per
+ *   frame and 4 per sample and channel).  NULL pointers, offsets that do not start at 0 or decrease, n_files outside [1, 65535],
+ *   a stream of 25 to 32 bits (refused by name) or outside the supported set, an unknown (0) total and a short workspace give
+ *   TTSB_ERR_INVALID_ARGUMENT before any CUDA call. */
+#define TTSB_FLAC_INFO_FIELDS 6
+#define TTSB_FLAC_OK 0
+#define TTSB_FLAC_NO_SYNC 1         /* no valid frame header (sync, codes, CRC-8) where a frame must start */
+#define TTSB_FLAC_BAD_FRAME 2       /* a reserved or invalid subframe, LPC or residual code, or non-zero padding */
+#define TTSB_FLAC_TRUNCATED 3       /* the data ends inside a frame or before STREAMINFO's total */
+#define TTSB_FLAC_CRC 4             /* the frame's CRC-16 (polynomial 0x8005) does not match */
+#define TTSB_FLAC_NUMBER 5          /* the coded frame or sample number is not the expected one */
+#define TTSB_FLAC_MISMATCH 6        /* block size, rate, channels or depth disagree with STREAMINFO */
+#define TTSB_FLAC_TOTAL 7           /* the frames hold more samples than STREAMINFO's total */
+int64_t ttsb_flac_decode_workspace_bytes(const int64_t* byte_offsets, const int64_t* stream_info, int n_files);  /* -1: invalid */
+int ttsb_flac_decode_batch(const uint8_t* data, const int64_t* byte_offsets, const int64_t* stream_info, int n_files,
+                           float* mono_out, int32_t* pcm_out, int32_t* status_out, void* workspace, int64_t workspace_bytes,
+                           void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Spectral envelope by WORLD's CheapTrick  (Audio.spectral_envelope_device; pyworld.cheaptrick(x, f0, t, fs, q1=-0.15,
  * f0_floor=71); tests/world_mcep_oracle.py restates the algorithm; the readings of WORLD's C++ are in DESIGN.md section 9)
  *   wav: fp32 clips packed end to end, clip c at samples sample_offsets[c] .. sample_offsets[c+1] - 1 (int32 (n_clips + 1), HOST

@@ -20,7 +20,7 @@ INCLUDE = PKG.parent / 'include'
 OUT = PKG / 'libttsb.so'
 OBJ_DIR = PKG / 'build'
 SOURCES = ['host.cu', 'gemm_tc.cu', 'attention_tc.cu', 'bgemm_tc.cu', 'attn_probs_tc.cu', 'rowops.cu', 'stft_mel.cu', 'train_ops.cu', 'alignment.cu', 'dp_nccl.cu', 'griffin_lim.cu', 'decode.cu', 'pitch.cu', 'conv1d_tc.cu',
-           'resample.cu', 'evaluate.cu', 'stft_general.cu', 'wavernn.cu', 'trim.cu', 'world_sp.cu']
+           'resample.cu', 'evaluate.cu', 'stft_general.cu', 'wavernn.cu', 'trim.cu', 'world_sp.cu', 'flac.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=default', '--expt-relaxed-constexpr']
 # pitch.cu restates WORLD's float64 C++, resample.cu resampy's float64 loop, evaluate.cu the float64 definition of MCD-DTW

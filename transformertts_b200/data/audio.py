@@ -6,6 +6,8 @@ StoneMask (data/audio.py:146-151) by ``ttsb_pitch_dio_stonemask``, wav loading a
 by ``ttsb_trim_silence_bounds``, and mel -> waveform by Griffin-Lim.  For the WORLD mel-cepstral distortion of
 ``evaluate_tts.py --mcep`` (no reference counterpart): WORLD's CheapTrick envelope by ``ttsb_cheaptrick`` and pysptk's sp2mc by
 ``ttsb_sp2mc`` (``world_mcep_batch``), and ``load_wavs``, which rebuilds recordings as ``create_training_data.py`` prepares them.
+``.flac`` recordings (librosa.load reads them through libsndfile) are decoded on the GPU by ``ttsb_flac_decode_batch``
+(``read_flac_batch``), a batch of files per call; the STREAMINFO's MD5 is not checked, as libsndfile does not check it.
 
 ``trim_long_silences`` (webrtcvad voice-activity detection) is not implemented: ``preprocess`` refuses it, and refuses
 ``trim_silence`` without ``trim_silence_top_db``.  ``load_wav`` refuses a file whose rate differs from ``sampling_rate``; such
@@ -74,6 +76,102 @@ def kaiser_best_half_window() -> np.ndarray:
 
 class TooShortToResample(ValueError):
     """A clip with no output sample to compute at the target rate."""
+
+
+FLAC_SKIPPED_BLOCKS = {1: 'PADDING', 2: 'APPLICATION', 3: 'SEEKTABLE', 4: 'VORBIS_COMMENT', 5: 'CUESHEET', 6: 'PICTURE'}
+
+
+class FlacStream:
+    """A .flac file read but not decoded: its bytes, where its frames start, and its STREAMINFO (RFC 9639 section 8.2)."""
+
+    def __init__(self, path, data: bytes):
+        self.path, self.data = str(path), data
+        name = self.path
+
+        def need(n, what):
+            if len(data) < n:
+                raise ValueError(f'{name}: truncated metadata ({what} needs {n} bytes, the file has {len(data)})')
+        need(4, 'the fLaC magic')
+        if data[:4] != b'fLaC':
+            raise ValueError(f'{name}: not a FLAC file (no fLaC magic)')
+        pos, first, last = 4, True, False
+        while not last:
+            need(pos + 4, 'a metadata block header')
+            kind, last, length = data[pos] & 0x7F, bool(data[pos] >> 7), int.from_bytes(data[pos + 1:pos + 4], 'big')
+            need(pos + 4 + length, f'metadata block type {kind}')
+            body = data[pos + 4:pos + 4 + length]
+            if first:
+                if kind != 0 or length != 34:
+                    raise ValueError(f'{name}: the first metadata block is type {kind} of {length} bytes, not a 34-byte STREAMINFO')
+                v = int.from_bytes(body[10:18], 'big')
+                self.min_block, self.max_block = int.from_bytes(body[0:2], 'big'), int.from_bytes(body[2:4], 'big')
+                self.sample_rate, self.channels = v >> 44, (v >> 41 & 7) + 1
+                self.bits_per_sample, self.total_samples = (v >> 36 & 31) + 1, v & ((1 << 36) - 1)
+            elif kind == 127:
+                raise ValueError(f'{name}: invalid metadata block type 127')
+            elif kind == 0:
+                raise ValueError(f'{name}: a second STREAMINFO block')
+            # PADDING, APPLICATION, SEEKTABLE, VORBIS_COMMENT, CUESHEET, PICTURE and reserved types carry nothing the decoder needs
+            first = False
+            pos += 4 + length
+        self.frame_offset = pos
+        if self.total_samples == 0:
+            raise ValueError(f'{name}: STREAMINFO gives an unknown (0) total sample count, which this decoder does not support')
+        if 25 <= self.bits_per_sample <= 32:
+            raise ValueError(f'{name}: {self.bits_per_sample}-bit FLAC is not supported (4 to 24 bits per sample)')
+        if self.bits_per_sample < 4:
+            raise ValueError(f'{name}: {self.bits_per_sample} bits per sample is not supported (4 to 24 bits per sample)')
+        if not 16 <= self.min_block <= self.max_block:
+            raise ValueError(f'{name}: STREAMINFO block sizes {self.min_block} to {self.max_block} (need 16 <= min <= max)')
+        if self.sample_rate == 0:
+            raise ValueError(f'{name}: STREAMINFO sample rate 0')
+
+    @classmethod
+    def read(cls, path):
+        with open(path, 'rb') as f:
+            return cls(path, f.read())
+
+    def stream_info(self):
+        """The row of ttsb_flac_decode_batch's stream_info table."""
+        return (self.channels, self.bits_per_sample, self.sample_rate, self.min_block, self.max_block, self.total_samples)
+
+
+class FlacDecodeError(ValueError):
+    """One or more streams of a FLAC batch are malformed; `failed` maps each such file to its reason."""
+
+    def __init__(self, failed: dict):
+        self.failed = failed
+        super().__init__('; '.join(f'{k}: {v}' for k, v in failed.items()))
+
+
+def flac_decode_streams(streams, device, pcm: bool = False) -> list:
+    """ttsb_flac_decode_batch on a list of FlacStream in one call -> per stream a dict: 'mono' (float32, what read_wav returns for
+    the same PCM as WAV), 'rate', 'pcm' (int32 (total, channels) with pcm=True) and 'error' (None, or the reason and frame index of
+    a malformed stream, whose samples are then zeros).  The other streams of the call decode normally."""
+    streams = list(streams)
+    if not streams:
+        return []
+    frames = [st.data[st.frame_offset:] for st in streams]
+    byte_off = np.concatenate([[0], np.cumsum([len(b) for b in frames])]).astype(np.int64)
+    totals = np.array([st.total_samples for st in streams], np.int64)
+    widths = totals * np.array([st.channels for st in streams], np.int64)
+    dev = torch.device(device)
+    with torch.cuda.device(dev):
+        blob = np.frombuffer(b''.join(frames), np.uint8)
+        data = torch.from_numpy(blob.copy()).to(dev) if len(blob) else torch.empty(0, dtype=torch.uint8, device=dev)
+        mono = torch.empty(int(totals.sum()), dtype=torch.float32, device=dev)
+        status = torch.empty((len(streams), 2), dtype=torch.int32, device=dev)
+        pcm_out = torch.empty(int(widths.sum()), dtype=torch.int32, device=dev) if pcm else None
+        lib.flac_decode_batch(data, byte_off, [st.stream_info() for st in streams], mono, status, pcm_out)
+        mono, status = mono.cpu().numpy(), status.cpu().numpy()
+        pcm_host = pcm_out.cpu().numpy() if pcm else None
+    out, mo, po = [], np.concatenate([[0], np.cumsum(totals)]), np.concatenate([[0], np.cumsum(widths)])
+    for i, st in enumerate(streams):
+        code, frame = int(status[i, 0]), int(status[i, 1])
+        err = None if code == 0 else f'{lib.FLAC_STATUS[code]} (frame {frame})'
+        out.append(dict(mono=mono[mo[i]:mo[i + 1]], rate=st.sample_rate, error=err,
+                        pcm=pcm_host[po[i]:po[i + 1]].reshape(-1, st.channels) if pcm else None))
+    return out
 
 
 def resampled_length(n_samples: int, sr_orig: int, sr_new: int) -> int:
@@ -556,10 +654,33 @@ class Audio:
             y = np.mean(y, axis=1)
         return y, sr
 
+    def read_flac_batch(self, paths) -> list:
+        """The decoding half of librosa.load for .flac files (data/audio.py:126-130; libsndfile reads FLAC) -> list of (float32 mono
+        samples, the file's own rate), all files decoded in one ttsb_flac_decode_batch call.  The samples equal read_wav's of the
+        same PCM stored as WAV, bit for bit.  Malformed metadata raises ValueError naming the file; malformed frames raise
+        FlacDecodeError naming every failed file, its reason and frame."""
+        streams = [p if isinstance(p, FlacStream) else FlacStream.read(p) for p in paths]
+        res = flac_decode_streams(streams, self.device)
+        failed = {st.path: r['error'] for st, r in zip(streams, res) if r['error']}
+        if failed:
+            raise FlacDecodeError(failed)
+        return [(r['mono'], r['rate']) for r in res]
+
+    def read_audio(self, path):
+        """read_wav, or read_flac_batch for a .flac file -> (float32 mono samples, the file's own rate)."""
+        if str(path).lower().endswith('.flac'):
+            return self.read_flac_batch([path])[0]
+        return self.read_wav(path)
+
     def read_for_batch(self, wav_path):
         """The per-file half of preparing a recording as create_training_data.py does (load_wavs): -> (samples, None), read and
         preprocessed up to the trim (all of preprocess without trim_silence), when the file is at sampling_rate; else (the raw mono
-        samples, the file's rate) for finish_batch to resample.  A file too short to resample raises TooShortToResample."""
+        samples, the file's rate) for finish_batch to resample.  A .flac file is returned undecoded, as (FlacStream, None), for
+        finish_batch to decode with the rest of the batch.  A file too short to resample raises TooShortToResample."""
+        if str(wav_path).lower().endswith('.flac'):
+            st = FlacStream.read(wav_path)
+            resampled_length(st.total_samples, st.sample_rate, self.sampling_rate)
+            return st, None
         y, sr = self.read_wav(wav_path)
         if sr == self.sampling_rate:
             return self._host_preprocess()(y), None
@@ -567,10 +688,16 @@ class Audio:
         return y, sr
 
     def finish_batch(self, items) -> list:
-        """The batch half of load_wavs on read_for_batch items: the off-rate clips resampled in one launch (resample_ragged) and
+        """The batch half of load_wavs on read_for_batch items: the FLAC files decoded in one call (read_flac_batch), after which
+        each takes the path of a WAV file's samples at its rate; the off-rate clips resampled in one launch (resample_ragged) and
         preprocessed; with trim_silence, every clip trimmed in one launch (trim_silence_ragged) and padded to the hop -> list of
         float32 arrays at sampling_rate, each what preprocess makes of the file's samples at that rate."""
         items = list(items)
+        flac = [c for c, (y, _) in enumerate(items) if isinstance(y, FlacStream)]
+        if flac:
+            preprocess = self._host_preprocess()
+            for c, (y, sr) in zip(flac, self.read_flac_batch([items[c][0] for c in flac])):
+                items[c] = (preprocess(y), None) if sr == self.sampling_rate else (y, sr)
         off = [c for c, (_, sr) in enumerate(items) if sr is not None]
         done = dict(zip(off, self.resample_ragged([items[c] for c in off]))) if off else {}
         preprocess = self._host_preprocess()
@@ -580,7 +707,8 @@ class Audio:
         return clips
 
     def load_wavs(self, wav_paths) -> list:
-        """Recordings as create_training_data.py prepares them before their mels: read_wav, GPU resampling of an off-rate file,
+        """Recordings as create_training_data.py prepares them before their mels: read_wav or the GPU FLAC decoder (one call for
+        all .flac files), GPU resampling of an off-rate file,
         volume normalisation, trim_silence when configured, the pad to the hop -> list of float32 arrays."""
         return self.finish_batch([self.read_for_batch(p) for p in wav_paths])
 
@@ -590,10 +718,10 @@ class Audio:
         return self.preprocess_before_trim if self.trim_silence else self.preprocess
 
     def load_wav(self, wav_path, preprocess: bool = True):
-        """reference: data/audio.py:126-130 (librosa.load(path, sr=sampling_rate)) -> (float32 samples, rate): read_wav, then
-        preprocess.  A file at another rate is refused here; read it with read_wav and resample it with resample_ragged (what
-        create_training_data.py does for a whole corpus)."""
-        y, sr = self.read_wav(wav_path)
+        """reference: data/audio.py:126-130 (librosa.load(path, sr=sampling_rate)) -> (float32 samples, rate): read_wav (or
+        read_flac_batch for a .flac file), then preprocess.  A file at another rate is refused here; read it with read_audio and
+        resample it with resample_ragged (what create_training_data.py does for a whole corpus)."""
+        y, sr = self.read_audio(wav_path)
         if sr != self.sampling_rate:
             raise ValueError(f'{wav_path}: sampled at {sr} Hz, expected {self.sampling_rate} Hz; read_wav + resample_ragged '
                              f'resample it')

@@ -67,9 +67,22 @@ def get_preprocessor_by_name(name: str) -> Callable:
     return {'ljspeech': ljspeech, 'post_processed_reader': post_processed_reader}[name.lower()]
 
 
+def scan_recordings(directory) -> dict:
+    """{stem: path} of every ``*.wav`` and ``*.flac`` below `directory` (recursively; datasets.py:13-16 scans ``*.wav``).  A stem
+    that exists as both a ``.wav`` and a ``.flac`` file is refused with ValueError naming it."""
+    root = Path(directory).expanduser().resolve()
+    wavs = {w.with_suffix('').name: w for w in root.rglob('*.wav')}
+    flacs = {w.with_suffix('').name: w for w in root.rglob('*.flac')}
+    both = sorted(set(wavs) & set(flacs))
+    if both:
+        raise ValueError(f'{both[0]} exists as both {wavs[both[0]]} and {flacs[both[0]]}'
+                         + (f' (and {len(both) - 1} more stems)' if len(both) > 1 else '') + '; keep one recording per name')
+    return {**wavs, **flacs}
+
+
 class DataReader:
-    """datasets.py:19-73.  With ``scan_wavs`` (datasets.py:13-16, 43-45), ``wav_paths`` maps the stem of every ``*.wav`` below
-    ``wav_directory`` (recursively) to its path."""
+    """datasets.py:19-73.  With ``scan_wavs`` (datasets.py:13-16, 43-45), ``wav_paths`` maps the stem of every ``*.wav`` and
+    ``*.flac`` below ``wav_directory`` (recursively) to its path (scan_recordings)."""
 
     def __init__(self, metadata_path, metadata_reading_function: Callable = None, training: bool = False, is_processed: bool = False,
                  wav_directory=None, scan_wavs: bool = False):
@@ -88,8 +101,7 @@ class DataReader:
         if scan_wavs:
             if self.wav_directory is None:
                 raise ValueError('scan_wavs needs a wav_directory (the wav_directory key of the paths settings)')
-            all_wavs = list(Path(self.wav_directory).expanduser().resolve().rglob('*.wav'))
-            self.wav_paths = {w.with_suffix('').name: w for w in all_wavs}
+            self.wav_paths = scan_recordings(self.wav_directory)
 
     KINDS = ('original', 'phonemized', 'train', 'valid')
 

@@ -43,6 +43,7 @@ EXPORTS = [
     'ttsb_trim_silence_workspace_bytes', 'ttsb_trim_silence_bounds',
     'ttsb_cheaptrick_workspace_bytes', 'ttsb_cheaptrick', 'ttsb_sp2mc',
     'ttsb_mcd_dtw_ceps_workspace_bytes', 'ttsb_mcd_dtw_ceps', 'ttsb_mcd_dtw_ceps_path_workspace_bytes', 'ttsb_mcd_dtw_ceps_path',
+    'ttsb_flac_decode_workspace_bytes', 'ttsb_flac_decode_batch',
 ]
 
 
@@ -106,6 +107,13 @@ class MhaArgs(C.Structure):
         ('kv_hi', C.c_void_p), ('kv_lo', C.c_void_p), ('ld_kv', C.c_int), ('Tk', C.c_int), ('causal', C.c_int),
         ('full_queries', C.c_int), ('weights_all', C.c_int),
     ]
+
+
+# include/ttsb.h: TTSB_FLAC_* (index = status code)
+FLAC_STATUS = ('ok', 'no valid frame header where a frame must start', 'a reserved or invalid subframe or residual code',
+               'the data ends inside a frame or before the STREAMINFO total', 'CRC-16 mismatch',
+               'unexpected frame or sample number', 'frame header disagrees with STREAMINFO',
+               'the frames hold more samples than the STREAMINFO total')
 
 
 class DecodeAttnArgs(C.Structure):
@@ -190,6 +198,10 @@ def load() -> C.CDLL:
                                       C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.ttsb_mcd_dtw_ceps_path.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                            C.c_double, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.ttsb_flac_decode_workspace_bytes.restype = C.c_int64
+    lib.ttsb_flac_decode_workspace_bytes.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+    lib.ttsb_flac_decode_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_int64, C.c_void_p]
     for name in EXPORTS:
         if not hasattr(lib, name):
             raise TtsbError(f'libttsb.so does not export {name}')
@@ -467,6 +479,38 @@ def trim_silence_bounds(wav, sample_offsets, top_db: float, bounds):
     ws = torch.empty(nb, dtype=torch.uint8, device=wav.device)
     _check(load().ttsb_trim_silence_bounds(ptr(wav), so, n, float(top_db), ptr(ws), C.c_int64(nb), ptr(bounds), _stream()),
            'ttsb_trim_silence_bounds')
+
+
+def _flac_tables(byte_offsets, infos):
+    import numpy as np
+    bo = np.ascontiguousarray(np.asarray(byte_offsets, dtype=np.int64))
+    n = len(infos)
+    if bo.ndim != 1 or len(bo) != n + 1:
+        raise TtsbError(f'{len(bo)} byte offsets for {n} files (need n_files + 1)')
+    info = np.asarray(infos, dtype=np.int64).reshape(-1)
+    if len(info) != 6 * n:
+        raise TtsbError(f'stream info must hold 6 values per file (include/ttsb.h: TTSB_FLAC_INFO_FIELDS), got {len(info)} for {n}')
+    return (C.c_int64 * len(bo))(*bo.tolist()), (C.c_int64 * len(info))(*info.tolist()), n
+
+
+def flac_decode_workspace_bytes(byte_offsets, infos) -> int:
+    """infos: per file (channels, bits_per_sample, sample_rate, min_block_size, max_block_size, total_samples)."""
+    bo, table, n = _flac_tables(byte_offsets, infos)
+    nb = int(load().ttsb_flac_decode_workspace_bytes(bo, table, n))
+    if nb < 0:
+        raise TtsbError(load().ttsb_last_error().decode())
+    return nb
+
+
+def flac_decode_batch(data, byte_offsets, infos, mono_out, status_out, pcm_out=None):
+    """Decode the frame bytes of every file of a packed batch of FLAC streams (include/ttsb.h: ttsb_flac_decode_batch).  data uint8,
+    mono_out fp32, status_out int32 (n_files, 2) and pcm_out int32 (optional) on the device; byte_offsets (n_files + 1) and infos
+    (flac_decode_workspace_bytes) are host sequences."""
+    bo, table, n = _flac_tables(byte_offsets, infos)
+    nb = flac_decode_workspace_bytes(byte_offsets, infos)
+    ws = torch.empty(max(nb, 16), dtype=torch.uint8, device=mono_out.device)
+    _check(load().ttsb_flac_decode_batch(ptr(data) if data.numel() else None, bo, table, n, ptr(mono_out), ptr(pcm_out),
+                                         ptr(status_out), ptr(ws), C.c_int64(nb), _stream()), 'ttsb_flac_decode_batch')
 
 
 # the longest shorter side of a pair ttsb_mcd_dtw takes (include/ttsb.h: TTSB_MCD_DTW_MAX_FRAMES)

@@ -262,16 +262,17 @@ class ValidationSet:
 
 def load_recordings(cm, names: Sequence[str], mels: Sequence[np.ndarray]) -> List[np.ndarray]:
     """The waveform of every line, rebuilt from ``wav_directory`` as create_training_data.py built the one its mel came from
-    (Audio.load_wavs at the config's audio settings: read_wav, GPU resampling of an off-rate file, volume normalisation,
+    (Audio.load_wavs at the config's audio settings: read_wav or the GPU FLAC decoder, GPU resampling of an off-rate file, volume normalisation,
     trim_silence when configured, the pad to the hop).  A line whose rebuilt waveform does not give its stored mel's frame count
     (1 + L // hop_length) is refused with ValueError; a missing wav_directory or file raises FileNotFoundError."""
     from ..data.audio import Audio
+    from ..data.datasets import scan_recordings
     if cm.wav_directory is None:
         raise FileNotFoundError('the recordings are read from the wav_directory of the paths settings, and the config has none')
-    wav_paths = {w.with_suffix('').name: w for w in Path(cm.wav_directory).expanduser().resolve().rglob('*.wav')}
+    wav_paths = scan_recordings(cm.wav_directory)
     missing = [n for n in names if n not in wav_paths]
     if missing:
-        raise FileNotFoundError(f'no recording {missing[0]}.wav below {cm.wav_directory}'
+        raise FileNotFoundError(f'no recording {missing[0]}.wav or .flac below {cm.wav_directory}'
                                 + (f' (and {len(missing) - 1} more)' if len(missing) > 1 else ''))
     audio = Audio.from_config(cm.config)
     wavs = audio.load_wavs([wav_paths[n] for n in names])
