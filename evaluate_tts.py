@@ -5,6 +5,7 @@
     python evaluate_tts.py --config CFG -p WEIGHTS_DIR --weights_glob 'step_*'          # every checkpoint, in step order
     python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder melgan --vocoder_checkpoint melgan.pt
     python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder hifigan --vocoder_checkpoint g_02500000 [--vocoder_config v1]
+    python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder bigvgan --vocoder_checkpoint bigvgan_generator.pt [--vocoder_config base]
     python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder wavernn --vocoder_checkpoint latest_weights.pyt
     python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder melgan --vocoder_checkpoint melgan.pt --f0    # + pitch / voicing
     python evaluate_tts.py --config CFG -p MODEL_DIR --vocoder melgan --vocoder_checkpoint melgan.pt --mcep  # + WORLD MCD
@@ -45,10 +46,11 @@ def parse_args(argv=None):
     parser.add_argument('--weights_glob', default=None, type=str, help="checkpoint directories under --path, e.g. 'step_*'")
     parser.add_argument('--outdir', '-o', dest='outdir', default=None, type=str)
     parser.add_argument('--n_ceps', default=24, type=int)
-    parser.add_argument('--vocoder', default=None, choices=('griffinlim', 'melgan', 'hifigan', 'wavernn'))
+    parser.add_argument('--vocoder', default=None, choices=('griffinlim', 'melgan', 'hifigan', 'bigvgan', 'wavernn'))
     parser.add_argument('--vocoder_checkpoint', default=None, type=str)
     parser.add_argument('--vocoder_config', default=None, type=str,
-                        help='HiFi-GAN config: a config.json path or v1 / v2 / v3 (default: config.json beside the checkpoint)')
+                        help='HiFi-GAN config (a config.json path or v1 / v2 / v3) or BigVGAN config (a config.json path or base / bigvgan); '
+                             'default: the config.json beside the checkpoint')
     parser.add_argument('--f0', action='store_true',
                         help='also score the F0 and voicing of the vocoded audio against the recorded frame pitch (needs --vocoder)')
     parser.add_argument('--mcep', action='store_true',
@@ -67,10 +69,10 @@ def parse_args(argv=None):
         parser.error(f'--mcep_order must be at least 1, got {args.mcep_order}')
     if args.mcep_alpha is not None and not abs(args.mcep_alpha) < 1:
         parser.error(f'--mcep_alpha must be in (-1, 1), got {args.mcep_alpha}')
-    if args.vocoder in ('melgan', 'hifigan', 'wavernn') and args.vocoder_checkpoint is None:
+    if args.vocoder in ('melgan', 'hifigan', 'bigvgan', 'wavernn') and args.vocoder_checkpoint is None:
         parser.error(f'--vocoder {args.vocoder} needs --vocoder_checkpoint PATH')
-    if args.vocoder_config is not None and args.vocoder != 'hifigan':
-        parser.error('--vocoder_config applies to --vocoder hifigan only')
+    if args.vocoder_config is not None and args.vocoder not in ('hifigan', 'bigvgan'):
+        parser.error('--vocoder_config applies to --vocoder hifigan and bigvgan only')
     return args
 
 

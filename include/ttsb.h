@@ -845,6 +845,28 @@ int ttsb_conv1d_ex_tc(const ttsb_conv1d_ex_args* a, void* stream);
 int ttsb_conv1d_out_tanh_ex(const void* in_hi, const void* in_lo, int ld_in, int channels, int halo, const int32_t* clip_offsets,
                             int n_clips, int drop_tail, const float* weight, float bias, void* workspace, int64_t workspace_bytes,
                             float* wav_out, void* stream);
+/* The same output layer with clamp(., -1, 1) in place of tanh (BigVGAN v2, use_tanh_at_final = false; pass bias 0 for a
+ * conv_post without bias).  Same arguments and refusals. */
+int ttsb_conv1d_out_clamp_ex(const void* in_hi, const void* in_lo, int ld_in, int channels, int halo, const int32_t* clip_offsets,
+                             int n_clips, int drop_tail, const float* weight, float bias, void* workspace, int64_t workspace_bytes,
+                             float* wav_out, void* stream);
+/* BigVGAN's anti-aliased periodic activation (Activation1d: UpSample1d, Snake / SnakeBeta, DownSample1d; model/bigvgan.py), one
+ * launch for a packed ragged batch.  in = hi (+ lo in bf16x3) planes in the layout above (`halo` rows, 0..
+ * TTSB_CONV1D_EX_MAX_HALO, ld columns, the first `channels` live); out = separate planes of the same layout.  Per clip c of
+ * L_c >= 1 rows and live channel ch, with x the clip's rows:
+ *   u[m] = 2 sum_i x[clamp(i - 5, 0, L - 1)] h_up[m + 15 - 2i]      m in [0, 2L), over the six i with 0 <= m + 15 - 2i <= 11
+ *   s[m] = u[m] + inv_beta[ch] sin^2(alpha[ch] u[m])
+ *   out[t] = sum_j h_down[j] s[clamp(2t + j - 5, 0, 2L - 1)]         t in [0, L), j = 0..11
+ * (F.pad(x, (5, 5), 'replicate'), 2 conv_transpose1d(stride 2), [15 : -15]; then F.pad(s, (5, 6), 'replicate'), conv1d(stride
+ * 2)).  fp32 arithmetic with full-range sinf, in a fixed order without atomics: a clip's output is bit-identical wherever it
+ * sits in the batch.  Columns [channels, ld) of clip rows are written as 0; halo rows are never written (zero-initialised
+ * planes keep the next conv's zero padding).  alpha, inv_beta: fp32 (channels) on the device; h_up, h_down: 12 fp32 taps each
+ * in HOST memory.  ld is a multiple of 8, the planes are 16-byte aligned and no output plane is an input plane.  workspace:
+ * ttsb_conv1d_workspace_bytes(n_clips) bytes.  NULL or misaligned planes, malformed offsets, channels > ld, aliased planes
+ * and a short workspace give TTSB_ERR_INVALID_ARGUMENT before any CUDA call. */
+int ttsb_snake_aa_ex(const void* in_hi, const void* in_lo, void* out_hi, void* out_lo, int ld, int channels, int halo,
+                     const int32_t* clip_offsets, int n_clips, const float* alpha, const float* inv_beta, const float* h_up,
+                     const float* h_down, int precision, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * WaveRNN generator (fatchord/WaveRNN, transformertts_b200/model/wavernn.py): the sample-rate recurrence of every fold of

@@ -5,6 +5,7 @@
     python predict_tts.py -t "phoneme string" ...
     python predict_tts.py -f lines.txt --vocoder melgan --vocoder_checkpoint melgan.pt ...
     python predict_tts.py -f lines.txt --vocoder hifigan --vocoder_checkpoint g_02500000 [--vocoder_config v1|config.json] ...
+    python predict_tts.py -f lines.txt --vocoder bigvgan --vocoder_checkpoint bigvgan_generator.pt [--vocoder_config base|bigvgan|config.json] ...
     python predict_tts.py -f lines.txt --vocoder wavernn --vocoder_checkpoint latest_weights.pyt ...
 
 Every input line is tokenised and the lines are turned into mels by ``ForwardTransformer.predict_batch`` (sorted by length,
@@ -16,7 +17,10 @@ reference's synthesis notebook does one line at a time; a line of T frames then 
 256 (T - 1)).  With ``--vocoder hifigan`` they go through a HiFi-GAN generator (``HiFiGANGenerator.vocode_batch``, a
 jik876/hifi-gan checkpoint; its config is ``--vocoder_config``, a config.json path or v1 / v2 / v3, by default the
 config.json beside the checkpoint), also 256 T samples per line; HiFi-GAN takes the MelGAN normaliser's log-mels, so a
-model with another ``normalizer`` is refused.  With ``--vocoder wavernn`` they go through a fatchord/WaveRNN generator
+model with another ``normalizer`` is refused.  ``--vocoder bigvgan`` does the same with an NVIDIA/BigVGAN generator
+(``BigVGANGenerator.vocode_batch``; config base / bigvgan or a config.json, by default the one beside the checkpoint), which
+also refuses a config whose ``sampling_rate``, ``num_mels``, ``hop_size`` or ``fmax`` differs from the model's audio
+settings.  With ``--vocoder wavernn`` they go through a fatchord/WaveRNN generator
 (``WaveRNNGenerator.vocode_batch``, batched folds of 11000 + 2 550 samples), line i sampled with seed i; its hop is the
 product of its upsample factors and must equal the model's, the model must use the ``WaveRNN`` normaliser, a line of T
 frames gives 275 (T - 1) samples at hop 275, and a line below 21 frames is refused.  Output:
@@ -53,15 +57,16 @@ def parse_args(argv=None):
     parser.add_argument('--store_mel', '-m', dest='store_mel', action='store_true')
     parser.add_argument('--verbose', '-v', dest='verbose', action='store_true')
     parser.add_argument('--single', '-s', dest='single', action='store_true')
-    parser.add_argument('--vocoder', dest='vocoder', default='griffinlim', choices=('griffinlim', 'melgan', 'hifigan', 'wavernn'))
+    parser.add_argument('--vocoder', dest='vocoder', default='griffinlim', choices=('griffinlim', 'melgan', 'hifigan', 'bigvgan', 'wavernn'))
     parser.add_argument('--vocoder_checkpoint', dest='vocoder_checkpoint', default=None, type=str)
     parser.add_argument('--vocoder_config', dest='vocoder_config', default=None, type=str,
-                        help='HiFi-GAN config: a config.json path or v1 / v2 / v3 (default: config.json beside the checkpoint)')
+                        help='HiFi-GAN config (a config.json path or v1 / v2 / v3) or BigVGAN config (a config.json path or base / bigvgan); '
+                             'default: the config.json beside the checkpoint')
     args = parser.parse_args(argv)
-    if args.vocoder in ('melgan', 'hifigan', 'wavernn') and args.vocoder_checkpoint is None:
+    if args.vocoder in ('melgan', 'hifigan', 'bigvgan', 'wavernn') and args.vocoder_checkpoint is None:
         parser.error(f'--vocoder {args.vocoder} needs --vocoder_checkpoint PATH')
-    if args.vocoder_config is not None and args.vocoder != 'hifigan':
-        parser.error('--vocoder_config applies to --vocoder hifigan only')
+    if args.vocoder_config is not None and args.vocoder not in ('hifigan', 'bigvgan'):
+        parser.error('--vocoder_config applies to --vocoder hifigan and bigvgan only')
     return args
 
 
@@ -119,9 +124,9 @@ def load_vocoder(name: str, checkpoint, config, model):
     """The generator --vocoder names (weights from checkpoint, HiFi-GAN's config from config) on the model's device, or None
     for Griffin-Lim, which Audio.reconstruct_waveform_batch runs.  A generator is refused when the samples it makes per mel frame
     differ from the model's hop_length: its audio would have the wrong length and pitch."""
-    if name in ('melgan', 'hifigan'):
-        from transformertts_b200.model import hifigan, melgan
-        upsampling = (melgan if name == 'melgan' else hifigan).HOP
+    if name in ('melgan', 'hifigan', 'bigvgan'):
+        from transformertts_b200.model import bigvgan, hifigan, melgan
+        upsampling = {'melgan': melgan, 'hifigan': hifigan, 'bigvgan': bigvgan}[name].HOP
         hop = int(model.config['hop_length'])
         if upsampling != hop:
             raise SystemExit(f'--vocoder {name}: the generator upsamples each mel frame to {upsampling} samples, but the audio '
@@ -129,13 +134,28 @@ def load_vocoder(name: str, checkpoint, config, model):
     if name == 'melgan':
         from transformertts_b200.model.melgan import MelGANGenerator
         return MelGANGenerator.from_checkpoint(checkpoint, device=model.device)
-    if name == 'hifigan':
+    if name in ('hifigan', 'bigvgan'):
         normalizer = model.config.get('normalizer')
         if normalizer != 'MelGAN':
-            raise SystemExit(f'--vocoder hifigan takes the MelGAN normaliser\'s log-mels (ln(max(S, 1e-5))); this model\'s normalizer '
-                             f'is {normalizer!r}, whose mels HiFi-GAN would misread')
+            label = 'HiFi-GAN' if name == 'hifigan' else 'BigVGAN'
+            raise SystemExit(f'--vocoder {name} takes the MelGAN normaliser\'s log-mels (ln(max(S, 1e-5))); this model\'s normalizer '
+                             f'is {normalizer!r}, whose mels {label} would misread')
+    if name == 'hifigan':
         from transformertts_b200.model.hifigan import HiFiGANGenerator
         return HiFiGANGenerator.from_checkpoint(checkpoint, config=config, device=model.device)
+    if name == 'bigvgan':
+        from transformertts_b200.model.bigvgan import BigVGANGenerator, check_audio, load_config
+        if config is None:
+            config = Path(checkpoint).parent / 'config.json'
+            if not config.exists():
+                raise SystemExit(f'--vocoder bigvgan: {config} not found; pass --vocoder_config (a config.json path or base / bigvgan)')
+        h = load_config(config)
+        c = model.config
+        try:
+            check_audio(h, c['sampling_rate'], c['mel_channels'], c['hop_length'], c.get('f_max'))
+        except ValueError as e:
+            raise SystemExit(f'--vocoder bigvgan: {e}')
+        return BigVGANGenerator.from_checkpoint(checkpoint, config=h, device=model.device)
     if name == 'wavernn':
         normalizer = model.config.get('normalizer')
         if normalizer != 'WaveRNN':

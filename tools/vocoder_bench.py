@@ -2,6 +2,7 @@
 
     python tools/vocoder_bench.py [--clips 64] [--reps 3] [--out DIR]
     python tools/vocoder_bench.py --vocoder hifigan [--config v1|v2|v3] [--clips 64] [--reps 3] [--out DIR]
+    python tools/vocoder_bench.py --vocoder bigvgan [--config base|bigvgan] [--clips 64] [--reps 3] [--out DIR]
     python tools/vocoder_bench.py --vocoder wavernn [--clips 64] [--reps 3] [--out DIR]
 
 Workload: that of tools/synth_bench.py -- `--clips` seeded ragged clips of 2-10 s (T_c uniform in 173..862 frames), mels from
@@ -21,6 +22,13 @@ With `--vocoder hifigan` the same clips go through a seeded HiFi-GAN generator o
 seed 0), without pad frames.  Paths: `module`, jik876's generator as a torch module in fp32 on the GPU (cuDNN, TF32 off), one
 clip per call as its inference.py runs it; `bf16x3` and `bf16`, HiFiGANGenerator.vocode_batch with all clips in one call.
 FLOPs count the useful products of every conv (a transposed conv's output row sums 2 of its k taps per input channel).
+
+With `--vocoder bigvgan` the same clips go through a seeded BigVGAN generator of `--config` (oracle/bigvgan_oracle.py, seed
+0, v1 final layer).  Paths: `module`, the oracle's layers as a torch module in fp32 on the GPU (cuDNN, TF32 off), one clip per
+call; `bf16x3` and `bf16`, BigVGANGenerator.vocode_batch with all clips in one call.  Also reported: the convs' FLOPs over the
+config's channels (useful) and over the padded columns the kernel runs (issued), and, from one more call of each mode under
+torch.profiler, the share of GPU time spent in the activation kernel and the bytes per second it achieves at the least
+traffic it needs (every column of every clip row read and written once per plane), against the H100 SXM's 3.35 TB/s.
 
 With `--vocoder wavernn` the workload is `--clips` seeded ragged clips of 1-10 s (T_c uniform in 81..802 frames at hop 275,
 22050 Hz) of WaveRNN-normalised mels (oracle/wavernn_oracle.make_mels), then one 10 s clip alone, through a seeded MOL
@@ -43,11 +51,13 @@ import torch
 
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 from oracle import audio_oracle as ao  # noqa: E402
+from oracle import bigvgan_oracle as bo  # noqa: E402
 from oracle import hifigan_oracle as ho  # noqa: E402
 from oracle import melgan_oracle as mo  # noqa: E402
 from oracle import wavernn_oracle as wo  # noqa: E402
 from transformertts_b200 import lib  # noqa: E402
 from transformertts_b200.data.audio import Audio  # noqa: E402
+from transformertts_b200.model import bigvgan as bg  # noqa: E402
 from transformertts_b200.model import hifigan as hg  # noqa: E402
 from transformertts_b200.model import melgan as mg  # noqa: E402
 
@@ -132,6 +142,62 @@ def hifigan_main(args, mels, lengths):
     return res
 
 
+def kernel_share(fn, name):
+    """One call under torch.profiler -> (GPU seconds of the kernels whose name contains `name`, GPU seconds of all kernels)."""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    mine = total = 0.0
+    for e in prof.key_averages():
+        t = getattr(e, 'device_time_total', None)
+        if t is None:
+            t = e.cuda_time_total
+        if e.key.startswith('Memcpy') or e.key.startswith('Memset'):
+            continue
+        total += t
+        if name in e.key:
+            mine += t
+    return mine / 1e6, total / 1e6
+
+
+def bigvgan_main(args, mels, lengths):
+    h = bg.load_config(args.config)
+    sd = bo.init_state_dict(h, seed=0)
+    module = bo.build(h, sd, dtype=torch.float32).cuda()
+
+    def per_clip():
+        with torch.no_grad():
+            return [module(torch.from_numpy(m).cuda()[None])[0, 0].cpu().numpy() for m in mels]
+
+    frames = int(lengths.sum())
+    res = dict(workload='bigvgan_vocode', config=args.config, clips=args.clips, frames=frames, min_frames=int(lengths.min()),
+               max_frames=int(lengths.max()), reps=args.reps, audio_s=round(float(256 * frames / 22050), 1),
+               stage_cols=bg.stage_cols(h))
+    fl = bg.conv_flops(h, frames)
+    res.update(conv_gflop_useful=round(fl['useful'] / 1e9, 1), conv_gflop_issued=round(fl['issued'] / 1e9, 1),
+               conv_useful_fraction=round(fl['useful'] / fl['issued'], 3))
+    t, _, w_ref = timed(per_clip, args.reps)
+    res.update(module_s=round(t, 4), module_audio_s_per_s=round(res['audio_s'] / t, 1))
+    del module
+    torch.cuda.empty_cache()
+    for prec in ('bf16x3', 'bf16'):
+        g = bg.BigVGANGenerator(h, device='cuda', precision=prec).load_state_dict(sd)
+        t, launches, w = timed(lambda: g.vocode_batch(mels), args.reps)
+        act_s, gpu_s = kernel_share(lambda: g.vocode_device(mels), 'snake_aa_kernel')
+        act_bytes = bg.activation_bytes(h, frames, prec == 'bf16x3')
+        res.update({f'{prec}_s': round(t, 4), f'{prec}_audio_s_per_s': round(res['audio_s'] / t, 1), f'{prec}_launches': launches,
+                    f'{prec}_conv_tflops_useful': round(fl['useful'] / t / 1e12, 2),
+                    f'{prec}_gpu_s': round(gpu_s, 4), f'{prec}_activation_s': round(act_s, 4),
+                    f'{prec}_activation_share': round(act_s / gpu_s, 3),
+                    f'{prec}_activation_tb_per_s': round(act_bytes / act_s / 1e12, 2),
+                    f'{prec}_activation_of_3p35_tb_per_s': round(act_bytes / act_s / 3.35e12, 3),
+                    f'{prec}_max_abs_diff_vs_module': float(max(np.abs(a - b).max() for a, b in zip(w, w_ref)))})
+        del g
+        torch.cuda.empty_cache()
+    return res
+
+
 def wavernn_torch_loop(net, fmels, target, overlap):
     """fatchord's generate() loop in torch on the GPU, the folds of all clips as one batch (before the crossfade)."""
     ms, auxs = [], []
@@ -205,9 +271,12 @@ def main():
     ap.add_argument('--clips', type=int, default=64)
     ap.add_argument('--reps', type=int, default=3)
     ap.add_argument('--out', default=None)
-    ap.add_argument('--vocoder', choices=('melgan', 'hifigan', 'wavernn'), default='melgan')
-    ap.add_argument('--config', default='v1', help='HiFi-GAN config: v1 / v2 / v3 or a config.json path')
+    ap.add_argument('--vocoder', choices=('melgan', 'hifigan', 'bigvgan', 'wavernn'), default='melgan')
+    ap.add_argument('--config', default=None, help='HiFi-GAN config: v1 (default) / v2 / v3 or a config.json path; BigVGAN config: '
+                                                   'base (default) / bigvgan or a config.json path')
     args = ap.parse_args()
+    if args.config is None:
+        args.config = 'base' if args.vocoder == 'bigvgan' else 'v1'
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     if args.vocoder == 'wavernn':
@@ -218,6 +287,8 @@ def main():
     mels = [audio.mel_spectrogram(ao.make_clips(1, 256 * (int(T) - 1), seed=500 + c)[0]).T for c, T in enumerate(lengths)]
     if args.vocoder == 'hifigan':
         return report(hifigan_main(args, mels, lengths), args)
+    if args.vocoder == 'bigvgan':
+        return report(bigvgan_main(args, mels, lengths), args)
     sd = mo.init_state_dict(seed=0)
     module = mo.build(sd, dtype=torch.float32).cuda()
     pad = torch.full((1, 80, mo.PAD_FRAMES), mo.PAD_VALUE, device='cuda')

@@ -4,7 +4,8 @@
 // load and a 128-row tile may span several clips.  The epilogue (one thread per row) maps the row to its clip, skips halo
 // rows, adds the bias, an optional residual and the multi-receptive-field sum, writes y and LeakyReLU(y) as bf16 hi/lo planes
 // and mirrors the rows next to each clip edge into the halos the next conv reads.  ttsb_conv1d_ex_tc takes the halo (up to 64
-// rows), up to 16 taps and the slope per call; ttsb_conv1d_out_tanh_ex is the generators' N = 1 output layer.
+// rows), up to 16 taps and the slope per call; ttsb_conv1d_out_tanh_ex (ttsb_conv1d_out_clamp_ex for BigVGAN v2) is the
+// generators' N = 1 output layer, and ttsb_snake_aa_ex BigVGAN's anti-aliased Snake activation on the same layout.
 #include <vector>
 
 #include "../../include/ttsb.h"
@@ -210,7 +211,9 @@ done:
 }
 
 // one thread per output sample: tanh(bias + 7-tap dot product over the padded channels), fixed summation order; the 3 rows of
-// padding on each side are the clip's halo rows (reflected for MelGAN, zeros for HiFi-GAN)
+// padding on each side are the clip's halo rows (reflected for MelGAN, zeros for HiFi-GAN).  kClamp: clamp(., -1, 1) instead of
+// tanh (BigVGAN v2's output layer)
+template <bool kClamp>
 __global__ void __launch_bounds__(256)
 conv1d_out_tanh_kernel(const __nv_bfloat16* __restrict__ in_hi, const __nv_bfloat16* __restrict__ in_lo, int ld_in, int channels, int halo,
                        const int32_t* __restrict__ tab, int n_clips, int drop_tail, const float* __restrict__ weight, float bias,
@@ -235,7 +238,115 @@ conv1d_out_tanh_kernel(const __nv_bfloat16* __restrict__ in_hi, const __nv_bfloa
         acc = fmaf(x, sw[k * channels + ch], acc);
       }
     }
-    wav_out[off_c - (size_t)c * drop_tail + j] = tanhf(acc);
+    wav_out[off_c - (size_t)c * drop_tail + j] = kClamp ? fminf(fmaxf(acc, -1.f), 1.f) : tanhf(acc);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// BigVGAN's anti-aliased periodic activation (Activation1d), per clip and channel, over the same ragged layout:
+//   u[m] = 2 sum_i x[clamp(i - 5, 0, L - 1)] h_up[m + 15 - 2i]        m in [0, 2L), the six i with the tap in [0, 12)
+//   s[m] = u[m] + inv_beta sin^2(alpha u[m])
+//   y[t] = sum_j h_down[j] s[clamp(2t + j - 5, 0, 2L - 1)]             t in [0, L)
+// A CTA takes SAA_ROWS rows of the packed layout (which may span clips) and 32 columns, one per lane.  It stages the input
+// rows [r0 - 6, r0 + SAA_ROWS + 6) in shared memory as fp32, computes both phases of s for the rows [r0 - 3, r0 + SAA_ROWS
+// + 3) and then the outputs; every index is clamped to the row's own clip, found in the uploaded clip table, so no clip
+// reads another's rows or the halos.  Each value is computed by one thread in a fixed order: a clip's output does not
+// depend on the tiling or the batch.
+constexpr int SAA_ROWS = 64;
+constexpr int SAA_THREADS = 256;
+constexpr int SAA_XPAD = 6;  // s rows r0 - 3 .. need x rows 3 further out
+constexpr int SAA_SPAD = 3;  // output row t reads s at positions 2t - 5 .. 2t + 6: rows t - 3 .. t + 3
+constexpr int SAA_XROWS = SAA_ROWS + 2 * SAA_XPAD;
+constexpr int SAA_SROWS = SAA_ROWS + 2 * SAA_SPAD;
+
+struct SnakeAAParams {
+  const __nv_bfloat16* in_hi;
+  const __nv_bfloat16* in_lo;
+  __nv_bfloat16* out_hi;
+  __nv_bfloat16* out_lo;
+  int ld, channels, halo, rows, n_clips;
+  const int32_t* tab;  // region start rows [n_clips + 1], then the clip_offsets prefix sums [n_clips + 1]
+  const float* alpha;
+  const float* inv_beta;
+  float h_up[12];
+  float h_down[12];
+};
+
+__global__ void __launch_bounds__(SAA_THREADS)
+snake_aa_kernel(const __grid_constant__ SnakeAAParams p) {
+  __shared__ float xs[SAA_XROWS][32];
+  __shared__ float ss[SAA_SROWS][2][32];
+  __shared__ int2 meta[SAA_XROWS];  // per staged row: (row of its clip's position 0, L), L = 0 for a halo row or outside
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r0 = blockIdx.x * SAA_ROWS;
+  const int col = blockIdx.y * 32 + lane;
+  const bool any_live = blockIdx.y * 32 < p.channels;  // CTA-uniform: all 32 columns are padding otherwise
+  const bool live = col < p.channels;
+  const int32_t* off = p.tab + p.n_clips + 1;
+  for (int k = threadIdx.x; k < SAA_XROWS; k += SAA_THREADS) {
+    const int g = r0 - SAA_XPAD + k;
+    int2 m = make_int2(0, 0);
+    if (g >= 0 && g < p.rows) {
+      const int c = find_clip(p.tab, p.n_clips, g);
+      const int base = __ldg(p.tab + c) + p.halo;
+      const int L = __ldg(off + c + 1) - __ldg(off + c);
+      if (g >= base && g < base + L) m = make_int2(base, L);
+    }
+    meta[k] = m;
+  }
+  __syncthreads();
+  if (any_live) {
+    for (int k = warp; k < SAA_XROWS; k += SAA_THREADS / 32) {
+      float v = 0.f;
+      if (live && meta[k].y) {
+        const size_t o = (size_t)(r0 - SAA_XPAD + k) * p.ld + col;
+        v = __bfloat162float(p.in_hi[o]);
+        if (p.in_lo) v += __bfloat162float(p.in_lo[o]);
+      }
+      xs[k][lane] = v;
+    }
+    __syncthreads();
+    const float a = live ? __ldg(p.alpha + col) : 0.f;
+    const float ib = live ? __ldg(p.inv_beta + col) : 0.f;
+    for (int k = warp; k < SAA_SROWS; k += SAA_THREADS / 32) {
+      const int2 m = meta[k + SAA_XPAD - SAA_SPAD];
+      if (!live || !m.y) continue;
+      const int pos = r0 - SAA_SPAD + k - m.x;  // position in the clip
+      const int xb = m.x - (r0 - SAA_XPAD);      // staged row of the clip's position 0
+#pragma unroll
+      for (int ph = 0; ph < 2; ++ph) {
+        // m = 2 pos + ph: i = pos + 2 + ph + q (q = 0..5) reads x[pos - 3 + ph + q] with tap 11 - ph - 2q
+        float acc = 0.f;
+#pragma unroll
+        for (int q = 0; q < 6; ++q) {
+          const int i = min(max(pos - 3 + ph + q, 0), m.y - 1);
+          acc = fmaf(xs[xb + i][lane], p.h_up[11 - ph - 2 * q], acc);
+        }
+        const float u = 2.f * acc;
+        const float sn = sinf(a * u);
+        ss[k][ph][lane] = fmaf(ib, sn * sn, u);
+      }
+    }
+    __syncthreads();
+  }
+  if (col >= p.ld) return;
+  for (int k = warp; k < SAA_ROWS; k += SAA_THREADS / 32) {
+    const int2 m = meta[k + SAA_XPAD];
+    if (!m.y) continue;  // a halo row (or past the end): never written
+    float y = 0.f;
+    if (live) {
+      const int t = r0 + k - m.x;
+      const int sb = m.x - (r0 - SAA_SPAD);  // s row of the clip's position 0
+#pragma unroll
+      for (int j = 0; j < 12; ++j) {
+        const int mm = min(max(2 * t + j - 5, 0), 2 * m.y - 1);
+        y = fmaf(p.h_down[j], ss[sb + (mm >> 1)][mm & 1][lane], y);
+      }
+    }
+    const size_t o = (size_t)(r0 + k) * p.ld + col;
+    const __nv_bfloat16 hi = __float2bfloat16_rn(y);
+    p.out_hi[o] = hi;
+    if (p.out_lo) p.out_lo[o] = __float2bfloat16_rn(y - __bfloat162float(hi));
   }
 }
 
@@ -399,6 +510,7 @@ static int conv1d_launch(const char* what, const ttsb_conv1d_ex_args* a, void* s
   return split ? conv_launch_tc<true>(tmA, tmW, p, stream) : conv_launch_tc<false>(tmA, tmW, p, stream);
 }
 
+template <bool kClamp>
 static int out_tanh_launch(const char* what, const void* in_hi, const void* in_lo, int ld_in, int channels, int halo,
                            const int32_t* clip_offsets, int n_clips, int drop_tail, const float* weight, float bias, void* workspace,
                            int64_t workspace_bytes, float* wav_out, void* stream_v) {
@@ -416,11 +528,65 @@ static int out_tanh_launch(const char* what, const void* in_hi, const void* in_l
   TTSB_CUDA_OK(cudaMemcpyAsync(workspace, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
   const int total = clip_offsets[n_clips];
   const int grid = min((total + 255) / 256, 8 * num_sms());
-  conv1d_out_tanh_kernel<<<grid, 256, 7 * channels * sizeof(float), stream>>>(
+  conv1d_out_tanh_kernel<kClamp><<<grid, 256, 7 * channels * sizeof(float), stream>>>(
       static_cast<const __nv_bfloat16*>(in_hi), static_cast<const __nv_bfloat16*>(in_lo), ld_in, channels, halo,
       static_cast<const int32_t*>(workspace), n_clips, drop_tail, weight, bias, total, wav_out);
   count_launch();
   return check_cuda(cudaGetLastError(), "conv1d_out_tanh_kernel launch");
+}
+
+static int snake_aa_launch(const void* in_hi, const void* in_lo, void* out_hi, void* out_lo, int ld, int channels, int halo,
+                           const int32_t* clip_offsets, int n_clips, const float* alpha, const float* inv_beta, const float* h_up,
+                           const float* h_down, int precision, void* workspace, int64_t workspace_bytes, void* stream_v) {
+  const char* what = "ttsb_snake_aa_ex";
+  if (precision != TTSB_PREC_BF16 && precision != TTSB_PREC_BF16X3) { set_last_error("%s: unknown precision", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  const bool split = precision == TTSB_PREC_BF16X3;
+  if (!in_hi || !out_hi || (split && (!in_lo || !out_lo))) {
+    set_last_error("%s: in_hi or out_hi is NULL, or in_lo or out_lo in bf16x3", what);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  if (!alpha || !inv_beta || !h_up || !h_down) { set_last_error("%s: alpha, inv_beta, h_up or h_down is NULL", what); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (ld < 8 || ld % 8) { set_last_error("%s: ld = %d must be a positive multiple of 8", what, ld); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (channels < 1 || channels > ld) { set_last_error("%s: channels = %d must be in [1, ld = %d]", what, channels, ld); return TTSB_ERR_INVALID_ARGUMENT; }
+  if (halo < 0 || halo > TTSB_CONV1D_EX_MAX_HALO) { set_last_error("%s: halo = %d must be in [0, %d]", what, halo, TTSB_CONV1D_EX_MAX_HALO); return TTSB_ERR_INVALID_ARGUMENT; }
+  const void* planes[4] = {in_hi, split ? in_lo : nullptr, out_hi, split ? out_lo : nullptr};
+  if ((reinterpret_cast<uintptr_t>(planes[0]) | reinterpret_cast<uintptr_t>(planes[1]) | reinterpret_cast<uintptr_t>(planes[2]) |
+       reinterpret_cast<uintptr_t>(planes[3])) % 16 || (reinterpret_cast<uintptr_t>(alpha) | reinterpret_cast<uintptr_t>(inv_beta)) % 4) {
+    set_last_error("%s: in_hi, in_lo, out_hi and out_lo must be 16-byte aligned, alpha and inv_beta 4-byte aligned", what);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  for (int o = 2; o < 4; ++o)
+    if (planes[o] && (planes[o] == planes[0] || planes[o] == planes[1] || (o == 3 && planes[3] == planes[2]))) {
+      set_last_error("%s: an output plane aliases an input plane or the other output plane (no in-place activation)", what);
+      return TTSB_ERR_INVALID_ARGUMENT;
+    }
+  std::vector<int32_t> tab;
+  long long rows = 0, out_rows = 0;
+  int rc = conv_table(what, clip_offsets, n_clips, 1, halo, 1, tab, &rows, &out_rows);
+  if (rc) return rc;
+  rc = check_workspace(what, workspace, workspace_bytes, n_clips);
+  if (rc) return rc;
+
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  SnakeAAParams p{};
+  p.in_hi = static_cast<const __nv_bfloat16*>(in_hi);
+  p.in_lo = split ? static_cast<const __nv_bfloat16*>(in_lo) : nullptr;
+  p.out_hi = static_cast<__nv_bfloat16*>(out_hi);
+  p.out_lo = split ? static_cast<__nv_bfloat16*>(out_lo) : nullptr;
+  p.ld = ld;
+  p.channels = channels;
+  p.halo = halo;
+  p.rows = (int)rows;
+  p.n_clips = n_clips;
+  p.tab = static_cast<const int32_t*>(workspace);
+  p.alpha = alpha;
+  p.inv_beta = inv_beta;
+  for (int j = 0; j < 12; ++j) { p.h_up[j] = h_up[j]; p.h_down[j] = h_down[j]; }
+  TTSB_CUDA_OK(cudaMemcpyAsync(workspace, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  const dim3 grid((unsigned)((rows + SAA_ROWS - 1) / SAA_ROWS), (unsigned)((ld + 31) / 32));
+  snake_aa_kernel<<<grid, SAA_THREADS, 0, stream>>>(p);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "snake_aa_kernel launch");
 }
 
 }  // namespace ttsb
@@ -447,6 +613,24 @@ extern "C" int ttsb_conv1d_out_tanh_ex(const void* in_hi, const void* in_lo, int
     set_last_error("ttsb_conv1d_out_tanh_ex: halo = %d must be in [3, %d]", halo, TTSB_CONV1D_EX_MAX_HALO);
     return TTSB_ERR_INVALID_ARGUMENT;
   }
-  return out_tanh_launch("ttsb_conv1d_out_tanh_ex", in_hi, in_lo, ld_in, channels, halo, clip_offsets, n_clips, drop_tail, weight, bias,
-                         workspace, workspace_bytes, wav_out, stream_v);
+  return out_tanh_launch<false>("ttsb_conv1d_out_tanh_ex", in_hi, in_lo, ld_in, channels, halo, clip_offsets, n_clips, drop_tail, weight,
+                                bias, workspace, workspace_bytes, wav_out, stream_v);
+}
+
+extern "C" int ttsb_conv1d_out_clamp_ex(const void* in_hi, const void* in_lo, int ld_in, int channels, int halo, const int32_t* clip_offsets,
+                                        int n_clips, int drop_tail, const float* weight, float bias, void* workspace, int64_t workspace_bytes,
+                                        float* wav_out, void* stream_v) {
+  if (halo < 3 || halo > TTSB_CONV1D_EX_MAX_HALO) {
+    set_last_error("ttsb_conv1d_out_clamp_ex: halo = %d must be in [3, %d]", halo, TTSB_CONV1D_EX_MAX_HALO);
+    return TTSB_ERR_INVALID_ARGUMENT;
+  }
+  return out_tanh_launch<true>("ttsb_conv1d_out_clamp_ex", in_hi, in_lo, ld_in, channels, halo, clip_offsets, n_clips, drop_tail, weight,
+                               bias, workspace, workspace_bytes, wav_out, stream_v);
+}
+
+extern "C" int ttsb_snake_aa_ex(const void* in_hi, const void* in_lo, void* out_hi, void* out_lo, int ld, int channels, int halo,
+                                const int32_t* clip_offsets, int n_clips, const float* alpha, const float* inv_beta, const float* h_up,
+                                const float* h_down, int precision, void* workspace, int64_t workspace_bytes, void* stream_v) {
+  return snake_aa_launch(in_hi, in_lo, out_hi, out_lo, ld, channels, halo, clip_offsets, n_clips, alpha, inv_beta, h_up, h_down, precision,
+                         workspace, workspace_bytes, stream_v);
 }

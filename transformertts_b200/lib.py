@@ -33,7 +33,7 @@ EXPORTS = [
     'ttsb_stft_mel_log_batch_workspace_bytes', 'ttsb_stft_mel_log_batch', 'ttsb_pitch_workspace_bytes', 'ttsb_pitch_dio_stonemask',
     'ttsb_dp_unique_id', 'ttsb_dp_init', 'ttsb_dp_allreduce_bucket', 'ttsb_dp_destroy',
     'ttsb_decode_attn_workspace_bytes', 'ttsb_decode_attn', 'ttsb_decode_prologue', 'ttsb_decode_commit',
-    'ttsb_conv1d_workspace_bytes', 'ttsb_conv1d_ex_tc', 'ttsb_conv1d_out_tanh_ex',
+    'ttsb_conv1d_workspace_bytes', 'ttsb_conv1d_ex_tc', 'ttsb_conv1d_out_tanh_ex', 'ttsb_conv1d_out_clamp_ex', 'ttsb_snake_aa_ex',
     'ttsb_resample_batch_workspace_bytes', 'ttsb_resample_batch',
     'ttsb_mcd_dtw_workspace_bytes', 'ttsb_mcd_dtw', 'ttsb_mcd_dtw_path_workspace_bytes', 'ttsb_mcd_dtw_path',
     'ttsb_stft_mel_log_ragged_workspace_bytes', 'ttsb_stft_mel_log_ragged', 'ttsb_mel_to_linear_ex',
@@ -150,8 +150,11 @@ def load() -> C.CDLL:
     lib.ttsb_stft_mel_log_batch_workspace_bytes.restype = C.c_int64
     lib.ttsb_pitch_workspace_bytes.restype = C.c_int64
     lib.ttsb_conv1d_workspace_bytes.restype = C.c_int64
-    lib.ttsb_conv1d_out_tanh_ex.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
-                                            C.c_float, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    for name in ('ttsb_conv1d_out_tanh_ex', 'ttsb_conv1d_out_clamp_ex'):
+        getattr(lib, name).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                       C.c_float, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.ttsb_snake_aa_ex.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]
     lib.ttsb_pitch_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double]
     lib.ttsb_pitch_dio_stonemask.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double,
                                              C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
@@ -989,6 +992,30 @@ def conv1d_out_tanh_ex(in_hi, in_lo, channels, halo, clip_offsets, drop_tail, we
                                           ptr(weight), C.c_float(bias), ptr(workspace),
                                           C.c_int64(workspace.numel() * workspace.element_size()), ptr(wav_out), _stream()),
            'ttsb_conv1d_out_tanh_ex')
+
+
+def conv1d_out_clamp_ex(in_hi, in_lo, channels, halo, clip_offsets, drop_tail, weight, bias, workspace, wav_out):
+    """conv1d_out_tanh_ex with clamp(., -1, 1) in place of tanh (include/ttsb.h: ttsb_conv1d_out_clamp_ex)."""
+    co, n = _host_offsets(clip_offsets)
+    _check(load().ttsb_conv1d_out_clamp_ex(ptr(in_hi), ptr(in_lo), in_hi.shape[-1], int(channels), int(halo), co, n, int(drop_tail),
+                                           ptr(weight), C.c_float(bias), ptr(workspace),
+                                           C.c_int64(workspace.numel() * workspace.element_size()), ptr(wav_out), _stream()),
+           'ttsb_conv1d_out_clamp_ex')
+
+
+def snake_aa_ex(src, dst, channels, halo, clip_offsets, alpha, inv_beta, h_up, h_down, workspace):
+    """BigVGAN's anti-aliased Snake activation over a packed ragged layout (include/ttsb.h: ttsb_snake_aa_ex).  src / dst:
+    (hi, lo) planes, lo None in bf16; clip_offsets: host sequence (n_clips + 1); alpha / inv_beta: fp32 (channels) device
+    tensors; h_up / h_down: 12 host taps each."""
+    co, n = _host_offsets(clip_offsets)
+    split = src[1] is not None
+    up = (C.c_float * 12)(*[float(v) for v in h_up])
+    down = (C.c_float * 12)(*[float(v) for v in h_down])
+    _check(load().ttsb_snake_aa_ex(ptr(src[0]), ptr(src[1]), ptr(dst[0]), ptr(dst[1]), src[0].shape[-1], int(channels), int(halo), co, n,
+                                   ptr(alpha), ptr(inv_beta), C.cast(up, C.c_void_p), C.cast(down, C.c_void_p),
+                                   PREC_BF16X3 if split else PREC_BF16, ptr(workspace),
+                                   C.c_int64(workspace.numel() * workspace.element_size()), _stream()),
+           'ttsb_snake_aa_ex')
 
 
 # ------------------------------------------------------------------------------------------------------------
