@@ -137,11 +137,58 @@ def test_duration_path_search_dp_equals_scipy_dijkstra():
     kernel runs the equivalent dynamic programme.  Both restated in oracle/alignment_oracle.py and compared here."""
     from oracle import alignment_oracle as ao
     rng = np.random.default_rng(0)
+    shapes = []
     for _ in range(25):
         M = int(rng.integers(5, 50))
-        N = int(rng.integers(3, min(M, 20) + 1))
+        shapes.append((M, int(rng.integers(3, min(M, 20) + 1))))
+    # more phonemes than frames (the path moves right inside rows), one row, one column, more columns than the 256 threads
+    # of the kernel's anti-diagonal loop
+    shapes += [(7, 30), (20, 45), (1, 9), (1, 2), (12, 1), (2, 1), (2, 300), (40, 257)]
+    for M, N in shapes:
         logits = rng.normal(0, 1, (M, N)) - 0.3 * N * np.abs(np.arange(M)[:, None] / M - np.arange(N)[None, :] / N)
         a = np.exp(logits)
         a = (a / a.sum(1, keepdims=True)).astype(np.float32)
         d_ref = ao.extract_durations_with_dijkstra(a)
-        assert d_ref.sum() == M and np.array_equal(d_ref, ao.durations_by_dynamic_programming(a))
+        assert d_ref.sum() == M and np.array_equal(d_ref, ao.durations_by_dynamic_programming(a)), (M, N)
+    # M = N = 1: the reference's path walk follows the source's predecessor (-9999) and fails; the DP answers [1]
+    with pytest.raises(IndexError):
+        ao.extract_durations_with_dijkstra(np.ones((1, 1), np.float32))
+    assert ao.durations_by_dynamic_programming(np.ones((1, 1), np.float32)).tolist() == [1]
+
+
+def test_vectorised_duration_dp_equals_the_loop():
+    """tests/test_gpu_duration_edges.py runs the DP over anti-diagonals (the large maps would take minutes as a Python double
+    loop): on small maps, random and plateau alike, it equals oracle/alignment_oracle.py's loop bit for bit."""
+    from oracle import alignment_oracle as ao
+    import test_gpu_duration_edges as gde
+    rng = np.random.default_rng(1)
+    maps = list(gde.plateau_maps().values())
+    for M, N in [(1, 1), (1, 7), (9, 1), (5, 5), (13, 40), (40, 13)]:
+        maps.append(gde.diagonal_maps(rng, 1, 1, M, N)[0, 0])
+        maps.append(np.round(rng.uniform(0, 1, (M, N)) * 3).astype(np.float32) / 3)   # few levels: many exact ties
+    for a in maps:
+        assert np.array_equal(gde.dp_durations(a), ao.durations_by_dynamic_programming(a)), a.shape
+
+
+def test_duration_edge_inputs_tell_wrong_oracles_apart():
+    """The exact assertions of tests/test_gpu_duration_edges.py would catch three plausible mistakes: each wrong variant of
+    the reference changes the result on at least one of that file's inputs (those that need no GPU-computed scores)."""
+    import test_gpu_duration_edges as gde
+    cases = {**gde.hand_scored_cases(), **gde.plateau_cases()}
+    right = {k: gde.durations_reference(*c) for k, c in cases.items()}
+
+    def changed(**variant):
+        return [k for k, c in cases.items() if not np.array_equal(right[k], gde.durations_reference(*c, **variant))]
+
+    assert changed(start=0)                          # cropping from row / column 0 instead of 1
+    assert 'tied_heads' in changed(argmax=gde.last_argmax)   # the best head by the last maximum
+    assert changed(order='uld')                      # tie order up before left
+    # the last maximum also changes the jumpiness of the score inputs (uniform, zero and tied rows)
+    for Tq, Tk, H, r in gde.SCORE_SHAPES:
+        if Tq > 2000:
+            continue
+        att, ml, pl = gde.make_score_inputs(Tq, Tk, H, seed=Tq * 7 + Tk)
+        right_jump = gde.scores_reference(att, ml, pl, r)[0]
+        wrong_jump = gde.scores_reference(att, ml, pl, r, argmax=gde.last_argmax)[0]
+        if Tk > 6:
+            assert not np.array_equal(right_jump, wrong_jump), (Tq, Tk, H, r)
