@@ -117,6 +117,60 @@ def test_glide_vibrato_and_gaps():
     assert not g[:38].any() and not g[135:].any()
 
 
+# the other sampling rates the project prepares data at, each at its usual hop (vrm 3 at all of them)
+RATES = [(8000, 80), (16000, 200), (44100, 512), (48000, 600), (96000, 1200)]
+
+
+@pytest.mark.parametrize('fs,hop', RATES)
+def test_world_fft_filters_equal_direct_linear_convolution_at_other_rates(fs, hop):
+    x = po.speech_like_clip(1.3, seed=fs, fs=float(fs))
+    bounds = po.boundary_f0s()
+    for a, b in zip(po.filtered_bands_fft(x, fs, bounds), po.filtered_bands_direct(x, fs, bounds)):
+        assert np.max(np.abs(a - b)) <= 1e-12 * np.max(np.abs(b))
+
+
+@pytest.mark.parametrize('fs,hop', RATES)
+def test_tones_glide_and_silence_at_other_rates(fs, hop):
+    fp = hop / fs * 1000
+    v = po.voice_range_minimum(fp, 71.0)
+    assert v == 3
+    for f in (90, 180, 350):
+        x = po.tone(f, 2.0, fs=float(fs), seed=f).astype(np.float64)
+        f0, t = po.dio(x, fs, fp)
+        sm = po.stonemask(x, f0, t, fs)
+        assert (f0[v:-v] > 0).all() and (sm[v:-v] > 0).all(), f
+        assert np.max(np.abs(sm[v:-v] / f - 1)) < TONE_TOL, f
+    x = po.glide(110, 220, 2.0, fs=float(fs), seed=1)
+    g = po.extract_pitch(x, fs, hop)
+    n = len(x)
+    track = 110 * 2.0 ** (np.arange(n) / n)
+    t = np.minimum(np.arange(len(g)) * hop, n - 1)
+    assert (g[v:-v] > 0).all() and np.max(np.abs(g[v:-v] / track[t][v:-v] - 1)) < GLIDE_TOL
+    assert not po.extract_pitch(np.zeros(fs, np.float32), fs, hop).any()
+
+
+def test_stonemask_upper_limit_at_8k():
+    # fs / 12 = 666.7 Hz is below f0_ceil at 8 kHz: DIO voices a 700 Hz tone and StoneMask zeroes it; at 16 kHz it is refined
+    for fs, hop, kept in ((8000, 80, False), (16000, 200, True)):
+        x = po.tone(700, 1.0, fs=float(fs), seed=1).astype(np.float64)
+        f0, t = po.dio(x, fs, hop / fs * 1000)
+        sm = po.stonemask(x, f0, t, fs)
+        assert np.count_nonzero(f0 > 8000 / 12.0) > 50
+        if kept:
+            assert (sm[3:-3] > 0).all() and np.max(np.abs(sm[3:-3] / 700 - 1)) < TONE_TOL
+        else:
+            assert not sm.any()
+
+
+@pytest.mark.parametrize('hop,vrm', [(64, 11), (128, 5), (256, 3), (275, 3), (FS * 5.0 / 1000, 7)])
+def test_fix_f0_contour_needs_more_than_voice_range_minimum_frames(hop, vrm):
+    fp = hop / FS * 1000
+    assert po.voice_range_minimum(fp, 71.0) == vrm
+    with pytest.raises(ValueError, match=f'more than {vrm}'):
+        po.fix_f0_contour(np.full(vrm, 100.0), np.full((7, vrm), 100.0), fp, 71.0, 0.1)
+    assert not po.fix_f0_contour(np.full(vrm + 1, 100.0), np.full((7, vrm + 1), 100.0), fp, 71.0, 0.1).any()
+
+
 def test_pitch_statistics_and_normalisation():
     a, b = np.array([0.0, 100.0, 200.0]), np.array([300.0, 0.0])
     mean, std = po.pitch_stats([a, b])

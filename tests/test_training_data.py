@@ -58,6 +58,32 @@ def test_pitch_refuses_malformed_offsets_without_gpu(cdll):
     assert lib.pitch_workspace_bytes([0, 1500, 4000], 22050, fp) > 0
 
 
+def test_pitch_workspace_refuses_band_count_band_length_and_short_clips(cdll):
+    from oracle import pitch_oracle as po
+    fs, fp = 22050, 256 / 22050 * 1000
+
+    def ws(lengths, f0_floor=71.0, channels_in_octave=2.0):
+        so = np.concatenate([[0], np.cumsum(lengths)]).tolist()
+        return cdll.ttsb_pitch_workspace_bytes(_i32(*so), len(lengths), fs, fp, f0_floor, 800.0, channels_in_octave)
+
+    # 71 .. 800 Hz: 16 bands at 4.5 channels per octave, 17 at 4.6
+    assert len(po.boundary_f0s(71.0, 800.0, 4.5)) == 16 and len(po.boundary_f0s(71.0, 800.0, 4.6)) == 17
+    assert ws([fs], channels_in_octave=4.5) > 0
+    assert ws([fs], channels_in_octave=4.6) == -1 and b'17 bands' in cdll.ttsb_last_error()
+    # band 0's low-pass has 4h taps, h = round(fs / (f0_floor sqrt 2) / 2), and must satisfy 2h <= round(fs / 50)
+    P = po.matlab_round(fs / 50.0)
+    fits = lambda floor: 2 * po.band_half_lengths(fs, po.boundary_f0s(floor, 800.0, 2.0))[0] <= P
+    assert fits(36.0) and not fits(35.0)
+    assert ws([fs], f0_floor=36.0) > 0
+    assert ws([fs], f0_floor=35.0) == -1 and b'band 0 low-pass longer than the low-cut margin' in cdll.ttsb_last_error()
+    # a clip of voice_range_minimum frames is refused, one of one frame more is accepted
+    vrm = po.voice_range_minimum(fp, 71.0)
+    L = next(L for L in range(1, 10 * 256) if po.n_frames(L, fs, fp) > vrm)
+    assert po.n_frames(L - 1, fs, fp) == vrm
+    assert ws([4000, L]) > 0
+    assert ws([4000, L - 1]) == -1 and b'voice_range_minimum' in cdll.ttsb_last_error()
+
+
 def _ref_normalize_volume(self, wav, increase_only=False, decrease_only=False):
     # reference data/audio.py:154-162, as written
     if increase_only and decrease_only:
