@@ -51,15 +51,20 @@ def _header_structs(header: str) -> dict:
     return structs
 
 
+def _mirrors(lib) -> dict:
+    """{header struct name: its ctypes mirror in lib.py}"""
+    return {'ttsb_pack_desc': lib.PackDesc, 'ttsb_gemm_args': lib.GemmArgs, 'ttsb_mha_args': lib.MhaArgs,
+            'ttsb_decode_attn_args': lib.DecodeAttnArgs, 'ttsb_bgemm_args': lib.BgemmArgs, 'ttsb_wgrad_args': lib.WgradArgs,
+            'ttsb_conv1d_ex_args': lib.Conv1dExArgs}
+
+
 def test_struct_layout_matches_header():
     """Every ctypes mirror in lib.py against its typedef struct: field names and order, C types, array lengths, offsets and
     size; and the constants lib.py mirrors of the header's #defines."""
     from transformertts_b200 import lib
     header = (ROOT / 'include' / 'ttsb.h').read_text()
     structs = _header_structs(header)
-    mirrors = {'ttsb_pack_desc': lib.PackDesc, 'ttsb_gemm_args': lib.GemmArgs, 'ttsb_mha_args': lib.MhaArgs,
-               'ttsb_decode_attn_args': lib.DecodeAttnArgs, 'ttsb_bgemm_args': lib.BgemmArgs, 'ttsb_wgrad_args': lib.WgradArgs,
-               'ttsb_conv1d_ex_args': lib.Conv1dExArgs}
+    mirrors = _mirrors(lib)
     assert set(structs) == set(mirrors)
     assert set(mirrors.values()) == {v for v in vars(lib).values() if isinstance(v, type) and issubclass(v, C.Structure)}
     scalars = {'int': C.c_int, 'int64_t': C.c_int64, 'long long': C.c_longlong, 'uint32_t': C.c_uint32, 'float': C.c_float}
@@ -86,6 +91,46 @@ def test_struct_layout_matches_header():
                          ('TTSB_CONV1D_SUM_NONE', lib.SUM_NONE), ('TTSB_CONV1D_SUM_WRITE', lib.SUM_WRITE),
                          ('TTSB_CONV1D_SUM_ADD', lib.SUM_ADD), ('TTSB_CONV1D_SUM_FINISH', lib.SUM_FINISH)):
         assert re.search(r'#define %s (\d+)' % macro, header).group(1) == str(value), macro
+
+
+def _header_prototypes(header: str) -> dict:
+    """{function name: (return type, [parameter types])} of every prototype in the header, types as written."""
+    protos = {}
+    for ret, name, params in re.findall(r'^[ \t]*((?:const\s+)?\w+[\s*]*?)\s*\b(ttsb_\w+)\s*\(([^)]*)\)\s*;',
+                                        re.sub(r'/\*.*?\*/', '', header, flags=re.S), re.M):
+        params = [] if params.strip() == 'void' else [re.fullmatch(r'\s*(.*?)\s*\w+\s*', p, re.S).group(1) for p in params.split(',')]
+        protos[name] = (ret, params)
+    return protos
+
+
+def test_signatures_match_header(cdll):
+    """lib.SIGNATURES against every prototype of include/ttsb.h: the same names, and for each the return type and the type of
+    every parameter in order.  A pointer maps to c_void_p, except a pointer to a ttsb_*_args struct, which maps to a pointer
+    to its ctypes mirror.  load() declares every row, and no other module declares libttsb signatures."""
+    from transformertts_b200 import lib
+    protos = _header_prototypes((ROOT / 'include' / 'ttsb.h').read_text())
+    assert len(protos) >= 100
+    assert set(lib.SIGNATURES) == set(protos)
+    mirrors = _mirrors(lib)
+    scalars = {'int': C.c_int, 'int32_t': C.c_int, 'int64_t': C.c_int64, 'uint32_t': C.c_uint32, 'float': C.c_float,
+               'double': C.c_double}
+
+    def ctype(decl: str):
+        base = re.sub(r'\bconst\b', '', decl).replace('*', ' ').strip()
+        if decl.count('*') == 1 and re.fullmatch(r'ttsb_\w+_args', base):
+            return C.POINTER(mirrors[base])
+        return C.c_void_p if '*' in decl else scalars[base]
+
+    for name, (ret, params) in protos.items():
+        restype, argtypes = lib.SIGNATURES[name]
+        assert restype is {'const char*': C.c_char_p, 'void': None, **scalars}[ret], (name, ret)
+        assert len(argtypes) == len(params), name
+        for i, (have, decl) in enumerate(zip(argtypes, params)):
+            assert have is ctype(decl), (name, i, decl)
+        assert getattr(cdll, name).restype is restype and list(getattr(cdll, name).argtypes) == argtypes, name
+    for f in ROOT.rglob('*.py'):
+        if f != ROOT / 'transformertts_b200' / 'lib.py' and '_ref' not in f.parts:
+            assert not re.search(r'\.(argtypes|restype)\s*=', f.read_text()), f
 
 
 def test_argument_validation_without_gpu(cdll):
